@@ -1,4 +1,4 @@
-/* tetranerf_b200.h -- C ABI of the B200-native Tetra-NeRF ray-sampling hot path.
+/* tetranerf_b200.h -- C ABI of the H100-native Tetra-NeRF ray-sampling hot path.
  *
  * Drop-in boundary: these entry points are what the reference's pybind module
  * `tetranerf_cpp_extension` (src/py_binding.cpp:433-449) binds for this path.  Plain pointers and
@@ -122,8 +122,8 @@ int tn_render(tn_tracer *h, const tn_render_config *cfg, const float *d_origins,
  * ray, NULL = the eval-mode bins) and the training-mode RGBRenderer (no nan_to_num, no clamp).  Backward continues from the buffers of
  * the LAST training forward: d_grad_rgb f32[R,3] (+ optional d_grad_acc f32[R]) -> d_grad_field f32[64,V] (interpolate_values_backward,
  * src/tetrahedra_tracer.cu:223-248) and the twelve MLP gradients in the order / layouts of tn_render_set_weights; use_gradient_scaling =
- * GradientScaler (model.py:195-205,625-630).  Every output element is written.  The MLP backward runs on tcgen05 (recompute + dX + dW
- * GEMMs per 128-sample tile, weight gradients resident in TMEM); no [samples,128] tensor is materialised in HBM. */
+ * GradientScaler (model.py:195-205,625-630).  Every output element is written.  The MLP backward runs on wgmma (recompute + dX + dW
+ * GEMMs per 64-sample tile); no [samples,128] tensor is materialised in HBM. */
 int tn_render_train_forward(tn_tracer *h, const tn_render_config *cfg, const float *d_origins, const float *d_directions, uint32_t R,
                             const float *d_jitter_coarse, const float *d_jitter_fine, float *d_rgb, float *d_acc, float *d_depth,
                             uint8_t *d_mask, void *stream);
@@ -145,7 +145,7 @@ int tn_render_set_profiling(tn_tracer *h, int enable);
 int tn_render_get_timings(tn_tracer *h, float *ms6);
 /* the same for the last tn_render_train_backward: ms3 = composite_bwd, mlp_bwd, finalize */
 int tn_render_get_backward_timings(tn_tracer *h, float *ms3);
-/* trace_rays picks between bit-identical implementations by batch size (measured crossovers, profiles/r2_trace_sweep.json):
+/* trace_rays picks between bit-identical implementations by batch size:
  * >= walk_min_rays (default 2^20): adjacency walk, 32 rays per warp (throughput);
  * solo range [lo, hi] below that (default empty): adjacency walk, one ray per warp with cooperating lanes;
  * otherwise, for meshes that cannot be walked, and as the exact stage the walks fall back to: warp-per-ray all-hits BVH gather. */
@@ -153,7 +153,7 @@ int tn_set_walk_min_rays(tn_tracer *h, uint32_t n);
 int tn_set_walk_solo_range(tn_tracer *h, uint32_t lo, uint32_t hi);
 /* [lo, hi] below walk_min_rays (checked before the solo range): adjacency walk with 8 rays per warp, 4 cooperating lanes per ray */
 int tn_set_walk_quad_range(tn_tracer *h, uint32_t lo, uint32_t hi);
-/* the quad walk of batches of up to n rays (default 10240) loads the records of all candidate next tetrahedra while the current one
+/* the quad walk of batches of up to n rays (default 65536) loads the records of all candidate next tetrahedra while the current one
  * is intersected instead of prefetching them (latency-bound regime); 0 = never.  Results are identical. */
 int tn_set_walk_quad_spec_max_rays(tn_tracer *h, uint32_t n);
 /* out2[0] = 1 if the loaded mesh takes the adjacency-walk fast path (conforming, convex hull); out2[1] = rays of the last
@@ -164,24 +164,16 @@ int tn_debug_trace_stats(tn_tracer *h, uint32_t *out2);
  * num, dist, n_active, ray_list, ebins_c, sbins_c, vi_c, bary_c, dens_c, ebins_f, vi_f, bary_f, out_f,
  * dirbias, field shadow, weight image */
 int tn_render_debug_buffers(tn_tracer *h, void **ptrs16);
-/* one 128x128 tile out = A[128,K] * W[128,K]^T through the tcgen05 bf16x3 path; K in {64,128}; synchronous */
+/* one 128x128 tile out = A[128,K] * W[128,K]^T through the wgmma bf16x3 path (A from registers); K in {64,128}; synchronous */
 int tn_debug_gemm_bf16x3(int device, const float *d_A, const float *d_W, uint32_t K, float *d_out, void *stream);
 /* probe of the shared-memory operand forms of the fused MLP backward: P, Q f32[128,128] staged as bf16 hi/lo blocks
  * ([rows][64 columns], 128-byte swizzle); mode 0: out = P Q^T (both K-major), 1: out = P Q (B MN-major), 2: out = P^T Q (both
  * MN-major); N in {64,128}; lbo / sbo / kstep (bytes) describe the MN-major descriptors; synchronous */
 int tn_debug_gemm_modes(int device, int mode, uint32_t N, uint32_t lbo, uint32_t sbo, uint32_t kstep, const float *d_P,
                         const float *d_Q, float *d_out, void *stream);
-/* microbenchmark behind tools/mma_rate.py: cycles for nrep x 8 tcgen05.mma (M128 N128 K16 bf16); mode bit 0: two accumulators,
- * bit 1: A from shared memory instead of TMEM, bit 2: concurrent tcgen05.ld/st traffic; h_out2 = {issue cycles, issue+drain} */
-int tn_debug_mma_rate(int device, int nrep, int mode, uint32_t boff, long long *h_out2);
-/* in-kernel timeline of the NEXT fine-pass k_mlp launches (tools/mlp_timeline.py): device buffer of >= 65001 u64, first word
- * zeroed by the caller; [1..n] = (tag << 40 | clock) records of CTA 0, [1000 + 8 b ..] per-CTA start/end/smid/tile counts.
- * NULL switches it off. */
+/* per-CTA record of the NEXT fine-pass k_mlp launches: device buffer of >= 65001 u64, zeroed by the caller; [1000 + 8 b + 0] =
+ * start (ns), [+1] = end (ns), [+3] = tiles processed by CTA b.  NULL switches it off. */
 int tn_debug_set_timeline(void *d_buf);
-/* CTA-pair (cta_group::2) MMA bring-up / rate probe: out[256,128] = P[256,128] Q[128,128]^T with bf16x3 products on a 2-CTA cluster
- * (M = 256, N = 128 per instruction, each CTA holds half of B); ts != 0 takes the A operand from TMEM; bswap swaps the B halves;
- * h_cyc = {issue cycles, issue + completion} of nrep x 24 MMAs. */
-int tn_debug_cg2(int device, int nrep, int bswap, int ts, const float *d_P, const float *d_Q, float *d_out, long long *h_cyc);
 /* rays of the last tn_debug_trace_stats call that needed the all-hits gather (subset of out2[1]) */
 uint32_t tn_debug_last_exact_count(void);
 

@@ -1,4 +1,4 @@
-"""GPU: tensor-core building blocks of the fused MLP (tcgen05 bf16x3 GEMM with A in TMEM) vs fp32/fp64 torch."""
+"""GPU: tensor-core building blocks of the fused MLP (wgmma bf16x3 GEMM with A from registers) vs fp32/fp64 torch."""
 import ctypes
 
 import numpy as np

@@ -1,5 +1,5 @@
-"""GPU parity of find_visited_cells / interpolate_values(+backward): vs the CPU oracle (bit-exact) and vs the
-reference's OWN kernels compiled from /root/reference into oracle/_ref (few-ulp, --use_fast_math there)."""
+"""GPU parity of find_visited_cells / interpolate_values(+backward): vs the CPU oracle (bit-exact) and vs what the
+reference's OWN kernels computed on the same inputs (tests/golden/ref_kernels.npz; few-ulp, --use_fast_math there)."""
 import ctypes
 from pathlib import Path
 
@@ -12,14 +12,17 @@ from tetranerf.b200 import synthetic as syn
 
 pytestmark = pytest.mark.gpu
 DEV = torch.device("cuda:0")
-REF_SO = Path(__file__).resolve().parents[1] / "oracle" / "_ref" / "libref_kernels.so"
+GOLDEN_REF = Path(__file__).resolve().parent / "golden" / "ref_kernels.npz"
 
 
 @pytest.fixture(scope="module")
 def traced(small_mesh):
+    return make_traced(*small_mesh)
+
+
+def make_traced(V, C):
     from tetranerf import cpp
 
-    V, C = small_mesh
     tr = cpp.TetrahedraTracer(DEV)
     tr.load_tetrahedra(torch.from_numpy(V).to(DEV), torch.from_numpy(C).to(DEV))
     o, d = syn.camera_rays(400)
@@ -125,46 +128,44 @@ def test_interpolate_autograd_matches_einsum(traced):
     torch.testing.assert_close(field.grad, f2.grad, rtol=1e-4, atol=1e-4)
 
 
-@pytest.mark.skipif(not REF_SO.exists(), reason="oracle/_ref not built (needs /root/reference at build time)")
-def test_against_reference_kernels(traced):
-    """oracle/_ref/libref_kernels.so = src/tetrahedra_tracer.cu of the reference, compiled unmodified for
-    sm_100a with the reference's flags (-O3 --use_fast_math).  Indices exact; floats within a few ulp."""
+def ref_kernel_case(traced):
+    """the inputs the reference kernels were run on (tests/golden/make_ref_kernels.py), with this repo's outputs for them"""
     from tetranerf import cpp
 
-    ref = ctypes.CDLL(str(REF_SO))
     tr, out, dist, V, C = traced
     srt = torch.sort(dist, dim=1).values.contiguous()
     R, S = srt.shape
-    M = out["visited_cells"].shape[1]
     g = tr.find_visited_cells(out["num_visited_cells"], out["visited_cells"], out["barycentric_coordinates"], out["hit_distances"],
                               out["vertex_indices"], srt)
-    mask = torch.zeros((R, S), dtype=torch.bool, device=DEV)
-    cell = torch.full((R, S), -1, dtype=torch.int32, device=DEV)
-    bary = torch.zeros((R, S, 3), dtype=torch.float32, device=DEV)
-    verts = torch.full((R, S, 4), -1, dtype=torch.int32, device=DEV)
-    p = lambda t: ctypes.c_void_p(t.data_ptr())
-    torch.cuda.synchronize()
-    rc = ref.ref_find_matched_cells(ctypes.c_size_t(R), ctypes.c_size_t(S), ctypes.c_size_t(M), p(torch.from_numpy(C).to(DEV)),
-                                    p(out["num_visited_cells"]), p(out["visited_cells"]), p(out["hit_distances"]),
-                                    p(out["barycentric_coordinates"]), p(srt), p(out["vertex_indices"]), p(cell), p(verts), p(mask), p(bary))
-    assert rc == 0
-    assert torch.equal(mask, g["mask"]) and torch.equal(cell, g["cell_indices"]) and torch.equal(verts, g["vertex_indices"])
-    torch.testing.assert_close(bary, g["barycentric_coordinates"], rtol=2e-6, atol=2e-6)
-    # interpolation forward: FFMA chain -> expect bit-exact; backward: atomics -> tolerance
     field = torch.from_numpy(syn.random_field(len(V), 64)).to(DEV)
-    N = R * S
-    res = torch.empty((64, N), dtype=torch.float32, device=DEV)
-    rc = ref.ref_interpolate_values4(ctypes.c_uint32(len(V)), ctypes.c_uint32(N), ctypes.c_uint32(64), p(g["vertex_indices"]),
-                                     p(g["barycentric_coordinates"]), p(field), p(res))
-    assert rc == 0
-    mine = cpp.interpolate_values(g["vertex_indices"], g["barycentric_coordinates"], field)
-    torch.testing.assert_close(mine.reshape(N, 64), res.T.contiguous(), rtol=1e-6, atol=1e-6)
-    frac_exact = (mine.reshape(N, 64) == res.T).float().mean().item()
-    assert frac_exact > 0.99, frac_exact
-    gin = torch.randn((N, 64), device=DEV)
-    gref = torch.zeros((64, len(V)), device=DEV)
-    rc = ref.ref_interpolate_values_backward4(ctypes.c_uint32(len(V)), ctypes.c_uint32(N), ctypes.c_uint32(64), p(g["vertex_indices"]),
-                                              p(g["barycentric_coordinates"]), p(gin.T.contiguous()), p(gref))
-    assert rc == 0
+    gin = torch.randn((R * S, 64), generator=torch.Generator().manual_seed(21)).to(DEV)
+    mine = cpp.interpolate_values(g["vertex_indices"], g["barycentric_coordinates"], field).reshape(R * S, 64)
     gmine = cpp.interpolate_values_backward(g["vertex_indices"], g["barycentric_coordinates"], field, gin)
-    torch.testing.assert_close(gmine, gref, rtol=1e-4, atol=1e-4)
+    return srt, g, field, gin, mine, gmine
+
+
+def ref_kernel_sample(N, V):
+    """the fixed subset of samples / vertices stored in the golden file (the full outputs are tens of MB)"""
+    rng = np.random.default_rng(1234)
+    return np.sort(rng.choice(N, 1536, replace=False))[::3], np.sort(rng.choice(V, 1024, replace=False))[::4]
+
+
+def test_against_reference_kernels(traced):
+    """tests/golden/ref_kernels.npz = a fixed sample of what src/tetrahedra_tracer.cu of the reference, compiled unmodified with
+    the reference's flags (-O3 --use_fast_math, oracle/Makefile), computed on these inputs.  Indices exact; floats within a few ulp."""
+    gold = np.load(GOLDEN_REF)
+    srt, g, field, gin, mine, gmine = ref_kernel_case(traced)
+    R, S = srt.shape
+    idx, vidx = ref_kernel_sample(R * S, field.shape[1])
+    assert np.array_equal(idx, gold["idx"]) and np.array_equal(vidx, gold["vidx"])
+    flat = lambda t, k: t.reshape(R * S, k).cpu().numpy()[idx]
+    assert np.array_equal(flat(g["mask"], 1)[:, 0], gold["mask"])
+    assert np.array_equal(flat(g["cell_indices"], 1)[:, 0], gold["cell"])
+    assert np.array_equal(flat(g["vertex_indices"], 4), gold["verts"])
+    torch.testing.assert_close(torch.from_numpy(flat(g["barycentric_coordinates"], 3)), torch.from_numpy(gold["bary"]), rtol=2e-6, atol=2e-6)
+    # interpolation forward: FFMA chain -> expect bit-exact; backward: atomics -> tolerance
+    ours = mine.cpu().numpy()[idx]
+    torch.testing.assert_close(torch.from_numpy(ours), torch.from_numpy(gold["interp"]), rtol=1e-6, atol=1e-6)
+    frac_exact = (ours == gold["interp"]).mean()
+    assert frac_exact > 0.99, frac_exact
+    torch.testing.assert_close(torch.from_numpy(gmine.cpu().numpy()[:, vidx]), torch.from_numpy(gold["grad"]), rtol=1e-4, atol=1e-4)

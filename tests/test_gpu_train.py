@@ -1,13 +1,12 @@
-"""GPU parity of the fused TRAINING step (tn_render_train_forward / _backward: stratified bins, training-mode renderer, tcgen05 MLP
+"""GPU parity of the fused TRAINING step (tn_render_train_forward / _backward: stratified bins, training-mode renderer, wgmma MLP
 backward, field-gradient scatter) against torch-CPU autograd through the oracle (oracle.render_train = model.py:520-662 in training
 mode).  Forward pixels within 1e-4 absolute.  Gradients: the oracle is differentiated twice, in float32 (what the reference computes)
 and in float64 (the truth); the fine-pass sample positions come out of an fp32 PDF inversion and move by ~1e-6 between any two
 implementations, so torch's own fp32 gradient already differs from the float64 one by up to ~6e-4 of the tensor's largest entry.
-Measured (profiles/r2_train_gradients.md): the gradient itself is ill-conditioned in fp32 -- sums over ~10^5 samples with cancelling
+Measured with the oracle alone: the gradient itself is ill-conditioned in fp32 -- sums over ~10^5 samples with cancelling
 terms -- so torch's OWN fp32 autograd differs from the float64 gradient by 1e-6 (heads) ... 8e-5 (third layer) ... 6e-4
 (tetrahedra_field) of the tensor's largest entry, even at identical sample positions; an rtol of 1e-4 against an fp32 reference is
-not a meaningful bar for the early layers.  The kernel (bf16x3 products: 2^-17 operands instead of 2^-24) lands within 1x ... 4.5x of
-that fp32 noise.  Bars, per tensor (tetrahedra_field and each of the twelve MLP parameters), in units of the tensor's largest entry:
+not a meaningful bar for the early layers.  The kernel computes with bf16x3 products (2^-17 operands instead of 2^-24).  Bars, per tensor (tetrahedra_field and each of the twelve MLP parameters), in units of the tensor's largest entry:
   (A) gradient arithmetic only: the float64 oracle evaluated AT THE KERNEL'S OWN fine-pass bins (detached in the reference, so this
       isolates everything that is differentiated: interpolation, MLP, heads, compositing, gradient scaling);
   (B) end to end, every stage independent (the oracle's own bins);
@@ -130,7 +129,7 @@ def test_fused_train_step_gradients(small_mesh, cfgname, gs):
 
 
 def test_fused_train_step_is_repeatable_and_many_tiles(medium_mesh):
-    """more tiles than SMs (dynamic tile scheduler, several tiles per CTA: TMEM-resident dW accumulation across tiles) and a second call on the
+    """more tiles than SMs (dynamic tile scheduler, several tiles per CTA, dW reductions from every tile) and a second call on the
     same renderer (workspace reuse, counters reset)"""
     from tetranerf.b200.render import RenderSettings
 

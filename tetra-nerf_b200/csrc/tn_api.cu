@@ -37,8 +37,8 @@ int tn_create(int device, tn_tracer **out) {
     int major = 0, minor = 0;
     cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, device);
     cudaDeviceGetAttribute(&minor, cudaDevAttrComputeCapabilityMinor, device);
-    if (major != 10)
-        return tn::fail(TN_ERR_CUDA, "tetranerf_b200 is built for sm_100a only; device has compute capability " + std::to_string(major) + "." +
+    if (major != 9 || minor != 0)
+        return tn::fail(TN_ERR_CUDA, "tetranerf_b200 is built for sm_90a (H100) only; device has compute capability " + std::to_string(major) + "." +
                                          std::to_string(minor));
     tn_tracer *h = new tn_tracer();
     h->device = device;
@@ -138,7 +138,7 @@ int tn_peer_free(int device, void *d_ptr) {
 }
 
 // batches with at least `n` rays take the adjacency-walk fast path of trace_rays (0 = always, UINT32_MAX = never);
-// measured crossover on B200 / 302k tetrahedra: ~10k rays (profiles/r1_trace_sweep.json)
+// (the default, 2^20, leaves batches of realistic size to the quad walk)
 extern "C" int tn_set_walk_min_rays(tn_tracer *h, uint32_t n) {
     if (!h) return tn::fail(TN_ERR_ARG, "null tracer");
     h->walk_min_rays = n;

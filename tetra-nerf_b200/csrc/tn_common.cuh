@@ -1,4 +1,4 @@
-// tn_common.cuh -- shared declarations of the B200-native Tetra-NeRF hot path (sm_100a only).
+// tn_common.cuh -- shared declarations of the H100-native Tetra-NeRF hot path (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -103,18 +103,17 @@ struct tn_tracer {
     uint32_t ovf_cap = 0;
     unsigned long long *d_walk_keys = nullptr;  // [R, M] (t, face) keys written by the adjacency walk
     size_t walk_keys_cap = 0;
-    // trace_rays picks between bit-identical implementations by batch size (measured on B200, 302k tetrahedra, profiles/r2_trace_sweep.json;
-    // trace time incl. L2 warm-up, ms at 1024 / 4096 / 8192 / 16384 / 65536 rays):
-    //   warp-per-ray all-hits BVH gather   0.19 / 0.31 / 0.57 / 1.02 / 3.51     <- below walk_quad_min_rays
-    //   walk, 8 rays per warp ("quad")     0.27 / 0.27 / 0.30 / 0.45 / 1.56     <- [walk_quad_min_rays, walk_min_rays)  (speculative record
-    //                                                                              loads up to walk_quad_spec_max_rays, prefetches above)
-    //   walk, 1 ray per warp ("solo")      0.26 / 0.35 / 0.55 / 1.00 / 3.57     (kept for tests / experiments: range empty by default)
-    //   walk, 32 rays per warp             0.66 / 0.67 / 0.68 / 0.81 / 1.95     <- >= walk_min_rays (fewest instructions per ray: only pays off
-    //                                                                              once the machine is full several times over)
+    // trace_rays picks between bit-identical implementations by batch size:
+    //   warp-per-ray all-hits BVH gather   <- below walk_quad_min_rays (latency of the few rays in flight dominates)
+    //   walk, 8 rays per warp ("quad")     <- [walk_quad_min_rays, walk_min_rays)  (speculative record loads up to walk_quad_spec_max_rays,
+    //                                         prefetches above)
+    //   walk, 1 ray per warp ("solo")      (kept for tests / experiments: range empty by default)
+    //   walk, 32 rays per warp             <- >= walk_min_rays (fewest instructions per ray: only pays off once the machine is full
+    //                                         several times over)
     uint32_t walk_min_rays = 1u << 20;
     uint32_t walk_solo_min_rays = 1, walk_solo_max_rays = 0;
     uint32_t walk_quad_min_rays = 3584, walk_quad_max_rays = 0xFFFFFFFFu;
-    uint32_t walk_quad_spec_max_rays = 10240;  // quad walk: batches up to this size load the candidate next records speculatively (tn_walk.cu)
+    uint32_t walk_quad_spec_max_rays = 65536;  // quad walk: batches up to this size load the candidate next records speculatively (tn_walk.cu)
     uint64_t launches = 0;
     tn::RenderState *render = nullptr;
 };

@@ -1,7 +1,6 @@
-// tn_mlp_debug.cu -- one-tile bf16x3 GEMM on tcgen05 used by tests to validate, in isolation, the pieces
-// the fused MLP kernel relies on: weight image (hi/lo bf16, 128-byte swizzle) staged by TMA bulk copy,
-// A operand written into TMEM by tcgen05.st (thread = row), tcgen05.mma kind::f16 with A from TMEM,
-// accumulator read back with tcgen05.ld.  out[128,128] = A[128,K] * W[128,K]^T with ~fp32 accuracy.
+// tn_mlp_debug.cu -- one-tile bf16x3 GEMMs on wgmma used by tests to validate, in isolation, the pieces the fused MLP kernels rely
+// on: the weight image (hi/lo bf16, 128-byte swizzle) staged by TMA bulk copy, A fragments in registers (thread layout of
+// tn_tc.cuh), and the K-major / MN-major shared-memory descriptors of the backward kernel.
 #include "tn_common.cuh"
 #include "tn_mlp_pack.cuh"
 #include "tn_tc.cuh"
@@ -9,76 +8,48 @@
 namespace tn {
 using namespace tc;
 
-__global__ void __launch_bounds__(160, 1) k_debug_gemm(const float *__restrict__ A, const uint8_t *__restrict__ wimg, uint32_t K,
+// out[128,128] = A[128,K] * W[128,K]^T: two warpgroups of 64 rows, A split into bf16 hi/lo register fragments, W from the forward
+// weight image (per 64-wide K block: hi 16 KB, lo 16 KB)
+__global__ void __launch_bounds__(256, 1) k_debug_gemm(const float *__restrict__ A, const uint8_t *__restrict__ wimg, uint32_t K,
                                                         float *__restrict__ out) {
     extern __shared__ __align__(1024) uint8_t smem[];
-    uint8_t *w_s = smem;  // K/64 * 32 KB
-    uint64_t *bars = reinterpret_cast<uint64_t *>(smem + 65536);
-    uint32_t *tmem_ptr = reinterpret_cast<uint32_t *>(smem + 65536 + 64);
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    uint64_t *bar = reinterpret_cast<uint64_t *>(smem + 65536);
     const uint32_t wbytes = (K / 64) * 32768u;
-    if (warp == 4) {
-        if (lane == 0) { mbar_init(&bars[0], 1); mbar_init(&bars[1], 1); fence_barrier_init(); }
-        __syncwarp();
-        tmem_alloc(tmem_ptr, 512);
-    }
-    fence_before_sync();
+    const uint32_t wg = threadIdx.x >> 7, warp = (threadIdx.x >> 5) & 3u, lane = threadIdx.x & 31u, g = lane >> 2, t = lane & 3u;
+    if (threadIdx.x == 0) { mbar_init(bar, 1); fence_barrier_init(); }
     __syncthreads();
-    fence_after_sync();
-    const uint32_t tbase = *tmem_ptr;
-    if (warp == 4) {
-        if (lane == 0) {
-            mbar_arrive_expect_tx(&bars[0], wbytes);
-            for (uint32_t off = 0; off < wbytes; off += 16384) tma_bulk_g2s(w_s + off, wimg + off, 16384, &bars[0]);
-        }
-    } else {
-        const uint32_t row = threadIdx.x;
-        const uint32_t lane_base = (uint32_t)(warp * 32) << 16;
-        for (uint32_t c = 0; c < K / 16; ++c) {  // 16 elements -> 8 packed columns
-            uint32_t hi[8], lo[8];
+    if (threadIdx.x == 0) {
+        mbar_arrive_expect_tx(bar, wbytes);
+        for (uint32_t off = 0; off < wbytes; off += 16384) tma_bulk_g2s(smem + off, wimg + off, 16384, bar);
+    }
+    const uint32_t r0 = wg * 64u + warp * 16u + g;
+    float d[64];
 #pragma unroll
-            for (int i = 0; i < 8; ++i) split_pack2(A[row * K + c * 16 + 2 * i], A[row * K + c * 16 + 2 * i + 1], hi[i], lo[i]);
-            tmem_st8(tbase + lane_base + 128 + c * 8, hi);
-            tmem_st8(tbase + lane_base + 192 + c * 8, lo);
-        }
-        tmem_st_wait();
-    }
-    fence_before_sync();
-    __syncthreads();
-    fence_after_sync();
-    if (warp == 4 && lane == 0) {
-        mbar_wait(&bars[0], 0);
-        const uint32_t idesc = make_idesc_bf16(128, 128);
-        uint32_t acc = 0;
-        for (uint32_t kb = 0; kb < K / 64; ++kb) {
-            const uint32_t w_hi = smem_u32(w_s + kb * 32768u), w_lo = w_hi + 16384u;
-            for (int term = 0; term < 3; ++term) {  // (A_hi,W_hi) (A_lo,W_hi) (A_hi,W_lo)
-                const uint32_t a_col = (term == 1 ? 192u : 128u) + kb * 32u;
-                const uint32_t wb = term == 2 ? w_lo : w_hi;
-                for (uint32_t k = 0; k < 4; ++k) {
-                    mma_ts(tbase, tbase + a_col + k * 8, make_desc_sw128(wb + k * 32u), idesc, acc);
-                    acc = 1;
-                }
-            }
-        }
-        mma_commit(&bars[1]);
-    }
-    if (warp < 4) {
-        mbar_wait(&bars[1], 0);
-        fence_after_sync();
-        const uint32_t row = threadIdx.x;
-        const uint32_t lane_base = (uint32_t)(warp * 32) << 16;
-        for (uint32_t ch = 0; ch < 4; ++ch) {
-            uint32_t r[32];
-            tmem_ld32(tbase + lane_base + ch * 32, r);
-            tmem_ld_wait();
+    for (int i = 0; i < 64; ++i) d[i] = 0.f;
+    mbar_wait(bar, 0);
+    const uint32_t ws = smem_u32(smem);
+    for (uint32_t kk = 0; kk < K / 16; ++kk) {
+        uint32_t ah[4], al[4];
 #pragma unroll
-            for (int i = 0; i < 32; ++i) out[row * 128 + ch * 32 + i] = __uint_as_float(r[i]);
+        for (int i = 0; i < 4; ++i) {
+            const uint32_t row = r0 + 8u * (i & 1), col = kk * 16u + 8u * (i >> 1) + 2u * t;
+            split_pack2(A[row * K + col], A[row * K + col + 1], ah[i], al[i]);
         }
+        const uint32_t wb = ws + (kk >> 2) * 32768u + (kk & 3u) * 32u;
+        wgmma_fence();
+        wgmma_rs_bf16_n128<0>(d, ah, make_desc(wb), 1u);
+        wgmma_rs_bf16_n128<0>(d, al, make_desc(wb), 1u);
+        wgmma_rs_bf16_n128<0>(d, ah, make_desc(wb + 16384u), 1u);
+        wgmma_commit();
+        wgmma_wait0();
     }
-    fence_before_sync();
-    __syncthreads();
-    if (warp == 4) tmem_dealloc(tbase, 512);
+    reg_fence(d);
+#pragma unroll
+    for (int j = 0; j < 16; ++j) {
+        const uint32_t c = 8u * j + 2u * t;
+        out[r0 * 128 + c] = d[4 * j]; out[r0 * 128 + c + 1] = d[4 * j + 1];
+        out[(r0 + 8) * 128 + c] = d[4 * j + 2]; out[(r0 + 8) * 128 + c + 1] = d[4 * j + 3];
+    }
 }
 
 }  // namespace tn
@@ -93,107 +64,45 @@ extern "C" int tn_debug_gemm_bf16x3(int device, const float *d_A, const float *d
     tn::launch_pack_weights(d_W, K, 0, K, img, s);
     const int smem = 65536 + 128;
     TN_CUDA(cudaFuncSetAttribute(tn::k_debug_gemm, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    tn::k_debug_gemm<<<1, 160, smem, s>>>(d_A, img, K, d_out);
+    tn::k_debug_gemm<<<1, 256, smem, s>>>(d_A, img, K, d_out);
     TN_CUDA(cudaGetLastError());
     TN_CUDA(cudaStreamSynchronize(s));
     cudaFree(img);
     return TN_OK;
 }
 
-// ---- microbenchmark: cycles per tcgen05.mma (M=128, N=128, K=16, bf16) in TS (A from TMEM) and SS (A from smem) mode ----
+// ---- the three operand forms of the fused MLP backward, from shared memory: ------------------------------------------------------
+// mode 0: out = P Q^T (A, B K-major)   mode 1: out = P Q (A K-major, B MN-major)   mode 2: out = P^T Q (A, B MN-major)
+// P, Q f32[128,128] are stored as bf16 hi/lo [row][64-column block] images (block stride 32 KB, lo 16 KB after hi); two
+// warpgroups own output rows 0..63 / 64..127.
 namespace tn {
-using namespace tc;
-__global__ void __launch_bounds__(160, 1) k_debug_mma_rate(long long *out, int nrep, int mode, uint32_t boff) {
-    extern __shared__ __align__(1024) uint8_t smem[];
-    uint64_t *bars = reinterpret_cast<uint64_t *>(smem + 212992);
-    uint32_t *tmem_ptr = reinterpret_cast<uint32_t *>(smem + 212992 + 64);
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    for (uint32_t i = threadIdx.x; i < 212992 / 4; i += blockDim.x) reinterpret_cast<uint32_t *>(smem)[i] = 0x3c003c00u;
-    if (warp == 4) {
-        if (lane == 0) { mbar_init(&bars[0], 1); fence_barrier_init(); }
-        __syncwarp();
-        tmem_alloc(tmem_ptr, 512);
-    }
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-    fence_before_sync();
-    __syncthreads();
-    fence_after_sync();
-    const uint32_t tbase = *tmem_ptr;
-    if (warp < 4 && (mode & 4)) {
-        // concurrent epilogue-like TMEM traffic on the other accumulator: ld 32 cols + st 16 cols in a loop
-        const uint32_t lane_base = (uint32_t)(warp * 32) << 16;
-        uint32_t r[32];
-        for (int it = 0; it < nrep * 6; ++it) {
-            tmem_ld32(tbase + lane_base + 256u + (uint32_t)(it & 3) * 32u, r);
-            tmem_ld_wait();
-            tmem_st16(tbase + lane_base + 384u + (uint32_t)(it & 3) * 16u, r);
-            tmem_st_wait();
+template <int MODE, int N>
+__device__ __forceinline__ void gemm_modes_body(uint32_t pa, uint32_t qa, uint32_t wg, uint32_t lbo, uint32_t sbo, uint32_t kstep, float (&d)[N / 2]) {
+    constexpr int TA = MODE == 2 ? 1 : 0, TB = MODE >= 1 ? 1 : 0;
+    wgmma_fence();
+    for (int term = 0; term < 3; ++term) {  // (P_hi,Q_hi) (P_lo,Q_hi) (P_hi,Q_lo)
+        const uint32_t po = term == 1 ? 16384u : 0u, qo = term == 2 ? 16384u : 0u;
+        for (uint32_t j = 0; j < 8; ++j) {  // 8 k-steps of 16
+            // K-major: k-step j lives in column block j/4 at byte 32 (j%4) of every row; MN-major: rows 16j.. of every block
+            const uint64_t da = TA ? make_desc(pa + po + wg * 32768u + j * kstep, lbo, sbo)
+                                   : make_desc(pa + po + (j >> 2) * 32768u + wg * 8192u + (j & 3u) * 32u);
+            const uint64_t db = TB ? make_desc(qa + qo + j * kstep, lbo, sbo) : make_desc(qa + qo + (j >> 2) * 32768u + (j & 3u) * 32u);
+            if constexpr (N == 128) wgmma_ss_bf16_n128<TA, TB>(d, da, db, 1u);
+            else wgmma_ss_bf16_n64<TA, TB>(d, da, db, 1u);
         }
     }
-    if (warp == 4 && lane == 0) {
-        const uint32_t idesc = make_idesc_bf16(128, 128);
-        const uint64_t dw = make_desc_sw128(smem_u32(smem + boff));
-        const long long t0 = clock64();
-        for (int r = 0; r < nrep; ++r) {
-#pragma unroll
-            for (int k = 0; k < 8; ++k) {
-                // mode 0: TS, one accumulator; 1: TS, two accumulators alternating; 2: SS, one accumulator; 3: SS two accumulators
-                const uint32_t d = tbase + ((mode & 1) ? (uint32_t)(k & 1) * 256u : 0u);
-                const uint64_t b = dw + (uint64_t)((k & 3) * 2 + (k >> 2) * 1024);
-                if ((mode & 3) < 2) mma_ts_c<true>(d, tbase + 128u + (uint32_t)k * 8u, b, idesc);
-                else mma_ss(d, dw + 4096ull + (uint64_t)((k & 3) * 2), b, idesc, 1);
-            }
-        }
-        const long long t1 = clock64();
-        mma_commit(&bars[0]);
-        mbar_wait(&bars[0], 0);
-        const long long t2 = clock64();
-        out[0] = t1 - t0;
-        out[1] = t2 - t0;
-    }
-    fence_before_sync();
-    __syncthreads();
-    if (warp == 4) tmem_dealloc(tbase, 512);
-}
-}  // namespace tn
-
-extern "C" int tn_debug_mma_rate(int device, int nrep, int mode, uint32_t boff, long long *h_out2) {
-    tn::DeviceGuard g(device);
-    long long *d = nullptr;
-    TN_CUDA(cudaMalloc(&d, 16));
-    const int smem = 212992 + 128;
-    TN_CUDA(cudaFuncSetAttribute(tn::k_debug_mma_rate, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    tn::k_debug_mma_rate<<<1, 160, smem>>>(d, nrep, mode, boff);
-    TN_CUDA(cudaDeviceSynchronize());
-    TN_CUDA(cudaMemcpy(h_out2, d, 16, cudaMemcpyDeviceToHost));
-    cudaFree(d);
-    return TN_OK;
+    wgmma_commit();
+    wgmma_wait0();
+    reg_fence(d);
 }
 
-// ---- probe for the operand forms of the fused MLP backward (tn_mlp_bwd.cuh): every operand is a [128 rows][128 cols] fp32
-// matrix staged in shared memory as bf16 hi/lo in the ONE layout the backward kernel uses -- per 64-column block:
-// [hi 16 KB][lo 16 KB], rows of 128 bytes, 128-byte swizzle -- and is read either K-major (the K index runs along the
-// columns) or MN-major (the K index runs along the ROWS; the M/N index along the columns: bit 15 / 16 of the instruction
-// descriptor).  mode 0: out = P Q^T (A, B K-major: the forward form);  mode 1: out = P Q (A K-major, B MN-major: dX = dA W);
-// mode 2: out = P^T Q (A, B MN-major: dW = dA^T H).  N in {64, 128} (mode 0: rows of Q; modes 1, 2: columns of Q).
-namespace tn {
-using namespace tc;
-__device__ __forceinline__ uint64_t make_desc_rt(uint32_t smem_addr, uint32_t lbo, uint32_t sbo) {
-    return (uint64_t)((smem_addr & 0x3FFFFu) >> 4) | ((uint64_t)((lbo >> 4) & 0x3FFFu) << 16) | ((uint64_t)((sbo >> 4) & 0x3FFFu) << 32) | (1ull << 46) |
-           (2ull << 61);
-}
-__global__ void __launch_bounds__(160, 1) k_debug_gemm2(const float *__restrict__ P, const float *__restrict__ Q, int mode, uint32_t N,
-                                                         uint32_t lbo, uint32_t sbo, uint32_t kstep, float *__restrict__ out) {
+template <int N>
+__global__ void __launch_bounds__(256, 1) k_debug_gemm2(const float *__restrict__ P, const float *__restrict__ Q, int mode, uint32_t lbo, uint32_t sbo,
+                                                         uint32_t kstep, float *__restrict__ out) {
     extern __shared__ __align__(1024) uint8_t smem[];
     uint8_t *p_s = smem, *q_s = smem + 65536;
-    uint64_t *bars = reinterpret_cast<uint64_t *>(smem + 131072);
-    uint32_t *tmem_ptr = reinterpret_cast<uint32_t *>(smem + 131072 + 64);
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    if (warp == 4) {
-        if (lane == 0) { mbar_init(&bars[0], 1); fence_barrier_init(); }
-        __syncwarp();
-        tmem_alloc(tmem_ptr, 128);
-    } else {
+    const uint32_t wg = threadIdx.x >> 7, warp = (threadIdx.x >> 5) & 3u, lane = threadIdx.x & 31u, g = lane >> 2, t = lane & 3u;
+    if (threadIdx.x < 128) {
         const uint32_t row = threadIdx.x;
         for (uint32_t k = 0; k < 128; k += 2) {
             uint32_t hi, lo;
@@ -205,198 +114,37 @@ __global__ void __launch_bounds__(160, 1) k_debug_gemm2(const float *__restrict_
             *reinterpret_cast<uint32_t *>(q_s + off) = hi;
             *reinterpret_cast<uint32_t *>(q_s + off + 16384u) = lo;
         }
-        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+        fence_proxy_async();
     }
-    fence_before_sync();
     __syncthreads();
-    fence_after_sync();
-    const uint32_t tbase = *tmem_ptr;
-    if (warp == 4 && lane == 0) {
-        const uint32_t idesc = make_idesc_bf16(128, N) | (mode == 2 ? (1u << 15) : 0u) | (mode >= 1 ? (1u << 16) : 0u);
-        const uint32_t pa = smem_u32(p_s), qa = smem_u32(q_s);
-        uint32_t acc = 0;
-        for (int term = 0; term < 3; ++term) {  // (P_hi,Q_hi) (P_lo,Q_hi) (P_hi,Q_lo)
-            const uint32_t po = term == 1 ? 16384u : 0u, qo = term == 2 ? 16384u : 0u;
-            for (uint32_t j = 0; j < 8; ++j) {  // 8 k-steps of 16
-                // K-major: k-step j lives in column block j/4 at byte 32 (j%4) of every row; MN-major: rows 16j.. of every block
-                const uint64_t da = mode == 2 ? make_desc_rt(pa + po + j * kstep, lbo, sbo) : make_desc_sw128(pa + po + (j >> 2) * 32768u + (j & 3u) * 32u);
-                const uint64_t db = mode >= 1 ? make_desc_rt(qa + qo + j * kstep, lbo, sbo) : make_desc_sw128(qa + qo + (j >> 2) * 32768u + (j & 3u) * 32u);
-                mma_ss(tbase, da, db, idesc, acc);
-                acc = 1;
-            }
-        }
-        mma_commit(&bars[0]);
-    }
-    if (warp < 4) {
-        mbar_wait(&bars[0], 0);
-        fence_after_sync();
-        const uint32_t row = threadIdx.x;
-        const uint32_t lane_base = (uint32_t)(warp * 32) << 16;
-        for (uint32_t ch = 0; ch < N / 32; ++ch) {
-            uint32_t r[32];
-            tmem_ld32(tbase + lane_base + ch * 32, r);
-            tmem_ld_wait();
+    const uint32_t pa = smem_u32(p_s), qa = smem_u32(q_s);
+    float d[N / 2];
 #pragma unroll
-            for (int i = 0; i < 32; ++i) out[row * 128 + ch * 32 + i] = __uint_as_float(r[i]);
-        }
+    for (int i = 0; i < N / 2; ++i) d[i] = 0.f;
+    if (mode == 0) gemm_modes_body<0, N>(pa, qa, wg, lbo, sbo, kstep, d);
+    else if (mode == 1) gemm_modes_body<1, N>(pa, qa, wg, lbo, sbo, kstep, d);
+    else gemm_modes_body<2, N>(pa, qa, wg, lbo, sbo, kstep, d);
+    const uint32_t r0 = wg * 64u + warp * 16u + g;
+#pragma unroll
+    for (int j = 0; j < N / 8; ++j) {
+        const uint32_t c = 8u * j + 2u * t;
+        out[r0 * 128 + c] = d[4 * j]; out[r0 * 128 + c + 1] = d[4 * j + 1];
+        out[(r0 + 8) * 128 + c] = d[4 * j + 2]; out[(r0 + 8) * 128 + c + 1] = d[4 * j + 3];
     }
-    fence_before_sync();
-    __syncthreads();
-    if (warp == 4) tmem_dealloc(tbase, 128);
 }
 }  // namespace tn
-
-// ---- CTA-pair MMA (cta_group::2): bring-up + rate probe ----------------------------------------------------------------------
-// out[256,128] = P[256,128] Q[128,128]^T with bf16x3 products.  Two CTAs of one cluster: CTA r holds A rows 128r..128r+127 and
-// HALF of B (64 of the 128 rows of Q); the leader (rank 0) issues M = 256, N = 128 MMAs, the accumulator rows 128r.. land in CTA
-// r's TMEM, one multicast commit releases the epilogue warps of both CTAs.  ts != 0: the A operand comes from TMEM (each CTA
-// copies its hi / lo A rows into its own TMEM columns 128.. first).  nrep > 1 repeats the 24 MMAs (accumulating) for the rate.
-namespace tn {
-__device__ __forceinline__ uint32_t cluster_ctarank() { uint32_t r; asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r)); return r; }
-__device__ __forceinline__ void cluster_sync_all() {
-    asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-    asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_alloc2(uint32_t *dst_smem, uint32_t ncols) {  // whole warp, in both CTAs of the pair
-    asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)), "r"(ncols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc2(uint32_t taddr, uint32_t ncols) {
-    asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void mma2_ss(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\ttcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(d_tmem),
-                 "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate) : "memory");
-}
-__device__ __forceinline__ void mma2_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\ttcgen05.mma.cta_group::2.kind::f16 [%0], [%1], %2, %3, p;\n\t}" ::"r"(d_tmem),
-                 "r"(a_tmem), "l"(b_desc), "r"(idesc), "r"(accumulate) : "memory");
-}
-__device__ __forceinline__ void mma2_commit_mc(uint64_t *bar, uint16_t mask) {
-    asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(smem_u32(bar)), "h"(mask) : "memory");
-}
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(160, 1)
-k_debug_cg2(const float *__restrict__ P, const float *__restrict__ Q, int nrep, int bswap, int ts, float *__restrict__ out, long long *__restrict__ cyc) {
-    extern __shared__ __align__(1024) uint8_t smem[];
-    uint8_t *p_s = smem, *q_s = smem + 65536;  // A: 2 K blocks x (hi 16K | lo 16K); B: 2 K blocks x (hi 8K | lo 8K)
-    uint64_t *bars = reinterpret_cast<uint64_t *>(smem + 98304);
-    uint32_t *tmem_ptr = reinterpret_cast<uint32_t *>(smem + 98304 + 64);
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const uint32_t rank = cluster_ctarank();
-    if (warp == 4) {
-        if (lane == 0) { mbar_init(&bars[0], 1); mbar_init(&bars[1], 1); fence_barrier_init(); }
-        __syncwarp();
-        tmem_alloc2(tmem_ptr, 256);
-    } else {
-        const uint32_t row = threadIdx.x;
-        for (uint32_t k = 0; k < 128; k += 2) {
-            uint32_t hi, lo;
-            const uint32_t off = (k >> 6) * 32768u + sw128_offset(row, k & 63u);
-            split_pack2(P[(128u * rank + row) * 128 + k], P[(128u * rank + row) * 128 + k + 1], hi, lo);
-            *reinterpret_cast<uint32_t *>(p_s + off) = hi;
-            *reinterpret_cast<uint32_t *>(p_s + off + 16384u) = lo;
-            if (row < 64) {
-                const uint32_t qrow = 64u * (rank ^ (uint32_t)bswap) + row;
-                const uint32_t qoff = (k >> 6) * 16384u + sw128_offset(row, k & 63u);
-                split_pack2(Q[qrow * 128 + k], Q[qrow * 128 + k + 1], hi, lo);
-                *reinterpret_cast<uint32_t *>(q_s + qoff) = hi;
-                *reinterpret_cast<uint32_t *>(q_s + qoff + 8192u) = lo;
-            }
-        }
-        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-    }
-    fence_before_sync();
-    __syncthreads();
-    fence_after_sync();
-    const uint32_t tbase = *tmem_ptr;
-    if (ts && warp < 4) {  // A operand into TMEM: columns 128..191 hi, 192..255 lo (packed pairs: column c holds K elements 2c, 2c+1)
-        const uint32_t row = threadIdx.x, lane_base = (uint32_t)(warp * 32) << 16;
-        for (uint32_t c0 = 0; c0 < 64; c0 += 8) {
-            uint32_t ph[8], pl[8];
-#pragma unroll
-            for (int i = 0; i < 8; ++i) {
-                const uint32_t k = 2 * (c0 + i);
-                split_pack2(P[(128u * rank + row) * 128 + k], P[(128u * rank + row) * 128 + k + 1], ph[i], pl[i]);
-            }
-            tmem_st8(tbase + lane_base + 128 + c0, ph);
-            tmem_st8(tbase + lane_base + 192 + c0, pl);
-        }
-        tmem_st_wait();
-    }
-    fence_before_sync();
-    cluster_sync_all();
-    fence_after_sync();
-    if (rank == 0 && warp == 4 && lane == 0) {
-        const uint32_t idesc = make_idesc_bf16(256, 128);
-        const uint32_t pa = smem_u32(p_s), qa = smem_u32(q_s);
-        const long long t0 = clock64();
-        uint32_t acc = 0;
-        for (int rep = 0; rep < nrep; ++rep) {
-            for (int term = 0; term < 3; ++term) {  // (P_hi,Q_hi) (P_lo,Q_hi) (P_hi,Q_lo)
-                const uint32_t po = term == 1 ? 16384u : 0u, qo = term == 2 ? 8192u : 0u;
-                for (uint32_t j = 0; j < 8; ++j) {  // 8 k-steps of 16
-                    const uint64_t db = make_desc_sw128(qa + qo + (j >> 2) * 16384u + (j & 3u) * 32u);
-                    if (ts) {
-                        mma2_ts(tbase, tbase + (term == 1 ? 192u : 128u) + j * 8u, db, idesc, acc);
-                    } else {
-                        const uint64_t da = make_desc_sw128(pa + po + (j >> 2) * 32768u + (j & 3u) * 32u);
-                        mma2_ss(tbase, da, db, idesc, acc);
-                    }
-                    acc = 1;
-                }
-            }
-        }
-        const long long t1 = clock64();
-        mma2_commit_mc(&bars[0], (uint16_t)3);
-        mbar_wait(&bars[0], 0);
-        const long long t2 = clock64();
-        cyc[0] = t1 - t0; cyc[1] = t2 - t0;
-    }
-    if (warp < 4) {
-        mbar_wait(&bars[0], 0);
-        fence_after_sync();
-        const uint32_t row = threadIdx.x;
-        const uint32_t lane_base = (uint32_t)(warp * 32) << 16;
-        for (uint32_t ch = 0; ch < 4; ++ch) {
-            uint32_t r[32];
-            tmem_ld32(tbase + lane_base + ch * 32, r);
-            tmem_ld_wait();
-#pragma unroll
-            for (int i = 0; i < 32; ++i) out[(128u * rank + row) * 128 + ch * 32 + i] = __uint_as_float(r[i]);
-        }
-    }
-    fence_before_sync();
-    cluster_sync_all();
-    if (warp == 4) tmem_dealloc2(tbase, 256);
-}
-}  // namespace tn
-
-// test hook: d_P f32[256,128], d_Q f32[128,128], d_out f32[256,128]; h_cyc = {issue cycles, issue + completion} of nrep x 24 MMAs
-extern "C" int tn_debug_cg2(int device, int nrep, int bswap, int ts, const float *d_P, const float *d_Q, float *d_out, long long *h_cyc) {
-    tn::DeviceGuard g(device);
-    const int smem = 98304 + 128;
-    long long *d_cyc = nullptr;
-    TN_CUDA(cudaMalloc((void **)&d_cyc, 16));
-    TN_CUDA(cudaMemset(d_cyc, 0, 16));
-    TN_CUDA(cudaFuncSetAttribute(tn::k_debug_cg2, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    tn::k_debug_cg2<<<2, 160, smem>>>(d_P, d_Q, nrep, bswap, ts, d_out, d_cyc);
-    TN_CUDA(cudaGetLastError());
-    TN_CUDA(cudaDeviceSynchronize());
-    TN_CUDA(cudaMemcpy(h_cyc, d_cyc, 16, cudaMemcpyDeviceToHost));
-    cudaFree(d_cyc);
-    return TN_OK;
-}
 
 // test hook: d_P, d_Q f32[128,128], d_out f32[128,128] (first N columns written); lbo / sbo / kstep in bytes describe the
-// MN-major operands (the backward kernel uses lbo = 32768 (next 64-column block), sbo = 1024 (next 8 rows), kstep = 2048)
+// MN-major operands (the test uses lbo = 32768 (next 64-column block), sbo = 1024 (next 8 rows), kstep = 2048 (16 rows))
 extern "C" int tn_debug_gemm_modes(int device, int mode, uint32_t N, uint32_t lbo, uint32_t sbo, uint32_t kstep, const float *d_P,
                                    const float *d_Q, float *d_out, void *stream) {
     if (mode < 0 || mode > 2 || (N != 64 && N != 128)) return tn::fail(TN_ERR_ARG, "tn_debug_gemm_modes: mode in 0..2, N in {64,128}");
     tn::DeviceGuard g(device);
     cudaStream_t s = (cudaStream_t)stream;
-    const int smem = 131072 + 128;
-    TN_CUDA(cudaFuncSetAttribute(tn::k_debug_gemm2, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    tn::k_debug_gemm2<<<1, 160, smem, s>>>(d_P, d_Q, mode, N, lbo, sbo, kstep, d_out);
+    const int smem = 131072;
+    auto k = N == 128 ? tn::k_debug_gemm2<128> : tn::k_debug_gemm2<64>;
+    TN_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    k<<<1, 256, smem, s>>>(d_P, d_Q, mode, lbo, sbo, kstep, d_out);
     TN_CUDA(cudaGetLastError());
     TN_CUDA(cudaStreamSynchronize(s));
     return TN_OK;

@@ -1,9 +1,9 @@
 // tn_pairing.cuh -- from the sorted (t, face) keys of one ray to its records: the pairing stage of trace_rays
 // (post_process_tetrahedra, src/optix/optix_trace_rays.cu:110-266, and the record emission of :216-225 with combine_indices :39-75).
 // One warp per ray, keys and scratch in shared memory.  Used by k_trace<0> (tn_trace.cu) on keys gathered through the BVH or provided
-// by a walk.  (Round 2 also ran it at the tail of the quad walk, each warp pairing the keys of its own rays that met eps-ties: 24 us
-// SLOWER than the separate exact-stage launch at 4096 rays -- a warp with two or three such rays pairs them one after the other,
-// ~15 us each, while the exact stage gives every listed ray a warp of its own.  Removed; profiles/README.md.)
+// by a walk.  (Running it at the tail of the quad walk instead, each warp pairing the keys of its own rays that met eps-ties, was
+// slower than the separate exact-stage launch: a warp with two or three such rays pairs them one after the other, while the exact
+// stage gives every listed ray a warp of its own.)
 #ifndef TN_PAIRING_CUH
 #define TN_PAIRING_CUH
 #include "tn_common.cuh"

@@ -1,4 +1,4 @@
-// tn_render.cu -- fused forward render: trace -> sample -> (interp+MLP on tcgen05) -> PDF -> (interp+MLP) -> composite.
+// tn_render.cu -- fused forward render: trace -> sample -> (interp+MLP on wgmma) -> PDF -> (interp+MLP) -> composite.
 //
 // Replaces TetrahedraNerf.get_outputs between trace_rays and the pixel (tetranerf/nerfstudio/model.py:531-662)
 // in eval mode, i.e. the un-vendored nerfstudio pieces it calls (restated in oracle/oracle.py):
@@ -52,8 +52,7 @@ struct RenderState {
     float *sbins_f = nullptr, *enc = nullptr;   // [R,S2+1] spacing bins of the fine pass, [R,27] encoded directions (per slot)
     float4 *dout = nullptr;            // [R*S2] gradients at the head pre-activations
     float *gshadow = nullptr, *gw = nullptr, *g_dirbias = nullptr;
-    uint8_t *scratch = nullptr;
-    size_t cap_train_R = 0, cap_train_S2 = 0, cap_scratch = 0;
+    size_t cap_train_R = 0, cap_train_S2 = 0;
     uint32_t gshadow_V = 0;
     // what the last training forward ran with (the backward continues from its buffers)
     bool train_valid = false;
@@ -84,7 +83,6 @@ void free_render(tn_tracer *h) {
     free_ws(r);
     cudaFree(r->fshadow); cudaFree(r->wimg); cudaFree(r->wimg16); cudaFree(r->bias); cudaFree(r->head); cudaFree(r->w4dir);
     cudaFree(r->wimg_bwd); cudaFree(r->sbins_f); cudaFree(r->enc); cudaFree(r->dout); cudaFree(r->gshadow); cudaFree(r->gw); cudaFree(r->g_dirbias);
-    cudaFree(r->scratch);
     for (auto &e : r->ev) if (e) cudaEventDestroy(e);
     for (auto &e : r->evb) if (e) cudaEventDestroy(e);
     delete r;
@@ -707,7 +705,7 @@ extern "C" int tn_render_set_weights(tn_tracer *h, const float *const *P, void *
 struct TrainFwd {
     const float *jit_c, *jit_f;
 };
-static int ensure_train_ws(RenderState *r, size_t R, size_t S2, uint32_t V, int sms);
+static int ensure_train_ws(RenderState *r, size_t R, size_t S2, uint32_t V);
 
 static int render_impl(tn_tracer *h, const tn_render_config *cfg, const float *d_origins, const float *d_directions, uint32_t R,
                        float *d_rgb, float *d_acc, float *d_depth, uint8_t *d_mask, const TrainFwd *tf, void *stream) {
@@ -727,10 +725,8 @@ static int render_impl(tn_tracer *h, const tn_render_config *cfg, const float *d
     cudaStream_t s = (cudaStream_t)stream;
     int rc = ensure_ws(r, R, M, Sc, S2);
     if (rc) return rc;
-    int sms = 148;
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, h->device);
     if (tf != nullptr) {
-        rc = ensure_train_ws(r, R, S2, r->V, sms);
+        rc = ensure_train_ws(r, R, S2, r->V);
         if (rc) return rc;
     }
     r->train_valid = false;
@@ -780,8 +776,13 @@ static int render_impl(tn_tracer *h, const tn_render_config *cfg, const float *d
     mc.n_active = r->n_active; mc.S = Sc; mc.vi = r->vi_c; mc.bary = r->bary_c; mc.fshadow = r->fshadow; mc.wimg = prec == 2 ? r->wimg16 : r->wimg;
     mc.bias = r->bias; mc.head = r->head; mc.dirbias = nullptr; mc.out = r->dens_c;
     mc.tile_ctr = r->n_active + 1;  // words 1, 2 of the zeroed 16-byte block: tile counters of the coarse / fine pass
-    const uint32_t tiles_c = (uint32_t)(((uint64_t)R * Sc + 127) / 128), tiles_f = (uint32_t)(((uint64_t)R * S2 + 127) / 128);
-    if (!single) k_coarse<<<std::min<uint32_t>(tiles_c, (uint32_t)sms), MLP_THREADS, MLP_SMEM_BYTES, s>>>(mc);
+    // one CTA per SM at most (the weight image fills its shared memory), MLP_WGS tiles of MLP_TILE samples in flight per CTA
+    int sms = 132;
+    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, h->device);
+    const uint64_t tiles_c = ((uint64_t)R * Sc + MLP_TILE - 1) / MLP_TILE, tiles_f = ((uint64_t)R * S2 + MLP_TILE - 1) / MLP_TILE;
+    const uint32_t grid_c = (uint32_t)std::min<uint64_t>((tiles_c + MLP_WGS - 1) / MLP_WGS, (uint64_t)sms);
+    const uint32_t grid_f = (uint32_t)std::min<uint64_t>((tiles_f + MLP_WGS - 1) / MLP_WGS, (uint64_t)sms);
+    if (!single) k_coarse<<<grid_c, MLP_THREADS, MLP_SMEM_BYTES, s>>>(mc);
     TN_EV(3);
     if (!single) k_sample_fine<<<gridR, SAMPLE_WARPS * 32, smem_sf, s>>>(p);
     else k_dirbias_only<<<gridR, SAMPLE_WARPS * 32, 0, s>>>(p);
@@ -792,7 +793,7 @@ static int render_impl(tn_tracer *h, const tn_render_config *cfg, const float *d
     else p.ebins_f = r->ebins_c;  // k_composite integrates over the coarse bins
     mf.timeline = g_timeline;
     mf.tile_ctr = r->n_active + 2;
-    k_fine<<<std::min<uint32_t>(tiles_f, (uint32_t)sms), MLP_THREADS, MLP_SMEM_BYTES, s>>>(mf);
+    k_fine<<<grid_f, MLP_THREADS, MLP_SMEM_BYTES, s>>>(mf);
     TN_EV(5);
     k_composite<<<gridR, SAMPLE_WARPS * 32, smem_c, s>>>(p);
     TN_EV(6);
@@ -807,7 +808,7 @@ static int render_impl(tn_tracer *h, const tn_render_config *cfg, const float *d
     return TN_OK;
 }
 
-static int ensure_train_ws(RenderState *r, size_t R, size_t S2, uint32_t V, int sms) {
+static int ensure_train_ws(RenderState *r, size_t R, size_t S2, uint32_t V) {
     if (R > r->cap_train_R || S2 > r->cap_train_S2) {
         cudaFree(r->sbins_f); cudaFree(r->enc); cudaFree(r->dout); cudaFree(r->g_dirbias);
         r->sbins_f = r->enc = r->g_dirbias = nullptr; r->dout = nullptr;
@@ -823,12 +824,6 @@ static int ensure_train_ws(RenderState *r, size_t R, size_t S2, uint32_t V, int 
         cudaFree(r->gshadow); r->gshadow = nullptr;
         TN_CUDA(cudaMalloc((void **)&r->gshadow, sizeof(float) * 64 * (size_t)V));
         r->gshadow_V = V;
-    }
-    const size_t need = (size_t)sms * BWD_SCRATCH_PER_CTA;
-    if (r->cap_scratch < need) {
-        cudaFree(r->scratch); r->scratch = nullptr;
-        TN_CUDA(cudaMalloc((void **)&r->scratch, need));
-        r->cap_scratch = need;
     }
     return TN_OK;
 }
@@ -858,7 +853,7 @@ extern "C" int tn_render_train_backward(tn_tracer *h, const float *d_grad_rgb, c
     if (!r || !r->train_valid) return fail(TN_ERR_STATE, "tn_render_train_backward: no training forward to continue from");
     DeviceGuard g(h->device);
     cudaStream_t s = (cudaStream_t)stream;
-    int sms = 148;
+    int sms = 132;
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, h->device);
     const uint32_t R = r->t_R, S2 = r->t_S2, V = r->V;
     TN_CUDA(cudaMemsetAsync(r->gw, 0, sizeof(float) * GW_TOTAL, s));
@@ -877,11 +872,11 @@ extern "C" int tn_render_train_backward(tn_tracer *h, const float *d_grad_rgb, c
     if (r->profile) cudaEventRecord(r->evb[1], s);
     MlpBwdParams bp{};
     bp.n_active = r->n_active; bp.S = S2; bp.vi = r->vi_f; bp.bary = r->bary_f; bp.fshadow = r->fshadow; bp.wimg = r->wimg_bwd;
-    bp.bias = r->bias; bp.head = r->head; bp.dirbias = r->dirbias; bp.dout = r->dout; bp.scratch = r->scratch; bp.gshadow = r->gshadow;
+    bp.bias = r->bias; bp.head = r->head; bp.dirbias = r->dirbias; bp.dout = r->dout; bp.gshadow = r->gshadow;
     bp.gw = r->gw; bp.g_dirbias = r->g_dirbias; bp.tile_ctr = r->n_active + 3;
     TN_CUDA(cudaFuncSetAttribute(k_mlp_bwd, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)BWD_SMEM_BYTES));
-    const uint32_t tiles = (uint32_t)(((uint64_t)R * S2 + 127) / 128);
-    k_mlp_bwd<<<std::min<uint32_t>(tiles, (uint32_t)sms), BWD_THREADS, BWD_SMEM_BYTES, s>>>(bp);
+    const uint64_t tiles = ((uint64_t)R * S2 + BWD_TILE - 1) / BWD_TILE;
+    k_mlp_bwd<<<(uint32_t)std::min<uint64_t>(tiles, (uint64_t)sms), BWD_THREADS, BWD_SMEM_BYTES, s>>>(bp);
     if (r->profile) cudaEventRecord(r->evb[2], s);
     k_dirbias_grads<<<(R + DBG_SLOTS - 1) / DBG_SLOTS, 256, 0, s>>>(r->n_active, r->g_dirbias, r->enc, r->gw);
     GradOut go{};
@@ -939,7 +934,7 @@ extern "C" int tn_render_get_backward_timings(tn_tracer *h, float *ms3) {
     return TN_OK;
 }
 
-// debug: clock64 timeline of CTA 0 of the NEXT fine k_mlp launches (device buffer of >= 65001 u64, first word zeroed by caller)
+// debug: per-CTA start / end / tile count of the NEXT fine k_mlp launches (device buffer of >= 65001 u64, zeroed by the caller)
 extern "C" int tn_debug_set_timeline(void *d_buf) { g_timeline = (unsigned long long *)d_buf; return TN_OK; }
 
 // test / debug hook: device pointers of the intermediate buffers of the last tn_render call

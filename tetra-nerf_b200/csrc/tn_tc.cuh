@@ -1,6 +1,7 @@
-// tn_tc.cuh -- thin inline-PTX wrappers for the sm_100a tensor-core path: mbarrier, TMA bulk copy,
-// TMEM allocation, tcgen05.mma (A from TMEM, B from shared memory), tcgen05.ld/st, plus the
-// bf16 hi/lo split used for "bf16x3" (fp32-accurate) products.
+// tn_tc.cuh -- thin inline-PTX wrappers for the sm_90a tensor-core path: mbarrier, TMA bulk copy,
+// warpgroup MMA (wgmma: A from registers or shared memory, B from shared memory, accumulator in
+// registers), shared-memory matrix descriptors, plus the bf16 hi/lo split used for "bf16x3"
+// (fp32-accurate) products.
 #pragma once
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
@@ -67,148 +68,99 @@ __device__ __forceinline__ void tma_bulk_g2s(void *dst_smem, const void *src_gme
                  : "memory");
 }
 
-// ---- TMEM ------------------------------------------------------------------------------------------
-__device__ __forceinline__ void tmem_alloc(uint32_t *dst_smem, uint32_t ncols) {  // whole warp
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)), "r"(ncols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {  // whole warp
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void fence_before_sync() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void fence_after_sync() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// D[tmem] (+)= A[tmem] * B[smem]^T, kind::f16 (bf16 inputs, fp32 accumulate), one CTA, M=128
-__device__ __forceinline__ void mma_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}" ::"r"(d_tmem),
-        "r"(a_tmem), "l"(b_desc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// same with a compile-time accumulate flag (no predicate register traffic in the issue loop)
-template <bool ACC>
-__device__ __forceinline__ void mma_ts_c(uint32_t d_tmem, uint32_t a_tmem, uint64_t b_desc, uint32_t idesc) {
-    if (ACC)
-        asm volatile("{\n\t.reg .pred p;\n\tsetp.eq.u32 p, 1, 1;\n\ttcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}" ::"r"(d_tmem),
-                     "r"(a_tmem), "l"(b_desc), "r"(idesc) : "memory");
-    else
-        asm volatile("{\n\t.reg .pred p;\n\tsetp.eq.u32 p, 1, 0;\n\ttcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}" ::"r"(d_tmem),
-                     "r"(a_tmem), "l"(b_desc), "r"(idesc) : "memory");
-}
-// D[tmem] (+)= A[smem] * B[smem]^T
-__device__ __forceinline__ void mma_ss(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(d_tmem),
-        "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-template <bool ACC>
-__device__ __forceinline__ void mma_ss_c(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc) {
-    if (ACC)
-        asm volatile("{\n\t.reg .pred p;\n\tsetp.eq.u32 p, 1, 1;\n\ttcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(d_tmem),
-                     "l"(a_desc), "l"(b_desc), "r"(idesc) : "memory");
-    else
-        asm volatile("{\n\t.reg .pred p;\n\tsetp.eq.u32 p, 1, 0;\n\ttcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(d_tmem),
-                     "l"(a_desc), "l"(b_desc), "r"(idesc) : "memory");
-}
-// Issue forms used by the fused MLP kernel.  They take BASE values plus compile-time offsets: the TMEM address of the
-// A operand is a_base + AOFF, the shared-memory descriptors are built from the LOW word (start address >> 4) base + OFF
-// and a constant high word (the same for every 128-byte-swizzle K-major operand).  The additions and the 64-bit
-// descriptor assembly happen inside the asm block, so the compiler sees only the few base registers -- with dozens of
-// unrolled MMAs it otherwise hoists every "base + constant" into a register, runs out, and parks them in local memory
-// (one LDL per MMA on the issue path).
-#define TN_DESC_HI_SW128 "0x40004040"   // SBO 1024 B (>>4) | version 1 (bit 46) | SWIZZLE_128B (2 << 61)
-template <bool ACC, uint32_t AOFF, uint32_t BOFF>
-__device__ __forceinline__ void mma_ts_o(uint32_t d_tmem, uint32_t a_base, uint32_t b_base_lo, uint32_t idesc) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t.reg .b32 hi, ta, tb;\n\t.reg .b64 db;\n\t"
-        "setp.eq.u32 p, 1, %6;\n\tadd.u32 ta, %1, %4;\n\tadd.u32 tb, %2, %5;\n\tmov.u32 hi, " TN_DESC_HI_SW128 ";\n\tmov.b64 db, {tb, hi};\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], [ta], db, %3, p;\n\t}" ::"r"(d_tmem), "r"(a_base), "r"(b_base_lo), "r"(idesc), "n"(AOFF), "n"(BOFF), "n"(ACC ? 1 : 0)
-        : "memory");
-}
-template <bool ACC, uint32_t AOFF, uint32_t BOFF>
-__device__ __forceinline__ void mma_ss_o(uint32_t d_tmem, uint32_t a_base_lo, uint32_t b_base_lo, uint32_t idesc) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t.reg .b32 hi, ta, tb;\n\t.reg .b64 da, db;\n\t"
-        "setp.eq.u32 p, 1, %6;\n\tadd.u32 ta, %1, %4;\n\tadd.u32 tb, %2, %5;\n\tmov.u32 hi, " TN_DESC_HI_SW128 ";\n\tmov.b64 da, {ta, hi};\n\tmov.b64 db, {tb, hi};\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], da, db, %3, p;\n\t}" ::"r"(d_tmem), "r"(a_base_lo), "r"(b_base_lo), "r"(idesc), "n"(AOFF), "n"(BOFF), "n"(ACC ? 1 : 0)
-        : "memory");
-}
-__device__ __forceinline__ uint32_t desc_lo(uint32_t smem_addr) { return (smem_addr & 0x3FFFFu) >> 4; }
-// all previously issued MMAs of this thread arrive on `bar` when they complete (implies fence::before_thread_sync)
-__device__ __forceinline__ void mma_commit(uint64_t *bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
+// ---- warpgroup MMA (wgmma) -------------------------------------------------------------------------
+// Every wgmma of this project is m64nNk16 with fp32 accumulation: one warpgroup (4 warps, 128 threads) owns 64 rows; warp w of
+// the warpgroup owns rows 16w..16w+15.  Register fragments (g = lane / 4, t = lane % 4):
+//   accumulator d[4j + e]: row 16w + g + 8 (e >> 1), column 8j + 2t + (e & 1)
+//   A operand of k-step kk, a[i] (two packed 16-bit values, low half first): row 16w + g + 8 (i & 1), columns 16kk + 8 (i >> 1) + 2t, +1
+// so the accumulator of one layer becomes the A operand of the next one in place: a[4kk + i] = pack(d[8kk + 2i], d[8kk + 2i + 1]).
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_wait0() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+// generic-proxy shared-memory stores -> visible to wgmma / TMA (async proxy); issue before the barrier that publishes them
+__device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+// keep the compiler from moving accumulator reads / writes across a wgmma batch
+template <int N>
+__device__ __forceinline__ void reg_fence(float (&d)[N]) {
+#pragma unroll
+    for (int i = 0; i < N; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
-__device__ __forceinline__ void mma_commit_a(uint32_t bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
+// shared-memory matrix descriptor (sm_90): operand stored as [rows][64 x 16-bit] blocks with 128-byte rows and the 128-byte
+// swizzle, 8-row groups 1024 bytes apart.  K-major operands: start = block + 32 bytes per k-step of 16, lbo unused, sbo = 1024.
+// MN-major operands (the same bytes with K running along the rows): start = block + 2048 bytes per k-step (16 rows),
+// lbo = distance of the next 64-wide MN block, sbo = 1024.
+__device__ __forceinline__ uint64_t make_desc(uint32_t smem_addr, uint32_t lbo = 16u, uint32_t sbo = 1024u) {
+    return (uint64_t)((smem_addr & 0x3FFFFu) >> 4) | ((uint64_t)((lbo >> 4) & 0x3FFFu) << 16) | ((uint64_t)((sbo >> 4) & 0x3FFFu) << 32) |
+           (1ull << 62);  // layout type 1: 128-byte swizzle
 }
 
-// instruction descriptor, kind::f16: bf16 x bf16 -> f32, A and B K-major, M=128, N given
-__host__ __device__ constexpr uint32_t make_idesc_bf16(uint32_t M, uint32_t N) {
-    return (1u << 4)            // D format: f32
-           | (1u << 7)          // A format: bf16
-           | (1u << 10)         // B format: bf16
-           | ((N >> 3) << 17)   // N / 8
-           | ((M >> 4) << 24);  // M / 16
-}
-// the same for fp16 operands (format code 0)
-__host__ __device__ constexpr uint32_t make_idesc_f16(uint32_t M, uint32_t N) {
-    return (1u << 4) | ((N >> 3) << 17) | ((M >> 4) << 24);
-}
-// shared-memory matrix descriptor: K-major operand stored as [rows][64 bf16] (128-byte rows) with the
-// 128-byte swizzle; 8-row groups are 1024 bytes apart (SBO); version 1 (sm_100).
-__device__ __forceinline__ uint64_t make_desc_sw128(uint32_t smem_addr) {
-    return (uint64_t)((smem_addr & 0x3FFFFu) >> 4) | ((uint64_t)(1024u >> 4) << 32) | (1ull << 46) | (2ull << 61);
-}
-
-// 32 lanes x 32 columns of fp32 -> 32 registers per thread (thread t <-> TMEM lane base+t)
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t *r) {
+// D[64x128] (+)= A[regs] * B[smem], bf16 operands, fp32 accumulation; TB = 1: B is MN-major
+template <int TB>
+__device__ __forceinline__ void wgmma_rs_bf16_n128(float (&d)[64], const uint32_t (&a)[4], uint64_t bdesc, uint32_t acc) {
     asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-          "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]),
-          "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]),
-          "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr)
-        : "memory");
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %69, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+        "{%64, %65, %66, %67}, %68, p, 1, 1, %70;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(acc), "n"(TB));
 }
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t *r) {
+// D[64x128] (+)= A[regs] * B[smem], f16 operands, fp32 accumulation; TB = 1: B is MN-major
+template <int TB>
+__device__ __forceinline__ void wgmma_rs_f16_n128(float (&d)[64], const uint32_t (&a)[4], uint64_t bdesc, uint32_t acc) {
     asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-          "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-        : "r"(taddr)
-        : "memory");
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %69, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+        "{%64, %65, %66, %67}, %68, p, 1, 1, %70;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(acc), "n"(TB));
 }
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tmem_st16(uint32_t taddr, const uint32_t *r) {
+// D[64x128] (+)= A[smem] * B[smem], bf16 operands; TA / TB = 1: that operand is MN-major
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_ss_bf16_n128(float (&d)[64], uint64_t adesc, uint64_t bdesc, uint32_t acc) {
     asm volatile(
-        "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], "
-        "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};" ::"r"(taddr),
-        "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]), "r"(r[10]),
-        "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15])
-        : "memory");
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+        "%64, %65, p, 1, 1, %67, %68;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "l"(adesc), "l"(bdesc), "r"(acc), "n"(TA), "n"(TB));
 }
-__device__ __forceinline__ void tmem_st8(uint32_t taddr, const uint32_t *r) {
-    asm volatile("tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};" ::"r"(taddr), "r"(r[0]), "r"(r[1]),
-                 "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7])
-                 : "memory");
+// D[64x64] (+)= A[regs] * B[smem], bf16 operands, fp32 accumulation; TB = 1: B is MN-major
+template <int TB>
+__device__ __forceinline__ void wgmma_rs_bf16_n64(float (&d)[32], const uint32_t (&a)[4], uint64_t bdesc, uint32_t acc) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %37, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
+        "{%32, %33, %34, %35}, %36, p, 1, 1, %38;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(acc), "n"(TB));
 }
-__device__ __forceinline__ void tmem_st4(uint32_t taddr, const uint32_t *r) {
-    asm volatile("tcgen05.st.sync.aligned.32x32b.x4.b32 [%0], {%1, %2, %3, %4};" ::"r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]) : "memory");
+// D[64x64] (+)= A[regs] * B[smem], f16 operands, fp32 accumulation; TB = 1: B is MN-major
+template <int TB>
+__device__ __forceinline__ void wgmma_rs_f16_n64(float (&d)[32], const uint32_t (&a)[4], uint64_t bdesc, uint32_t acc) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %37, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
+        "{%32, %33, %34, %35}, %36, p, 1, 1, %38;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(acc), "n"(TB));
 }
-__device__ __forceinline__ void tmem_ld4(uint32_t taddr, uint32_t *r) {
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x4.b32 {%0, %1, %2, %3}, [%4];" : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(taddr) : "memory");
+// D[64x64] (+)= A[smem] * B[smem], bf16 operands; TA / TB = 1: that operand is MN-major
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_ss_bf16_n64(float (&d)[32], uint64_t adesc, uint64_t bdesc, uint32_t acc) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
+        "%32, %33, p, 1, 1, %35, %36;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "l"(adesc), "l"(bdesc), "r"(acc), "n"(TA), "n"(TB));
 }
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
 
 // ---- bf16 hi/lo split: x ~= hi + lo with hi = bf16(x), lo = bf16(x - hi) -----------------------------
 // packs elements (e0 -> bits [15:0], e1 -> bits [31:16]) so that element 2c sits in the low half of column c

@@ -1,4 +1,4 @@
-// tn_trace.cu -- trace_rays / trace_rays_triangles on sm_100a without OptiX.
+// tn_trace.cu -- trace_rays / trace_rays_triangles on sm_90a without OptiX.
 //
 // Replaces src/optix/optix_trace_rays.cu (+ the OptiX host runtime in src/tetrahedra_tracer.cpp:137-176,
 // 342-587).  One WARP per ray:
@@ -312,7 +312,9 @@ int launch_prefetch(tn_tracer *h, const void *const *extra, const size_t *extra_
     add(m.xyz, sizeof(float) * 3 * (size_t)m.V);
     for (int i = 0; i < nextra; ++i) add(extra[i], extra_bytes[i]);
     a.n = n;
-    k_l2_prefetch<<<148, 128, 0, s>>>(a);
+    int sms = 132;
+    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, h->device);
+    k_l2_prefetch<<<sms, 128, 0, s>>>(a);
     h->launches += 1;
     TN_CUDA(cudaGetLastError());
     return TN_OK;
@@ -333,7 +335,7 @@ static int launch_trace(tn_tracer *h, int mode, const float *o, const float *d, 
     static const int windowed_env = [] { const char *e = getenv("TETRANERF_B200_WINDOWED_PAIRING"); return e ? atoi(e) : 1; }();  // A/B switch
     p.windowed = windowed_env;
     auto kern = mode == 0 ? k_trace<0> : k_trace<1>;
-    int sms = 148;
+    int sms = 132;
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, h->device);
     auto launch = [&](uint32_t nblocks_wanted) -> int {
         const size_t smem = (size_t)TRACE_WARPS * ((size_t)p.hcap * 8 + (size_t)p.scap * 4 + (size_t)p.lcap * 4);

@@ -366,7 +366,7 @@ __global__ void __launch_bounds__(32) k_walk_coop(const WalkParams p) {
 // Same outputs, classification and fallbacks as k_walk / k_walk_coop (the same algorithm).  A 4096-ray batch is 512 warps = 3.5 per
 // SM: the walk is a serial chain of L2 round trips per ray, so what matters at this size is how many instructions are issued per
 // step and how many chains are in flight per scheduler.  One ray per warp (k_walk_coop) issues a full warp instruction stream per
-// ray (28 warps per SM fight for issue slots); 32 rays per warp (k_walk) leaves 128 warps for 148 SMs.  Here a warp instruction
+// ray (28 warps per SM fight for issue slots); 32 rays per warp (k_walk) leaves 128 warps for 132 SMs.  Here a warp instruction
 // stream serves 8 rays: lane j of a quad owns vertex j and the face opposite to it, exactly as in k_walk_coop.
 // SPEC: the records of all candidate next tetrahedra (the neighbours across the three faces the ray did not enter through) are LOADED
 // while the current one is intersected and the right one is selected afterwards, instead of prefetched into L1: ncu (round 2) put 25 %

@@ -144,7 +144,7 @@ class GradientScaler(torch.autograd.Function):
 
 
 class TetrahedraNerf(Model):
-    """Tetra-NeRF model on the B200-native tracer.  Buffers `tetrahedra_vertices` f32[V,3], `tetrahedra_cells`
+    """Tetra-NeRF model on the H100-native tracer.  Buffers `tetrahedra_vertices` f32[V,3], `tetrahedra_cells`
     i32[T,4] and parameter `tetrahedra_field` f32[field_dim,V] keep the reference's names and shapes
     (model.py:239-255) so checkpoints interchange."""
 
@@ -305,7 +305,7 @@ class TetrahedraNerf(Model):
         return self._get_outputs_unfused(ray_bundle, origins, directions)
 
     def _get_outputs_fused_train(self, origins, directions):
-        """training step on the fused CUDA pipeline: ONE differentiable op (forward + tcgen05 backward) instead of the reference's op
+        """training step on the fused CUDA pipeline: ONE differentiable op (forward + wgmma backward) instead of the reference's op
         sequence; the stratified draws are the same two torch.rand calls the reference makes (model.py:169-174, PDFSampler)."""
         from ..b200.render import PARAM_ORDER, FusedTrainRender, RenderSettings
 

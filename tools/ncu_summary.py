@@ -1,4 +1,4 @@
-"""summarise an .ncu-rep (ncu --set full) into the per-kernel figures profiles/*_ncu_summary.json carries:
+"""summarise an .ncu-rep (ncu --set full) into per-kernel figures (one JSON object per kernel):
 python tools/ncu_summary.py <report.ncu-rep> [command string] > summary.json"""
 import csv, io, json, subprocess, sys
 rep = sys.argv[1]
