@@ -107,6 +107,13 @@ def test_interpolate_values_vs_oracle(traced, D, Cdim):
     np.testing.assert_allclose(gb.cpu().numpy(), refb, rtol=1e-5, atol=1e-5)  # atomics: order differs
 
 
+def test_interpolate_values_unsupported_dimension():
+    from tetranerf import cpp
+
+    with pytest.raises(RuntimeError, match="Unsupported interpolation dimension"):  # py_binding.cpp:273-275
+        cpp.interpolate_values(torch.zeros((1, 5), dtype=torch.int32, device=DEV), torch.zeros((1, 4), device=DEV), torch.zeros((2, 3), device=DEV))
+
+
 def test_interpolate_autograd_matches_einsum(traced):
     """the reference's own test identity, tests/test_tetrahedra_tracer.py:410-416,442-453"""
     from tetranerf.utils.extension import interpolate_values

@@ -57,7 +57,6 @@ struct MlpParams {
     const float *dirbias;      // FINE: [n_active,128]  = b4 + W4[:, :27] . enc(dir)
     float *out;                // COARSE: density [rows] ; FINE: (sigma,r,g,b) [rows,4]
     uint32_t *tile_ctr;        // device counter (zeroed before the launch): dynamic tile scheduler
-    unsigned long long *timeline;  // debug: per-CTA (start ns, end ns, tiles) at [1000 + 8 cta ..]; nullptr in production
 };
 
 constexpr uint32_t MLP_NO_TILE = 0xFFFFFFFFu;  // sentinel: the scheduler has run dry
@@ -169,11 +168,6 @@ __global__ void __launch_bounds__(MLP_THREADS, 1) k_mlp(const MlpParams p) {
         mbar_init(w_bar, 1);
         fence_barrier_init();
     }
-    if (p.timeline != nullptr && threadIdx.x == 0) {
-        unsigned long long ns;
-        asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(ns));
-        p.timeline[1000 + 8 * blockIdx.x] = ns;
-    }
     for (uint32_t i = threadIdx.x; i < 516; i += MLP_THREADS) const_cast<float *>(head_s)[i] = p.head[i];
     if (tid == 0) {  // first tile of each warpgroup: static; the following ones come from the global counter
         const uint32_t first = blockIdx.x * MLP_WGS + wg;
@@ -187,7 +181,6 @@ __global__ void __launch_bounds__(MLP_THREADS, 1) k_mlp(const MlpParams p) {
     const uint32_t wsm = smem_u32(smem);
     const float *wd = head_s, *wc = head_s + 128;
     bool weights_ready = false;
-    uint32_t ntl = 0;
 
 #pragma unroll 1
     for (uint32_t n = 0;; ++n) {
@@ -198,7 +191,6 @@ __global__ void __launch_bounds__(MLP_THREADS, 1) k_mlp(const MlpParams p) {
             const uint32_t nx = gridDim.x * MLP_WGS + atomicAdd(p.tile_ctr, 1u);
             slots[2 * wg + ((n + 1u) & 1u)] = nx < ntiles ? nx : MLP_NO_TILE;
         }
-        ++ntl;
         const uint64_t row0 = (uint64_t)tile * MLP_TILE + warp * 16u + g, row1 = row0 + 8u;
 
         uint32_t ah[32], al[32];
@@ -291,12 +283,6 @@ __global__ void __launch_bounds__(MLP_THREADS, 1) k_mlp(const MlpParams p) {
         }
     }
     if (!weights_ready) mbar_wait(w_bar, 0);  // a warpgroup without a tile still lets the weight copy land before the CTA exits
-    if (p.timeline != nullptr && tid == 0) {
-        atomicAdd(p.timeline + 1000 + 8 * blockIdx.x + 3, (unsigned long long)ntl);
-        unsigned long long ns;
-        asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(ns));
-        atomicMax(p.timeline + 1000 + 8 * blockIdx.x + 1, ns);
-    }
 }
 
 }  // namespace tn

@@ -21,8 +21,6 @@
 
 namespace tn {
 
-static unsigned long long *g_timeline = nullptr;
-
 int launch_trace_internal(tn_tracer *h, const float *o, const float *d, uint32_t R, uint32_t M, uint32_t *num, uint32_t *cells, float *bary,
                           float *dist, uint32_t *verts, int dense, cudaStream_t s);
 
@@ -791,7 +789,6 @@ static int render_impl(tn_tracer *h, const tn_render_config *cfg, const float *d
     mf.S = S2; mf.dirbias = r->dirbias; mf.out = r->out_f;
     if (!single) { mf.vi = r->vi_f; mf.bary = r->bary_f; }
     else p.ebins_f = r->ebins_c;  // k_composite integrates over the coarse bins
-    mf.timeline = g_timeline;
     mf.tile_ctr = r->n_active + 2;
     k_fine<<<grid_f, MLP_THREADS, MLP_SMEM_BYTES, s>>>(mf);
     TN_EV(5);
@@ -933,9 +930,6 @@ extern "C" int tn_render_get_backward_timings(tn_tracer *h, float *ms3) {
     for (int i = 0; i < 3; ++i) TN_CUDA(cudaEventElapsedTime(&ms3[i], r->evb[i], r->evb[i + 1]));
     return TN_OK;
 }
-
-// debug: per-CTA start / end / tile count of the NEXT fine k_mlp launches (device buffer of >= 65001 u64, zeroed by the caller)
-extern "C" int tn_debug_set_timeline(void *d_buf) { g_timeline = (unsigned long long *)d_buf; return TN_OK; }
 
 // test / debug hook: device pointers of the intermediate buffers of the last tn_render call
 extern "C" int tn_render_debug_buffers(tn_tracer *h, void **ptrs16) {

@@ -15,22 +15,6 @@ from ..utils.extension import tetranerf_cpp_extension as ext
 _lib = ext._lib
 _vp = C.c_void_p
 
-
-class _Cfg(C.Structure):
-    _fields_ = [("max_ray_triangles", C.c_uint32), ("num_samples", C.c_uint32), ("num_fine_samples", C.c_uint32),
-                ("use_biased_sampler", C.c_uint32), ("far_plane", C.c_float), ("background", C.c_float * 3)]
-
-
-_lib.tn_render_set_field.argtypes = [_vp, _vp, C.c_uint32, C.c_uint32, _vp]
-_lib.tn_render_set_weights.argtypes = [_vp, C.POINTER(_vp), _vp]
-_lib.tn_render.argtypes = [_vp, C.POINTER(_Cfg), _vp, _vp, C.c_uint32, _vp, _vp, _vp, _vp, _vp]
-_lib.tn_render_train_forward.argtypes = [_vp, C.POINTER(_Cfg), _vp, _vp, C.c_uint32, _vp, _vp, _vp, _vp, _vp, _vp, _vp]
-_lib.tn_render_train_backward.argtypes = [_vp, _vp, _vp, C.c_int, _vp, C.POINTER(_vp), _vp]
-_lib.tn_render_debug_buffers.argtypes = [_vp, C.POINTER(_vp)]
-_lib.tn_render_set_profiling.argtypes = [_vp, C.c_int]
-_lib.tn_render_set_mlp_precision.argtypes = [_vp, C.c_int]
-_lib.tn_render_get_timings.argtypes = [_vp, C.POINTER(C.c_float)]
-_lib.tn_render_get_backward_timings.argtypes = [_vp, C.POINTER(C.c_float)]
 KERNEL_NAMES = ["trace", "sample_coarse", "mlp_coarse", "sample_fine", "mlp_fine", "composite"]
 
 PARAM_ORDER = [
@@ -59,6 +43,11 @@ class RenderSettings:
     @staticmethod
     def tetra_nerf_original():  # registration.py:20-46
         return RenderSettings()
+
+
+def _config(settings: RenderSettings) -> "ext._Cfg":
+    return ext._Cfg(settings.max_intersected_triangles, settings.num_samples, settings.num_fine_samples, int(settings.use_biased_sampler),
+                    float(settings.far_plane), (C.c_float * 3)(*settings.background))
 
 
 class FusedRenderer:
@@ -101,8 +90,7 @@ class FusedRenderer:
                 "depth": torch.empty((R, 1), dtype=torch.float32, device=dev),
                 "ray_mask": torch.empty((R,), dtype=torch.bool, device=dev),
             }
-        cfg = _Cfg(settings.max_intersected_triangles, settings.num_samples, settings.num_fine_samples, int(settings.use_biased_sampler),
-                   float(settings.far_plane), (C.c_float * 3)(*settings.background))
+        cfg = _config(settings)
         ext._check(_lib.tn_render(tr.handle, C.byref(cfg), origins.data_ptr(), directions.data_ptr(), R, out["rgb"].data_ptr(),
                                   out["accumulation"].data_ptr(), out["depth"].data_ptr(), out["ray_mask"].data_ptr(), self._stream()))
         return out
@@ -122,8 +110,7 @@ class FusedRenderer:
                 raise RuntimeError(f"{n} must be a contiguous float32 [{R}, {w}] tensor on the tracer's device")
         out = {"rgb": torch.empty((R, 3), dtype=torch.float32, device=dev), "accumulation": torch.empty((R, 1), dtype=torch.float32, device=dev),
                "depth": torch.empty((R, 1), dtype=torch.float32, device=dev), "ray_mask": torch.empty((R,), dtype=torch.bool, device=dev)}
-        cfg = _Cfg(settings.max_intersected_triangles, settings.num_samples, settings.num_fine_samples, int(settings.use_biased_sampler),
-                   float(settings.far_plane), (C.c_float * 3)(*settings.background))
+        cfg = _config(settings)
         ext._check(_lib.tn_render_train_forward(tr.handle, C.byref(cfg), origins.data_ptr(), directions.data_ptr(), R,
                                                 jitter_coarse.data_ptr() if jitter_coarse is not None else None,
                                                 jitter_fine.data_ptr() if jitter_fine is not None else None, out["rgb"].data_ptr(),

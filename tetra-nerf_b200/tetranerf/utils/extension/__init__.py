@@ -7,18 +7,11 @@ is a ctypes shim over the C ABI in include/tetranerf_b200.h; when the shared lib
 use raises RuntimeError (the reference defers its ImportError the same way, :3-21) -- there is no CPU
 or PyTorch fallback.
 """
-import os
-
 import torch
 
 _LOAD_ERROR = None
 try:
-    # Two interchangeable bindings of the same C ABI: the ctypes shim (default: no compile step beyond the CUDA library) and the
-    # compiled pybind11 module of the same name (csrc/py_binding.cpp, built by build.py into _pybind/); TETRANERF_B200_BINDING picks.
-    if os.environ.get("TETRANERF_B200_BINDING", "ctypes") == "pybind":
-        from ._pybind import tetranerf_cpp_extension as cpp
-    else:
-        from . import tetranerf_cpp_extension as cpp
+    from . import tetranerf_cpp_extension as cpp
 except (ImportError, OSError) as _e:  # library not built
     _LOAD_ERROR = _e
 

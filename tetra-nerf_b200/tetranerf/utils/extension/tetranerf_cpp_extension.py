@@ -5,6 +5,9 @@ Same class / function names, argument checks and error behaviour (RuntimeError) 
 binding; tensors in, tensors out.  All device work is hand-written CUDA in the shared library, launched
 on torch's current stream; there is no CPU fallback (importing this module without the built library
 raises, and a non-CUDA device raises exactly like py_binding.cpp:31-33).
+
+This module is where the package declares the C ABI to ctypes: the signatures of every entry point it calls, including the
+fused-render ones that tetranerf.b200.render calls through `_lib`.
 """
 from __future__ import annotations
 
@@ -32,7 +35,6 @@ _lib.tn_trace_rays.argtypes = [_vp, _vp, _vp, _u32, _u32, _vp, _vp, _vp, _vp, _v
 _lib.tn_trace_rays_triangles.argtypes = [_vp, _vp, _vp, _u32, _u32, _vp, _vp, _vp, _vp, _vp, _vp]
 _lib.tn_find_tetrahedra.argtypes = [_vp, _vp, _u32, _vp, _vp, _vp, _vp]
 _lib.tn_find_visited_cells.argtypes = [_vp, _u32, _u32, _u32] + [_vp] * 11
-_lib.tn_interpolate_values.argtypes = [_i, _u32, _u32, _u32, _u32, _vp, _vp, _vp, _vp, _vp, _vp]
 _lib.tn_interpolate_values_backward.argtypes = [_i, _u32, _u32, _u32, _u32, _vp, _vp, _vp, _vp, _vp, _vp]
 _lib.tn_make_field_shadow.argtypes = [_i, _u32, _u32, _vp, _vp, _vp]
 _lib.tn_interpolate_values_shadow.argtypes = [_i, _u32, _u32, _u32, _u32, _vp, _vp, _vp, _vp, _vp]
@@ -43,6 +45,23 @@ _lib.tn_set_walk_quad_range.argtypes = [_vp, _u32, _u32]
 _lib.tn_set_walk_quad_spec_max_rays.argtypes = [_vp, _u32]
 _lib.tn_launch_count.restype = C.c_uint64
 _lib.tn_launch_count.argtypes = [_vp]
+
+
+class _Cfg(C.Structure):  # tn_render_config
+    _fields_ = [("max_ray_triangles", C.c_uint32), ("num_samples", C.c_uint32), ("num_fine_samples", C.c_uint32),
+                ("use_biased_sampler", C.c_uint32), ("far_plane", C.c_float), ("background", C.c_float * 3)]
+
+
+_lib.tn_render_set_field.argtypes = [_vp, _vp, _u32, _u32, _vp]
+_lib.tn_render_set_weights.argtypes = [_vp, C.POINTER(_vp), _vp]
+_lib.tn_render.argtypes = [_vp, C.POINTER(_Cfg), _vp, _vp, _u32, _vp, _vp, _vp, _vp, _vp]
+_lib.tn_render_train_forward.argtypes = [_vp, C.POINTER(_Cfg), _vp, _vp, _u32, _vp, _vp, _vp, _vp, _vp, _vp, _vp]
+_lib.tn_render_train_backward.argtypes = [_vp, _vp, _vp, _i, _vp, C.POINTER(_vp), _vp]
+_lib.tn_render_debug_buffers.argtypes = [_vp, C.POINTER(_vp)]
+_lib.tn_render_set_profiling.argtypes = [_vp, _i]
+_lib.tn_render_set_mlp_precision.argtypes = [_vp, _i]
+_lib.tn_render_get_timings.argtypes = [_vp, C.POINTER(C.c_float)]
+_lib.tn_render_get_backward_timings.argtypes = [_vp, C.POINTER(C.c_float)]
 
 LIBRARY_PATH = str(_LIB_PATH)
 
