@@ -15,6 +15,7 @@
  */
 #ifndef TETRANERF_B200_H
 #define TETRANERF_B200_H
+#include <stddef.h>
 #include <stdint.h>
 #ifdef __cplusplus
 extern "C" {
@@ -87,6 +88,14 @@ int tn_interpolate_values_shadow(int device, uint32_t D, uint32_t N, uint32_t C,
  *   a row-major [V,C] accumulator filled with 16-byte vector reductions and transposed at the end (needs C % 4 == 0). */
 int tn_interpolate_values_backward(int device, uint32_t D, uint32_t N, uint32_t C, uint32_t V, const uint32_t *d_vi,
                                    const float *d_w, const float *d_grad_in, float *d_grad_field, float *d_scratch, void *stream);
+/* The same gradient, bitwise reproducible: identical inputs give identical bits on every run (same build, same GPU model), whatever
+ * the scheduling.  The vertex slots are sorted by vertex (stable radix sort) and each vertex sums its contributions in input order;
+ * the products are the ones above, only the summation order differs (so results differ from tn_interpolate_values_backward by
+ * rounding).  Any C; N * D < 2^31.  d_workspace == NULL: *workspace_bytes receives the size the call needs and nothing else happens;
+ * otherwise d_workspace holds *workspace_bytes (>= that size) bytes of device memory used only during the call (stream-ordered). */
+int tn_interpolate_values_backward_deterministic(int device, uint32_t D, uint32_t N, uint32_t C, uint32_t V, const uint32_t *d_vi,
+                                                 const float *d_w, const float *d_grad_in, float *d_grad_field, void *d_workspace,
+                                                 size_t *workspace_bytes, void *stream);
 
 /* ---- fused forward render (new; replaces model.py:531-662 between trace_rays and the pixel) -------
  * Weights are passed once (tn_render_set_weights) in nerfstudio state-dict layout and repacked on
@@ -126,6 +135,16 @@ int tn_render_train_forward(tn_tracer *h, const tn_render_config *cfg, const flo
                             uint8_t *d_mask, void *stream);
 int tn_render_train_backward(tn_tracer *h, const float *d_grad_rgb, const float *d_grad_acc, int use_gradient_scaling, float *d_grad_field,
                              float *const *d_grad_params12, void *stream);
+/* Deterministic mode of the fused training step (enable != 0; initial value: 1 if the environment variable TETRANERF_B200_DETERMINISTIC
+ * is 1, else 0).  Read by tn_render_train_forward; tn_render_train_backward continues in the mode of the forward it belongs to.  With
+ * identical inputs, on the same build and GPU model, forward outputs and every gradient are then bitwise identical from run to run and
+ * process to process, whatever the backward grid size and whatever order warps claim work in: slots go to rays in ray order (an
+ * exclusive scan instead of an atomic counter), the backward assigns its 64-sample tiles to 256 fixed partitions with private
+ * accumulators, and every sum (weight gradients, column sums, per-ray bias gradients, the per-vertex field gradient after a stable sort
+ * by vertex) is reduced in a fixed order.  Forward outputs (rgb, accumulation, depth, ray_mask) equal those of the default mode bit for
+ * bit; gradients differ from it by rounding (another summation order).  Costs extra device memory: ~0.9 GB at 8192 rays x 257 fine
+ * samples (the [samples,64] feature gradient, the sort, partition partials).  The eval render (tn_render) is unaffected. */
+int tn_render_set_deterministic(tn_tracer *h, int enable);
 /* ---- multi-GPU: final gather of the rendered pixels (north_star; tetranerf/nerfstudio/pipeline.py:53-58 is the reference's only
  * multi-GPU mechanism).  One process per GPU; each rank owns a gathered-pixel buffer f32[world * rays_per_rank, 6]
  * (r, g, b, accumulation, depth, mask) allocated with tn_peer_alloc, whose 64-byte CUDA IPC handle the ranks exchange and map
@@ -153,6 +172,8 @@ int tn_set_walk_quad_range(tn_tracer *h, uint32_t lo, uint32_t hi);
 /* the quad walk of batches of up to n rays (default 65536) loads the records of all candidate next tetrahedra while the current one
  * is intersected instead of prefetching them (latency-bound regime); 0 = never.  Results are identical. */
 int tn_set_walk_quad_spec_max_rays(tn_tracer *h, uint32_t n);
+/* test hook: number of CTAs of the backward MLP kernel of tn_render_train_backward (0 = default, one per SM) */
+int tn_render_set_backward_grid(tn_tracer *h, uint32_t ctas);
 /* out2[0] = 1 if the loaded mesh takes the adjacency-walk fast path (conforming, convex hull); out2[1] = rays of the last
  * trace_rays call that needed the exact sort/pairing or all-hits stage.  Synchronises. */
 int tn_debug_trace_stats(tn_tracer *h, uint32_t *out2);

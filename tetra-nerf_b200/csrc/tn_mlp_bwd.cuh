@@ -19,7 +19,16 @@
 // weight gradients of a tile (two M = 64 halves per layer) are added to the global accumulators with vector reductions.
 // The weights stream through a two-stage TMA ring in the fixed order of the 14 stages a tile consumes.
 // Shared memory: ring 2 x 32 KB | X 16 KB | H1, H2, H3, dA 32 KB each | heads, column sums, barriers.
+//
+// Deterministic mode (k_mlp_bwd<true>, tn_render_set_deterministic): the same arithmetic per tile, but no reduction whose order depends
+// on scheduling.  The tiles are split statically into BWD_PARTS contiguous partitions (independent of the grid size); a CTA takes
+// partitions blockIdx.x, blockIdx.x + gridDim.x, ... and their tiles in order, and accumulates dW and the column sums of each partition
+// in a partition-private slice of `part` with plain read-modify-write.  The four warps keep separate column sums, combined in warp
+// order when a partition ends.  The per-ray direction-bias gradient goes to one partial row per (tile, ray, warp) and dX rows are
+// stored to `dx`; tn_render.cu reduces all of these in a fixed order.
 #pragma once
+#include <type_traits>
+
 #include "tn_common.cuh"
 #include "tn_mlp.cuh"
 #include "tn_tc.cuh"
@@ -58,9 +67,35 @@ struct MlpBwdParams {
     float *g_dirbias;           // [n_active,128] gradient at the per-ray direction bias (zeroed by the caller)
     uint32_t *tile_ctr;
 };
+// deterministic mode (k_mlp_bwd<true>): gw, g_dirbias, gshadow and tile_ctr are not used
+struct MlpBwdDetParams : MlpBwdParams {
+    float *part;                // [BWD_PARTS][BWD_PART_STRIDE] per-partition dW and column sums (GW_* offsets)
+    float *gdb_part;            // [4 (ntiles + n_active)][128] direction-bias gradient partials, row 4 (tile + slot) + warp
+    float *dx;                  // [rows,64] gradient at the interpolated features
+};
+template <bool DET>
+using MlpBwdParamsT = typename std::conditional<DET, MlpBwdDetParams, MlpBwdParams>::type;
 // offsets (floats) inside gw
 constexpr uint32_t GW_W1 = 0, GW_W2 = 8192, GW_W3 = 24576, GW_W4B = 40960, GW_B1 = 57344, GW_B2 = 57472, GW_B3 = 57600, GW_WD = 57728, GW_WC = 57856,
                    GW_SUMS = 58240 /* sum ds, sum dz_r, dz_g, dz_b */, GW_W4DIR = 58244 /* [128][27] */, GW_B4 = 61700, GW_TOTAL = 61828;
+
+// deterministic mode: fixed tile partitions; a partition's slice holds gw[0, GW_SUMS): dW1..dW4b and the 7 column sums (b1 b2 b3 wd wc)
+constexpr uint32_t BWD_PARTS = 256;
+constexpr uint32_t BWD_PART_STRIDE = GW_SUMS;
+constexpr uint32_t BWD_DET_OFF_BARS = BWD_OFF_SUMS + 4 * 7 * 512;  // column sums per warp [4][7][128]
+constexpr uint32_t BWD_DET_SMEM_BYTES = BWD_DET_OFF_BARS + 32;
+static_assert(BWD_DET_SMEM_BYTES <= 232448, "k_mlp_bwd<true> shared memory exceeds 227 KB");
+// partition q holds tiles [part_lo(q), part_lo(q + 1))
+__host__ __device__ __forceinline__ uint32_t bwd_part_lo(uint32_t q, uint32_t ntiles) { return (uint32_t)(((uint64_t)q * ntiles) / BWD_PARTS); }
+__host__ __device__ __forceinline__ uint32_t bwd_part_of(uint32_t tile, uint32_t ntiles) {
+    return (uint32_t)((((uint64_t)tile + 1) * BWD_PARTS - 1) / ntiles);
+}
+// first tile of the first non-empty partition q0, q0 + step, ... (MLP_NO_TILE: none)
+__device__ __forceinline__ uint32_t bwd_det_first(uint32_t q, uint32_t step, uint32_t ntiles) {
+    for (; q < BWD_PARTS; q += step)
+        if (bwd_part_lo(q, ntiles) < bwd_part_lo(q + 1, ntiles)) return bwd_part_lo(q, ntiles);
+    return MLP_NO_TILE;
+}
 
 __device__ __forceinline__ void red_add_v2(float *dst, float a, float b) {
     asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(dst), "f"(a), "f"(b) : "memory");
@@ -96,19 +131,27 @@ __device__ __forceinline__ void st_pair(uint32_t base, uint32_t R, uint32_t j, u
 
 // sum over the 64 rows of the tile of (s0, s1) = this thread's two-row partial sums of columns c, c+1: reduced over the eight
 // threads of a warp that share t, then added into the shared-memory column sums (four warps)
-__device__ __forceinline__ void colsum2(float *dst, uint32_t c, float s0, float s1, uint32_t lane) {
+// (deterministic mode: into the warp's own copy of the sums, [warp][7][128], without atomics)
+template <bool DET = false>
+__device__ __forceinline__ void colsum2(float *dst, uint32_t c, float s0, float s1, uint32_t lane, uint32_t warp = 0) {
 #pragma unroll
     for (int m = 4; m <= 16; m <<= 1) {
         s0 += __shfl_xor_sync(0xffffffffu, s0, m);
         s1 += __shfl_xor_sync(0xffffffffu, s1, m);
     }
-    if (lane < 4) { atomicAdd(dst + c, s0); atomicAdd(dst + c + 1, s1); }
+    if constexpr (DET) {
+        if (lane < 4) { float *w = dst + warp * (7u * 128u); w[c] += s0; w[c + 1] += s1; }
+    } else {
+        if (lane < 4) { atomicAdd(dst + c, s0); atomicAdd(dst + c + 1, s1); }
+    }
 }
 
 // dW (+)= dA^T H for one M = 64 half of the output features: A = dA (MN-major, half mh of its columns), B = H (MN-major, NB
-// 64-column blocks), K = the tile's 64 rows; bf16x3.  Result added to gw[dst + out * (64 NB) + in].
-template <int NB>
-__device__ __forceinline__ void dw_half(uint32_t sDA, uint32_t sHb, uint32_t h_lo_off, uint32_t mh, float *dst, uint32_t warp, uint32_t g, uint32_t t) {
+// 64-column blocks), K = the tile's 64 rows; bf16x3.  Result added to gw[dst + out * (64 NB) + in] (deterministic mode: every
+// thread owns its addresses, plain read-modify-write, or a store for the first tile of a partition).
+template <int NB, bool DET = false>
+__device__ __forceinline__ void dw_half(uint32_t sDA, uint32_t sHb, uint32_t h_lo_off, uint32_t mh, float *dst, uint32_t warp, uint32_t g, uint32_t t,
+                                        bool first = false) {
     using namespace tc;
     float d[32 * NB];
 #pragma unroll
@@ -132,7 +175,14 @@ __device__ __forceinline__ void dw_half(uint32_t sDA, uint32_t sHb, uint32_t h_l
 #pragma unroll
     for (int j = 0; j < 4 * NB * 2; ++j) {
         const float4 q = quad_of_row(make_float2(d[4 * j], d[4 * j + 1]), make_float2(d[4 * j + 2], d[4 * j + 3]), t);
-        red_add_v4(dst + (size_t)o * (64u * NB) + 8u * j + 4u * (t >> 1), q.x, q.y, q.z, q.w);
+        if constexpr (DET) {
+            float4 *a = reinterpret_cast<float4 *>(dst + (size_t)o * (64u * NB) + 8u * j + 4u * (t >> 1));
+            float4 r = q;
+            if (!first) { const float4 b = *a; r = make_float4(b.x + q.x, b.y + q.y, b.z + q.z, b.w + q.w); }
+            *a = r;
+        } else {
+            red_add_v4(dst + (size_t)o * (64u * NB) + 8u * j + 4u * (t >> 1), q.x, q.y, q.z, q.w);
+        }
     }
 }
 
@@ -149,28 +199,37 @@ __device__ __forceinline__ void frag_pair(float x0, float x1, float y0, float y1
     tc::split_pack2(y0, y1, ah[i + 1], al[i + 1]);
 }
 
-__global__ void __launch_bounds__(BWD_THREADS, 1) k_mlp_bwd(const MlpBwdParams p) {
+template <bool DET>
+__global__ void __launch_bounds__(BWD_THREADS, 1) k_mlp_bwd(const MlpBwdParamsT<DET> p) {
     using namespace tc;
     extern __shared__ __align__(1024) uint8_t tn_bwd_smem[];
+    constexpr uint32_t OFF_BARS = DET ? BWD_DET_OFF_BARS : BWD_OFF_BARS;
     uint8_t *smem = tn_bwd_smem;
     float *head_s = reinterpret_cast<float *>(smem + BWD_OFF_HEAD);  // wd[128], wc[3][128]
     float *sums = reinterpret_cast<float *>(smem + BWD_OFF_SUMS);
-    uint64_t *ring_full = reinterpret_cast<uint64_t *>(smem + BWD_OFF_BARS);
-    volatile uint32_t *slots = reinterpret_cast<volatile uint32_t *>(smem + BWD_OFF_BARS + 16);
+    uint64_t *ring_full = reinterpret_cast<uint64_t *>(smem + OFF_BARS);
+    volatile uint32_t *slots = reinterpret_cast<volatile uint32_t *>(smem + OFF_BARS + 16);
 
     const uint32_t tid = threadIdx.x, warp = tid >> 5, lane = tid & 31u, g = lane >> 2, t = lane & 3u;
     const uint32_t n_active = *p.n_active;
     const uint64_t total_rows = (uint64_t)n_active * p.S;
     const uint32_t ntiles = (uint32_t)((total_rows + BWD_TILE - 1) / BWD_TILE);
-    if (blockIdx.x >= ntiles) return;
+    uint32_t first_tile = blockIdx.x;
+    if constexpr (DET) {
+        if (ntiles == 0) return;
+        first_tile = bwd_det_first(blockIdx.x, gridDim.x, ntiles);
+        if (first_tile == MLP_NO_TILE) return;
+    } else {
+        if (blockIdx.x >= ntiles) return;
+    }
 
     if (tid == 0) {
         mbar_init(&ring_full[0], 1); mbar_init(&ring_full[1], 1);
         fence_barrier_init();
-        slots[0] = blockIdx.x;
+        slots[0] = first_tile;
     }
     for (uint32_t i = tid; i < 512; i += BWD_THREADS) head_s[i] = p.head[i];
-    for (uint32_t i = tid; i < 7 * 128; i += BWD_THREADS) sums[i] = 0.f;
+    for (uint32_t i = tid; i < (DET ? 4u : 1u) * 7 * 128; i += BWD_THREADS) sums[i] = 0.f;
     __syncthreads();
     const uint32_t sR = smem_u32(smem + BWD_OFF_RING), sX = smem_u32(smem + BWD_OFF_X), sH = smem_u32(smem + BWD_OFF_H), sDA = smem_u32(smem + BWD_OFF_DA);
     const float *wd = head_s, *wc = head_s + 128;
@@ -207,9 +266,23 @@ __global__ void __launch_bounds__(BWD_THREADS, 1) k_mlp_bwd(const MlpBwdParams p
         wg_sync(0);
         const uint32_t tile = slots[n & 1u];
         if (tile == MLP_NO_TILE) break;
+        // deterministic mode: the partition of the tile, and whether the tile opens / closes it
+        uint32_t part_q = 0;
+        bool part_first = false, part_last = false;
+        if constexpr (DET) {
+            part_q = bwd_part_of(tile, ntiles);
+            part_first = tile == bwd_part_lo(part_q, ntiles);
+            part_last = tile + 1u == bwd_part_lo(part_q + 1u, ntiles);
+        }
+        float *gw = p.gw;
+        if constexpr (DET) gw = p.part + (size_t)part_q * BWD_PART_STRIDE;
         if (tid == 0) {
-            const uint32_t nx = gridDim.x + atomicAdd(p.tile_ctr, 1u);
-            slots[(n + 1u) & 1u] = nx < ntiles ? nx : MLP_NO_TILE;
+            if constexpr (DET) {
+                slots[(n + 1u) & 1u] = part_last ? bwd_det_first(part_q + gridDim.x, gridDim.x, ntiles) : tile + 1u;
+            } else {
+                const uint32_t nx = gridDim.x + atomicAdd(p.tile_ctr, 1u);
+                slots[(n + 1u) & 1u] = nx < ntiles ? nx : MLP_NO_TILE;
+            }
         }
         const uint32_t R0 = warp * 16u + g, R1 = R0 + 8u;
         const uint64_t row0 = (uint64_t)tile * BWD_TILE + R0, row1 = row0 + 8u;
@@ -289,7 +362,7 @@ __global__ void __launch_bounds__(BWD_THREADS, 1) k_mlp_bwd(const MlpBwdParams p
                 st_pair(hb, R0, (uint32_t)j, t, 16384u, ah[i], al[i]);
                 st_pair(hb, R1, (uint32_t)j, t, 16384u, ah[i + 1], al[i + 1]);
                 if (l == 2)  // d wd[k] = sum_s d sigma_pre[s] H3[s,k]
-                    colsum2(sums + 3 * 128, c, g0.x * x0 + g1.x * y0, g0.x * x1 + g1.x * y1, lane);
+                    colsum2<DET>(sums + 3 * 128, c, g0.x * x0 + g1.x * y0, g0.x * x1 + g1.x * y1, lane, warp);
             }
             mask[l] = mk;
         }
@@ -327,9 +400,9 @@ __global__ void __launch_bounds__(BWD_THREADS, 1) k_mlp_bwd(const MlpBwdParams p
                 const float v0 = d[4 * j] + b0.x, v1 = d[4 * j + 1] + b0.y, v2 = d[4 * j + 2] + b1.x, v3 = d[4 * j + 3] + b1.y;
                 const float x0 = fmaxf(v0, 0.f), x1 = fmaxf(v1, 0.f), y0 = fmaxf(v2, 0.f), y1 = fmaxf(v3, 0.f);  // H4
                 // d wc[ch][k] = sum_s d z_ch[s] H4[s,k]
-                colsum2(sums + 4 * 128, c, g0.y * x0 + g1.y * y0, g0.y * x1 + g1.y * y1, lane);
-                colsum2(sums + 5 * 128, c, g0.z * x0 + g1.z * y0, g0.z * x1 + g1.z * y1, lane);
-                colsum2(sums + 6 * 128, c, g0.w * x0 + g1.w * y0, g0.w * x1 + g1.w * y1, lane);
+                colsum2<DET>(sums + 4 * 128, c, g0.y * x0 + g1.y * y0, g0.y * x1 + g1.y * y1, lane, warp);
+                colsum2<DET>(sums + 5 * 128, c, g0.z * x0 + g1.z * y0, g0.z * x1 + g1.z * y1, lane, warp);
+                colsum2<DET>(sums + 6 * 128, c, g0.w * x0 + g1.w * y0, g0.w * x1 + g1.w * y1, lane, warp);
                 // dA4 = (d z . wc) * (H4 > 0)
                 const float wa0 = wc[c], wa1 = wc[c + 1], wb0 = wc[128 + c], wb1 = wc[128 + c + 1], wc0 = wc[256 + c], wc1 = wc[256 + c + 1];
                 d[4 * j] = v0 > 0.f ? fmaf(g0.w, wc0, fmaf(g0.z, wb0, g0.y * wa0)) : 0.f;
@@ -356,7 +429,11 @@ __global__ void __launch_bounds__(BWD_THREADS, 1) k_mlp_bwd(const MlpBwdParams p
                         s0 += __shfl_xor_sync(0xffffffffu, s0, m);
                         s1 += __shfl_xor_sync(0xffffffffu, s1, m);
                     }
-                    if (lane < 4) red_add_v2(p.g_dirbias + (size_t)sl * 128 + 8u * j + 2u * t, s0, s1);
+                    if constexpr (DET) {
+                        if (lane < 4) *reinterpret_cast<float2 *>(p.gdb_part + (4 * ((size_t)tile + sl) + warp) * 128 + 8u * j + 2u * t) = make_float2(s0, s1);
+                    } else {
+                        if (lane < 4) red_add_v2(p.g_dirbias + (size_t)sl * 128 + 8u * j + 2u * t, s0, s1);
+                    }
                 }
             }
             publish();
@@ -364,10 +441,10 @@ __global__ void __launch_bounds__(BWD_THREADS, 1) k_mlp_bwd(const MlpBwdParams p
         // ---------- layers 4, 3, 2: dW_l += dA_l^T H_{l-1}; dH_{l-1} = dA_l W_l; dA_{l-1} = dH_{l-1} * (H_{l-1} > 0) ----------
 #pragma unroll 1
         for (int l = 2; l >= 0; --l) {
-            float *gdst = p.gw + (l == 2 ? GW_W4B : (l == 1 ? GW_W3 : GW_W2));
+            float *gdst = gw + (l == 2 ? GW_W4B : (l == 1 ? GW_W3 : GW_W2));
             const uint32_t hb = sH + 32768u * (uint32_t)l;  // H3, H2, H1
-            dw_half<2>(sDA, hb, 16384u, 0, gdst, warp, g, t);
-            dw_half<2>(sDA, hb, 16384u, 1, gdst, warp, g, t);
+            dw_half<2, DET>(sDA, hb, 16384u, 0, gdst, warp, g, t, part_first);
+            dw_half<2, DET>(sDA, hb, 16384u, 1, gdst, warp, g, t, part_first);
             uint32_t w = ring_acquire(true);
             zero(d);
             wgmma_fence();
@@ -402,7 +479,7 @@ __global__ void __launch_bounds__(BWD_THREADS, 1) k_mlp_bwd(const MlpBwdParams p
                 }
                 const uint32_t m = (uint32_t)(mk >> (4 * j)) & 15u;
                 e0 = (m & 1u) ? e0 : 0.f; e1 = (m & 2u) ? e1 : 0.f; e2 = (m & 4u) ? e2 : 0.f; e3 = (m & 8u) ? e3 : 0.f;
-                colsum2(bsum, c, e0 + e2, e1 + e3, lane);
+                colsum2<DET>(bsum, c, e0 + e2, e1 + e3, lane, warp);
                 frag_pair(e0, e1, e2, e3, j, ah, al);
                 const int i = 4 * (j >> 1) + 2 * (j & 1);
                 st_pair(sDA, R0, (uint32_t)j, t, 16384u, ah[i], al[i]);
@@ -411,8 +488,8 @@ __global__ void __launch_bounds__(BWD_THREADS, 1) k_mlp_bwd(const MlpBwdParams p
             publish();
         }
         // ---------- layer 1: dW1 += dA1^T X; dX = dA1 W1 -> field gradient (interpolate_values_backward, tetrahedra_tracer.cu:231-247) ----------
-        dw_half<1>(sDA, sX, 8192u, 0, p.gw + GW_W1, warp, g, t);
-        dw_half<1>(sDA, sX, 8192u, 1, p.gw + GW_W1, warp, g, t);
+        dw_half<1, DET>(sDA, sX, 8192u, 0, gw + GW_W1, warp, g, t, part_first);
+        dw_half<1, DET>(sDA, sX, 8192u, 1, gw + GW_W1, warp, g, t, part_first);
         {
             const uint32_t w = ring_acquire(more_tiles);  // the last stage of the tile: the next one is the next tile's layer 1
             float dx[32];
@@ -433,7 +510,13 @@ __global__ void __launch_bounds__(BWD_THREADS, 1) k_mlp_bwd(const MlpBwdParams p
 #pragma unroll
             for (int j = 0; j < 8; ++j) q[j] = quad_of_row(make_float2(dx[4 * j], dx[4 * j + 1]), make_float2(dx[4 * j + 2], dx[4 * j + 3]), t);
             const uint64_t row = (t & 1u) ? row1 : row0;
-            if (row < total_rows) {
+            if constexpr (DET) {  // dX rows to HBM; the field gradient is summed per vertex in a fixed order afterwards
+                if (row < total_rows) {
+                    float4 *dst = reinterpret_cast<float4 *>(p.dx + row * 64 + 4u * (t >> 1));
+#pragma unroll
+                    for (int j = 0; j < 8; ++j) dst[2 * j] = q[j];
+                }
+            } else if (row < total_rows) {
                 const uint4 v = __ldg(p.vi + row);
                 if (v.x != TN_EMPTY) {
                     const float b0 = __ldg(p.bary + 3 * row), b1 = __ldg(p.bary + 3 * row + 1), b2 = __ldg(p.bary + 3 * row + 2);
@@ -449,7 +532,21 @@ __global__ void __launch_bounds__(BWD_THREADS, 1) k_mlp_bwd(const MlpBwdParams p
                 }
             }
         }
+        if constexpr (DET) {
+            // the partition is complete: its column sums (all written before the barrier of the last publish()) -> its slice, the
+            // four warps in order; each thread owns one column and clears it for the next partition
+            if (part_last) {
+                const uint32_t c = tid;
+#pragma unroll 1
+                for (uint32_t k = 0; k < 7; ++k) {
+                    float *s = sums + k * 128 + c;
+                    gw[GW_B1 + k * 128 + c] = ((s[0] + s[896]) + s[1792]) + s[2688];
+                    s[0] = 0.f; s[896] = 0.f; s[1792] = 0.f; s[2688] = 0.f;
+                }
+            }
+        }
     }
+    if constexpr (DET) return;
     // ---------- flush the column sums ----------
     __syncthreads();
     for (uint32_t c = tid; c < 128; c += BWD_THREADS) {

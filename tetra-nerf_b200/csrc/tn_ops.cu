@@ -7,6 +7,8 @@
 //             its result differs by a few ulp and is checked against oracle/_ref on the GPU box);
 //   interp  : out = fma(w_k, F[v_{k+1}], out) for k = 0..D-2, then fma(1 - sum(w), F[v_0], out)
 //             -- the FFMA chain nvcc emits for tetrahedra_tracer.cu:211-219.
+#include <cub/cub.cuh>
+
 #include "tn_common.cuh"
 
 namespace tn {
@@ -284,6 +286,57 @@ static int interp_bwd(uint32_t N, uint32_t C, uint32_t V, const uint32_t *vi, co
     return TN_OK;
 }
 
+// ---- deterministic interpolate_values_backward --------------------------------------------------------------------------------
+// The (vertex, entry) pairs of the N x D vertex slots (entry = i * D + k) are sorted by vertex with a stable radix sort (the input is
+// in entry order, so equal vertices keep it); then one warp per vertex sums w_k g[i] over its entries in that order into a row-major
+// [V,C] accumulator, which is transposed to [C,V].  The products are the reference's (__fmul_rn(w_k, g)); only the order of the sum
+// is fixed, so the result does not depend on scheduling.
+__global__ void k_ivb_keys(uint32_t n, uint32_t V, const uint32_t *__restrict__ vi, uint32_t *__restrict__ keys, uint32_t *__restrict__ vals) {
+    const uint32_t e = blockIdx.x * blockDim.x + threadIdx.x;
+    if (e >= n) return;
+    const uint32_t v = vi[e];
+    keys[e] = v < V ? v : V;  // empty slots (E) sort behind every vertex
+    vals[e] = e;
+}
+__device__ __forceinline__ uint32_t lower_bound_keys(const uint32_t *__restrict__ a, uint32_t n, uint32_t x) {
+    uint32_t lo = 0, hi = n;
+    while (lo < hi) { const uint32_t mid = (lo + hi) >> 1; if (__ldg(a + mid) < x) lo = mid + 1; else hi = mid; }
+    return lo;
+}
+template <int D>
+__global__ void __launch_bounds__(256) k_ivb_det(uint32_t V, uint32_t C, uint32_t n, const uint32_t *__restrict__ keys, const uint32_t *__restrict__ vals,
+                                                 const float *__restrict__ w, const float *__restrict__ gin, float *__restrict__ grow) {
+    const uint32_t v = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31u;
+    if (v >= V) return;
+    const uint32_t lo = lower_bound_keys(keys, n, v), hi = lower_bound_keys(keys, n, v + 1);
+    for (uint32_t c0 = 0; c0 < C; c0 += 32) {
+        const uint32_t c = c0 + lane;
+        float acc = 0.f;
+        for (uint32_t b = lo; b < hi; b += 32) {
+            uint32_t i = 0;
+            float wk = 0.f;
+            if (b + lane < hi) {  // this lane's entry: sample i, vertex slot k (k_interp_bwd: slot k >= 1 has w[k-1], slot 0 the rest)
+                const uint32_t e = __ldg(vals + b + lane), k = e % D;
+                i = e / D;
+                if (k > 0) wk = __ldg(w + (size_t)i * (D - 1) + k - 1);
+                else {
+                    float weight = 0.f;
+#pragma unroll
+                    for (int q = 0; q < D - 1; ++q) weight = __fadd_rn(weight, __ldg(w + (size_t)i * (D - 1) + q));
+                    wk = __fsub_rn(1.0f, weight);
+                }
+            }
+            const uint32_t m = min(32u, hi - b);
+            for (uint32_t j = 0; j < m; ++j) {
+                const uint32_t ij = __shfl_sync(0xffffffffu, i, j);
+                const float wj = __shfl_sync(0xffffffffu, wk, j);
+                if (c < C) acc = __fadd_rn(acc, __fmul_rn(wj, __ldg(gin + (size_t)ij * C + c)));
+            }
+        }
+        if (c < C) grow[(size_t)v * C + c] = acc;
+    }
+}
+
 }  // namespace tn
 
 extern "C" int tn_find_visited_cells(tn_tracer *h, uint32_t R, uint32_t S, uint32_t M, const uint32_t *d_num, const uint32_t *d_cells,
@@ -352,6 +405,50 @@ extern "C" int tn_interpolate_values_backward(int device, uint32_t D, uint32_t N
         default: return tn::fail(TN_ERR_ARG, "Unsupported interpolation dimension with value " + std::to_string(D));
     }
     if (rc) return rc;
+    TN_CUDA(cudaGetLastError());
+    return TN_OK;
+}
+
+// workspace: keys and values of the sort (in | out), the [V,C] accumulator, CUB temporary storage; each part 256-byte aligned
+extern "C" int tn_interpolate_values_backward_deterministic(int device, uint32_t D, uint32_t N, uint32_t C, uint32_t V, const uint32_t *d_vi,
+                                                           const float *d_w, const float *d_grad_in, float *d_grad_field, void *d_workspace,
+                                                           size_t *workspace_bytes, void *stream) {
+    if (!workspace_bytes) return tn::fail(TN_ERR_ARG, "tn_interpolate_values_backward_deterministic: null workspace_bytes");
+    if (D != 2 && D != 3 && D != 4 && D != 6) return tn::fail(TN_ERR_ARG, "Unsupported interpolation dimension with value " + std::to_string(D));
+    const uint64_t n64 = (uint64_t)N * D;
+    if (n64 > 0x7FFFFFFFull) return tn::fail(TN_ERR_ARG, "tn_interpolate_values_backward_deterministic: N * D must stay below 2^31");
+    tn::DeviceGuard g(device);
+    cudaStream_t s = (cudaStream_t)stream;
+    const uint32_t n = (uint32_t)n64;
+    const int end_bit = 32 - __builtin_clz(V | 1u);  // keys are <= V
+    auto al = [](size_t b) { return (b + 255) & ~(size_t)255; };
+    size_t cub_bytes = 0;
+    TN_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, cub_bytes, (const uint32_t *)nullptr, (uint32_t *)nullptr, (const uint32_t *)nullptr,
+                                            (uint32_t *)nullptr, (int)n, 0, end_bit, s));
+    const size_t kb = al(sizeof(uint32_t) * (size_t)n), sb = al(sizeof(float) * (size_t)V * C);
+    const size_t need = 4 * kb + sb + al(cub_bytes);
+    if (!d_workspace) { *workspace_bytes = need; return TN_OK; }
+    if (*workspace_bytes < need) return tn::fail(TN_ERR_ARG, "tn_interpolate_values_backward_deterministic: workspace too small");
+    if ((size_t)C * V == 0) return TN_OK;
+    if (N == 0) {
+        TN_CUDA(cudaMemsetAsync(d_grad_field, 0, sizeof(float) * (size_t)C * V, s));
+        return TN_OK;
+    }
+    uint8_t *ws = (uint8_t *)d_workspace;
+    uint32_t *k0 = (uint32_t *)ws, *k1 = (uint32_t *)(ws + kb), *v0 = (uint32_t *)(ws + 2 * kb), *v1 = (uint32_t *)(ws + 3 * kb);
+    float *grow = (float *)(ws + 4 * kb);
+    void *tmp = ws + 4 * kb + sb;
+    tn::k_ivb_keys<<<(n + 255) / 256, 256, 0, s>>>(n, V, d_vi, k0, v0);
+    TN_CUDA(cub::DeviceRadixSort::SortPairs(tmp, cub_bytes, k0, k1, v0, v1, (int)n, 0, end_bit, s));
+    const uint32_t blocks = (uint32_t)(((uint64_t)V * 32 + 255) / 256);
+    switch (D) {
+        case 2: tn::k_ivb_det<2><<<blocks, 256, 0, s>>>(V, C, n, k1, v1, d_w, d_grad_in, grow); break;
+        case 3: tn::k_ivb_det<3><<<blocks, 256, 0, s>>>(V, C, n, k1, v1, d_w, d_grad_in, grow); break;
+        case 4: tn::k_ivb_det<4><<<blocks, 256, 0, s>>>(V, C, n, k1, v1, d_w, d_grad_in, grow); break;
+        default: tn::k_ivb_det<6><<<blocks, 256, 0, s>>>(V, C, n, k1, v1, d_w, d_grad_in, grow); break;
+    }
+    dim3 tb(32, 8), tg((V + 31) / 32, (C + 31) / 32);
+    tn::k_transpose<<<tg, tb, 0, s>>>(grow, d_grad_field, V, C, true);  // [V,C] -> [C,V]
     TN_CUDA(cudaGetLastError());
     return TN_OK;
 }

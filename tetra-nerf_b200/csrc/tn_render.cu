@@ -14,6 +14,7 @@
 #include <vector>
 
 #include <cstdlib>
+#include <cub/cub.cuh>
 #include "tn_common.cuh"
 #include "tn_mlp.cuh"
 #include "tn_mlp_bwd.cuh"
@@ -63,6 +64,21 @@ struct RenderState {
     bool profile = false;
     cudaEvent_t ev[7] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
     cudaEvent_t evb[4] = {nullptr, nullptr, nullptr, nullptr};  // backward: start | composite_bwd | mlp_bwd | finalize
+    // deterministic mode (tn_render_set_deterministic): ordered slots in the training forward, fixed-order reductions in its backward
+    bool det = false;                  // mode of the next training forward (initial value: TETRANERF_B200_DETERMINISTIC)
+    bool t_det = false;                // mode the last training forward ran in: its backward continues in it
+    uint32_t bwd_grid = 0;             // CTAs of the backward MLP kernel (test hook; 0 = default)
+    uint32_t *ray_flag = nullptr, *ray_slot = nullptr;  // [R] ray has hits, its slot (exclusive scan)
+    size_t cap_slot_R = 0;
+    void *cub_tmp = nullptr;           // CUB scan / sort temporary storage
+    size_t cub_tmp_bytes = 0;
+    float *det_part = nullptr;         // [BWD_PARTS][BWD_PART_STRIDE] per-partition dW / column sums
+    float *det_gdb = nullptr;          // [4 (ntiles + R)][128] direction-bias gradient partials
+    float *det_dx = nullptr;           // [R*S2,64] feature gradient per sample
+    float4 *det_sums = nullptr;        // [R] head-bias gradient per slot
+    float *det_dbg = nullptr;          // [R/64][128*28] partial W4dir / b4 gradients per block of k_dirbias_grads
+    uint32_t *det_keys = nullptr, *det_vals = nullptr;  // [2][R*S2*4] (vertex, sample row * 4 + k) pairs, sort input | output
+    size_t cap_det_R = 0, cap_det_S2 = 0;
 };
 
 static void free_ws(RenderState *r) {
@@ -81,6 +97,8 @@ void free_render(tn_tracer *h) {
     free_ws(r);
     cudaFree(r->fshadow); cudaFree(r->wimg); cudaFree(r->wimg16); cudaFree(r->bias); cudaFree(r->head); cudaFree(r->w4dir);
     cudaFree(r->wimg_bwd); cudaFree(r->sbins_f); cudaFree(r->enc); cudaFree(r->dout); cudaFree(r->gshadow); cudaFree(r->gw); cudaFree(r->g_dirbias);
+    cudaFree(r->ray_flag); cudaFree(r->ray_slot); cudaFree(r->cub_tmp); cudaFree(r->det_part); cudaFree(r->det_gdb); cudaFree(r->det_dx);
+    cudaFree(r->det_sums); cudaFree(r->det_dbg); cudaFree(r->det_keys); cudaFree(r->det_vals);
     for (auto &e : r->ev) if (e) cudaEventDestroy(e);
     for (auto &e : r->evb) if (e) cudaEventDestroy(e);
     delete r;
@@ -92,6 +110,8 @@ static RenderState *state(tn_tracer *h) {
         h->render = new RenderState();
         const char *e = getenv("TETRANERF_B200_MLP_PREC");  // 2 / 3: initial operand precision of the inference MLP (tn_render_set_mlp_precision)
         if (e && (atoi(e) == 2 || atoi(e) == 3)) h->render->mlp_prec = atoi(e);
+        const char *d = getenv("TETRANERF_B200_DETERMINISTIC");  // 1: initial value of tn_render_set_deterministic
+        if (d && atoi(d) == 1) h->render->det = true;
     }
     return h->render;
 }
@@ -157,6 +177,7 @@ struct SampleParams {
     // gather_rank * gather_stride + ray of EVERY rank's gathered buffer (peer[k] is mapped peer memory: stores travel over NVLink)
     float *peer[8];
     uint32_t gather_world, gather_rank, gather_stride;
+    const uint32_t *ray_slot;     // deterministic mode: slot of every ray with hits (exclusive scan of num > 0)
 };
 
 // lane 0 writes the local outputs; lanes < gather_world each post the pixel to one rank's gathered buffer (three 8-byte stores)
@@ -260,6 +281,9 @@ __host__ __device__ __forceinline__ size_t seg_arr(uint32_t M) { return (size_t)
 __host__ __device__ __forceinline__ size_t coarse_floats(uint32_t M, uint32_t Sc, uint32_t biased) { return seg_arr(M) * (biased ? 2 : 1) + (size_t)Sc + 2; }
 __host__ __device__ __forceinline__ size_t fine_floats(uint32_t M, uint32_t Smax) { return seg_arr(M) + 4 * ((size_t)Smax + 2); }
 
+// ORDERED (deterministic mode): the slot of a ray is its rank among the rays with hits (p.ray_slot), so slot order = ray order;
+// otherwise slots are claimed with an atomic counter
+template <bool ORDERED>
 __global__ void __launch_bounds__(SAMPLE_WARPS * 32) k_sample_coarse(const SampleParams p) {
     extern __shared__ float sm[];
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -270,13 +294,21 @@ __global__ void __launch_bounds__(SAMPLE_WARPS * 32) k_sample_coarse(const Sampl
     float *pm = sm + (size_t)warp * coarse_floats(M, S, p.biased);
     float *cum = pm + A, *e = cum + (p.biased ? A : 0);
     const uint32_t n = p.num[ray];
+    if constexpr (ORDERED) {
+        if (ray == p.R - 1 && lane == 0) *p.n_active = p.ray_slot[ray] + (n > 0 ? 1u : 0u);
+    }
     if (n == 0) {  // model.py:640-650 : background colour, accumulation 0, depth = collider far plane
         store_pixel(p, ray, lane, p.bg0, p.bg1, p.bg2, 0.f, p.far_plane, 0);
         return;
     }
     uint32_t slot = 0;
-    if (lane == 0) { slot = atomicAdd(p.n_active, 1u); p.ray_list[slot] = ray; p.mask[ray] = 1; }
-    slot = __shfl_sync(0xffffffffu, slot, 0);
+    if constexpr (ORDERED) {
+        slot = p.ray_slot[ray];
+        if (lane == 0) { p.ray_list[slot] = ray; p.mask[ray] = 1; }
+    } else {
+        if (lane == 0) { slot = atomicAdd(p.n_active, 1u); p.ray_list[slot] = ray; p.mask[ray] = 1; }
+        slot = __shfl_sync(0xffffffffu, slot, 0);
+    }
     const size_t row = (size_t)ray * M;
     const float near = __ldg(&p.dist[row]).x, far = __ldg(&p.dist[row + n - 1]).y;
     for (uint32_t k = lane; k < n; k += 32) {
@@ -504,8 +536,10 @@ struct CompositeBwdParams {
     const float *grad_rgb, *grad_acc;  // [R,3], [R] or nullptr
     float bg0, bg1, bg2;
     float4 *dout;                      // [slot * S2 + j]
-    float *sums;                       // 4 floats: sum d sigma_pre, sum d z_r, d z_g, d z_b (bias gradients of the two heads)
+    float *sums;                       // 4 floats: sum d sigma_pre, sum d z_r, d z_g, d z_b (bias gradients of the two heads);
+                                       // deterministic mode: [n_active] float4, one per slot (summed in slot order by k_det_sum_slots)
 };
+template <bool DET>
 __global__ void __launch_bounds__(SAMPLE_WARPS * 32) k_composite_bwd(const CompositeBwdParams p) {
     extern __shared__ float sm[];
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -554,15 +588,21 @@ __global__ void __launch_bounds__(SAMPLE_WARPS * 32) k_composite_bwd(const Compo
         s0 += o.x; s1 += o.y; s2 += o.z; s3 += o.w;
     }
     s0 = warp_sum_f(s0); s1 = warp_sum_f(s1); s2 = warp_sum_f(s2); s3 = warp_sum_f(s3);
-    if (lane == 0) { atomicAdd(p.sums, s0); atomicAdd(p.sums + 1, s1); atomicAdd(p.sums + 2, s2); atomicAdd(p.sums + 3, s3); }
+    if constexpr (DET) {
+        if (lane == 0) reinterpret_cast<float4 *>(p.sums)[slot] = make_float4(s0, s1, s2, s3);
+    } else {
+        if (lane == 0) { atomicAdd(p.sums, s0); atomicAdd(p.sums + 1, s1); atomicAdd(p.sums + 2, s2); atomicAdd(p.sums + 3, s3); }
+    }
 }
 
 // ---- after k_mlp_bwd: the direction part of mlp_head.layers.0 (W4[:, :27], b4) from the per-ray bias gradients: W4dir[k][j] =
 // sum_slot g_dirbias[slot][k] enc[slot][j], b4[k] = sum_slot g_dirbias[slot][k].  One block per 64 slots, 256 threads: thread t owns
-// hidden unit k = t & 127 and 14 of the 28 columns (27 encoding entries + the bias column of ones); partial sums -> atomicAdd.
-constexpr uint32_t DBG_SLOTS = 64;
+// hidden unit k = t & 127 and 14 of the 28 columns (27 encoding entries + the bias column of ones); partial sums -> atomicAdd
+// (deterministic mode: -> part[block][k * 28 + column], summed in block order by k_det_reduce_dbg).
+constexpr uint32_t DBG_SLOTS = 64, DBG_PART = 128 * 28;
+template <bool DET>
 __global__ void __launch_bounds__(256) k_dirbias_grads(const uint32_t *__restrict__ n_active, const float *__restrict__ g_dirbias, const float *__restrict__ enc,
-                                                        float *__restrict__ gw) {
+                                                        float *__restrict__ gw, float *__restrict__ part) {
     __shared__ float s_enc[DBG_SLOTS][28];
     const uint32_t n = *n_active, s0 = blockIdx.x * DBG_SLOTS;
     if (s0 >= n) return;
@@ -584,8 +624,109 @@ __global__ void __launch_bounds__(256) k_dirbias_grads(const uint32_t *__restric
 #pragma unroll
     for (int j = 0; j < 14; ++j) {
         const uint32_t col = j0 + (uint32_t)j;
-        atomicAdd(col < 27 ? gw + GW_W4DIR + k * 27 + col : gw + GW_B4 + k, acc[j]);
+        if constexpr (DET) part[(size_t)blockIdx.x * DBG_PART + k * 28 + col] = acc[j];
+        else atomicAdd(col < 27 ? gw + GW_W4DIR + k * 27 + col : gw + GW_B4 + k, acc[j]);
     }
+}
+
+// ---- deterministic mode: the reductions of the backward in a fixed order ----------------------------------------------------------------
+// slot flags for the ordered slot assignment of the training forward
+__global__ void k_ray_flags(uint32_t R, const uint32_t *__restrict__ num, uint32_t *__restrict__ flag) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < R) flag[i] = num[i] > 0 ? 1u : 0u;
+}
+// dW and the seven column sums: the non-empty partitions in index order
+__global__ void k_det_reduce_parts(const uint32_t *__restrict__ n_active, uint32_t S, const float *__restrict__ part, float *__restrict__ gw) {
+    const uint32_t e = blockIdx.x * blockDim.x + threadIdx.x;
+    if (e >= BWD_PART_STRIDE) return;
+    const uint32_t ntiles = (uint32_t)(((uint64_t)*n_active * S + BWD_TILE - 1) / BWD_TILE);
+    float acc = 0.f;
+    for (uint32_t q = 0; q < BWD_PARTS; ++q)
+        if (bwd_part_lo(q, ntiles) < bwd_part_lo(q + 1, ntiles)) acc += part[(size_t)q * BWD_PART_STRIDE + e];
+    gw[e] = acc;
+}
+// head-bias gradients: per-slot sums -> one block, strided sequential sums then a fixed tree
+__global__ void __launch_bounds__(256) k_det_sum_slots(const uint32_t *__restrict__ n_active, const float4 *__restrict__ part, float *__restrict__ out) {
+    __shared__ float4 s[256];
+    const uint32_t n = *n_active, t = threadIdx.x;
+    float4 a = make_float4(0.f, 0.f, 0.f, 0.f);
+    for (uint32_t i = t; i < n; i += 256) { const float4 v = part[i]; a.x += v.x; a.y += v.y; a.z += v.z; a.w += v.w; }
+    s[t] = a;
+    __syncthreads();
+    for (uint32_t h = 128; h > 0; h >>= 1) {
+        if (t < h) { const float4 b = s[t + h]; s[t].x += b.x; s[t].y += b.y; s[t].z += b.z; s[t].w += b.w; }
+        __syncthreads();
+    }
+    if (t == 0) { out[0] = s[0].x; out[1] = s[0].y; out[2] = s[0].z; out[3] = s[0].w; }
+}
+// per-ray direction-bias gradient: the partial rows of the 16-row warp blocks b that hold the ray's samples, in block order
+// (k_mlp_bwd<true> wrote block b = 4 tile + warp's partial for ray `slot` to row 4 (tile + slot) + warp)
+__global__ void __launch_bounds__(128) k_det_dirbias(const uint32_t *__restrict__ n_active, uint32_t S, const float *__restrict__ gdb_part,
+                                                     float *__restrict__ g_dirbias) {
+    const uint32_t slot = blockIdx.x, k = threadIdx.x;
+    if (slot >= *n_active) return;
+    const uint64_t r0 = (uint64_t)slot * S, r1 = r0 + S - 1;
+    float acc = 0.f;
+    for (uint64_t b = r0 / 16; b <= r1 / 16; ++b) acc += __ldg(gdb_part + (4 * (b / 4 + slot) + (b & 3)) * 128 + k);
+    g_dirbias[(size_t)slot * 128 + k] = acc;
+}
+// W4dir / b4: the per-block partials of k_dirbias_grads<true> in block order
+__global__ void k_det_reduce_dbg(const uint32_t *__restrict__ n_active, const float *__restrict__ part, float *__restrict__ gw) {
+    const uint32_t e = blockIdx.x * blockDim.x + threadIdx.x;  // k * 28 + column
+    if (e >= DBG_PART) return;
+    const uint32_t nb = (*n_active + DBG_SLOTS - 1) / DBG_SLOTS;
+    float acc = 0.f;
+    for (uint32_t b = 0; b < nb; ++b) acc += part[(size_t)b * DBG_PART + e];
+    const uint32_t k = e / 28, col = e % 28;
+    gw[col < 27 ? GW_W4DIR + k * 27 + col : GW_B4 + k] = acc;
+}
+// field gradient, step 1: (vertex, entry) pairs of every sample row, entry = row * 4 + k; rows past the active samples and empty
+// samples get the key V (sorted behind every vertex)
+__global__ void k_det_field_keys(const uint32_t *__restrict__ n_active, uint32_t S, uint32_t n, uint32_t V, const uint4 *__restrict__ vi,
+                                 uint32_t *__restrict__ keys, uint32_t *__restrict__ vals) {
+    const uint32_t e = blockIdx.x * blockDim.x + threadIdx.x;
+    if (e >= n) return;
+    const uint64_t row = e >> 2, total = (uint64_t)*n_active * S;
+    uint32_t key = V;
+    if (row < total) {
+        const uint4 v = __ldg(vi + row);
+        if (v.x != TN_EMPTY) { const uint32_t k = e & 3u; key = k == 0 ? v.x : (k == 1 ? v.y : (k == 2 ? v.z : v.w)); }
+    }
+    keys[e] = key;
+    vals[e] = e;
+}
+__device__ __forceinline__ uint32_t lower_bound_u32(const uint32_t *__restrict__ a, uint32_t n, uint32_t x) {
+    uint32_t lo = 0, hi = n;
+    while (lo < hi) { const uint32_t mid = (lo + hi) >> 1; if (__ldg(a + mid) < x) lo = mid + 1; else hi = mid; }
+    return lo;
+}
+// step 2 (after the stable sort by vertex): one warp per vertex sums w_k dX[row] over its entries in sorted (= row) order -> [V,64]
+__global__ void __launch_bounds__(256) k_det_field_grad(uint32_t V, uint32_t n, const uint32_t *__restrict__ keys, const uint32_t *__restrict__ vals,
+                                                        const float *__restrict__ bary, const float *__restrict__ dx, float *__restrict__ gshadow) {
+    const uint32_t v = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31u;
+    if (v >= V) return;
+    const uint32_t lo = lower_bound_u32(keys, n, v), hi = lower_bound_u32(keys, n, v + 1);
+    float2 acc = make_float2(0.f, 0.f);
+    for (uint32_t b = lo; b < hi; b += 32) {
+        uint32_t e = 0;
+        float w = 0.f;
+        if (b + lane < hi) {  // the weight of this lane's entry: (1 - b0 - b1 - b2, b0, b1, b2)[k], as k_mlp_bwd
+            e = __ldg(vals + b + lane);
+            const float *c = bary + 3 * (size_t)(e >> 2);
+            const float b0 = __ldg(c), b1 = __ldg(c + 1), b2 = __ldg(c + 2);
+            const uint32_t k = e & 3u;
+            w = k == 0 ? 1.0f - ((b0 + b1) + b2) : (k == 1 ? b0 : (k == 2 ? b1 : b2));
+        }
+        const uint32_t m = min(32u, hi - b);
+        for (uint32_t j = 0; j < m; ++j) {
+            const uint32_t ej = __shfl_sync(0xffffffffu, e, j);
+            const float wj = __shfl_sync(0xffffffffu, w, j);
+            const float2 x = __ldg(reinterpret_cast<const float2 *>(dx + (size_t)(ej >> 2) * 64) + lane);
+            acc.x = fmaf(wj, x.x, acc.x);
+            acc.y = fmaf(wj, x.y, acc.y);
+        }
+    }
+    reinterpret_cast<float2 *>(gshadow + (size_t)v * 64)[lane] = acc;
 }
 struct GradOut { float *p[12]; };
 __global__ void k_scatter_grads(const float *__restrict__ gw, const GradOut o) {
@@ -637,6 +778,50 @@ static int ensure_ws(RenderState *r, size_t R, size_t M, size_t Sc, size_t S2) {
     A(r->ebins_f, 4 * R * (S2 + 1)); A(r->bary_f, 12 * R * S2); A(r->out_f, 16 * R * S2); A(r->dirbias, 512 * R); A(r->vi_f, 16 * R * S2);
 #undef A
     r->cap_R = R; r->cap_M = M; r->cap_Sc = Sc; r->cap_S2 = S2;
+    return TN_OK;
+}
+
+static int ensure_cub_tmp(RenderState *r, size_t bytes) {
+    if (bytes <= r->cub_tmp_bytes) return TN_OK;
+    cudaFree(r->cub_tmp); r->cub_tmp = nullptr; r->cub_tmp_bytes = 0;
+    TN_CUDA(cudaMalloc(&r->cub_tmp, bytes));
+    r->cub_tmp_bytes = bytes;
+    return TN_OK;
+}
+
+// deterministic mode, forward: slot of every ray = number of rays with hits before it (exclusive scan)
+static int ordered_slots(RenderState *r, uint32_t R, cudaStream_t s) {
+    if (R > r->cap_slot_R) {
+        cudaFree(r->ray_flag); cudaFree(r->ray_slot); r->ray_flag = r->ray_slot = nullptr; r->cap_slot_R = 0;
+        TN_CUDA(cudaMalloc((void **)&r->ray_flag, 4 * (size_t)R));
+        TN_CUDA(cudaMalloc((void **)&r->ray_slot, 4 * (size_t)R));
+        r->cap_slot_R = R;
+    }
+    size_t bytes = 0;
+    TN_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, bytes, r->ray_flag, r->ray_slot, (int)R, s));
+    int rc = ensure_cub_tmp(r, bytes);
+    if (rc) return rc;
+    k_ray_flags<<<(R + 255) / 256, 256, 0, s>>>(R, r->num, r->ray_flag);
+    TN_CUDA(cub::DeviceScan::ExclusiveSum(r->cub_tmp, bytes, r->ray_flag, r->ray_slot, (int)R, s));
+    return TN_OK;
+}
+
+// deterministic mode, backward workspace for R rays of S2 fine samples
+static int ensure_det_ws(RenderState *r, size_t R, size_t S2) {
+    if (!r->det_part) TN_CUDA(cudaMalloc((void **)&r->det_part, sizeof(float) * BWD_PARTS * (size_t)BWD_PART_STRIDE));
+    if (R <= r->cap_det_R && S2 <= r->cap_det_S2) return TN_OK;
+    cudaFree(r->det_gdb); cudaFree(r->det_dx); cudaFree(r->det_sums); cudaFree(r->det_dbg); cudaFree(r->det_keys); cudaFree(r->det_vals);
+    r->det_gdb = r->det_dx = r->det_dbg = nullptr; r->det_sums = nullptr; r->det_keys = r->det_vals = nullptr;
+    r->cap_det_R = r->cap_det_S2 = 0;
+    R = std::max(R, r->cap_det_R); S2 = std::max(S2, r->cap_det_S2);
+    const size_t rows = R * S2, ntiles = (rows + BWD_TILE - 1) / BWD_TILE;
+    TN_CUDA(cudaMalloc((void **)&r->det_gdb, sizeof(float) * 4 * (ntiles + R) * 128));
+    TN_CUDA(cudaMalloc((void **)&r->det_dx, sizeof(float) * 64 * rows));
+    TN_CUDA(cudaMalloc((void **)&r->det_sums, sizeof(float4) * R));
+    TN_CUDA(cudaMalloc((void **)&r->det_dbg, sizeof(float) * DBG_PART * ((R + DBG_SLOTS - 1) / DBG_SLOTS)));
+    TN_CUDA(cudaMalloc((void **)&r->det_keys, sizeof(uint32_t) * 2 * 4 * rows));
+    TN_CUDA(cudaMalloc((void **)&r->det_vals, sizeof(uint32_t) * 2 * 4 * rows));
+    r->cap_det_R = R; r->cap_det_S2 = S2;
     return TN_OK;
 }
 
@@ -715,6 +900,9 @@ static int render_impl(tn_tracer *h, const tn_render_config *cfg, const float *d
     const uint32_t M = cfg->max_ray_triangles, Sc = cfg->num_samples, Sf = cfg->num_fine_samples;
     if (Sc == 0 || Sc > 4096 || Sf > 4096) return fail(TN_ERR_ARG, "tn_render: num_samples must be in [1,4096]");
     if (tf != nullptr && Sf == 0) return fail(TN_ERR_ARG, "tn_render_train_forward: the fused training step needs num_fine_samples > 0");
+    const bool det = tf != nullptr && r->det;
+    if (det && (uint64_t)R * (Sc + Sf + 1) * 4 > 0x7FFFFFFFull)
+        return fail(TN_ERR_ARG, "tn_render_train_forward: deterministic mode takes at most 2^29 fine samples per call (split the batch)");
     if (R == 0) return TN_OK;
     if ((uint64_t)R * (uint64_t)(Sc + Sf + 1) >= (1ull << 32)) return fail(TN_ERR_ARG, "tn_render: rays x samples must stay below 2^32 per call (split the batch)");
     const bool single = Sf == 0;                       // one pass only: the colours come from the coarse samples
@@ -759,7 +947,8 @@ static int render_impl(tn_tracer *h, const tn_render_config *cfg, const float *d
     const size_t smem_sc = SAMPLE_WARPS * sizeof(float) * coarse_floats(M, Sc, p.biased);
     const size_t smem_sf = SAMPLE_WARPS * sizeof(float) * fine_floats(M, Smax);
     const size_t smem_c = SAMPLE_WARPS * sizeof(float) * 2 * ((size_t)S2 + 2);
-    TN_CUDA(cudaFuncSetAttribute(k_sample_coarse, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_sc));
+    auto k_coarse_sample = det ? k_sample_coarse<true> : k_sample_coarse<false>;
+    TN_CUDA(cudaFuncSetAttribute(k_coarse_sample, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_sc));
     TN_CUDA(cudaFuncSetAttribute(k_sample_fine, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_sf));
     TN_CUDA(cudaFuncSetAttribute(k_composite, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_c));
     auto k_coarse = prec == 2 ? k_mlp<false, 2> : k_mlp<false, 3>;
@@ -768,7 +957,13 @@ static int render_impl(tn_tracer *h, const tn_render_config *cfg, const float *d
     TN_CUDA(cudaFuncSetAttribute(k_fine, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)MLP_SMEM_BYTES));
     const uint32_t gridR = (R + SAMPLE_WARPS - 1) / SAMPLE_WARPS;
 
-    k_sample_coarse<<<gridR, SAMPLE_WARPS * 32, smem_sc, s>>>(p);
+    if (det) {
+        rc = ordered_slots(r, R, s);
+        if (rc) return rc;
+        p.ray_slot = r->ray_slot;
+        h->launches += 2;
+    }
+    k_coarse_sample<<<gridR, SAMPLE_WARPS * 32, smem_sc, s>>>(p);
     TN_EV(2);
     MlpParams mc{};
     mc.n_active = r->n_active; mc.S = Sc; mc.vi = r->vi_c; mc.bary = r->bary_c; mc.fshadow = r->fshadow; mc.wimg = prec == 2 ? r->wimg16 : r->wimg;
@@ -799,6 +994,7 @@ static int render_impl(tn_tracer *h, const tn_render_config *cfg, const float *d
     TN_CUDA(cudaGetLastError());
     if (tf != nullptr) {
         r->train_valid = true;
+        r->t_det = det;
         r->t_R = R; r->t_M = M; r->t_Sc = Sc; r->t_Sf = Sf; r->t_S2 = S2;
         r->t_bg[0] = cfg->background[0]; r->t_bg[1] = cfg->background[1]; r->t_bg[2] = cfg->background[2];
     }
@@ -853,29 +1049,67 @@ extern "C" int tn_render_train_backward(tn_tracer *h, const float *d_grad_rgb, c
     int sms = 132;
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, h->device);
     const uint32_t R = r->t_R, S2 = r->t_S2, V = r->V;
+    const bool det = r->t_det;
+    if (det) {
+        const int rc = ensure_det_ws(r, R, S2);
+        if (rc) return rc;
+    }
     TN_CUDA(cudaMemsetAsync(r->gw, 0, sizeof(float) * GW_TOTAL, s));
-    TN_CUDA(cudaMemsetAsync(r->gshadow, 0, sizeof(float) * 64 * (size_t)V, s));
-    TN_CUDA(cudaMemsetAsync(r->g_dirbias, 0, 512 * (size_t)R, s));
-    TN_CUDA(cudaMemsetAsync(r->n_active + 3, 0, 4, s));  // tile counter of the backward kernel (word 3 of the 16-byte block)
+    if (!det) {  // (deterministic mode writes every element of these)
+        TN_CUDA(cudaMemsetAsync(r->gshadow, 0, sizeof(float) * 64 * (size_t)V, s));
+        TN_CUDA(cudaMemsetAsync(r->g_dirbias, 0, 512 * (size_t)R, s));
+        TN_CUDA(cudaMemsetAsync(r->n_active + 3, 0, 4, s));  // tile counter of the backward kernel (word 3 of the 16-byte block)
+    }
     CompositeBwdParams cb{};
     cb.S2 = S2; cb.use_gradient_scaling = use_gradient_scaling ? 1u : 0u; cb.n_active = r->n_active; cb.ray_list = r->ray_list;
     cb.ebins_f = r->ebins_f; cb.sbins_f = r->sbins_f; cb.out_f = r->out_f; cb.grad_rgb = d_grad_rgb; cb.grad_acc = d_grad_acc;
-    cb.bg0 = r->t_bg[0]; cb.bg1 = r->t_bg[1]; cb.bg2 = r->t_bg[2]; cb.dout = r->dout; cb.sums = r->gw + GW_SUMS;
+    cb.bg0 = r->t_bg[0]; cb.bg1 = r->t_bg[1]; cb.bg2 = r->t_bg[2]; cb.dout = r->dout; cb.sums = det ? (float *)r->det_sums : r->gw + GW_SUMS;
     const size_t smem_cb = SAMPLE_WARPS * sizeof(float) * 4 * ((size_t)S2 + 2);
-    TN_CUDA(cudaFuncSetAttribute(k_composite_bwd, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_cb));
+    auto k_cbwd = det ? k_composite_bwd<true> : k_composite_bwd<false>;
+    TN_CUDA(cudaFuncSetAttribute(k_cbwd, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_cb));
     const uint32_t gridR = (R + SAMPLE_WARPS - 1) / SAMPLE_WARPS;
     if (r->profile) cudaEventRecord(r->evb[0], s);
-    k_composite_bwd<<<gridR, SAMPLE_WARPS * 32, smem_cb, s>>>(cb);
+    k_cbwd<<<gridR, SAMPLE_WARPS * 32, smem_cb, s>>>(cb);
     if (r->profile) cudaEventRecord(r->evb[1], s);
     MlpBwdParams bp{};
     bp.n_active = r->n_active; bp.S = S2; bp.vi = r->vi_f; bp.bary = r->bary_f; bp.fshadow = r->fshadow; bp.wimg = r->wimg_bwd;
     bp.bias = r->bias; bp.head = r->head; bp.dirbias = r->dirbias; bp.dout = r->dout; bp.gshadow = r->gshadow;
     bp.gw = r->gw; bp.g_dirbias = r->g_dirbias; bp.tile_ctr = r->n_active + 3;
-    TN_CUDA(cudaFuncSetAttribute(k_mlp_bwd, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)BWD_SMEM_BYTES));
     const uint64_t tiles = ((uint64_t)R * S2 + BWD_TILE - 1) / BWD_TILE;
-    k_mlp_bwd<<<(uint32_t)std::min<uint64_t>(tiles, (uint64_t)sms), BWD_THREADS, BWD_SMEM_BYTES, s>>>(bp);
-    if (r->profile) cudaEventRecord(r->evb[2], s);
-    k_dirbias_grads<<<(R + DBG_SLOTS - 1) / DBG_SLOTS, 256, 0, s>>>(r->n_active, r->g_dirbias, r->enc, r->gw);
+    if (!det) {
+        TN_CUDA(cudaFuncSetAttribute(k_mlp_bwd<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)BWD_SMEM_BYTES));
+        const uint32_t grid = r->bwd_grid ? r->bwd_grid : (uint32_t)std::min<uint64_t>(tiles, (uint64_t)sms);
+        k_mlp_bwd<false><<<grid, BWD_THREADS, BWD_SMEM_BYTES, s>>>(bp);
+        if (r->profile) cudaEventRecord(r->evb[2], s);
+        k_dirbias_grads<false><<<(R + DBG_SLOTS - 1) / DBG_SLOTS, 256, 0, s>>>(r->n_active, r->g_dirbias, r->enc, r->gw, nullptr);
+    } else {
+        // the same stages with every reduction in a fixed order (header of tn_mlp_bwd.cuh); the grid only decides which CTA runs
+        // which partition, never what is summed in which order
+        MlpBwdDetParams dp{};
+        static_cast<MlpBwdParams &>(dp) = bp;
+        dp.part = r->det_part; dp.gdb_part = r->det_gdb; dp.dx = r->det_dx;
+        TN_CUDA(cudaFuncSetAttribute(k_mlp_bwd<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)BWD_DET_SMEM_BYTES));
+        const uint32_t grid = r->bwd_grid ? r->bwd_grid : std::min<uint32_t>(BWD_PARTS, (uint32_t)sms);
+        k_mlp_bwd<true><<<grid, BWD_THREADS, BWD_DET_SMEM_BYTES, s>>>(dp);
+        if (r->profile) cudaEventRecord(r->evb[2], s);
+        k_det_reduce_parts<<<(BWD_PART_STRIDE + 255) / 256, 256, 0, s>>>(r->n_active, S2, r->det_part, r->gw);
+        k_det_sum_slots<<<1, 256, 0, s>>>(r->n_active, r->det_sums, r->gw + GW_SUMS);
+        k_det_dirbias<<<R, 128, 0, s>>>(r->n_active, S2, r->det_gdb, r->g_dirbias);
+        k_dirbias_grads<true><<<(R + DBG_SLOTS - 1) / DBG_SLOTS, 256, 0, s>>>(r->n_active, r->g_dirbias, r->enc, r->gw, r->det_dbg);
+        k_det_reduce_dbg<<<(DBG_PART + 255) / 256, 256, 0, s>>>(r->n_active, r->det_dbg, r->gw);
+        // field gradient: stable sort of (vertex, row * 4 + k) by vertex, then per-vertex sums in row order
+        const uint32_t n = (uint32_t)(4 * (uint64_t)R * S2);
+        const int end_bit = 32 - __builtin_clz(V | 1u);  // keys are <= V
+        uint32_t *k0 = r->det_keys, *k1 = r->det_keys + n, *v0 = r->det_vals, *v1 = r->det_vals + n;
+        size_t bytes = 0;
+        TN_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, bytes, k0, k1, v0, v1, (int)n, 0, end_bit, s));
+        const int rc = ensure_cub_tmp(r, bytes);
+        if (rc) return rc;
+        k_det_field_keys<<<(n + 255) / 256, 256, 0, s>>>(r->n_active, S2, n, V, (const uint4 *)r->vi_f, k0, v0);
+        TN_CUDA(cub::DeviceRadixSort::SortPairs(r->cub_tmp, bytes, k0, k1, v0, v1, (int)n, 0, end_bit, s));
+        k_det_field_grad<<<(uint32_t)(((uint64_t)V * 32 + 255) / 256), 256, 0, s>>>(V, n, k1, v1, r->bary_f, r->det_dx, r->gshadow);
+        h->launches += 9;
+    }
     GradOut go{};
     for (int i = 0; i < 12; ++i) {
         if (!d_grad_params12[i]) return fail(TN_ERR_ARG, "tn_render_train_backward: null parameter gradient pointer");
@@ -886,6 +1120,22 @@ extern "C" int tn_render_train_backward(tn_tracer *h, const float *d_grad_rgb, c
     if (r->profile) cudaEventRecord(r->evb[3], s);
     h->launches += 5;
     TN_CUDA(cudaGetLastError());
+    return TN_OK;
+}
+
+// deterministic mode of the fused training step (see the header): applies from the next tn_render_train_forward on
+extern "C" int tn_render_set_deterministic(tn_tracer *h, int enable) {
+    if (!h) return fail(TN_ERR_ARG, "null tracer");
+    DeviceGuard g(h->device);
+    state(h)->det = enable != 0;
+    return TN_OK;
+}
+
+// test hook: CTAs of the backward MLP kernel (0 = default: one per SM, capped by the tiles / partitions)
+extern "C" int tn_render_set_backward_grid(tn_tracer *h, uint32_t ctas) {
+    if (!h) return fail(TN_ERR_ARG, "null tracer");
+    DeviceGuard g(h->device);
+    state(h)->bwd_grid = ctas;
     return TN_OK;
 }
 

@@ -99,7 +99,9 @@ class FusedRenderer:
     def train_forward(self, origins: torch.Tensor, directions: torch.Tensor, settings: RenderSettings, jitter_coarse: Optional[torch.Tensor] = None,
                       jitter_fine: Optional[torch.Tensor] = None):
         """training-mode forward (stratified bins from the given uniform draws f32[R,S_c+1] / f32[R,S_f+1]; None = eval bins; RGB renderer
-        without clamp).  Keeps the per-sample buffers the backward continues from."""
+        without clamp).  Keeps the per-sample buffers the backward continues from.  Runs in deterministic mode (bitwise reproducible
+        outputs and gradients, see tn_render_set_deterministic) when `torch.are_deterministic_algorithms_enabled()` or
+        TETRANERF_B200_DETERMINISTIC=1; the backward continues in the mode of its forward."""
         tr = self.tracer
         tr._check_float_dim3(origins, "ray_origins")
         tr._check_float_dim3(directions, "ray_directions")
@@ -111,6 +113,7 @@ class FusedRenderer:
         out = {"rgb": torch.empty((R, 3), dtype=torch.float32, device=dev), "accumulation": torch.empty((R, 1), dtype=torch.float32, device=dev),
                "depth": torch.empty((R, 1), dtype=torch.float32, device=dev), "ray_mask": torch.empty((R,), dtype=torch.bool, device=dev)}
         cfg = _config(settings)
+        ext._check(_lib.tn_render_set_deterministic(tr.handle, int(ext.deterministic_enabled())))
         ext._check(_lib.tn_render_train_forward(tr.handle, C.byref(cfg), origins.data_ptr(), directions.data_ptr(), R,
                                                 jitter_coarse.data_ptr() if jitter_coarse is not None else None,
                                                 jitter_fine.data_ptr() if jitter_fine is not None else None, out["rgb"].data_ptr(),
@@ -134,6 +137,10 @@ class FusedRenderer:
         """operand precision of the inference MLP: 2 = f16w2 (default: fp16 activations x fp16 hi/lo weights, ~2.6e-5 absolute on
         unit-scale density / colour, inside the 1e-4 per-sample bar), 3 = bf16x3 (fp32-level, ~5e-7).  Training always runs bf16x3."""
         ext._check(_lib.tn_render_set_mlp_precision(self.tracer.handle, int(prec)))
+
+    def set_backward_grid(self, ctas: int) -> None:
+        """test hook: CTAs of the backward MLP kernel (0 = default, one per SM)"""
+        ext._check(_lib.tn_render_set_backward_grid(self.tracer.handle, int(ctas)))
 
     def set_profiling(self, enable: bool) -> None:
         ext._check(_lib.tn_render_set_profiling(self.tracer.handle, int(enable)))

@@ -36,6 +36,7 @@ _lib.tn_trace_rays_triangles.argtypes = [_vp, _vp, _vp, _u32, _u32, _vp, _vp, _v
 _lib.tn_find_tetrahedra.argtypes = [_vp, _vp, _u32, _vp, _vp, _vp, _vp]
 _lib.tn_find_visited_cells.argtypes = [_vp, _u32, _u32, _u32] + [_vp] * 11
 _lib.tn_interpolate_values_backward.argtypes = [_i, _u32, _u32, _u32, _u32, _vp, _vp, _vp, _vp, _vp, _vp]
+_lib.tn_interpolate_values_backward_deterministic.argtypes = [_i, _u32, _u32, _u32, _u32, _vp, _vp, _vp, _vp, _vp, C.POINTER(C.c_size_t), _vp]
 _lib.tn_make_field_shadow.argtypes = [_i, _u32, _u32, _vp, _vp, _vp]
 _lib.tn_interpolate_values_shadow.argtypes = [_i, _u32, _u32, _u32, _u32, _vp, _vp, _vp, _vp, _vp]
 _lib.tn_debug_trace_stats.argtypes = [_vp, C.POINTER(_u32)]
@@ -62,6 +63,8 @@ _lib.tn_render_set_profiling.argtypes = [_vp, _i]
 _lib.tn_render_set_mlp_precision.argtypes = [_vp, _i]
 _lib.tn_render_get_timings.argtypes = [_vp, C.POINTER(C.c_float)]
 _lib.tn_render_get_backward_timings.argtypes = [_vp, C.POINTER(C.c_float)]
+_lib.tn_render_set_deterministic.argtypes = [_vp, _i]
+_lib.tn_render_set_backward_grid.argtypes = [_vp, _u32]
 
 LIBRARY_PATH = str(_LIB_PATH)
 
@@ -73,6 +76,12 @@ def _check(rc: int):
 
 def _stream(device: torch.device) -> int:
     return torch.cuda.current_stream(device).cuda_stream
+
+
+def deterministic_enabled() -> bool:
+    """Whether the custom ops run in their bitwise-reproducible mode: `torch.use_deterministic_algorithms(True)` or the environment
+    variable TETRANERF_B200_DETERMINISTIC=1.  Read on every call."""
+    return torch.are_deterministic_algorithms_enabled() or os.environ.get("TETRANERF_B200_DETERMINISTIC", "0") == "1"
 
 
 def _require(cond: bool, msg: str):
@@ -343,6 +352,13 @@ def interpolate_values_backward(vertex_indices, barycentric_coordinates, field, 
     dev = grad_in.device
     grad_field = torch.empty((Cdim, V), dtype=torch.float32, device=dev)
     grad_in = grad_in.contiguous()
+    if deterministic_enabled():  # sorted by vertex, summed in input order: bitwise reproducible
+        nbytes = C.c_size_t(0)
+        args = (dev.index, D, N, Cdim, V, vertex_indices.data_ptr(), barycentric_coordinates.data_ptr(), grad_in.data_ptr(), grad_field.data_ptr())
+        _check(_lib.tn_interpolate_values_backward_deterministic(*args, None, C.byref(nbytes), _stream(dev)))
+        workspace = torch.empty((max(int(nbytes.value), 1),), dtype=torch.uint8, device=dev)
+        _check(_lib.tn_interpolate_values_backward_deterministic(*args, workspace.data_ptr(), C.byref(nbytes), _stream(dev)))
+        return grad_field
     # row-major [V,C] accumulator for the vector-reduction path (worth it once there is more than a handful of samples)
     scratch = torch.empty((V, Cdim), dtype=torch.float32, device=dev) if (Cdim % 4 == 0 and N >= 1024) else None
     _check(_lib.tn_interpolate_values_backward(dev.index, D, N, Cdim, V, vertex_indices.data_ptr(), barycentric_coordinates.data_ptr(),
