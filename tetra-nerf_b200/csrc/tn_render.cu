@@ -10,6 +10,7 @@
 //   k_mlp<true>     : interpolate_values + mlp_base + density + mlp_head + colour head (:596-621)
 //   k_composite     : get_weights, RGB / accumulation / median-depth renderers, scatter to rays (:632-662)
 // Per-ray kernels use one warp per ray with the ray's segments staged in shared memory.
+#include <atomic>
 #include <cmath>
 #include <vector>
 
@@ -37,6 +38,7 @@ struct RenderState {
     float *head = nullptr;     // wd[128] wc[3][128] bd bc[3]
     float *w4dir = nullptr;    // [128][27] + b4[128]
     bool have_weights = false;
+    uint64_t gen = 0;          // generation of field + weights: a fresh value from next_generation() on every set_field / set_weights
     // workspace
     size_t cap_R = 0, cap_M = 0, cap_Sc = 0, cap_S2 = 0;
     uint32_t *num = nullptr, *cells = nullptr, *verts = nullptr;
@@ -46,9 +48,9 @@ struct RenderState {
     uint4 *vi_c = nullptr;
     float *ebins_f = nullptr, *bary_f = nullptr, *out_f = nullptr, *dirbias = nullptr;
     uint4 *vi_f = nullptr;
-    // training (tn_render_train_forward / _backward): backward weight image, per-sample head gradients, accumulators
+    // training: backward weight image, per-sample head gradients, accumulators (scratch of every backward, saved state or not)
     uint8_t *wimg_bwd = nullptr;       // 7 stages of 32 KB (tn_mlp_bwd.cuh)
-    float *sbins_f = nullptr, *enc = nullptr;   // [R,S2+1] spacing bins of the fine pass, [R,27] encoded directions (per slot)
+    float *sbins_f = nullptr, *enc = nullptr;   // tn_render_train_forward: [R,S2+1] spacing bins of the fine pass, [R,27] encoded directions (per slot)
     float4 *dout = nullptr;            // [R*S2] gradients at the head pre-activations
     float *gshadow = nullptr, *gw = nullptr, *g_dirbias = nullptr;
     size_t cap_train_R = 0, cap_train_S2 = 0;
@@ -103,6 +105,12 @@ void free_render(tn_tracer *h) {
     for (auto &e : r->evb) if (e) cudaEventDestroy(e);
     delete r;
     h->render = nullptr;
+}
+
+// generations are unique across tracers, so a saved state recorded on one tracer never matches another tracer's field and weights
+static uint64_t next_generation() {
+    static std::atomic<uint64_t> g{0};
+    return ++g;
 }
 
 static RenderState *state(tn_tracer *h) {
@@ -837,6 +845,7 @@ extern "C" int tn_render_set_field(tn_tracer *h, const float *d_field, uint32_t 
     if (r->V != V) { cudaFree(r->fshadow); r->fshadow = nullptr; TN_CUDA(cudaMalloc((void **)&r->fshadow, sizeof(float) * 64 * (size_t)V)); r->V = V; }
     k_transpose64<<<(V + 31) / 32, dim3(32, 8), 0, (cudaStream_t)stream>>>(d_field, r->fshadow, V);
     h->launches += 1;
+    r->gen = next_generation();
     TN_CUDA(cudaGetLastError());
     return TN_OK;
 }
@@ -879,14 +888,59 @@ extern "C" int tn_render_set_weights(tn_tracer *h, const float *const *P, void *
     launch_pack_weights(P[4], 128, 0, 128, r->wimg_bwd + 3 * BWD_STAGE, s, 16384u, 32768u);
     launch_pack_weights(P[6], 155, 27, 128, r->wimg_bwd + 5 * BWD_STAGE, s, 16384u, 32768u);
     h->launches += 13;
+    r->gen = next_generation();
     TN_CUDA(cudaGetLastError());
     r->have_weights = true;
     return TN_OK;
 }
 
-// training-mode inputs of the forward (nullptr = eval)
+// the buffers a training forward leaves for its backward: the tracer's own (tn_render_train_forward, the "last call") or those of a
+// caller's saved-state blob (tn_render_train_forward_saved)
+struct TrainBufs {
+    uint32_t *n_active;        // 16-byte block: active rays | tile counter of the coarse pass | of the fine pass | (unused)
+    uint32_t *ray_list;        // [R] slot -> ray
+    float *ebins_f, *sbins_f;  // [R,S2+1] euclidean / spacing bins of the fine pass
+    uint4 *vi_f;               // [R*S2] matched vertices
+    float *bary_f;             // [R*S2,3] their weights
+    float *out_f;              // [R*S2] (sigma, r, g, b) head pre-activations
+    float *dirbias, *enc;      // [R,128] direction bias, [R,27] encoded direction
+};
+static TrainBufs own_bufs(RenderState *r) {
+    return TrainBufs{r->n_active, r->ray_list, r->ebins_f, r->sbins_f, r->vi_f, r->bary_f, r->out_f, r->dirbias, r->enc};
+}
+
+// saved-state blob of tn_render_train_forward_saved: this header, then the TrainBufs arrays, each 256-byte aligned
+constexpr uint32_t SAVED_MAGIC = 0x53564e54u;  // "TNVS"
+struct SavedHeader {
+    uint32_t magic, R, M, Sc, Sf, S2, det, pad;
+    float bg[3];
+    uint32_t pad2;
+    uint64_t gen;              // RenderState::gen at the forward
+};
+constexpr size_t SAVED_ALIGN = 256;
+static_assert(sizeof(SavedHeader) <= SAVED_ALIGN, "saved-state header exceeds its slot");
+// bytes of the blob for R rays of S2 fine samples; with base != nullptr also the array pointers inside it
+static size_t saved_layout(size_t R, size_t S2, uint8_t *base, TrainBufs *b) {
+    size_t off = SAVED_ALIGN;  // header
+    auto take = [&](size_t bytes) { uint8_t *p = base ? base + off : nullptr; off += (bytes + SAVED_ALIGN - 1) / SAVED_ALIGN * SAVED_ALIGN; return p; };
+    TrainBufs t{};
+    t.n_active = (uint32_t *)take(16);
+    t.ray_list = (uint32_t *)take(4 * R);
+    t.ebins_f = (float *)take(4 * R * (S2 + 1));
+    t.sbins_f = (float *)take(4 * R * (S2 + 1));
+    t.vi_f = (uint4 *)take(16 * R * S2);
+    t.bary_f = (float *)take(12 * R * S2);
+    t.out_f = (float *)take(16 * R * S2);
+    t.dirbias = (float *)take(512 * R);
+    t.enc = (float *)take(4 * 27 * R);
+    if (b) *b = t;
+    return off;
+}
+
+// training-mode inputs of the forward (nullptr = eval); saved == nullptr: the tracer's own buffers
 struct TrainFwd {
     const float *jit_c, *jit_f;
+    const TrainBufs *saved;
 };
 static int ensure_train_ws(RenderState *r, size_t R, size_t S2, uint32_t V);
 
@@ -916,8 +970,9 @@ static int render_impl(tn_tracer *h, const tn_render_config *cfg, const float *d
         if (rc) return rc;
     }
     r->train_valid = false;
+    const TrainBufs b = tf != nullptr && tf->saved != nullptr ? *tf->saved : own_bufs(r);
     const int prec = tf != nullptr ? 3 : r->mlp_prec;  // the training forward keeps bf16x3 (its backward recomputes in bf16x3)
-    TN_CUDA(cudaMemsetAsync(r->n_active, 0, 16, s));
+    TN_CUDA(cudaMemsetAsync(b.n_active, 0, 16, s));
 #define TN_EV(i) do { if (r->profile) cudaEventRecord(r->ev[i], s); } while (0)
     TN_EV(0);  // the "trace" interval includes the L2 warm-up it exists for
     {   // L2 warm-up of everything read-only that the step gathers from (mesh tables, field shadow, weight image)
@@ -932,12 +987,12 @@ static int render_impl(tn_tracer *h, const tn_render_config *cfg, const float *d
     SampleParams p{};
     p.R = R; p.M = M; p.Sc = Sc; p.Sf = Sf; p.S2 = S2; p.biased = cfg->use_biased_sampler;
     p.num = r->num; p.dist = (const float2 *)r->dist; p.verts = (const uint4 *)r->verts; p.bary = r->bary;
-    p.o = d_origins; p.d = d_directions; p.n_active = r->n_active; p.ray_list = r->ray_list;
+    p.o = d_origins; p.d = d_directions; p.n_active = b.n_active; p.ray_list = b.ray_list;
     p.ebins_c = r->ebins_c; p.sbins_c = r->sbins_c; p.bary_c = r->bary_c; p.vi_c = r->vi_c; p.dens_c = r->dens_c;
-    p.ebins_f = r->ebins_f; p.bary_f = r->bary_f; p.vi_f = r->vi_f; p.dirbias = r->dirbias; p.w4dir = r->w4dir; p.out_f = r->out_f;
+    p.ebins_f = b.ebins_f; p.bary_f = b.bary_f; p.vi_f = b.vi_f; p.dirbias = b.dirbias; p.w4dir = r->w4dir; p.out_f = b.out_f;
     p.rgb = d_rgb; p.acc = d_acc; p.depth = d_depth; p.mask = d_mask;
     p.far_plane = cfg->far_plane; p.bg0 = cfg->background[0]; p.bg1 = cfg->background[1]; p.bg2 = cfg->background[2];
-    if (tf != nullptr) { p.train = 1; p.jit_c = tf->jit_c; p.jit_f = tf->jit_f; p.sbins_f = r->sbins_f; p.enc = r->enc; }
+    if (tf != nullptr) { p.train = 1; p.jit_c = tf->jit_c; p.jit_f = tf->jit_f; p.sbins_f = b.sbins_f; p.enc = b.enc; }
     if (r->gather_world) {
         if (R > r->gather_stride) return fail(TN_ERR_ARG, "tn_render: more rays than the gathered-pixel buffers were sized for (tn_render_set_gather)");
         for (int k = 0; k < 8; ++k) p.peer[k] = r->peer[k];
@@ -966,9 +1021,9 @@ static int render_impl(tn_tracer *h, const tn_render_config *cfg, const float *d
     k_coarse_sample<<<gridR, SAMPLE_WARPS * 32, smem_sc, s>>>(p);
     TN_EV(2);
     MlpParams mc{};
-    mc.n_active = r->n_active; mc.S = Sc; mc.vi = r->vi_c; mc.bary = r->bary_c; mc.fshadow = r->fshadow; mc.wimg = prec == 2 ? r->wimg16 : r->wimg;
+    mc.n_active = b.n_active; mc.S = Sc; mc.vi = r->vi_c; mc.bary = r->bary_c; mc.fshadow = r->fshadow; mc.wimg = prec == 2 ? r->wimg16 : r->wimg;
     mc.bias = r->bias; mc.head = r->head; mc.dirbias = nullptr; mc.out = r->dens_c;
-    mc.tile_ctr = r->n_active + 1;  // words 1, 2 of the zeroed 16-byte block: tile counters of the coarse / fine pass
+    mc.tile_ctr = b.n_active + 1;  // words 1, 2 of the zeroed 16-byte block: tile counters of the coarse / fine pass
     // one CTA per SM at most (the weight image fills its shared memory), MLP_WGS tiles of MLP_TILE samples in flight per CTA
     int sms = 132;
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, h->device);
@@ -981,10 +1036,10 @@ static int render_impl(tn_tracer *h, const tn_render_config *cfg, const float *d
     else k_dirbias_only<<<gridR, SAMPLE_WARPS * 32, 0, s>>>(p);
     TN_EV(4);
     MlpParams mf = mc;
-    mf.S = S2; mf.dirbias = r->dirbias; mf.out = r->out_f;
-    if (!single) { mf.vi = r->vi_f; mf.bary = r->bary_f; }
+    mf.S = S2; mf.dirbias = b.dirbias; mf.out = b.out_f;
+    if (!single) { mf.vi = b.vi_f; mf.bary = b.bary_f; }
     else p.ebins_f = r->ebins_c;  // k_composite integrates over the coarse bins
-    mf.tile_ctr = r->n_active + 2;
+    mf.tile_ctr = b.n_active + 2;
     k_fine<<<grid_f, MLP_THREADS, MLP_SMEM_BYTES, s>>>(mf);
     TN_EV(5);
     k_composite<<<gridR, SAMPLE_WARPS * 32, smem_c, s>>>(p);
@@ -992,7 +1047,7 @@ static int render_impl(tn_tracer *h, const tn_render_config *cfg, const float *d
 #undef TN_EV
     h->launches += 5;
     TN_CUDA(cudaGetLastError());
-    if (tf != nullptr) {
+    if (tf != nullptr && tf->saved == nullptr) {
         r->train_valid = true;
         r->t_det = det;
         r->t_R = R; r->t_M = M; r->t_Sc = Sc; r->t_Sf = Sf; r->t_S2 = S2;
@@ -1032,24 +1087,21 @@ extern "C" int tn_render(tn_tracer *h, const tn_render_config *cfg, const float 
 extern "C" int tn_render_train_forward(tn_tracer *h, const tn_render_config *cfg, const float *d_origins, const float *d_directions, uint32_t R,
                                        const float *d_jitter_coarse, const float *d_jitter_fine, float *d_rgb, float *d_acc, float *d_depth,
                                        uint8_t *d_mask, void *stream) {
-    TrainFwd tf{d_jitter_coarse, d_jitter_fine};
+    TrainFwd tf{d_jitter_coarse, d_jitter_fine, nullptr};
     return render_impl(h, cfg, d_origins, d_directions, R, d_rgb, d_acc, d_depth, d_mask, &tf, stream);
 }
 
-// backward of the LAST tn_render_train_forward: d_grad_rgb f32[R,3] (dL/d rgb), d_grad_acc f32[R] or NULL (dL/d accumulation) ->
-// d_grad_field f32[64,V] and the twelve MLP parameter gradients (same order / layouts as tn_render_set_weights); every output element
-// is written.  The coarse pass carries no gradient (PDFSampler detaches its bins).  No [samples,128] tensor touches HBM.
-extern "C" int tn_render_train_backward(tn_tracer *h, const float *d_grad_rgb, const float *d_grad_acc, int use_gradient_scaling,
-                                        float *d_grad_field, float *const *d_grad_params12, void *stream) {
-    if (!h || !d_grad_rgb || !d_grad_field || !d_grad_params12) return fail(TN_ERR_ARG, "null argument");
+// backward of a training forward of R rays x S2 fine samples whose buffers are `b`, in the mode (det) and with the background it ran
+// with: d_grad_rgb f32[R,3] (dL/d rgb), d_grad_acc f32[R] or NULL (dL/d accumulation) -> d_grad_field f32[64,V] and the twelve MLP
+// parameter gradients (same order / layouts as tn_render_set_weights); every output element is written.  Reads `b` and the field /
+// weights; writes only the tracer's gradient scratch.  The coarse pass carries no gradient (PDFSampler detaches its bins).  No
+// [samples,128] tensor touches HBM.
+static int train_backward_impl(tn_tracer *h, const TrainBufs &b, uint32_t R, uint32_t S2, bool det, const float *bg, const float *d_grad_rgb,
+                               const float *d_grad_acc, int use_gradient_scaling, float *d_grad_field, float *const *d_grad_params12, cudaStream_t s) {
     RenderState *r = h->render;
-    if (!r || !r->train_valid) return fail(TN_ERR_STATE, "tn_render_train_backward: no training forward to continue from");
-    DeviceGuard g(h->device);
-    cudaStream_t s = (cudaStream_t)stream;
     int sms = 132;
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, h->device);
-    const uint32_t R = r->t_R, S2 = r->t_S2, V = r->V;
-    const bool det = r->t_det;
+    const uint32_t V = r->V;
     if (det) {
         const int rc = ensure_det_ws(r, R, S2);
         if (rc) return rc;
@@ -1058,12 +1110,13 @@ extern "C" int tn_render_train_backward(tn_tracer *h, const float *d_grad_rgb, c
     if (!det) {  // (deterministic mode writes every element of these)
         TN_CUDA(cudaMemsetAsync(r->gshadow, 0, sizeof(float) * 64 * (size_t)V, s));
         TN_CUDA(cudaMemsetAsync(r->g_dirbias, 0, 512 * (size_t)R, s));
-        TN_CUDA(cudaMemsetAsync(r->n_active + 3, 0, 4, s));  // tile counter of the backward kernel (word 3 of the 16-byte block)
+        // tile counter of the backward kernel: word 3 of the tracer's own 16-byte block (scratch even when `b` is a saved state)
+        TN_CUDA(cudaMemsetAsync(r->n_active + 3, 0, 4, s));
     }
     CompositeBwdParams cb{};
-    cb.S2 = S2; cb.use_gradient_scaling = use_gradient_scaling ? 1u : 0u; cb.n_active = r->n_active; cb.ray_list = r->ray_list;
-    cb.ebins_f = r->ebins_f; cb.sbins_f = r->sbins_f; cb.out_f = r->out_f; cb.grad_rgb = d_grad_rgb; cb.grad_acc = d_grad_acc;
-    cb.bg0 = r->t_bg[0]; cb.bg1 = r->t_bg[1]; cb.bg2 = r->t_bg[2]; cb.dout = r->dout; cb.sums = det ? (float *)r->det_sums : r->gw + GW_SUMS;
+    cb.S2 = S2; cb.use_gradient_scaling = use_gradient_scaling ? 1u : 0u; cb.n_active = b.n_active; cb.ray_list = b.ray_list;
+    cb.ebins_f = b.ebins_f; cb.sbins_f = b.sbins_f; cb.out_f = b.out_f; cb.grad_rgb = d_grad_rgb; cb.grad_acc = d_grad_acc;
+    cb.bg0 = bg[0]; cb.bg1 = bg[1]; cb.bg2 = bg[2]; cb.dout = r->dout; cb.sums = det ? (float *)r->det_sums : r->gw + GW_SUMS;
     const size_t smem_cb = SAMPLE_WARPS * sizeof(float) * 4 * ((size_t)S2 + 2);
     auto k_cbwd = det ? k_composite_bwd<true> : k_composite_bwd<false>;
     TN_CUDA(cudaFuncSetAttribute(k_cbwd, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_cb));
@@ -1072,8 +1125,8 @@ extern "C" int tn_render_train_backward(tn_tracer *h, const float *d_grad_rgb, c
     k_cbwd<<<gridR, SAMPLE_WARPS * 32, smem_cb, s>>>(cb);
     if (r->profile) cudaEventRecord(r->evb[1], s);
     MlpBwdParams bp{};
-    bp.n_active = r->n_active; bp.S = S2; bp.vi = r->vi_f; bp.bary = r->bary_f; bp.fshadow = r->fshadow; bp.wimg = r->wimg_bwd;
-    bp.bias = r->bias; bp.head = r->head; bp.dirbias = r->dirbias; bp.dout = r->dout; bp.gshadow = r->gshadow;
+    bp.n_active = b.n_active; bp.S = S2; bp.vi = b.vi_f; bp.bary = b.bary_f; bp.fshadow = r->fshadow; bp.wimg = r->wimg_bwd;
+    bp.bias = r->bias; bp.head = r->head; bp.dirbias = b.dirbias; bp.dout = r->dout; bp.gshadow = r->gshadow;
     bp.gw = r->gw; bp.g_dirbias = r->g_dirbias; bp.tile_ctr = r->n_active + 3;
     const uint64_t tiles = ((uint64_t)R * S2 + BWD_TILE - 1) / BWD_TILE;
     if (!det) {
@@ -1081,7 +1134,7 @@ extern "C" int tn_render_train_backward(tn_tracer *h, const float *d_grad_rgb, c
         const uint32_t grid = r->bwd_grid ? r->bwd_grid : (uint32_t)std::min<uint64_t>(tiles, (uint64_t)sms);
         k_mlp_bwd<false><<<grid, BWD_THREADS, BWD_SMEM_BYTES, s>>>(bp);
         if (r->profile) cudaEventRecord(r->evb[2], s);
-        k_dirbias_grads<false><<<(R + DBG_SLOTS - 1) / DBG_SLOTS, 256, 0, s>>>(r->n_active, r->g_dirbias, r->enc, r->gw, nullptr);
+        k_dirbias_grads<false><<<(R + DBG_SLOTS - 1) / DBG_SLOTS, 256, 0, s>>>(b.n_active, r->g_dirbias, b.enc, r->gw, nullptr);
     } else {
         // the same stages with every reduction in a fixed order (header of tn_mlp_bwd.cuh); the grid only decides which CTA runs
         // which partition, never what is summed in which order
@@ -1092,11 +1145,11 @@ extern "C" int tn_render_train_backward(tn_tracer *h, const float *d_grad_rgb, c
         const uint32_t grid = r->bwd_grid ? r->bwd_grid : std::min<uint32_t>(BWD_PARTS, (uint32_t)sms);
         k_mlp_bwd<true><<<grid, BWD_THREADS, BWD_DET_SMEM_BYTES, s>>>(dp);
         if (r->profile) cudaEventRecord(r->evb[2], s);
-        k_det_reduce_parts<<<(BWD_PART_STRIDE + 255) / 256, 256, 0, s>>>(r->n_active, S2, r->det_part, r->gw);
-        k_det_sum_slots<<<1, 256, 0, s>>>(r->n_active, r->det_sums, r->gw + GW_SUMS);
-        k_det_dirbias<<<R, 128, 0, s>>>(r->n_active, S2, r->det_gdb, r->g_dirbias);
-        k_dirbias_grads<true><<<(R + DBG_SLOTS - 1) / DBG_SLOTS, 256, 0, s>>>(r->n_active, r->g_dirbias, r->enc, r->gw, r->det_dbg);
-        k_det_reduce_dbg<<<(DBG_PART + 255) / 256, 256, 0, s>>>(r->n_active, r->det_dbg, r->gw);
+        k_det_reduce_parts<<<(BWD_PART_STRIDE + 255) / 256, 256, 0, s>>>(b.n_active, S2, r->det_part, r->gw);
+        k_det_sum_slots<<<1, 256, 0, s>>>(b.n_active, r->det_sums, r->gw + GW_SUMS);
+        k_det_dirbias<<<R, 128, 0, s>>>(b.n_active, S2, r->det_gdb, r->g_dirbias);
+        k_dirbias_grads<true><<<(R + DBG_SLOTS - 1) / DBG_SLOTS, 256, 0, s>>>(b.n_active, r->g_dirbias, b.enc, r->gw, r->det_dbg);
+        k_det_reduce_dbg<<<(DBG_PART + 255) / 256, 256, 0, s>>>(b.n_active, r->det_dbg, r->gw);
         // field gradient: stable sort of (vertex, row * 4 + k) by vertex, then per-vertex sums in row order
         const uint32_t n = (uint32_t)(4 * (uint64_t)R * S2);
         const int end_bit = 32 - __builtin_clz(V | 1u);  // keys are <= V
@@ -1105,9 +1158,9 @@ extern "C" int tn_render_train_backward(tn_tracer *h, const float *d_grad_rgb, c
         TN_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, bytes, k0, k1, v0, v1, (int)n, 0, end_bit, s));
         const int rc = ensure_cub_tmp(r, bytes);
         if (rc) return rc;
-        k_det_field_keys<<<(n + 255) / 256, 256, 0, s>>>(r->n_active, S2, n, V, (const uint4 *)r->vi_f, k0, v0);
+        k_det_field_keys<<<(n + 255) / 256, 256, 0, s>>>(b.n_active, S2, n, V, b.vi_f, k0, v0);
         TN_CUDA(cub::DeviceRadixSort::SortPairs(r->cub_tmp, bytes, k0, k1, v0, v1, (int)n, 0, end_bit, s));
-        k_det_field_grad<<<(uint32_t)(((uint64_t)V * 32 + 255) / 256), 256, 0, s>>>(V, n, k1, v1, r->bary_f, r->det_dx, r->gshadow);
+        k_det_field_grad<<<(uint32_t)(((uint64_t)V * 32 + 255) / 256), 256, 0, s>>>(V, n, k1, v1, b.bary_f, r->det_dx, r->gshadow);
         h->launches += 9;
     }
     GradOut go{};
@@ -1121,6 +1174,81 @@ extern "C" int tn_render_train_backward(tn_tracer *h, const float *d_grad_rgb, c
     h->launches += 5;
     TN_CUDA(cudaGetLastError());
     return TN_OK;
+}
+
+// backward of the LAST tn_render_train_forward
+extern "C" int tn_render_train_backward(tn_tracer *h, const float *d_grad_rgb, const float *d_grad_acc, int use_gradient_scaling,
+                                        float *d_grad_field, float *const *d_grad_params12, void *stream) {
+    if (!h || !d_grad_rgb || !d_grad_field || !d_grad_params12) return fail(TN_ERR_ARG, "null argument");
+    RenderState *r = h->render;
+    if (!r || !r->train_valid) return fail(TN_ERR_STATE, "tn_render_train_backward: no training forward to continue from");
+    DeviceGuard g(h->device);
+    return train_backward_impl(h, own_bufs(r), r->t_R, r->t_S2, r->t_det, r->t_bg, d_grad_rgb, d_grad_acc, use_gradient_scaling, d_grad_field,
+                               d_grad_params12, (cudaStream_t)stream);
+}
+
+// ---- the training pair with per-call saved state: everything the backward reads that a later call could overwrite goes to the
+// caller's blob (header + TrainBufs, saved_layout), so any number of forwards can be in flight and each backward continues from its
+// own.  The gradient scratch (dout, accumulators, deterministic-mode buffers) stays in the tracer: it is dead once a backward returns.
+static int saved_shape(const tn_render_config *cfg, uint32_t R, uint32_t *S2) {
+    if (!cfg) return fail(TN_ERR_ARG, "null argument");
+    if (R == 0) return fail(TN_ERR_ARG, "tn_render_train_forward_saved: no rays");
+    if (cfg->num_fine_samples == 0) return fail(TN_ERR_ARG, "tn_render_train_forward: the fused training step needs num_fine_samples > 0");
+    *S2 = cfg->num_samples + cfg->num_fine_samples + 1;
+    return TN_OK;
+}
+
+extern "C" int tn_render_train_saved_bytes(tn_tracer *h, const tn_render_config *cfg, uint32_t R, size_t *bytes) {
+    if (!h || !bytes) return fail(TN_ERR_ARG, "null argument");
+    uint32_t S2 = 0;
+    const int rc = saved_shape(cfg, R, &S2);
+    if (rc) return rc;
+    *bytes = saved_layout(R, S2, nullptr, nullptr);
+    return TN_OK;
+}
+
+extern "C" int tn_render_train_forward_saved(tn_tracer *h, const tn_render_config *cfg, const float *d_origins, const float *d_directions,
+                                             uint32_t R, const float *d_jitter_coarse, const float *d_jitter_fine, float *d_rgb, float *d_acc,
+                                             float *d_depth, uint8_t *d_mask, void *d_saved, size_t saved_bytes, void *stream) {
+    if (!h || !d_saved) return fail(TN_ERR_ARG, "null argument");
+    uint32_t S2 = 0;
+    int rc = saved_shape(cfg, R, &S2);
+    if (rc) return rc;
+    if ((uintptr_t)d_saved % SAVED_ALIGN) return fail(TN_ERR_ARG, "tn_render_train_forward_saved: d_saved must be 256-byte aligned");
+    TrainBufs b{};
+    if (saved_bytes < saved_layout(R, S2, (uint8_t *)d_saved, &b))
+        return fail(TN_ERR_ARG, "tn_render_train_forward_saved: saved_bytes is smaller than tn_render_train_saved_bytes");
+    TrainFwd tf{d_jitter_coarse, d_jitter_fine, &b};
+    rc = render_impl(h, cfg, d_origins, d_directions, R, d_rgb, d_acc, d_depth, d_mask, &tf, stream);
+    if (rc) return rc;
+    RenderState *r = h->render;
+    const SavedHeader hd{SAVED_MAGIC, R, cfg->max_ray_triangles, cfg->num_samples, cfg->num_fine_samples, S2, r->det ? 1u : 0u, 0,
+                         {cfg->background[0], cfg->background[1], cfg->background[2]}, 0, r->gen};
+    DeviceGuard g(h->device);
+    // pageable source: staged before the call returns, so `hd` may go out of scope
+    TN_CUDA(cudaMemcpyAsync(d_saved, &hd, sizeof(hd), cudaMemcpyHostToDevice, (cudaStream_t)stream));
+    return TN_OK;
+}
+
+extern "C" int tn_render_train_backward_saved(tn_tracer *h, const void *d_saved, const float *d_grad_rgb, const float *d_grad_acc,
+                                              int use_gradient_scaling, float *d_grad_field, float *const *d_grad_params12, void *stream) {
+    if (!h || !d_saved || !d_grad_rgb || !d_grad_field || !d_grad_params12) return fail(TN_ERR_ARG, "null argument");
+    RenderState *r = h->render;
+    if (!r || !r->n_active) return fail(TN_ERR_STATE, "tn_render_train_backward_saved: no training forward on this tracer");
+    DeviceGuard g(h->device);
+    cudaStream_t s = (cudaStream_t)stream;
+    // the launch shapes depend on the call's R and S2: read the header back (waits until the stream has reached this backward)
+    SavedHeader hd{};
+    TN_CUDA(cudaMemcpyAsync(&hd, d_saved, sizeof(hd), cudaMemcpyDeviceToHost, s));
+    TN_CUDA(cudaStreamSynchronize(s));
+    if (hd.magic != SAVED_MAGIC) return fail(TN_ERR_STATE, "tn_render_train_backward_saved: d_saved holds no training forward");
+    if (hd.gen != r->gen)
+        return fail(TN_ERR_STATE, "tn_render_train_backward_saved: the field or the weights changed (tn_render_set_field / "
+                                  "tn_render_set_weights) since the forward, or the forward ran on another tracer");
+    TrainBufs b{};
+    saved_layout(hd.R, hd.S2, (uint8_t *)d_saved, &b);
+    return train_backward_impl(h, b, hd.R, hd.S2, hd.det != 0, hd.bg, d_grad_rgb, d_grad_acc, use_gradient_scaling, d_grad_field,
+                               d_grad_params12, s);
 }
 
 // deterministic mode of the fused training step (see the header): applies from the next tn_render_train_forward on

@@ -50,6 +50,15 @@ def _config(settings: RenderSettings) -> "ext._Cfg":
                     float(settings.far_plane), (C.c_float * 3)(*settings.background))
 
 
+@dataclass
+class TrainState:
+    """what one FusedRenderer.train_forward_saved call keeps for its backward: the saved-state blob (device memory from torch's
+    allocator, freed with this object whether or not the backward ever runs) and the call's ray count"""
+
+    blob: torch.Tensor
+    R: int
+
+
 class FusedRenderer:
     def __init__(self, tracer: "ext.TetrahedraTracer"):
         self.tracer = tracer
@@ -96,12 +105,8 @@ class FusedRenderer:
         return out
 
     # ---- fused training step ------------------------------------------------------------------------------------------------------
-    def train_forward(self, origins: torch.Tensor, directions: torch.Tensor, settings: RenderSettings, jitter_coarse: Optional[torch.Tensor] = None,
-                      jitter_fine: Optional[torch.Tensor] = None):
-        """training-mode forward (stratified bins from the given uniform draws f32[R,S_c+1] / f32[R,S_f+1]; None = eval bins; RGB renderer
-        without clamp).  Keeps the per-sample buffers the backward continues from.  Runs in deterministic mode (bitwise reproducible
-        outputs and gradients, see tn_render_set_deterministic) when `torch.are_deterministic_algorithms_enabled()` or
-        TETRANERF_B200_DETERMINISTIC=1; the backward continues in the mode of its forward."""
+    def _train_args(self, origins, directions, settings, jitter_coarse, jitter_fine):
+        """checks the inputs of a training forward, allocates its outputs and sets the mode of the call -> (R, outputs, C arguments)"""
         tr = self.tracer
         tr._check_float_dim3(origins, "ray_origins")
         tr._check_float_dim3(directions, "ray_directions")
@@ -112,26 +117,63 @@ class FusedRenderer:
                 raise RuntimeError(f"{n} must be a contiguous float32 [{R}, {w}] tensor on the tracer's device")
         out = {"rgb": torch.empty((R, 3), dtype=torch.float32, device=dev), "accumulation": torch.empty((R, 1), dtype=torch.float32, device=dev),
                "depth": torch.empty((R, 1), dtype=torch.float32, device=dev), "ray_mask": torch.empty((R,), dtype=torch.bool, device=dev)}
-        cfg = _config(settings)
         ext._check(_lib.tn_render_set_deterministic(tr.handle, int(ext.deterministic_enabled())))
-        ext._check(_lib.tn_render_train_forward(tr.handle, C.byref(cfg), origins.data_ptr(), directions.data_ptr(), R,
-                                                jitter_coarse.data_ptr() if jitter_coarse is not None else None,
-                                                jitter_fine.data_ptr() if jitter_fine is not None else None, out["rgb"].data_ptr(),
-                                                out["accumulation"].data_ptr(), out["depth"].data_ptr(), out["ray_mask"].data_ptr(), self._stream()))
+        args = [tr.handle, C.byref(_config(settings)), origins.data_ptr(), directions.data_ptr(), R,
+                jitter_coarse.data_ptr() if jitter_coarse is not None else None, jitter_fine.data_ptr() if jitter_fine is not None else None,
+                out["rgb"].data_ptr(), out["accumulation"].data_ptr(), out["depth"].data_ptr(), out["ray_mask"].data_ptr()]
+        return R, out, args
+
+    def _train_backward(self, entry, lead, grad_rgb, grad_acc, num_vertices, use_gradient_scaling):
+        """runs a training backward, entry(*lead, grads in, gradients out, stream) -> (grad_field, {name: gradient})"""
+        grad_rgb = grad_rgb.contiguous()
+        if grad_acc is not None:
+            grad_acc = grad_acc.contiguous()
+        gfield = torch.empty((64, num_vertices), dtype=torch.float32, device=self.device)
+        gps = [torch.empty(sh, dtype=torch.float32, device=self.device) for sh in _SHAPES]
+        arr = (_vp * 12)(*[t.data_ptr() for t in gps])
+        ext._check(entry(*lead, grad_rgb.data_ptr(), grad_acc.data_ptr() if grad_acc is not None else None, int(use_gradient_scaling),
+                         gfield.data_ptr(), arr, self._stream()))
+        return gfield, dict(zip(PARAM_ORDER, gps))
+
+    def train_forward(self, origins: torch.Tensor, directions: torch.Tensor, settings: RenderSettings, jitter_coarse: Optional[torch.Tensor] = None,
+                      jitter_fine: Optional[torch.Tensor] = None):
+        """training-mode forward (stratified bins from the given uniform draws f32[R,S_c+1] / f32[R,S_f+1]; None = eval bins; RGB renderer
+        without clamp).  Keeps the per-sample buffers the backward continues from in the tracer, until the next render call (see
+        train_forward_saved for a forward with its own saved state).  Runs in deterministic mode (bitwise reproducible outputs and
+        gradients, see tn_render_set_deterministic) when `torch.are_deterministic_algorithms_enabled()` or TETRANERF_B200_DETERMINISTIC=1;
+        the backward continues in the mode of its forward."""
+        _, out, args = self._train_args(origins, directions, settings, jitter_coarse, jitter_fine)
+        ext._check(_lib.tn_render_train_forward(*args, self._stream()))
         return out
 
     def train_backward(self, grad_rgb: torch.Tensor, grad_acc: Optional[torch.Tensor], num_vertices: int, use_gradient_scaling: bool = False):
         """backward of the last train_forward: -> (grad_field f32[64,V], {state-dict name: gradient} for the twelve MLP parameters)"""
-        dev = self.device
-        grad_rgb = grad_rgb.contiguous()
-        if grad_acc is not None:
-            grad_acc = grad_acc.contiguous()
-        gfield = torch.empty((64, num_vertices), dtype=torch.float32, device=dev)
-        gps = [torch.empty(sh, dtype=torch.float32, device=dev) for sh in _SHAPES]
-        arr = (_vp * 12)(*[t.data_ptr() for t in gps])
-        ext._check(_lib.tn_render_train_backward(self.tracer.handle, grad_rgb.data_ptr(), grad_acc.data_ptr() if grad_acc is not None else None,
-                                                 int(use_gradient_scaling), gfield.data_ptr(), arr, self._stream()))
-        return gfield, dict(zip(PARAM_ORDER, gps))
+        return self._train_backward(_lib.tn_render_train_backward, [self.tracer.handle], grad_rgb, grad_acc, num_vertices, use_gradient_scaling)
+
+    def train_saved_bytes(self, R: int, settings: RenderSettings) -> int:
+        """device bytes of the saved state of one training forward of R rays"""
+        n = C.c_size_t()
+        ext._check(_lib.tn_render_train_saved_bytes(self.tracer.handle, C.byref(_config(settings)), int(R), C.byref(n)))
+        return n.value
+
+    def train_forward_saved(self, origins: torch.Tensor, directions: torch.Tensor, settings: RenderSettings,
+                            jitter_coarse: Optional[torch.Tensor] = None, jitter_fine: Optional[torch.Tensor] = None):
+        """train_forward whose backward state goes to a blob of its own instead of the tracer -> (outputs, TrainState).  Any number of
+        these can be in flight; train_backward_saved(state, ...) continues from the one it is given."""
+        R, out, args = self._train_args(origins, directions, settings, jitter_coarse, jitter_fine)
+        blob = torch.empty((self.train_saved_bytes(R, settings),), dtype=torch.uint8, device=self.device)
+        ext._check(_lib.tn_render_train_forward_saved(*args, blob.data_ptr(), blob.numel(), self._stream()))
+        return out, TrainState(blob, R)
+
+    def train_backward_saved(self, state: "TrainState", grad_rgb: torch.Tensor, grad_acc: Optional[torch.Tensor], num_vertices: int,
+                             use_gradient_scaling: bool = False):
+        """backward of the train_forward_saved call that returned `state`; outputs as train_backward.  Raises RuntimeError if
+        set_field / set_weights ran since that forward.  Waits until the stream has reached it (it reads the call's shape back)."""
+        if tuple(grad_rgb.shape) != (state.R, 3) or (grad_acc is not None and grad_acc.numel() != state.R):
+            raise RuntimeError(f"the forward rendered {state.R} rays: grad_rgb must be [{state.R}, 3] and grad_acc [{state.R}], got "
+                               f"{tuple(grad_rgb.shape)} and {None if grad_acc is None else tuple(grad_acc.shape)}")
+        return self._train_backward(_lib.tn_render_train_backward_saved, [self.tracer.handle, state.blob.data_ptr()], grad_rgb, grad_acc,
+                                    num_vertices, use_gradient_scaling)
 
     def set_mlp_precision(self, prec: int) -> None:
         """operand precision of the inference MLP: 2 = f16w2 (default: fp16 activations x fp16 hi/lo weights, ~2.6e-5 absolute on
@@ -166,20 +208,25 @@ class FusedRenderer:
 
 
 class FusedTrainRender(torch.autograd.Function):
-    """TetrahedraNerf.get_outputs in training mode as ONE differentiable op: forward = tn_render_train_forward, backward =
-    tn_render_train_backward (gradients for `tetrahedra_field` and the twelve MLP parameters; none for rays or jitter).
-    The renderer must already hold the current field / weights (FusedRenderer.set_field / set_weights)."""
+    """TetrahedraNerf.get_outputs in training mode as ONE differentiable op: forward = tn_render_train_forward_saved, backward =
+    tn_render_train_backward_saved (gradients for `tetrahedra_field` and the twelve MLP parameters; none for rays or jitter).
+    The renderer must already hold the current field / weights (FusedRenderer.set_field / set_weights).  Every call keeps its own
+    saved state (~115 MB at 8192 rays x 257 fine samples, freed with the graph), so calls compose like any autograd op: several
+    forwards before one backward, other renders in between, retain_graph.  A backward after an in-place change of the field or a
+    parameter, or after set_field / set_weights on the renderer, raises RuntimeError."""
 
     @staticmethod
     def forward(ctx, fr, settings, use_gradient_scaling, origins, directions, jitter_coarse, jitter_fine, field, *params):
-        out = fr.train_forward(origins, directions, settings, jitter_coarse, jitter_fine)
-        ctx.fr, ctx.nv, ctx.gs = fr, field.shape[1], bool(use_gradient_scaling)
+        out, state = fr.train_forward_saved(origins, directions, settings, jitter_coarse, jitter_fine)
+        ctx.fr, ctx.state, ctx.gs = fr, state, bool(use_gradient_scaling)
+        ctx.save_for_backward(field, *params)  # their version counters reject a backward after an in-place change
         ctx.mark_non_differentiable(out["depth"], out["ray_mask"])
         return out["rgb"], out["accumulation"], out["depth"], out["ray_mask"]
 
     @staticmethod
     def backward(ctx, g_rgb, g_acc, _g_depth, _g_mask):
+        field = ctx.saved_tensors[0]
         if g_rgb is None:
-            g_rgb = torch.zeros((g_acc.shape[0], 3), dtype=torch.float32, device=g_acc.device)
-        gfield, gp = ctx.fr.train_backward(g_rgb, g_acc.reshape(-1) if g_acc is not None else None, ctx.nv, ctx.gs)
+            g_rgb = torch.zeros((ctx.state.R, 3), dtype=torch.float32, device=field.device)
+        gfield, gp = ctx.fr.train_backward_saved(ctx.state, g_rgb, g_acc.reshape(-1) if g_acc is not None else None, field.shape[1], ctx.gs)
         return (None, None, None, None, None, None, None, gfield) + tuple(gp[n] for n in PARAM_ORDER)
