@@ -255,6 +255,7 @@ class RenderConfig:
     field_dim: int = 64
     hidden_size: int = 128
     far_plane: float = 6.0  # nerfstudio ModelConfig.collider_params default {"near_plane": 2.0, "far_plane": 6.0}
+    background: tuple = (1.0, 1.0, 1.0)  # RGBRenderer background colour (model.py:258): "white" = (1, 1, 1), "black" = (0, 0, 0)
 
     @staticmethod
     def tetra_nerf():  # registration.py:48-61
@@ -395,8 +396,10 @@ def pdf_bins(cfg: RenderConfig, spacing_bins, weights, nears, fars, histogram_pa
 
 
 def render(mesh: OracleMesh, field: torch.Tensor, params: Dict[str, torch.Tensor], origins, directions, cfg: RenderConfig,
-           nthreads: int = 0, return_aux: bool = False):
-    """TetrahedraNerf.get_outputs in eval mode, background white (model.py:520-662)."""
+           nthreads: int = 0, return_aux: bool = False, fine_euclid=None):
+    """TetrahedraNerf.get_outputs in eval mode, background cfg.background (model.py:520-662).  fine_euclid f32[R',S2+1] (non-empty
+    rays, in ray order): evaluate the fine pass at THESE bin edges instead of the coarse pass + PDF sampler, as render_train does --
+    so that per-sample values can be compared at an implementation's own sample positions."""
     o = torch.as_tensor(np.asarray(origins), dtype=torch.float32).reshape(-1, 3)
     d = torch.as_tensor(np.asarray(directions), dtype=torch.float32).reshape(-1, 3)
     R = o.shape[0]
@@ -406,7 +409,8 @@ def render(mesh: OracleMesh, field: torch.Tensor, params: Dict[str, torch.Tensor
     nears = hd[:, 0, 0][:, None]
     fars = torch.gather(hd[:, :, 1], 1, (num_visited[:, None].long() - 1).clamp_min(0))
     ray_mask = num_visited > 0
-    rgb = torch.ones((R, 3), dtype=torch.float32)
+    bg = torch.tensor(cfg.background, dtype=torch.float32)
+    rgb = bg.expand(R, 3).clone()
     acc = torch.zeros((R, 1), dtype=torch.float32)
     depth = torch.full((R, 1), cfg.far_plane, dtype=torch.float32)
     aux = {"trace": tr}
@@ -425,7 +429,9 @@ def render(mesh: OracleMesh, field: torch.Tensor, params: Dict[str, torch.Tensor
             fv = interpolate_values(tc["vertex_indices"], tc["barycentric_coordinates"], fld, nthreads=nthreads)
             return torch.from_numpy(fv), tc
 
-        if cfg.num_fine_samples > 0:
+        if fine_euclid is not None:
+            euclid = torch.as_tensor(fine_euclid, dtype=torch.float32)
+        elif cfg.num_fine_samples > 0:
             fv, tc = field_at(euclid)
             base = mlp_base(params, fv)
             density_coarse = density_head(params, base)
@@ -440,10 +446,10 @@ def render(mesh: OracleMesh, field: torch.Tensor, params: Dict[str, torch.Tensor
         colors = color_head(params, base, enc)
         deltas = (euclid[:, 1:] - euclid[:, :-1])[..., None]
         weights = get_weights(deltas, sigmas)
-        # RGBRenderer (eval: nan_to_num, white background, clamp), AccumulationRenderer, DepthRenderer("median")
+        # RGBRenderer (eval: nan_to_num, background, clamp), AccumulationRenderer, DepthRenderer("median")
         comp = torch.sum(weights * torch.nan_to_num(colors), dim=-2)
         accum = torch.sum(weights, dim=-2)
-        rgb_r = torch.clamp(comp + 1.0 * (1.0 - accum), 0.0, 1.0)
+        rgb_r = torch.clamp(comp + bg * (1.0 - accum), 0.0, 1.0)
         steps = (euclid[:, 1:] + euclid[:, :-1]) / 2
         cumw = torch.cumsum(weights[..., 0], dim=-1)
         split = torch.ones((weights.shape[0], 1)) * 0.5
@@ -496,7 +502,8 @@ def render_train(mesh: OracleMesh, field: torch.Tensor, params: Dict[str, torch.
                  jitter_coarse=None, jitter_fine=None, use_gradient_scaling: bool = False, nthreads: int = 0, fine_euclid=None):
     """TetrahedraNerf.get_outputs in TRAINING mode (model.py:520-662) in differentiable torch-CPU fp32: `field` and the entries of `params`
     may require grad.  jitter_coarse f32[R,S_c+1] / jitter_fine f32[R,S_f+1] are the uniform draws of the two stratified samplers, indexed by
-    RAY (the reference draws them with torch.rand on the non-empty rays).  Training-mode renderer: white background, no nan_to_num / clamp.
+    RAY (the reference draws them with torch.rand on the non-empty rays).  Training-mode renderer: background cfg.background, no nan_to_num /
+    clamp.
     fine_euclid f32[R',S2+1] (non-empty rays, in ray order): use THESE fine-pass bin edges instead of running the coarse pass and the PDF
     sampler -- the bins are detached (non-differentiable) in the reference, so the gradient arithmetic of an implementation can be checked
     at the implementation's own sample positions, which move by ~1e-6 between any two fp32 PDF inversions."""
@@ -546,13 +553,14 @@ def render_train(mesh: OracleMesh, field: torch.Tensor, params: Dict[str, torch.
     weights = get_weights(deltas, sigmas)
     comp = torch.sum(weights * colors, dim=-2)
     accum = torch.sum(weights, dim=-2)
-    rgb_r = comp + 1.0 * (1.0 - accum)  # RGBRenderer in training: no nan_to_num, no clamp
+    bg = torch.tensor(cfg.background, dtype=comp.dtype)
+    rgb_r = comp + bg * (1.0 - accum)  # RGBRenderer in training: no nan_to_num, no clamp
     steps = (euclid[:, 1:] + euclid[:, :-1]) / 2
     cumw = torch.cumsum(weights[..., 0].detach(), dim=-1)
     mi = torch.clamp(torch.searchsorted(cumw, torch.ones((weights.shape[0], 1)) * 0.5, side="left"), 0, steps.shape[-1] - 1)
     depth_r = torch.gather(steps, dim=-1, index=mi)
     idx = torch.nonzero(ray_mask).flatten()
-    rgb = torch.ones((R, 3), dtype=rgb_r.dtype).index_copy(0, idx, rgb_r)  # (dtype follows the inputs: tests also run this in float64)
+    rgb = bg.expand(R, 3).clone().index_copy(0, idx, rgb_r)  # (dtype follows the inputs: tests also run this in float64)
     acc = torch.zeros((R, 1), dtype=rgb_r.dtype).index_copy(0, idx, accum)
     depth = torch.full((R, 1), cfg.far_plane, dtype=depth_r.dtype).index_copy(0, idx, depth_r)
     return {"rgb": rgb, "accumulation": acc, "depth": depth, "ray_mask": ray_mask,

@@ -22,14 +22,15 @@ def _from_ptr(ptr, shape, dtype):
     return t
 
 
-def setup(V, C, field_kind="normal", prec=3):
+def setup(V, C, field_kind="normal", prec=3, field=None, params=None):
+    """field / params default to syn.random_field(kind=field_kind) and the torch-default network"""
     from tetranerf import cpp
     from tetranerf.b200.render import FusedRenderer
 
     tr = cpp.TetrahedraTracer(DEV)
     tr.load_tetrahedra(torch.from_numpy(V).to(DEV), torch.from_numpy(C).to(DEV))
-    field = syn.random_field(len(V), 64, seed=3, kind=field_kind)
-    params = orc.init_mlp_params(0)
+    field = syn.random_field(len(V), 64, seed=3, kind=field_kind) if field is None else field
+    params = orc.init_mlp_params(0) if params is None else params
     fr = FusedRenderer(tr)
     fr.set_field(torch.from_numpy(field).to(DEV))
     fr.set_weights(params)
@@ -38,7 +39,9 @@ def setup(V, C, field_kind="normal", prec=3):
 
 
 # prec: operand precision of the tensor-core MLP -- 3 = bf16x3 (fp32-level), 2 = f16w2 (fp16 activations x fp16 hi/lo weights, 2 MMAs per
-# product).  BOTH are held to the same bars: the north-star tolerance of 1e-4 absolute per sample and per pixel.
+# product).  On this (torch-default, unit-scale) network BOTH are held to the same bars: 1e-4 absolute per sample and per pixel.  f16w2's
+# per-sample error is relative to the activations (~4.9e-4 sigma, 1.8e-4 colour on a trained-NeRF-like network: tests/test_gpu_opaque.py,
+# DESIGN 4.2); its pixels stay within 1e-4 there too.
 @pytest.mark.parametrize("prec", [3, 2])
 @pytest.mark.parametrize("cfgname", ["tetra_nerf", "tetra_nerf_original", "small_uniform", "small_biased"])
 @pytest.mark.parametrize("field_kind", ["normal", "init"])

@@ -23,13 +23,13 @@ DEV = torch.device("cuda:0")
 GRAD_TOL = 1e-4
 
 
-def _setup(V, C, field):
+def _setup(V, C, field, params=None):
     from tetranerf import cpp
     from tetranerf.b200.render import FusedRenderer
 
     tr = cpp.TetrahedraTracer(DEV)
     tr.load_tetrahedra(torch.from_numpy(V).to(DEV), torch.from_numpy(C).to(DEV))
-    params = orc.init_mlp_params(0)
+    params = orc.init_mlp_params(0) if params is None else params
     fr = FusedRenderer(tr)
     fr.set_field(torch.from_numpy(field).to(DEV))
     fr.set_weights(params)
@@ -70,11 +70,14 @@ def _check(name, got, f32, f64, f64_same_bins, failures):
         failures.append((name, arith, err, noise))
 
 
-def _run(V, C, o, d, st, oc, gs, seed, field_kind="normal", mesh=None):
+def _run(V, C, o, d, st, oc, gs, seed, field_kind="normal", mesh=None, field=None, params=None, details=None):
+    """field / params default to syn.random_field(kind=field_kind) and the torch-default network; the background is st's / oc's.
+    details (a dict), if given, receives the kernel's gradients ("gfield", "gp") and the float64 oracle at the kernel's own fine bins
+    ("gfield_f64", "gp_f64", "out_f64": its forward, with the per-sample aux)."""
     from tetranerf.b200.render import PARAM_ORDER
 
-    field = syn.random_field(len(V), 64, seed=3, kind=field_kind)
-    tr, fr, params = _setup(V, C, field)
+    field = syn.random_field(len(V), 64, seed=3, kind=field_kind) if field is None else field
+    tr, fr, params = _setup(V, C, field, params)
     g = torch.Generator().manual_seed(seed)
     R = len(o)
     jc = torch.rand((R, st.num_samples + 1), generator=g)
@@ -102,7 +105,9 @@ def _run(V, C, o, d, st, oc, gs, seed, field_kind="normal", mesh=None):
     ray_list = _from_ptr(bufs["ray_list"], (n_act,), torch.int32).cpu().long()
     eb = _from_ptr(bufs["ebins_f"], (n_act, S2 + 1), torch.float32).cpu()
     fine = eb[torch.argsort(ray_list)]
-    _, gfsb, gpsb = _oracle_grads(V, C, field, params, o, d, oc, jc, jf, target, gs, mesh, dtype=torch.float64, fine_euclid=fine)
+    out_sb, gfsb, gpsb = _oracle_grads(V, C, field, params, o, d, oc, jc, jf, target, gs, mesh, dtype=torch.float64, fine_euclid=fine)
+    if details is not None:
+        details.update(gfield=gfield, gp=gp, gfield_f64=gfsb, gp_f64=gpsb, out_f64=out_sb)
     failures = []
     _check("tetrahedra_field", gfield, gf32, gf64, gfsb, failures)
     for n in PARAM_ORDER:

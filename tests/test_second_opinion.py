@@ -70,13 +70,29 @@ def test_pdf_bins_merge_and_inversion():
 def test_whole_ray_render_against_definitions(small_mesh):
     """oracle.render (torch fp32, upstream code order) vs per-ray float64 evaluation from the definitions: interpolation by
     explicit weights, MLP in float64, product-form weights, scan-based PDF inversion, sorted() merge, loop median depth."""
+    from tetranerf.b200 import synthetic as syn
+
+    V, _ = small_mesh
+    _whole_ray_render(small_mesh, syn.random_field(len(V), 64, seed=3), orc.init_mlp_params(0), (1.0, 1.0, 1.0))
+
+
+def test_whole_ray_render_with_background_on_surface_scene(small_mesh):
+    """the same on the semi-transparent surface scene (1 - acc spans most of (0, 1)) and an asymmetric background colour, so that
+    a swapped or dropped channel of the background shows"""
+    from tetranerf.b200 import synthetic as syn
+
+    V, _ = small_mesh
+    field, params = syn.surface_scene(V, 10, orc.init_mlp_params(0))
+    _whole_ray_render(small_mesh, field, params, (0.1, 0.6, 0.3))
+
+
+def _whole_ray_render(small_mesh, field, params, background):
     V, C = small_mesh
     from tetranerf.b200 import synthetic as syn
 
-    field = syn.random_field(len(V), 64, seed=3)
-    params = orc.init_mlp_params(0)
     o, d = syn.camera_rays(24, seed=5)
-    cfg = orc.RenderConfig(num_samples=32, num_fine_samples=24, use_biased_sampler=True)
+    o[3] = [5, 5, 5]; d[3] = [1, 0, 0]  # empty ray: the background
+    cfg = orc.RenderConfig(num_samples=32, num_fine_samples=24, use_biased_sampler=True, background=background)
     mesh = orc.OracleMesh(V, C)
     ref = orc.render(mesh, torch.from_numpy(field), params, o, d, cfg, return_aux=True)
     tr = ref["aux"]["trace"]
@@ -98,6 +114,7 @@ def test_whole_ray_render_against_definitions(small_mesh):
 
     worst = 0.0
     rows = [r for r in range(len(o)) if tr["num_visited_cells"][r] > 0]
+    assert ref["rgb"][3].tolist() == list(np.float32(background)) and not bool(ref["ray_mask"][3])
     for r in rows:
         n = int(tr["num_visited_cells"][r])
         seg = [(float(tr["hit_distances"][r, k, 0]), float(tr["hit_distances"][r, k, 1])) for k in range(n)]
@@ -111,7 +128,7 @@ def test_whole_ray_render_against_definitions(small_mesh):
         eu2 = [b * far + (1 - b) * near for b in sb2]
         mids2 = [(eu2[j] + eu2[j + 1]) / 2 for j in range(len(eu2) - 1)]
         sig, col = so2.mlp_forward(params, features_at(r, mids2), enc)
-        rgb, acc, dep = so2.composite(eu2, sig, col)
+        rgb, acc, dep = so2.composite(eu2, sig, col, background=background)
         worst = max(worst, float(np.abs(np.array(rgb) - ref["rgb"][r].numpy()).max()), abs(acc - float(ref["accumulation"][r])))
     print("whole-ray render: fp32 restatement vs float64 definitions, max |rgb/acc| diff", worst)
     assert worst < 5e-5

@@ -176,8 +176,9 @@ class FusedRenderer:
                                     num_vertices, use_gradient_scaling)
 
     def set_mlp_precision(self, prec: int) -> None:
-        """operand precision of the inference MLP: 2 = f16w2 (default: fp16 activations x fp16 hi/lo weights, ~2.6e-5 absolute on
-        unit-scale density / colour, inside the 1e-4 per-sample bar), 3 = bf16x3 (fp32-level, ~5e-7).  Training always runs bf16x3."""
+        """operand precision of the inference MLP: 2 = f16w2 (default: fp16 activations x fp16 hi/lo weights; per-sample error relative
+        to the activations -- ~2.6e-5 absolute on unit-scale density / colour, ~4.9e-4 relative on large densities -- pixels within
+        1e-4), 3 = bf16x3 (fp32-level, ~5e-7).  Training always runs bf16x3."""
         ext._check(_lib.tn_render_set_mlp_precision(self.tracer.handle, int(prec)))
 
     def set_backward_grid(self, ctas: int) -> None:

@@ -1,6 +1,7 @@
 """VERDICT r1 item 4: is there a cheaper operand split than bf16x3 (3 MMAs per product) that holds the 1e-4 per-sample bar?
 CPU emulation of the fused MLP's arithmetic (exact products of the split operands, fp32 accumulation) on the bench's field /
-weights: per-sample density and colour against float64.  Run: python tools/split_accuracy.py"""
+weights: per-sample density and colour against float64; then the same on the opaque surface network of synthetic.surface_scene, where
+f16w2's error turns out relative to the activations (density ~4e-4 |sigma|).  Run: python tools/split_accuracy.py"""
 import os, sys
 R = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path[:0] = [R, R + "/tetra-nerf_b200"]
@@ -41,9 +42,8 @@ def linear(a, w, bias, scheme):
     return acc.double() + bias
 
 
-def mlp(scheme):
-    p = params
-    h = x0
+def mlp(scheme, p=params, x=x0):
+    h = x
     for l in range(3):
         h = torch.relu(linear(h, p[f"mlp_base.layers.{l}.weight"], p[f"mlp_base.layers.{l}.bias"], scheme))
     # the heads are fp32 FMAs in the kernel, the direction part of mlp_head is a per-ray fp32 bias: only the 128 hidden inputs of
@@ -68,18 +68,32 @@ SCHEMES = {
 }
 
 
-def errors():
-    """{scheme: (max |sigma err|, max |colour err|)} against float64"""
-    ref_s, ref_c = mlp(None)
+def surface_inputs(sharpness):
+    """(params, interpolated features) of synthetic.surface_scene(sharpness) on 4000 random points, in float64"""
+    pts = np.random.default_rng(1).random((4000, 3))
+    fld, p = syn.surface_scene(pts, sharpness, orc.init_mlp_params(0))
+    f = torch.from_numpy(fld).double().T.contiguous()
+    return {k: v.double() for k, v in p.items()}, (f[idx] * b[..., None]).sum(1)
+
+
+def errors(p=params, x=x0):
+    """{scheme: (max |sigma err|, max |colour err|, 99.9th percentiles, max |sigma err| / sigma where sigma > 1)} against float64"""
+    ref_s, ref_c = mlp(None, p, x)
     out = {}
+    big = ref_s > 1.0
     for name, sc in SCHEMES.items():
-        s, c = mlp(sc)
+        s, c = mlp(sc, p, x)
         out[name] = ((s - ref_s).abs().max().item(), (c - ref_c).abs().max().item(),
-                     (s - ref_s).abs().flatten().quantile(0.999).item(), (c - ref_c).abs().flatten().quantile(0.999).item())
+                     (s - ref_s).abs().flatten().quantile(0.999).item(), (c - ref_c).abs().flatten().quantile(0.999).item(),
+                     ((s - ref_s).abs()[big] / ref_s[big]).max().item() if bool(big.any()) else 0.0)
     return out
 
 
 if __name__ == "__main__":
     print(f"{N} samples; max / 99.9th-percentile absolute error against float64 (bar: 1e-4 per sample)")
-    for name, (es, ec, qs, qc) in errors().items():
+    for name, (es, ec, qs, qc, _) in errors().items():
         print(f"{name:58s} sigma {es:.2e} / {qs:.2e}   colour {ec:.2e} / {qc:.2e}")
+    for k in (10, 100, 1000):
+        print(f"surface network, sharpness {k}: max |sigma err|, relative where sigma > 1, max |colour err|")
+        for name, (es, ec, _, _, rel) in errors(*surface_inputs(k)).items():
+            print(f"  {name:56s} sigma {es:.2e} (relative {rel:.2e})   colour {ec:.2e}")
