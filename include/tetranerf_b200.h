@@ -163,6 +163,25 @@ int tn_render_train_backward_saved(tn_tracer *h, const void *d_saved, const floa
  * bit; gradients differ from it by rounding (another summation order).  Costs extra device memory: ~0.9 GB at 8192 rays x 257 fine
  * samples (the [samples,64] feature gradient, the sort, partition partials).  The eval render (tn_render) is unaffected. */
 int tn_render_set_deterministic(tn_tracer *h, int enable);
+/* ---- surface extraction: the density iso-surface sigma = level of the field as a triangle mesh, by marching tetrahedra on the loaded
+ * mesh (DESIGN.md §4.6).  sigma is the density the renderer uses (density head of mlp_base, no GradientScaler), always evaluated in
+ * bf16x3.  A vertex is inside when sigma(F[:, v]) >= level; every mesh edge (a, b), a < b, with one end inside and one outside gives one
+ * output vertex, placed on the edge by two rounds of 64 density evaluations and a linear interpolation in the last 1/4096 bracket (the
+ * crossing nearest a); a tetrahedron with 1 or 3 inside vertices gives one triangle, one with 2 gives two; normals point from inside to
+ * outside.  Vertex normals: normalised sums of the unnormalised face normals; vertex colours: the colour head at the vertex's features
+ * seen along -normal.  Vertices are ordered by edge (a, b), faces by tetrahedron then by the case table; the output is bitwise
+ * reproducible and is not cleaned up (degenerate triangles are kept, so connectivity stays exact).
+ * tn_surface_extract runs the extraction into a workspace the tracer owns and keeps (2.6 KB per crossing edge, 76 bytes per face, 16 per
+ * tetrahedron, 32 per mesh vertex) and returns the
+ * counts: it reads them back, so it waits until the stream has reached it.  It reads the mesh, field and weights only: a pending
+ * training backward (tracer-held or saved) is unaffected.  TN_ERR_STATE without mesh, field or weights; TN_ERR_ARG if level is not
+ * finite and > 0 or the field's vertex count differs from the mesh's.  An empty surface (level above or below every vertex) is not an
+ * error: both counts are 0.
+ * tn_surface_copy copies the last extraction out: d_vertices, d_normals, d_colors f32[N,3], d_faces u32[F,3] (indices into the
+ * vertices), d_face_tet u32[F] (the tetrahedron of each face); a NULL pointer skips that output.  TN_ERR_STATE if no extraction ran, or
+ * tn_render_set_field, tn_render_set_weights or tn_load_tetrahedra ran since it. */
+int tn_surface_extract(tn_tracer *h, float level, uint32_t *n_vertices, uint32_t *n_faces, void *stream);
+int tn_surface_copy(tn_tracer *h, float *d_vertices, float *d_normals, float *d_colors, uint32_t *d_faces, uint32_t *d_face_tet, void *stream);
 /* ---- multi-GPU: final gather of the rendered pixels (north_star; tetranerf/nerfstudio/pipeline.py:53-58 is the reference's only
  * multi-GPU mechanism).  One process per GPU; each rank owns a gathered-pixel buffer f32[world * rays_per_rank, 6]
  * (r, g, b, accumulation, depth, mask) allocated with tn_peer_alloc, whose 64-byte CUDA IPC handle the ranks exchange and map

@@ -57,6 +57,7 @@ int tn_destroy(tn_tracer *h) {
     tn::DeviceGuard g(h->device);
     cudaDeviceSynchronize();
     tn::free_render(h);
+    tn::free_surface(h);
     tn::free_mesh(h);
     cudaFree(h->d_flags);
     cudaFree(h->d_ovf_list);
@@ -82,6 +83,7 @@ int tn_load_tetrahedra(tn_tracer *h, const float *d_xyz, uint32_t V, const uint3
     if (!h) return tn::fail(TN_ERR_ARG, "null tracer");
     if (!d_xyz || !d_cells) return tn::fail(TN_ERR_ARG, "load_tetrahedra: null pointer");
     tn::DeviceGuard g(h->device);
+    h->mesh_gen = tn::next_generation();  // any earlier surface extraction is stale from here on, even if the build fails
     return tn::build_mesh(h, d_xyz, V, d_cells, T, (cudaStream_t)stream);
 }
 

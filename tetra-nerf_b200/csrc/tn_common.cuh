@@ -92,6 +92,7 @@ struct Mesh {
 };
 
 struct RenderState;
+struct SurfaceState;
 
 }  // namespace tn
 
@@ -115,7 +116,9 @@ struct tn_tracer {
     uint32_t walk_quad_min_rays = 3584, walk_quad_max_rays = 0xFFFFFFFFu;
     uint32_t walk_quad_spec_max_rays = 65536;  // quad walk: batches up to this size load the candidate next records speculatively (tn_walk.cu)
     uint64_t launches = 0;
+    uint64_t mesh_gen = 0;  // a fresh next_generation() on every tn_load_tetrahedra (a surface extraction records it)
     tn::RenderState *render = nullptr;
+    tn::SurfaceState *surface = nullptr;
 };
 
 namespace tn {
@@ -134,6 +137,18 @@ struct FaceTables {
 int build_faces_device(const float *d_xyz, uint32_t V, const uint32_t *d_cells, uint32_t T, cudaStream_t s, FaceTables &out, int *launches);
 void free_mesh(tn_tracer *h);
 void free_render(tn_tracer *h);
+void free_surface(tn_tracer *h);
+// a value no earlier call returned (tn_render.cu): the generation of a field, weights or mesh
+uint64_t next_generation();
+// the field and weights of the fused render as the surface extraction reads them; TN_ERR_STATE unless both were set
+struct RenderInputs {
+    const float *fshadow;   // [V,64]
+    uint32_t V;
+    const uint8_t *wimg;    // bf16 hi/lo weight image of k_mlp<*, 3>
+    const float *bias, *head, *w4dir;
+    uint64_t gen;           // generation of field + weights
+};
+int render_inputs(tn_tracer *h, RenderInputs *out);
 int launch_walk(tn_tracer *h, const float *o, const float *d, uint32_t R, uint32_t M, uint32_t *num, uint32_t *cells, float *bary,
                 float *dist, uint32_t *verts, unsigned long long *keys, uint32_t *list, uint32_t *list_count, int kind, cudaStream_t s);
 int launch_tail_fill(tn_tracer *h, uint32_t R, uint32_t M, const uint32_t *num, uint32_t *cells, float *bary, float *dist, uint32_t *verts,

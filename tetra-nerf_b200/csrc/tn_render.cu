@@ -17,6 +17,7 @@
 #include <cstdlib>
 #include <cub/cub.cuh>
 #include "tn_common.cuh"
+#include "tn_direnc.cuh"
 #include "tn_mlp.cuh"
 #include "tn_mlp_bwd.cuh"
 #include "tn_mlp_pack.cuh"
@@ -108,9 +109,16 @@ void free_render(tn_tracer *h) {
 }
 
 // generations are unique across tracers, so a saved state recorded on one tracer never matches another tracer's field and weights
-static uint64_t next_generation() {
+uint64_t next_generation() {
     static std::atomic<uint64_t> g{0};
     return ++g;
+}
+
+int render_inputs(tn_tracer *h, RenderInputs *out) {
+    const RenderState *r = h->render;
+    if (!r || !r->fshadow || !r->have_weights) return TN_ERR_STATE;
+    *out = RenderInputs{r->fshadow, r->V, r->wimg, r->bias, r->head, r->w4dir, r->gen};
+    return TN_OK;
 }
 
 static RenderState *state(tn_tracer *h) {
@@ -386,22 +394,7 @@ __device__ void weights_from_density(float *dd, float *tr, uint32_t S, int lane)
 __device__ __forceinline__ void dir_bias(const SampleParams &p, uint32_t ray, uint32_t slot, int lane) {
     const float dx = p.d[3 * (size_t)ray], dy = p.d[3 * (size_t)ray + 1], dz = p.d[3 * (size_t)ray + 2];
     float enc[27];
-    {
-        const float dd[3] = {dx, dy, dz};
-        const float two_pi = 6.283185307179586f, half_pi = 1.5707963267948966f;
-#pragma unroll
-        for (int a = 0; a < 3; ++a) {
-            const float sc = two_pi * dd[a];
-#pragma unroll
-            for (int f = 0; f < 4; ++f) {
-                const float freq = f == 0 ? 1.0f : (f == 1 ? 2.5198421f : (f == 2 ? 6.3496042f : 16.0f));  // 2**linspace(0,4,4)
-                const float si = sc * freq;
-                enc[a * 4 + f] = sinf(si);
-                enc[12 + a * 4 + f] = sinf(si + half_pi);
-            }
-            enc[24 + a] = dd[a];
-        }
-    }
+    encode_direction(dx, dy, dz, enc);
     if (p.train) {
 #pragma unroll
         for (int k = 0; k < 27; ++k) if (lane == k) p.enc[(size_t)slot * 27 + k] = enc[k];

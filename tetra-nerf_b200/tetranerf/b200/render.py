@@ -175,6 +175,29 @@ class FusedRenderer:
         return self._train_backward(_lib.tn_render_train_backward_saved, [self.tracer.handle, state.blob.data_ptr()], grad_rgb, grad_acc,
                                     num_vertices, use_gradient_scaling)
 
+    # ---- surface extraction ---------------------------------------------------------------------------------------------------------
+    def extract_surface(self, level: float) -> Dict[str, torch.Tensor]:
+        """the density iso-surface sigma = level (finite, > 0) of the current field and weights, by marching tetrahedra on the tracer's
+        mesh (tn_surface_extract; DESIGN §4.6) -> device tensors `vertices`, `normals`, `colors` f32[N,3], `faces` i32[F,3] and
+        `face_tetrahedra` i32[F], in the mesh's frame.  Empty tensors when the level lies above or below every vertex density.  Waits
+        until the stream has reached it (the counts are read back)."""
+        tr, dev = self.tracer, self.device
+        n, f = C.c_uint32(0), C.c_uint32(0)
+        with torch.cuda.device(dev):
+            ext._check(_lib.tn_surface_extract(tr.handle, C.c_float(float(level)), C.byref(n), C.byref(f), self._stream()))
+            N, F = int(n.value), int(f.value)
+            out = {"vertices": torch.empty((N, 3), dtype=torch.float32, device=dev), "normals": torch.empty((N, 3), dtype=torch.float32, device=dev),
+                   "colors": torch.empty((N, 3), dtype=torch.float32, device=dev), "faces": torch.empty((F, 3), dtype=torch.int32, device=dev),
+                   "face_tetrahedra": torch.empty((F,), dtype=torch.int32, device=dev)}
+            self.copy_surface(out)
+        return out
+
+    def copy_surface(self, out: Dict[str, torch.Tensor]) -> None:
+        """copies the last extraction into `out` (the tensors extract_surface allocates); raises RuntimeError if set_field, set_weights or
+        load_tetrahedra ran since it"""
+        ext._check(_lib.tn_surface_copy(self.tracer.handle, out["vertices"].data_ptr(), out["normals"].data_ptr(), out["colors"].data_ptr(),
+                                        out["faces"].data_ptr(), out["face_tetrahedra"].data_ptr(), self._stream()))
+
     def set_mlp_precision(self, prec: int) -> None:
         """operand precision of the inference MLP: 2 = f16w2 (default: fp16 activations x fp16 hi/lo weights; per-sample error relative
         to the activations -- ~2.6e-5 absolute on unit-scale density / colour, ~4.9e-4 relative on large densities -- pixels within

@@ -267,10 +267,15 @@ class TetrahedraNerf(Model):
         return self.renderer_rgb.get_background_color(self.renderer_rgb.background_color, shape, device)
 
     # ---- fused inference path ---------------------------------------------------------------------------
-    def _fused_supported(self) -> bool:
+    def _fused_unsupported(self) -> List[str]:
+        """the config options, as `name=value`, that keep this model off the fused CUDA pipeline"""
         c = self.config
-        return (c.field_dim == 64 and c.hidden_size == 128 and c.num_density_layers == 3 and c.num_color_layers == 1
-                and c.input_fourier_frequencies == 0 and c.appearance_embed_dim == 0 and c.background_color in ("white", "black"))
+        want = {"field_dim": (64,), "hidden_size": (128,), "num_density_layers": (3,), "num_color_layers": (1,), "input_fourier_frequencies": (0,),
+                "appearance_embed_dim": (0,), "background_color": ("white", "black")}
+        return [f"{k}={getattr(c, k)!r}" for k, ok in want.items() if getattr(c, k) not in ok]
+
+    def _fused_supported(self) -> bool:
+        return not self._fused_unsupported()
 
     def _fused_renderer(self):
         from ..b200.render import FusedRenderer
@@ -367,6 +372,18 @@ class TetrahedraNerf(Model):
             accumulation[ray_mask] = self.renderer_accumulation(weights)
             depth[ray_mask] = self.renderer_depth(weights, samples)
         return {"rgb": rgb, "accumulation": accumulation, "depth": depth, "ray_mask": ray_mask}
+
+    # ---- geometry export -----------------------------------------------------------------------------------------------------------------
+    def extract_surface(self, level: float) -> Dict[str, torch.Tensor]:
+        """the density iso-surface sigma = level of the trained field as a triangle mesh, by marching tetrahedra on the model's own
+        tetrahedra (FusedRenderer.extract_surface): device tensors `vertices`, `normals`, `colors` f32[N,3], `faces` i32[F,3],
+        `face_tetrahedra` i32[F], in the model's (nerfstudio) frame, the one the renders use.  `tetranerf.b200.surface.write_ply` writes
+        it out.  Needs the fused pipeline: raises RuntimeError naming the options that rule it out."""
+        bad = self._fused_unsupported()
+        if bad:
+            raise RuntimeError(f"extract_surface runs on the fused CUDA pipeline, which does not support {', '.join(bad)}")
+        with torch.no_grad():
+            return self._fused_renderer().extract_surface(level)
 
     def get_loss_dict(self, outputs, batch, metrics_dict=None) -> Dict[str, torch.Tensor]:
         image = batch["image"].to(outputs["rgb"].device)

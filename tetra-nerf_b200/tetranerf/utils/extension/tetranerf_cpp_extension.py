@@ -68,6 +68,8 @@ _lib.tn_render_get_timings.argtypes = [_vp, C.POINTER(C.c_float)]
 _lib.tn_render_get_backward_timings.argtypes = [_vp, C.POINTER(C.c_float)]
 _lib.tn_render_set_deterministic.argtypes = [_vp, _i]
 _lib.tn_render_set_backward_grid.argtypes = [_vp, _u32]
+_lib.tn_surface_extract.argtypes = [_vp, C.c_float, C.POINTER(_u32), C.POINTER(_u32), _vp]
+_lib.tn_surface_copy.argtypes = [_vp, _vp, _vp, _vp, _vp, _vp, _vp]
 
 LIBRARY_PATH = str(_LIB_PATH)
 
