@@ -87,34 +87,73 @@ __device__ __forceinline__ void to_operand(float e0, float e1, uint32_t &hi, uin
     else tc::split_pack2(e0, e1, hi, lo);
 }
 
-// the interpolated features of the thread's two rows, as the layer-0 A fragments (K = 64: 4 k-steps x 4 registers).
-// tetrahedra_tracer.cu:203-220: v1*b0, + v2*b1, + v3*b2, + v0*w0 (fused multiply-adds), per feature.
-template <int PREC>
-__device__ __forceinline__ void gather_rows(const uint4 *__restrict__ vi, const float *__restrict__ bary, const float *__restrict__ fshadow, uint64_t row0,
-                                            uint64_t total_rows, uint32_t t, uint32_t (&xh)[16], uint32_t (&xl)[16]) {
+// the sample indices of the thread's two rows (row0, row0 + 8): matched vertex ids and barycentric weights.  A row at or past
+// total_rows reads as unmatched.
+struct GatherRows {
+    uint4 v[2];
+    float b[2][3];
+};
+__device__ __forceinline__ GatherRows load_gather_rows(const uint4 *__restrict__ vi, const float *__restrict__ bary, uint64_t row0, uint64_t total_rows) {
+    GatherRows r;
 #pragma unroll
     for (int rr = 0; rr < 2; ++rr) {
         const uint64_t row = row0 + 8u * rr;
-        uint4 v = make_uint4(TN_EMPTY, TN_EMPTY, TN_EMPTY, TN_EMPTY);
-        float b0 = 0.f, b1 = 0.f, b2 = 0.f;
+        r.v[rr] = make_uint4(TN_EMPTY, TN_EMPTY, TN_EMPTY, TN_EMPTY);
+        r.b[rr][0] = r.b[rr][1] = r.b[rr][2] = 0.f;
         if (row < total_rows) {
-            v = __ldg(vi + row);
-            b0 = __ldg(bary + 3 * row); b1 = __ldg(bary + 3 * row + 1); b2 = __ldg(bary + 3 * row + 2);
+            r.v[rr] = __ldg(vi + row);
+            r.b[rr][0] = __ldg(bary + 3 * row); r.b[rr][1] = __ldg(bary + 3 * row + 1); r.b[rr][2] = __ldg(bary + 3 * row + 2);
         }
-        const bool m = v.x != TN_EMPTY;
+    }
+    return r;
+}
+// brings the 128-byte line of p into L1 (no register is written, nothing waits for it)
+__device__ __forceinline__ void prefetch_l1(const void *p) { asm volatile("prefetch.global.L1 [%0];" ::"l"(p)); }
+// the lines load_gather_rows will read for the same rows
+__device__ __forceinline__ void prefetch_gather_rows(const uint4 *vi, const float *bary, uint64_t row0, uint64_t total_rows) {
+#pragma unroll
+    for (int rr = 0; rr < 2; ++rr) {
+        const uint64_t row = row0 + 8u * rr;
+        if (row < total_rows) {
+            prefetch_l1(vi + row);
+            prefetch_l1(bary + 3 * row);
+        }
+    }
+}
+
+// the interpolated features of the thread's two rows, as the layer-0 A fragments (K = 64: 4 k-steps x 4 registers).
+// tetrahedra_tracer.cu:203-220: v1*b0, + v2*b1, + v3*b2, + v0*w0 (fused multiply-adds), per feature.
+// All 64 field loads of the two rows are issued before the first one is consumed, so a thread has its whole gather in flight at
+// once instead of one L2 round trip per column pair.  The loads are unconditional: an unmatched row reads vertex 0's features and
+// its result is replaced by 0 (a branch around the loads would keep the compiler from hoisting them over the FMAs).
+template <int PREC>
+__device__ __forceinline__ void gather_rows(const GatherRows &r, const float *__restrict__ fshadow, uint32_t t, uint32_t (&xh)[16], uint32_t (&xl)[16]) {
+    float2 a[2][4][8];  // [row][vertex][column pair]
+#pragma unroll
+    for (int rr = 0; rr < 2; ++rr) {
+        const uint4 v = r.v[rr].x != TN_EMPTY ? r.v[rr] : make_uint4(0u, 0u, 0u, 0u);
+        const uint32_t vs[4] = {v.x, v.y, v.z, v.w};
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+            const float *f = fshadow + (size_t)vs[k] * 64 + 2 * t;
+#pragma unroll
+            for (int c = 0; c < 8; ++c) a[rr][k][c] = ldg_stream2(f + 8 * c);
+        }
+    }
+#pragma unroll
+    for (int rr = 0; rr < 2; ++rr) {
+        const bool m = r.v[rr].x != TN_EMPTY;
+        const float b0 = r.b[rr][0], b1 = r.b[rr][1], b2 = r.b[rr][2];
         const float w0 = __fsub_rn(1.0f, __fadd_rn(__fadd_rn(b0, b1), b2));
-        const float *f0 = fshadow + (size_t)v.x * 64 + 2 * t, *f1 = fshadow + (size_t)v.y * 64 + 2 * t;
-        const float *f2 = fshadow + (size_t)v.z * 64 + 2 * t, *f3 = fshadow + (size_t)v.w * 64 + 2 * t;
 #pragma unroll
         for (int c = 0; c < 8; ++c) {  // column pair 8c + 2t, +1  ->  k-step c / 2, register 2 (c & 1) + rr
-            float2 o = make_float2(0.f, 0.f);
-            if (m) {
-                const float2 a0 = ldg_stream2(f0 + 8 * c), a1 = ldg_stream2(f1 + 8 * c), a2 = ldg_stream2(f2 + 8 * c), a3 = ldg_stream2(f3 + 8 * c);
-                o.x = __fmaf_rn(b0, a1.x, 0.f); o.y = __fmaf_rn(b0, a1.y, 0.f);
-                o.x = __fmaf_rn(b1, a2.x, o.x); o.y = __fmaf_rn(b1, a2.y, o.y);
-                o.x = __fmaf_rn(b2, a3.x, o.x); o.y = __fmaf_rn(b2, a3.y, o.y);
-                o.x = __fmaf_rn(w0, a0.x, o.x); o.y = __fmaf_rn(w0, a0.y, o.y);
-            }
+            const float2 a0 = a[rr][0][c], a1 = a[rr][1][c], a2 = a[rr][2][c], a3 = a[rr][3][c];
+            float2 o;
+            o.x = __fmaf_rn(b0, a1.x, 0.f); o.y = __fmaf_rn(b0, a1.y, 0.f);
+            o.x = __fmaf_rn(b1, a2.x, o.x); o.y = __fmaf_rn(b1, a2.y, o.y);
+            o.x = __fmaf_rn(b2, a3.x, o.x); o.y = __fmaf_rn(b2, a3.y, o.y);
+            o.x = __fmaf_rn(w0, a0.x, o.x); o.y = __fmaf_rn(w0, a0.y, o.y);
+            if (!m) o = make_float2(0.f, 0.f);
             const int i = 4 * (c >> 1) + 2 * (c & 1) + rr;
             to_operand<PREC>(o.x, o.y, xh[i], xl[i]);
         }
@@ -169,9 +208,16 @@ __global__ void __launch_bounds__(MLP_THREADS, 1) k_mlp(const MlpParams p) {
         fence_barrier_init();
     }
     for (uint32_t i = threadIdx.x; i < 516; i += MLP_THREADS) const_cast<float *>(head_s)[i] = p.head[i];
-    if (tid == 0) {  // first tile of each warpgroup: static; the following ones come from the global counter
+    // tile scheduler: the tile of round n sits in slots[2 wg + (n & 1)] from round n - 1 on, so a warpgroup knows its next tile for
+    // the whole of the current round.  The first tile of each warpgroup is static, the following ones come from the global counter.
+    auto draw = [&]() {
+        const uint32_t nx = gridDim.x * MLP_WGS + atomicAdd(p.tile_ctr, 1u);
+        return nx < ntiles ? nx : MLP_NO_TILE;
+    };
+    if (tid == 0) {
         const uint32_t first = blockIdx.x * MLP_WGS + wg;
         slots[2 * wg] = first < ntiles ? first : MLP_NO_TILE;
+        slots[2 * wg + 1] = draw();
     }
     __syncthreads();
     if (threadIdx.x == 0) {
@@ -181,22 +227,33 @@ __global__ void __launch_bounds__(MLP_THREADS, 1) k_mlp(const MlpParams p) {
     const uint32_t wsm = smem_u32(smem);
     const float *wd = head_s, *wc = head_s + 128;
     bool weights_ready = false;
+    const uint32_t lrow = warp * 16u + g;  // the thread's first row within a tile
+    uint32_t tile = slots[2 * wg];
 
 #pragma unroll 1
     for (uint32_t n = 0;; ++n) {
         wg_sync(wg);
-        const uint32_t tile = slots[2 * wg + (n & 1u)];
         if (tile == MLP_NO_TILE) break;
-        if (tid == 0) {  // draw the tile of the next round now: the atomic's latency hides under this one
-            const uint32_t nx = gridDim.x * MLP_WGS + atomicAdd(p.tile_ctr, 1u);
-            slots[2 * wg + ((n + 1u) & 1u)] = nx < ntiles ? nx : MLP_NO_TILE;
-        }
-        const uint64_t row0 = (uint64_t)tile * MLP_TILE + warp * 16u + g, row1 = row0 + 8u;
+        const uint32_t next = slots[2 * wg + ((n + 1u) & 1u)];
+        // draw the tile of round n + 2 into this round's slot (every thread read it in round n - 1, before the barrier above)
+        if (tid == 0) slots[2 * wg + (n & 1u)] = draw();
+        const uint64_t row0 = (uint64_t)tile * MLP_TILE + lrow, row1 = row0 + 8u;
+        const float *db0 = nullptr, *db1 = nullptr;  // FINE: the per-ray bias rows of layer 4
 
         uint32_t ah[32], al[32];
         {
             uint32_t xh[16], xl[16];
-            gather_rows<PREC>(p.vi, p.bary, p.fshadow, row0, total_rows, t, xh, xl);
+            gather_rows<PREC>(load_gather_rows(p.vi, p.bary, row0, total_rows), p.fshadow, t, xh, xl);
+            // Into L1 while this tile's MMAs run: the next tile's indices, so its gather starts with the field loads, and (FINE) this
+            // tile's bias rows of layer 4, read right after that layer's MMA wait.  Prefetches hold no registers: keeping the 14
+            // index words of the next tile in registers instead spills k_mlp<true, 3> at its 168-register limit.
+            if (next != MLP_NO_TILE) prefetch_gather_rows(p.vi, p.bary, (uint64_t)next * MLP_TILE + lrow, total_rows);
+            if (FINE) {
+                db0 = p.dirbias + (size_t)((uint32_t)min(row0, total_rows - 1) / p.S) * 128;
+                db1 = p.dirbias + (size_t)((uint32_t)min(row1, total_rows - 1) / p.S) * 128;
+                prefetch_l1(db0 + 32 * t);  // the four threads of a row cover its four 128-byte lines
+                prefetch_l1(db1 + 32 * t);
+            }
             if (!weights_ready) { mbar_wait(w_bar, 0); weights_ready = true; }
             float d[64];
             layer_mma<PREC, 4>(d, xh, xl, wsm + mlp_off_layer(0));
@@ -238,8 +295,6 @@ __global__ void __launch_bounds__(MLP_THREADS, 1) k_mlp(const MlpParams p) {
             // layer 4: per-ray bias (b4 + the direction part of W4), ReLU, colour-head partial dot products
             float d[64];
             layer_mma<PREC, 8>(d, ah, al, wsm + mlp_off_layer(3));
-            const float *db0 = p.dirbias + (size_t)((uint32_t)min(row0, total_rows - 1) / p.S) * 128;
-            const float *db1 = p.dirbias + (size_t)((uint32_t)min(row1, total_rows - 1) / p.S) * 128;
 #pragma unroll
             for (int j = 0; j < 16; ++j) {
                 const int c = 8 * j + 2 * (int)t;
@@ -281,6 +336,7 @@ __global__ void __launch_bounds__(MLP_THREADS, 1) k_mlp(const MlpParams p) {
                 }
             }
         }
+        tile = next;
     }
     if (!weights_ready) mbar_wait(w_bar, 0);  // a warpgroup without a tile still lets the weight copy land before the CTA exits
 }

@@ -297,7 +297,7 @@ __global__ void __launch_bounds__(BWD_THREADS, 1) k_mlp_bwd(const MlpBwdParamsT<
         // ---------- forward layer 1; X also goes to shared memory for dW1 ----------
         {
             uint32_t xh[16], xl[16];
-            gather_rows<3>(p.vi, p.bary, p.fshadow, row0, total_rows, t, xh, xl);
+            gather_rows<3>(load_gather_rows(p.vi, p.bary, row0, total_rows), p.fshadow, t, xh, xl);
 #pragma unroll
             for (int c = 0; c < 8; ++c) {
                 const int i = 4 * (c >> 1) + 2 * (c & 1);
