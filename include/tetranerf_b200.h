@@ -122,6 +122,13 @@ int tn_render_set_weights(tn_tracer *h, const float *const *d_params12, void *st
 /* d_rgb f32[R,3], d_acc f32[R,1], d_depth f32[R,1], d_mask u8[R] */
 int tn_render(tn_tracer *h, const tn_render_config *cfg, const float *d_origins, const float *d_directions, uint32_t R,
               float *d_rgb, float *d_acc, float *d_depth, uint8_t *d_mask, void *stream);
+/* tn_render plus the normal map d_normals f32[R,3] (every element written): per sample the exact gradient of the density
+ * pre-activation (reverse pass through mlp_base in the render's operand precision, then grad = cof(E) q / det(E) on the matched
+ * tetrahedron), n = -grad / |grad|, composited with the weights of rgb and normalised (nerfstudio NormalsRenderer(normalize=True));
+ * (0,0,0) on empty rays.  rgb, acc, depth and mask are the same bits as tn_render's.  TN_ERR_ARG while a fused pixel gather is set
+ * (tn_render_set_gather).  DESIGN.md §4.7. */
+int tn_render_normals(tn_tracer *h, const tn_render_config *cfg, const float *d_origins, const float *d_directions, uint32_t R,
+                      float *d_rgb, float *d_acc, float *d_depth, uint8_t *d_mask, float *d_normals, void *stream);
 /* ---- fused training step (SURVEY.md §8f-1): TetrahedraNerf.get_outputs in training mode (model.py:520-662) + its autograd backward.
  * Forward = the fused pipeline with the stratified bins of training (model.py:169-174 for the coarse pass, PDFSampler train_stratified
  * for the fine pass; the uniform [0,1) draws come from the caller, d_jitter_coarse f32[R,S_c+1] / d_jitter_fine f32[R,S_f+1] indexed by
@@ -219,6 +226,9 @@ int tn_debug_trace_stats(tn_tracer *h, uint32_t *out2);
  * num, dist, n_active, ray_list, ebins_c, sbins_c, vi_c, bary_c, dens_c, ebins_f, vi_f, bary_f, out_f,
  * dirbias, field shadow, weight image */
 int tn_render_debug_buffers(tn_tracer *h, void **ptrs16);
+/* device pointer of the per-sample density gradient of the last tn_render_normals call: float4 (x, y, z, 0) per sample, in the
+ * slot order of the pass that gives the colours (vi_f / bary_f; vi_c / bary_c when num_fine_samples = 0) */
+int tn_render_debug_normals_grad(tn_tracer *h, void **ptr);
 /* one 128x128 tile out = A[128,K] * W[128,K]^T through the wgmma bf16x3 path (A from registers); K in {64,128}; synchronous */
 int tn_debug_gemm_bf16x3(int device, const float *d_A, const float *d_W, uint32_t K, float *d_out, void *stream);
 /* probe of the shared-memory operand forms of the fused MLP backward: P, Q f32[128,128] staged as bf16 hi/lo blocks

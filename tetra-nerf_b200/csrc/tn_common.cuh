@@ -149,6 +149,23 @@ struct RenderInputs {
     uint64_t gen;           // generation of field + weights
 };
 int render_inputs(tn_tracer *h, RenderInputs *out);
+// the normal map of a fused render (tn_normals.cu), launched after its composite on the render's own buffers
+struct NormalsLaunch {
+    const uint32_t *n_active, *ray_list;  // active rays, slot -> ray
+    uint32_t *tile_ctr;                   // zeroed device counter
+    uint32_t S, R, prec;                  // samples per ray of the pass that gives the colours, rays, operand precision (2 / 3)
+    const uint4 *vi;                      // [n_active*S] matched vertex ids of that pass
+    const float *bary;                    // [n_active*S,3]
+    const float *ebins;                   // [n_active,S+1] its euclidean bin edges
+    const float *out_f;                   // [n_active*S] (sigma, r, g, b)
+    const float *fshadow;                 // [V,64]
+    const uint8_t *wimg;                  // weight image of k_mlp<*, prec>
+    const float *bias, *head;
+    const float *xyz;                     // [V,3] mesh vertex positions
+    float4 *grad;                         // out: [n_active*S] density gradient (x, y, z, 0)
+    float *normals;                       // out: [R,3]
+};
+int launch_normals(const NormalsLaunch &a, int sms, cudaStream_t s);
 int launch_walk(tn_tracer *h, const float *o, const float *d, uint32_t R, uint32_t M, uint32_t *num, uint32_t *cells, float *bary,
                 float *dist, uint32_t *verts, unsigned long long *keys, uint32_t *list, uint32_t *list_count, int kind, cudaStream_t s);
 int launch_tail_fill(tn_tracer *h, uint32_t R, uint32_t M, const uint32_t *num, uint32_t *cells, float *bary, float *dist, uint32_t *verts,

@@ -17,6 +17,7 @@
 #include <cstdlib>
 #include <cub/cub.cuh>
 #include "tn_common.cuh"
+#include "tn_composite.cuh"
 #include "tn_direnc.cuh"
 #include "tn_mlp.cuh"
 #include "tn_mlp_bwd.cuh"
@@ -82,6 +83,9 @@ struct RenderState {
     float *det_dbg = nullptr;          // [R/64][128*28] partial W4dir / b4 gradients per block of k_dirbias_grads
     uint32_t *det_keys = nullptr, *det_vals = nullptr;  // [2][R*S2*4] (vertex, sample row * 4 + k) pairs, sort input | output
     size_t cap_det_R = 0, cap_det_S2 = 0;
+    // normal map (tn_render_normals): density gradient per sample of the last normals render
+    float4 *grad_n = nullptr;
+    size_t cap_grad_n = 0;
 };
 
 static void free_ws(RenderState *r) {
@@ -102,6 +106,7 @@ void free_render(tn_tracer *h) {
     cudaFree(r->wimg_bwd); cudaFree(r->sbins_f); cudaFree(r->enc); cudaFree(r->dout); cudaFree(r->gshadow); cudaFree(r->gw); cudaFree(r->g_dirbias);
     cudaFree(r->ray_flag); cudaFree(r->ray_slot); cudaFree(r->cub_tmp); cudaFree(r->det_part); cudaFree(r->det_gdb); cudaFree(r->det_dx);
     cudaFree(r->det_sums); cudaFree(r->det_dbg); cudaFree(r->det_keys); cudaFree(r->det_vals);
+    cudaFree(r->grad_n);
     for (auto &e : r->ev) if (e) cudaEventDestroy(e);
     for (auto &e : r->evb) if (e) cudaEventDestroy(e);
     delete r;
@@ -210,32 +215,6 @@ __device__ __forceinline__ void store_pixel(const SampleParams &p, uint32_t ray,
     }
 }
 
-__device__ __forceinline__ float warp_incl_scan_f(float v, int lane) {
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-        const float t = __shfl_up_sync(0xffffffffu, v, o);
-        if (lane >= o) v += t;
-    }
-    return v;
-}
-__device__ __forceinline__ float warp_sum_f(float v) {
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-    return v;
-}
-// in-place inclusive scan of a[0..n) in shared memory by one warp; returns the total
-__device__ float smem_scan_add(float *a, uint32_t n, int lane) {
-    float carry = 0.f;
-    for (uint32_t base = 0; base < n; base += 32) {
-        const uint32_t i = base + lane;
-        float v = i < n ? a[i] : 0.f;
-        v = warp_incl_scan_f(v, lane) + carry;
-        if (i < n) a[i] = v;
-        carry = __shfl_sync(0xffffffffu, v, 31);
-    }
-    __syncwarp();
-    return carry;
-}
 __device__ void smem_scan_max(const float *in, float *out, uint32_t n, int lane) {
     float carry = -3.0e38f;
     for (uint32_t base = 0; base < n; base += 32) {
@@ -251,11 +230,6 @@ __device__ void smem_scan_max(const float *in, float *out, uint32_t n, int lane)
         carry = __shfl_sync(0xffffffffu, v, 31);
     }
     __syncwarp();
-}
-__device__ __forceinline__ float nan_to_num_f(float x) {  // torch.nan_to_num defaults
-    if (isnan(x)) return 0.f;
-    if (isinf(x)) return x > 0 ? 3.4028234663852886e38f : -3.4028234663852886e38f;
-    return x;
 }
 // torch.linspace(start, end, steps)[i] for float32 (symmetric fill of ATen's linspace kernel)
 __device__ __forceinline__ float linspace_f(float start, float end, uint32_t steps, uint32_t i) {
@@ -373,20 +347,6 @@ __global__ void __launch_bounds__(SAMPLE_WARPS * 32) k_sample_coarse(const Sampl
         p.vi_c[g] = vi;
         p.bary_c[3 * g] = b0; p.bary_c[3 * g + 1] = b1; p.bary_c[3 * g + 2] = b2;
     }
-}
-
-// RaySamples.get_weights on staged deltas/densities: w[j] (in place over `dd`), using `tr` as scratch
-__device__ void weights_from_density(float *dd, float *tr, uint32_t S, int lane) {
-    for (uint32_t j = lane; j < S; j += 32) tr[j] = dd[j];
-    __syncwarp();
-    smem_scan_add(tr, S, lane);  // inclusive cumsum of delta*density
-    for (uint32_t j = lane; j < S; j += 32) {
-        const float excl = j == 0 ? 0.f : tr[j - 1];
-        const float alpha = 1.f - expf(-dd[j]);
-        const float T = expf(-excl);
-        dd[j] = nan_to_num_f(alpha * T);
-    }
-    __syncwarp();
 }
 
 // direction encoding folded into a per-ray bias of mlp_head (model.py:607-620): dirbias[slot] = b4 + W4[:, :27] . enc(dir)
@@ -938,7 +898,7 @@ struct TrainFwd {
 static int ensure_train_ws(RenderState *r, size_t R, size_t S2, uint32_t V);
 
 static int render_impl(tn_tracer *h, const tn_render_config *cfg, const float *d_origins, const float *d_directions, uint32_t R,
-                       float *d_rgb, float *d_acc, float *d_depth, uint8_t *d_mask, const TrainFwd *tf, void *stream) {
+                       float *d_rgb, float *d_acc, float *d_depth, uint8_t *d_mask, const TrainFwd *tf, float *d_normals, void *stream) {
     if (!h || !cfg) return fail(TN_ERR_ARG, "null argument");
     RenderState *r = h->render;
     if (!r || !r->fshadow || !r->have_weights) return fail(TN_ERR_STATE, "tn_render: call tn_render_set_field and tn_render_set_weights first");
@@ -958,6 +918,11 @@ static int render_impl(tn_tracer *h, const tn_render_config *cfg, const float *d
     cudaStream_t s = (cudaStream_t)stream;
     int rc = ensure_ws(r, R, M, Sc, S2);
     if (rc) return rc;
+    if (d_normals != nullptr && (size_t)R * S2 > r->cap_grad_n) {
+        cudaFree(r->grad_n); r->grad_n = nullptr; r->cap_grad_n = 0;
+        TN_CUDA(cudaMalloc((void **)&r->grad_n, sizeof(float4) * (size_t)R * S2));
+        r->cap_grad_n = (size_t)R * S2;
+    }
     if (tf != nullptr) {
         rc = ensure_train_ws(r, R, S2, r->V);
         if (rc) return rc;
@@ -1040,6 +1005,16 @@ static int render_impl(tn_tracer *h, const tn_render_config *cfg, const float *d
 #undef TN_EV
     h->launches += 5;
     TN_CUDA(cudaGetLastError());
+    if (d_normals != nullptr) {  // after the six timed intervals: the density gradient at the samples that give the colours, composited
+        NormalsLaunch nl{};
+        nl.n_active = b.n_active; nl.ray_list = b.ray_list; nl.tile_ctr = b.n_active + 3;  // word 3 of the zeroed block
+        nl.S = S2; nl.R = R; nl.prec = (uint32_t)prec; nl.vi = mf.vi; nl.bary = mf.bary; nl.ebins = p.ebins_f; nl.out_f = b.out_f;
+        nl.fshadow = r->fshadow; nl.wimg = mf.wimg; nl.bias = r->bias; nl.head = r->head; nl.xyz = h->mesh.xyz; nl.grad = r->grad_n;
+        nl.normals = d_normals;
+        rc = launch_normals(nl, sms, s);
+        if (rc) return rc;
+        h->launches += 2;
+    }
     if (tf != nullptr && tf->saved == nullptr) {
         r->train_valid = true;
         r->t_det = det;
@@ -1071,7 +1046,16 @@ static int ensure_train_ws(RenderState *r, size_t R, size_t S2, uint32_t V) {
 
 extern "C" int tn_render(tn_tracer *h, const tn_render_config *cfg, const float *d_origins, const float *d_directions, uint32_t R,
                          float *d_rgb, float *d_acc, float *d_depth, uint8_t *d_mask, void *stream) {
-    return render_impl(h, cfg, d_origins, d_directions, R, d_rgb, d_acc, d_depth, d_mask, nullptr, stream);
+    return render_impl(h, cfg, d_origins, d_directions, R, d_rgb, d_acc, d_depth, d_mask, nullptr, nullptr, stream);
+}
+
+// tn_render plus the normal map d_normals f32[R,3] (DESIGN.md §4.7; tn_normals.cu)
+extern "C" int tn_render_normals(tn_tracer *h, const tn_render_config *cfg, const float *d_origins, const float *d_directions, uint32_t R,
+                                 float *d_rgb, float *d_acc, float *d_depth, uint8_t *d_mask, float *d_normals, void *stream) {
+    if (!h || !d_normals) return fail(TN_ERR_ARG, "null argument");
+    if (h->render && h->render->gather_world)
+        return fail(TN_ERR_ARG, "tn_render_normals: the fused pixel gather (tn_render_set_gather) carries no normals; switch it off first");
+    return render_impl(h, cfg, d_origins, d_directions, R, d_rgb, d_acc, d_depth, d_mask, nullptr, d_normals, stream);
 }
 
 // ---- fused training step (SURVEY §8f-1; model.py:520-662 in training mode + autograd) ------------------------------------------------
@@ -1081,7 +1065,7 @@ extern "C" int tn_render_train_forward(tn_tracer *h, const tn_render_config *cfg
                                        const float *d_jitter_coarse, const float *d_jitter_fine, float *d_rgb, float *d_acc, float *d_depth,
                                        uint8_t *d_mask, void *stream) {
     TrainFwd tf{d_jitter_coarse, d_jitter_fine, nullptr};
-    return render_impl(h, cfg, d_origins, d_directions, R, d_rgb, d_acc, d_depth, d_mask, &tf, stream);
+    return render_impl(h, cfg, d_origins, d_directions, R, d_rgb, d_acc, d_depth, d_mask, &tf, nullptr, stream);
 }
 
 // backward of a training forward of R rays x S2 fine samples whose buffers are `b`, in the mode (det) and with the background it ran
@@ -1212,7 +1196,7 @@ extern "C" int tn_render_train_forward_saved(tn_tracer *h, const tn_render_confi
     if (saved_bytes < saved_layout(R, S2, (uint8_t *)d_saved, &b))
         return fail(TN_ERR_ARG, "tn_render_train_forward_saved: saved_bytes is smaller than tn_render_train_saved_bytes");
     TrainFwd tf{d_jitter_coarse, d_jitter_fine, &b};
-    rc = render_impl(h, cfg, d_origins, d_directions, R, d_rgb, d_acc, d_depth, d_mask, &tf, stream);
+    rc = render_impl(h, cfg, d_origins, d_directions, R, d_rgb, d_acc, d_depth, d_mask, &tf, nullptr, stream);
     if (rc) return rc;
     RenderState *r = h->render;
     const SavedHeader hd{SAVED_MAGIC, R, cfg->max_ray_triangles, cfg->num_samples, cfg->num_fine_samples, S2, r->det ? 1u : 0u, 0,
@@ -1309,5 +1293,13 @@ extern "C" int tn_render_debug_buffers(tn_tracer *h, void **ptrs16) {
     void *v[16] = {r->num, r->dist, r->n_active, r->ray_list, r->ebins_c, r->sbins_c, r->vi_c, r->bary_c,
                    r->dens_c, r->ebins_f, r->vi_f, r->bary_f, r->out_f, r->dirbias, r->fshadow, r->wimg};
     for (int i = 0; i < 16; ++i) ptrs16[i] = v[i];
+    return TN_OK;
+}
+
+// test hook: device pointer of the per-sample density gradient of the last tn_render_normals call, float4 (x, y, z, 0) per sample in
+// the slot order of the pass that gives the colours (vi_f / bary_f, or vi_c / bary_c in single-pass configurations)
+extern "C" int tn_render_debug_normals_grad(tn_tracer *h, void **ptr) {
+    if (!h || !h->render || !h->render->grad_n) return fail(TN_ERR_STATE, "no normals render");
+    *ptr = h->render->grad_n;
     return TN_OK;
 }

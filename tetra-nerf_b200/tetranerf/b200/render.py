@@ -86,7 +86,10 @@ class FusedRenderer:
         ext._check(_lib.tn_render_set_weights(self.tracer.handle, arr, self._stream()))
         self._keep = ts  # repacked on the stream; keep sources alive until then
 
-    def render(self, origins: torch.Tensor, directions: torch.Tensor, settings: RenderSettings, out: Optional[dict] = None):
+    def render(self, origins: torch.Tensor, directions: torch.Tensor, settings: RenderSettings, out: Optional[dict] = None, normals: bool = False):
+        """eval-mode render -> `rgb` f32[R,3], `accumulation` / `depth` f32[R,1], `ray_mask` bool[R]; normals=True adds `normals`
+        f32[R,3]: the composited unit normal of the density field (nerfstudio's "normals" output, (0, 0, 0) on empty rays; DESIGN §4.7).
+        The other outputs are the same bits as without normals.  Not available while a fused pixel gather is set."""
         tr = self.tracer
         tr._check_float_dim3(origins, "ray_origins")
         tr._check_float_dim3(directions, "ray_directions")
@@ -100,8 +103,14 @@ class FusedRenderer:
                 "ray_mask": torch.empty((R,), dtype=torch.bool, device=dev),
             }
         cfg = _config(settings)
-        ext._check(_lib.tn_render(tr.handle, C.byref(cfg), origins.data_ptr(), directions.data_ptr(), R, out["rgb"].data_ptr(),
-                                  out["accumulation"].data_ptr(), out["depth"].data_ptr(), out["ray_mask"].data_ptr(), self._stream()))
+        args = [tr.handle, C.byref(cfg), origins.data_ptr(), directions.data_ptr(), R, out["rgb"].data_ptr(), out["accumulation"].data_ptr(),
+                out["depth"].data_ptr(), out["ray_mask"].data_ptr()]
+        if normals:
+            if "normals" not in out:
+                out["normals"] = torch.empty((R, 3), dtype=torch.float32, device=dev)
+            ext._check(_lib.tn_render_normals(*args, out["normals"].data_ptr(), self._stream()))
+        else:
+            ext._check(_lib.tn_render(*args, self._stream()))
         return out
 
     # ---- fused training step ------------------------------------------------------------------------------------------------------
@@ -222,6 +231,12 @@ class FusedRenderer:
         arr = (C.c_float * 3)()
         ext._check(_lib.tn_render_get_backward_timings(self.tracer.handle, arr))
         return {n: float(arr[i]) for i, n in enumerate(["composite_bwd", "mlp_bwd", "finalize"])}
+
+    def debug_normals_grad(self) -> int:
+        """test hook: device pointer of the per-sample density gradient (float4 per sample, slot order) of the last normals render"""
+        ptr = _vp()
+        ext._check(_lib.tn_render_debug_normals_grad(self.tracer.handle, C.byref(ptr)))
+        return ptr.value
 
     def debug_buffers(self):
         arr = (_vp * 16)()

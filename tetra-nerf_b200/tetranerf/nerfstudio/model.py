@@ -72,6 +72,8 @@ class TetrahedraNerfConfig(ModelConfig):
     background_color: Literal["random", "last_sample", "black", "white"] = "white"
     appearance_embed_dim: int = 0
     use_occupancy_field: bool = False
+    render_normals: bool = False
+    """eval renders also return "normals" f32[R,3], the composited normal of the density field (fused path only; training ignores it)"""
 
     def __post_init__(self):
         if self.tetrahedra_path is not None and self.num_tetrahedra_vertices is None:
@@ -297,13 +299,17 @@ class TetrahedraNerf(Model):
     def get_outputs(self, ray_bundle: RayBundle):
         assert self.collider is not None
         origins, directions = ray_bundle.origins.contiguous(), ray_bundle.directions.contiguous()
-        if not self.training and not torch.is_grad_enabled() and self._fused_supported():
+        normals = self.config.render_normals and not self.training
+        if normals and self._fused_unsupported():
+            raise RuntimeError(f"render_normals runs on the fused CUDA pipeline, which does not support {', '.join(self._fused_unsupported())}")
+        if normals or (not self.training and not torch.is_grad_enabled() and self._fused_supported()):
             from ..b200.render import RenderSettings
 
             bg = (1.0, 1.0, 1.0) if self.config.background_color == "white" else (0.0, 0.0, 0.0)
             st = RenderSettings(self.config.max_intersected_triangles, self.config.num_samples, self.config.num_fine_samples,
                                 self.config.use_biased_sampler, float(self.collider.far_plane), bg)
-            return self._fused_renderer().render(origins, directions, st)
+            with torch.no_grad():
+                return self._fused_renderer().render(origins, directions, st, normals=normals)
         if self.training and torch.is_grad_enabled() and self._fused_supported() and self.config.num_fine_samples > 0 \
                 and os.environ.get("TETRANERF_B200_UNFUSED_TRAIN", "0") != "1":
             return self._get_outputs_fused_train(origins, directions)
@@ -396,6 +402,8 @@ class TetrahedraNerf(Model):
         acc = _apply_colormap(outputs["accumulation"])
         depth = _apply_depth_colormap(outputs["depth"], accumulation=outputs["accumulation"])
         images = {"img": torch.cat([image, rgb], dim=1), "accumulation": torch.cat([acc], dim=1), "depth": torch.cat([depth], dim=1)}
+        if "normals" in outputs:  # unit normals in [-1, 1] shown as colours in [0, 1]
+            images["normals"] = (outputs["normals"] + 1.0) / 2.0
         # [H, W, C] -> [1, C, H, W]
         im, pr = torch.moveaxis(image, -1, 0)[None, ...], torch.moveaxis(rgb, -1, 0)[None, ...]
         metrics = {"psnr": float(_psnr(im, pr)), "nerfstudio_ssim": float(_ssim(im, pr))}

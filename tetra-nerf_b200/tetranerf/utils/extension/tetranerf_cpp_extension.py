@@ -56,6 +56,8 @@ class _Cfg(C.Structure):  # tn_render_config
 _lib.tn_render_set_field.argtypes = [_vp, _vp, _u32, _u32, _vp]
 _lib.tn_render_set_weights.argtypes = [_vp, C.POINTER(_vp), _vp]
 _lib.tn_render.argtypes = [_vp, C.POINTER(_Cfg), _vp, _vp, _u32, _vp, _vp, _vp, _vp, _vp]
+_lib.tn_render_normals.argtypes = [_vp, C.POINTER(_Cfg), _vp, _vp, _u32, _vp, _vp, _vp, _vp, _vp, _vp]
+_lib.tn_render_debug_normals_grad.argtypes = [_vp, C.POINTER(_vp)]
 _lib.tn_render_train_forward.argtypes = [_vp, C.POINTER(_Cfg), _vp, _vp, _u32, _vp, _vp, _vp, _vp, _vp, _vp, _vp]
 _lib.tn_render_train_backward.argtypes = [_vp, _vp, _vp, _i, _vp, C.POINTER(_vp), _vp]
 _lib.tn_render_train_saved_bytes.argtypes = [_vp, C.POINTER(_Cfg), _u32, C.POINTER(C.c_size_t)]
