@@ -147,7 +147,7 @@ int tn_render_train_backward(tn_tracer *h, const float *d_grad_rgb, const float 
  * their backwards, in any order, and a backward can run more than once.  tn_render_train_saved_bytes gives the size of one call's state
  * (R >= 1 rays, cfg as for the forward; ~115 MB at 8192 rays x 257 fine samples).  tn_render_train_forward_saved takes the arguments of
  * tn_render_train_forward plus d_saved (256-byte aligned, saved_bytes >= that size) and writes into it everything its backward reads that
- * a later call could overwrite: a header (R, M, S_c, S_f, S2, background, deterministic mode, generation of field and weights), the
+ * a later call could overwrite: a header (R, M, S_c, S_f, S2, background, deterministic mode, generations of field and weights and of the mesh), the
  * slot -> ray map and active count, the fine-pass samples (matched vertices, weights, (sigma, rgb) pre-activations, bins, spacing bins),
  * the per-ray direction bias and encoding.  tn_render_train_backward_saved computes the gradients of that forward (outputs as
  * tn_render_train_backward, d_grad_rgb f32[R,3] of the forward's R).  It reads d_saved, the field and the weights, and uses the tracer's
@@ -160,6 +160,16 @@ int tn_render_train_forward_saved(tn_tracer *h, const tn_render_config *cfg, con
                                   uint8_t *d_mask, void *d_saved, size_t saved_bytes, void *stream);
 int tn_render_train_backward_saved(tn_tracer *h, const void *d_saved, const float *d_grad_rgb, const float *d_grad_acc,
                                    int use_gradient_scaling, float *d_grad_field, float *const *d_grad_params12, void *stream);
+/* tn_render_train_backward_saved plus the gradients at the forward's ray origins and directions, d_grad_origins / d_grad_directions
+ * f32[R,3] (either may be NULL; every element of a non-NULL one is written, 0 on empty rays).  The sample distances are constants:
+ * a fine sample sits at x = o + t d, t the midpoint of its bin; dL/dx = E^-T q on its tetrahedron (q_k = dL/df . (F_vk - F_v0), solved in
+ * float64 from the fp32 mesh positions), dL/do = sum dL/dx, dL/dd = sum t dL/dx + the direction encoding's term.  The other outputs are
+ * those of tn_render_train_backward_saved (bitwise in the deterministic mode).  dL/do is bitwise reproducible in both modes, dL/dd in
+ * the deterministic mode.  Also returns TN_ERR_STATE if tn_load_tetrahedra ran since the forward (it reads the mesh positions).  The
+ * default mode keeps the [samples,64] feature gradient for it (0.54 GB at 8192 rays x 257 fine samples).  DESIGN.md §4.8. */
+int tn_render_train_backward_saved_rays(tn_tracer *h, const void *d_saved, const float *d_grad_rgb, const float *d_grad_acc,
+                                        int use_gradient_scaling, float *d_grad_field, float *const *d_grad_params12, float *d_grad_origins,
+                                        float *d_grad_directions, void *stream);
 /* Deterministic mode of the fused training step (enable != 0; initial value: 1 if the environment variable TETRANERF_B200_DETERMINISTIC
  * is 1, else 0).  Read by tn_render_train_forward; tn_render_train_backward continues in the mode of the forward it belongs to.  With
  * identical inputs, on the same build and GPU model, forward outputs and every gradient are then bitwise identical from run to run and
@@ -229,6 +239,9 @@ int tn_render_debug_buffers(tn_tracer *h, void **ptrs16);
 /* device pointer of the per-sample density gradient of the last tn_render_normals call: float4 (x, y, z, 0) per sample, in the
  * slot order of the pass that gives the colours (vi_f / bary_f; vi_c / bary_c when num_fine_samples = 0) */
 int tn_render_debug_normals_grad(tn_tracer *h, void **ptr);
+/* device pointer of dL/dx per fine sample of the last tn_render_train_backward_saved_rays call: float4 (x, y, z, 0) per sample, in the
+ * slot order of its forward (0 for unmatched samples and flat tetrahedra) */
+int tn_render_debug_ray_grads(tn_tracer *h, void **ptr);
 /* one 128x128 tile out = A[128,K] * W[128,K]^T through the wgmma bf16x3 path (A from registers); K in {64,128}; synchronous */
 int tn_debug_gemm_bf16x3(int device, const float *d_A, const float *d_W, uint32_t K, float *d_out, void *stream);
 /* probe of the shared-memory operand forms of the fused MLP backward: P, Q f32[128,128] staged as bf16 hi/lo blocks

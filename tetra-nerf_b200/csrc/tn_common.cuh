@@ -166,6 +166,22 @@ struct NormalsLaunch {
     float *normals;                       // out: [R,3]
 };
 int launch_normals(const NormalsLaunch &a, int sms, cudaStream_t s);
+// gradients of a training step at the ray origins and directions (tn_ray_grads.cu), launched at the end of its backward
+struct RayGradsLaunch {
+    const uint32_t *n_active, *ray_list;  // active rays, slot -> ray
+    uint32_t S, R;                        // fine samples per ray, rays of the forward
+    const float *ebins;                   // [n_active,S+1] euclidean bin edges of the fine pass
+    const uint4 *vi;                      // [n_active*S] matched vertex ids
+    const float *dx;                      // [n_active*S,64] gradient at the interpolated features
+    const float *fshadow;                 // [V,64]
+    const float *xyz;                     // [V,3] mesh vertex positions
+    const float *enc;                     // [n_active,27] encoded directions (entries 24..26: the direction itself)
+    const float *g_dirbias;               // [n_active,128] gradient at the per-ray direction bias
+    const float *w4dir;                   // [128][27] W4[:, :27]
+    float4 *gx;                           // out: [n_active*S] dL/dx per sample (x, y, z, 0)
+    float *grad_o, *grad_d;               // out: [R,3] each, or nullptr
+};
+int launch_ray_grads(const RayGradsLaunch &a, cudaStream_t s);
 int launch_walk(tn_tracer *h, const float *o, const float *d, uint32_t R, uint32_t M, uint32_t *num, uint32_t *cells, float *bary,
                 float *dist, uint32_t *verts, unsigned long long *keys, uint32_t *list, uint32_t *list_count, int kind, cudaStream_t s);
 int launch_tail_fill(tn_tracer *h, uint32_t R, uint32_t M, const uint32_t *num, uint32_t *cells, float *bary, float *dist, uint32_t *verts,

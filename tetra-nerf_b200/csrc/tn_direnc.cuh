@@ -24,4 +24,17 @@ __device__ __forceinline__ void encode_direction(float dx, float dy, float dz, f
     }
 }
 
+// the Jacobian of encode_direction: entry k depends on the direction's component `axis` only; returns d enc[k] / d d_axis
+// (sin(s f d_a) -> s f cos(s f d_a), sin(s f d_a + pi/2) -> s f cos(s f d_a + pi/2), d_a -> 1; s = 2 pi)
+__device__ __forceinline__ float encode_direction_deriv(int k, float dx, float dy, float dz, int &axis) {
+    const float two_pi = 6.283185307179586f, half_pi = 1.5707963267948966f;
+    if (k >= 24) { axis = k - 24; return 1.0f; }
+    const int a = (k % 12) / 4, f = k % 4;
+    axis = a;
+    const float da = a == 0 ? dx : (a == 1 ? dy : dz);
+    const float freq = f == 0 ? 1.0f : (f == 1 ? 2.5198421f : (f == 2 ? 6.3496042f : 16.0f));
+    const float si = two_pi * da * freq;
+    return two_pi * freq * cosf(k < 12 ? si : si + half_pi);
+}
+
 }  // namespace tn

@@ -73,8 +73,13 @@ struct MlpBwdDetParams : MlpBwdParams {
     float *gdb_part;            // [4 (ntiles + n_active)][128] direction-bias gradient partials, row 4 (tile + slot) + warp
     float *dx;                  // [rows,64] gradient at the interpolated features
 };
-template <bool DET>
-using MlpBwdParamsT = typename std::conditional<DET, MlpBwdDetParams, MlpBwdParams>::type;
+// default mode with ray gradients (k_mlp_bwd<false, true>): the field-gradient scatter as k_mlp_bwd<false>, and the dX rows stored to
+// `dx` as well (tn_ray_grads.cu reads them)
+struct MlpBwdDxParams : MlpBwdParams {
+    float *dx;                  // [rows,64] gradient at the interpolated features
+};
+template <bool DET, bool DX>
+using MlpBwdParamsT = typename std::conditional<DET, MlpBwdDetParams, typename std::conditional<DX, MlpBwdDxParams, MlpBwdParams>::type>::type;
 // offsets (floats) inside gw
 constexpr uint32_t GW_W1 = 0, GW_W2 = 8192, GW_W3 = 24576, GW_W4B = 40960, GW_B1 = 57344, GW_B2 = 57472, GW_B3 = 57600, GW_WD = 57728, GW_WC = 57856,
                    GW_SUMS = 58240 /* sum ds, sum dz_r, dz_g, dz_b */, GW_W4DIR = 58244 /* [128][27] */, GW_B4 = 61700, GW_TOTAL = 61828;
@@ -199,8 +204,9 @@ __device__ __forceinline__ void frag_pair(float x0, float x1, float y0, float y1
     tc::split_pack2(y0, y1, ah[i + 1], al[i + 1]);
 }
 
-template <bool DET>
-__global__ void __launch_bounds__(BWD_THREADS, 1) k_mlp_bwd(const MlpBwdParamsT<DET> p) {
+// DX: store the dX rows to p.dx (always so in the deterministic mode)
+template <bool DET, bool DX = DET>
+__global__ void __launch_bounds__(BWD_THREADS, 1) k_mlp_bwd(const MlpBwdParamsT<DET, DX> p) {
     using namespace tc;
     extern __shared__ __align__(1024) uint8_t tn_bwd_smem[];
     constexpr uint32_t OFF_BARS = DET ? BWD_DET_OFF_BARS : BWD_OFF_BARS;
@@ -517,6 +523,11 @@ __global__ void __launch_bounds__(BWD_THREADS, 1) k_mlp_bwd(const MlpBwdParamsT<
                     for (int j = 0; j < 8; ++j) dst[2 * j] = q[j];
                 }
             } else if (row < total_rows) {
+                if constexpr (DX) {
+                    float4 *dst = reinterpret_cast<float4 *>(p.dx + row * 64 + 4u * (t >> 1));
+#pragma unroll
+                    for (int j = 0; j < 8; ++j) dst[2 * j] = q[j];
+                }
                 const uint4 v = __ldg(p.vi + row);
                 if (v.x != TN_EMPTY) {
                     const float b0 = __ldg(p.bary + 3 * row), b1 = __ldg(p.bary + 3 * row + 1), b2 = __ldg(p.bary + 3 * row + 2);

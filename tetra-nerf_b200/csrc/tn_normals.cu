@@ -19,6 +19,7 @@
 #include "tn_common.cuh"
 #include "tn_composite.cuh"
 #include "tn_mlp.cuh"
+#include "tn_tetsolve.cuh"
 
 namespace tn {
 
@@ -279,26 +280,8 @@ __global__ void __launch_bounds__(NRM_THREADS, 1) k_mlp_normals(const NormalsPar
                 if (v.x != TN_EMPTY) {
                     // E from the fp32 positions, cofactors and determinant in float64 (exact differences; no cancellation in slivers)
                     const uint32_t vs[4] = {v.x, v.y, v.z, v.w};
-                    double x[4][3];
-#pragma unroll
-                    for (int k = 0; k < 4; ++k)
-#pragma unroll
-                        for (int c = 0; c < 3; ++c) x[k][c] = (double)__ldg(p.xyz + 3 * (size_t)vs[k] + c);
-                    double e[3][3];
-#pragma unroll
-                    for (int k = 0; k < 3; ++k)
-#pragma unroll
-                        for (int c = 0; c < 3; ++c) e[k][c] = x[k + 1][c] - x[0][c];
-                    // cof(E) columns: e2 x e3, e3 x e1, e1 x e2; det = e1 . (e2 x e3)
-                    double cf[3][3];
-#pragma unroll
-                    for (int k = 0; k < 3; ++k) {
-                        const double *a = e[(k + 1) % 3], *b = e[(k + 2) % 3];
-                        cf[k][0] = a[1] * b[2] - a[2] * b[1];
-                        cf[k][1] = a[2] * b[0] - a[0] * b[2];
-                        cf[k][2] = a[0] * b[1] - a[1] * b[0];
-                    }
-                    const double det = e[0][0] * cf[0][0] + e[0][1] * cf[0][1] + e[0][2] * cf[0][2];
+                    double cf[3][3], det;
+                    tet_cofactors(p.xyz, vs, cf, det);
                     if (det != 0.0) {
                         const float q0 = t == 0 ? q[0][0] : q[1][0], q1 = t == 0 ? q[0][1] : q[1][1], q2 = t == 0 ? q[0][2] : q[1][2];
                         const double sc = ldexp(1.0, wexp) / det;  // undo the seed's power of two

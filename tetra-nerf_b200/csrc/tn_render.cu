@@ -86,6 +86,11 @@ struct RenderState {
     // normal map (tn_render_normals): density gradient per sample of the last normals render
     float4 *grad_n = nullptr;
     size_t cap_grad_n = 0;
+    // ray gradients (tn_render_train_backward_saved_rays): dX rows of the default mode (the deterministic mode keeps them in det_dx),
+    // dL/dx per sample of the last such backward
+    float *ray_dx = nullptr;
+    float4 *ray_gx = nullptr;
+    size_t cap_ray_dx = 0, cap_ray_gx = 0;
 };
 
 static void free_ws(RenderState *r) {
@@ -106,7 +111,7 @@ void free_render(tn_tracer *h) {
     cudaFree(r->wimg_bwd); cudaFree(r->sbins_f); cudaFree(r->enc); cudaFree(r->dout); cudaFree(r->gshadow); cudaFree(r->gw); cudaFree(r->g_dirbias);
     cudaFree(r->ray_flag); cudaFree(r->ray_slot); cudaFree(r->cub_tmp); cudaFree(r->det_part); cudaFree(r->det_gdb); cudaFree(r->det_dx);
     cudaFree(r->det_sums); cudaFree(r->det_dbg); cudaFree(r->det_keys); cudaFree(r->det_vals);
-    cudaFree(r->grad_n);
+    cudaFree(r->grad_n); cudaFree(r->ray_dx); cudaFree(r->ray_gx);
     for (auto &e : r->ev) if (e) cudaEventDestroy(e);
     for (auto &e : r->evb) if (e) cudaEventDestroy(e);
     delete r;
@@ -869,6 +874,7 @@ struct SavedHeader {
     float bg[3];
     uint32_t pad2;
     uint64_t gen;              // RenderState::gen at the forward
+    uint64_t mesh_gen;         // tn_tracer::mesh_gen at the forward (the ray gradients read the mesh positions)
 };
 constexpr size_t SAVED_ALIGN = 256;
 static_assert(sizeof(SavedHeader) <= SAVED_ALIGN, "saved-state header exceeds its slot");
@@ -1073,8 +1079,13 @@ extern "C" int tn_render_train_forward(tn_tracer *h, const tn_render_config *cfg
 // parameter gradients (same order / layouts as tn_render_set_weights); every output element is written.  Reads `b` and the field /
 // weights; writes only the tracer's gradient scratch.  The coarse pass carries no gradient (PDFSampler detaches its bins).  No
 // [samples,128] tensor touches HBM.
+// rays != nullptr: also the gradients at the ray origins / directions (tn_ray_grads.cu); either output may be null
+struct RayGradOut {
+    float *grad_o, *grad_d;
+};
 static int train_backward_impl(tn_tracer *h, const TrainBufs &b, uint32_t R, uint32_t S2, bool det, const float *bg, const float *d_grad_rgb,
-                               const float *d_grad_acc, int use_gradient_scaling, float *d_grad_field, float *const *d_grad_params12, cudaStream_t s) {
+                               const float *d_grad_acc, int use_gradient_scaling, float *d_grad_field, float *const *d_grad_params12, cudaStream_t s,
+                               const RayGradOut *rays = nullptr) {
     RenderState *r = h->render;
     int sms = 132;
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, h->device);
@@ -1082,6 +1093,19 @@ static int train_backward_impl(tn_tracer *h, const TrainBufs &b, uint32_t R, uin
     if (det) {
         const int rc = ensure_det_ws(r, R, S2);
         if (rc) return rc;
+    }
+    const size_t rows = (size_t)R * S2;
+    if (rays != nullptr) {
+        if (!det && rows > r->cap_ray_dx) {
+            cudaFree(r->ray_dx); r->ray_dx = nullptr; r->cap_ray_dx = 0;
+            TN_CUDA(cudaMalloc((void **)&r->ray_dx, sizeof(float) * 64 * rows));
+            r->cap_ray_dx = rows;
+        }
+        if (rows > r->cap_ray_gx) {
+            cudaFree(r->ray_gx); r->ray_gx = nullptr; r->cap_ray_gx = 0;
+            TN_CUDA(cudaMalloc((void **)&r->ray_gx, sizeof(float4) * rows));
+            r->cap_ray_gx = rows;
+        }
     }
     TN_CUDA(cudaMemsetAsync(r->gw, 0, sizeof(float) * GW_TOTAL, s));
     if (!det) {  // (deterministic mode writes every element of these)
@@ -1107,9 +1131,17 @@ static int train_backward_impl(tn_tracer *h, const TrainBufs &b, uint32_t R, uin
     bp.gw = r->gw; bp.g_dirbias = r->g_dirbias; bp.tile_ctr = r->n_active + 3;
     const uint64_t tiles = ((uint64_t)R * S2 + BWD_TILE - 1) / BWD_TILE;
     if (!det) {
-        TN_CUDA(cudaFuncSetAttribute(k_mlp_bwd<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)BWD_SMEM_BYTES));
         const uint32_t grid = r->bwd_grid ? r->bwd_grid : (uint32_t)std::min<uint64_t>(tiles, (uint64_t)sms);
-        k_mlp_bwd<false><<<grid, BWD_THREADS, BWD_SMEM_BYTES, s>>>(bp);
+        if (rays == nullptr) {
+            TN_CUDA(cudaFuncSetAttribute(k_mlp_bwd<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)BWD_SMEM_BYTES));
+            k_mlp_bwd<false><<<grid, BWD_THREADS, BWD_SMEM_BYTES, s>>>(bp);
+        } else {  // the same backward, storing the dX rows for k_ray_grads as well
+            MlpBwdDxParams xp{};
+            static_cast<MlpBwdParams &>(xp) = bp;
+            xp.dx = r->ray_dx;
+            TN_CUDA(cudaFuncSetAttribute(k_mlp_bwd<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)BWD_SMEM_BYTES));
+            k_mlp_bwd<false, true><<<grid, BWD_THREADS, BWD_SMEM_BYTES, s>>>(xp);
+        }
         if (r->profile) cudaEventRecord(r->evb[2], s);
         k_dirbias_grads<false><<<(R + DBG_SLOTS - 1) / DBG_SLOTS, 256, 0, s>>>(b.n_active, r->g_dirbias, b.enc, r->gw, nullptr);
     } else {
@@ -1144,6 +1176,15 @@ static int train_backward_impl(tn_tracer *h, const TrainBufs &b, uint32_t R, uin
     for (int i = 0; i < 12; ++i) {
         if (!d_grad_params12[i]) return fail(TN_ERR_ARG, "tn_render_train_backward: null parameter gradient pointer");
         go.p[i] = d_grad_params12[i];
+    }
+    if (rays != nullptr) {  // after the direction-bias gradient is complete
+        RayGradsLaunch rl{};
+        rl.n_active = b.n_active; rl.ray_list = b.ray_list; rl.S = S2; rl.R = R; rl.ebins = b.ebins_f; rl.vi = b.vi_f;
+        rl.dx = det ? r->det_dx : r->ray_dx; rl.fshadow = r->fshadow; rl.xyz = h->mesh.xyz; rl.enc = b.enc; rl.g_dirbias = r->g_dirbias;
+        rl.w4dir = r->w4dir; rl.gx = r->ray_gx; rl.grad_o = rays->grad_o; rl.grad_d = rays->grad_d;
+        const int rc = launch_ray_grads(rl, s);
+        if (rc) return rc;
+        h->launches += 1;
     }
     k_scatter_grads<<<(128 * 155 + 255) / 256, 256, 0, s>>>(r->gw, go);
     k_transpose_v64<<<(V + 31) / 32, dim3(32, 8), 0, s>>>(r->gshadow, d_grad_field, V);
@@ -1200,15 +1241,15 @@ extern "C" int tn_render_train_forward_saved(tn_tracer *h, const tn_render_confi
     if (rc) return rc;
     RenderState *r = h->render;
     const SavedHeader hd{SAVED_MAGIC, R, cfg->max_ray_triangles, cfg->num_samples, cfg->num_fine_samples, S2, r->det ? 1u : 0u, 0,
-                         {cfg->background[0], cfg->background[1], cfg->background[2]}, 0, r->gen};
+                         {cfg->background[0], cfg->background[1], cfg->background[2]}, 0, r->gen, h->mesh_gen};
     DeviceGuard g(h->device);
     // pageable source: staged before the call returns, so `hd` may go out of scope
     TN_CUDA(cudaMemcpyAsync(d_saved, &hd, sizeof(hd), cudaMemcpyHostToDevice, (cudaStream_t)stream));
     return TN_OK;
 }
 
-extern "C" int tn_render_train_backward_saved(tn_tracer *h, const void *d_saved, const float *d_grad_rgb, const float *d_grad_acc,
-                                              int use_gradient_scaling, float *d_grad_field, float *const *d_grad_params12, void *stream) {
+static int backward_saved(tn_tracer *h, const void *d_saved, const float *d_grad_rgb, const float *d_grad_acc, int use_gradient_scaling,
+                          float *d_grad_field, float *const *d_grad_params12, const RayGradOut *rays, void *stream) {
     if (!h || !d_saved || !d_grad_rgb || !d_grad_field || !d_grad_params12) return fail(TN_ERR_ARG, "null argument");
     RenderState *r = h->render;
     if (!r || !r->n_active) return fail(TN_ERR_STATE, "tn_render_train_backward_saved: no training forward on this tracer");
@@ -1222,10 +1263,27 @@ extern "C" int tn_render_train_backward_saved(tn_tracer *h, const void *d_saved,
     if (hd.gen != r->gen)
         return fail(TN_ERR_STATE, "tn_render_train_backward_saved: the field or the weights changed (tn_render_set_field / "
                                   "tn_render_set_weights) since the forward, or the forward ran on another tracer");
+    if (rays != nullptr && hd.mesh_gen != h->mesh_gen)
+        return fail(TN_ERR_STATE, "tn_render_train_backward_saved_rays: tn_load_tetrahedra ran since the forward (the ray gradients read "
+                                  "the mesh positions)");
     TrainBufs b{};
     saved_layout(hd.R, hd.S2, (uint8_t *)d_saved, &b);
     return train_backward_impl(h, b, hd.R, hd.S2, hd.det != 0, hd.bg, d_grad_rgb, d_grad_acc, use_gradient_scaling, d_grad_field,
-                               d_grad_params12, s);
+                               d_grad_params12, s, rays);
+}
+
+extern "C" int tn_render_train_backward_saved(tn_tracer *h, const void *d_saved, const float *d_grad_rgb, const float *d_grad_acc,
+                                              int use_gradient_scaling, float *d_grad_field, float *const *d_grad_params12, void *stream) {
+    return backward_saved(h, d_saved, d_grad_rgb, d_grad_acc, use_gradient_scaling, d_grad_field, d_grad_params12, nullptr, stream);
+}
+
+// tn_render_train_backward_saved plus the gradients at the ray origins / directions of the forward, f32[R,3] each (either may be NULL;
+// 0 on empty rays); DESIGN.md §4.8
+extern "C" int tn_render_train_backward_saved_rays(tn_tracer *h, const void *d_saved, const float *d_grad_rgb, const float *d_grad_acc,
+                                                   int use_gradient_scaling, float *d_grad_field, float *const *d_grad_params12,
+                                                   float *d_grad_origins, float *d_grad_directions, void *stream) {
+    const RayGradOut rays{d_grad_origins, d_grad_directions};
+    return backward_saved(h, d_saved, d_grad_rgb, d_grad_acc, use_gradient_scaling, d_grad_field, d_grad_params12, &rays, stream);
 }
 
 // deterministic mode of the fused training step (see the header): applies from the next tn_render_train_forward on
@@ -1301,5 +1359,13 @@ extern "C" int tn_render_debug_buffers(tn_tracer *h, void **ptrs16) {
 extern "C" int tn_render_debug_normals_grad(tn_tracer *h, void **ptr) {
     if (!h || !h->render || !h->render->grad_n) return fail(TN_ERR_STATE, "no normals render");
     *ptr = h->render->grad_n;
+    return TN_OK;
+}
+
+// test hook: device pointer of dL/dx per fine sample of the last tn_render_train_backward_saved_rays call, float4 (x, y, z, 0) per sample
+// in the slot order of that call's forward (0 for unmatched samples and flat tetrahedra)
+extern "C" int tn_render_debug_ray_grads(tn_tracer *h, void **ptr) {
+    if (!h || !h->render || !h->render->ray_gx) return fail(TN_ERR_STATE, "no backward with ray gradients");
+    *ptr = h->render->ray_gx;
     return TN_OK;
 }

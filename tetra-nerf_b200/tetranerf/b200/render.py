@@ -132,8 +132,8 @@ class FusedRenderer:
                 out["rgb"].data_ptr(), out["accumulation"].data_ptr(), out["depth"].data_ptr(), out["ray_mask"].data_ptr()]
         return R, out, args
 
-    def _train_backward(self, entry, lead, grad_rgb, grad_acc, num_vertices, use_gradient_scaling):
-        """runs a training backward, entry(*lead, grads in, gradients out, stream) -> (grad_field, {name: gradient})"""
+    def _train_backward(self, entry, lead, grad_rgb, grad_acc, num_vertices, use_gradient_scaling, tail=()):
+        """runs a training backward, entry(*lead, grads in, gradients out, *tail, stream) -> (grad_field, {name: gradient})"""
         grad_rgb = grad_rgb.contiguous()
         if grad_acc is not None:
             grad_acc = grad_acc.contiguous()
@@ -141,7 +141,7 @@ class FusedRenderer:
         gps = [torch.empty(sh, dtype=torch.float32, device=self.device) for sh in _SHAPES]
         arr = (_vp * 12)(*[t.data_ptr() for t in gps])
         ext._check(entry(*lead, grad_rgb.data_ptr(), grad_acc.data_ptr() if grad_acc is not None else None, int(use_gradient_scaling),
-                         gfield.data_ptr(), arr, self._stream()))
+                         gfield.data_ptr(), arr, *tail, self._stream()))
         return gfield, dict(zip(PARAM_ORDER, gps))
 
     def train_forward(self, origins: torch.Tensor, directions: torch.Tensor, settings: RenderSettings, jitter_coarse: Optional[torch.Tensor] = None,
@@ -175,14 +175,24 @@ class FusedRenderer:
         return out, TrainState(blob, R)
 
     def train_backward_saved(self, state: "TrainState", grad_rgb: torch.Tensor, grad_acc: Optional[torch.Tensor], num_vertices: int,
-                             use_gradient_scaling: bool = False):
+                             use_gradient_scaling: bool = False, grad_origins: bool = False, grad_directions: bool = False):
         """backward of the train_forward_saved call that returned `state`; outputs as train_backward.  Raises RuntimeError if
-        set_field / set_weights ran since that forward.  Waits until the stream has reached it (it reads the call's shape back)."""
+        set_field / set_weights ran since that forward.  Waits until the stream has reached it (it reads the call's shape back).
+        grad_origins / grad_directions: also the gradients at the forward's ray origins / directions (the sample distances held fixed;
+        DESIGN §4.8) -> (grad_field, grads, grad_origins f32[R,3] or None, grad_directions f32[R,3] or None), 0 on empty rays; then it
+        also raises RuntimeError if load_tetrahedra ran since that forward."""
         if tuple(grad_rgb.shape) != (state.R, 3) or (grad_acc is not None and grad_acc.numel() != state.R):
             raise RuntimeError(f"the forward rendered {state.R} rays: grad_rgb must be [{state.R}, 3] and grad_acc [{state.R}], got "
                                f"{tuple(grad_rgb.shape)} and {None if grad_acc is None else tuple(grad_acc.shape)}")
-        return self._train_backward(_lib.tn_render_train_backward_saved, [self.tracer.handle, state.blob.data_ptr()], grad_rgb, grad_acc,
-                                    num_vertices, use_gradient_scaling)
+        lead = [self.tracer.handle, state.blob.data_ptr()]
+        if not (grad_origins or grad_directions):
+            return self._train_backward(_lib.tn_render_train_backward_saved, lead, grad_rgb, grad_acc, num_vertices, use_gradient_scaling)
+        go = torch.empty((state.R, 3), dtype=torch.float32, device=self.device) if grad_origins else None
+        gd = torch.empty((state.R, 3), dtype=torch.float32, device=self.device) if grad_directions else None
+        tail = (go.data_ptr() if go is not None else None, gd.data_ptr() if gd is not None else None)
+        gfield, gp = self._train_backward(_lib.tn_render_train_backward_saved_rays, lead, grad_rgb, grad_acc, num_vertices,
+                                          use_gradient_scaling, tail)
+        return gfield, gp, go, gd
 
     # ---- surface extraction ---------------------------------------------------------------------------------------------------------
     def extract_surface(self, level: float) -> Dict[str, torch.Tensor]:
@@ -238,6 +248,12 @@ class FusedRenderer:
         ext._check(_lib.tn_render_debug_normals_grad(self.tracer.handle, C.byref(ptr)))
         return ptr.value
 
+    def debug_ray_grads(self) -> int:
+        """test hook: device pointer of dL/dx per fine sample (float4 per sample, slot order) of the last backward with ray gradients"""
+        ptr = _vp()
+        ext._check(_lib.tn_render_debug_ray_grads(self.tracer.handle, C.byref(ptr)))
+        return ptr.value
+
     def debug_buffers(self):
         arr = (_vp * 16)()
         ext._check(_lib.tn_render_debug_buffers(self.tracer.handle, arr))
@@ -248,7 +264,9 @@ class FusedRenderer:
 
 class FusedTrainRender(torch.autograd.Function):
     """TetrahedraNerf.get_outputs in training mode as ONE differentiable op: forward = tn_render_train_forward_saved, backward =
-    tn_render_train_backward_saved (gradients for `tetrahedra_field` and the twelve MLP parameters; none for rays or jitter).
+    tn_render_train_backward_saved (gradients for `tetrahedra_field` and the twelve MLP parameters; none for the jitter).  When
+    `origins` / `directions` require grad, the backward also returns their gradients (tn_render_train_backward_saved_rays, DESIGN §4.8:
+    the sample distances held fixed, as nerfstudio's samplers feed a camera optimizer), so a pose correction upstream of the rays learns.
     The renderer must already hold the current field / weights (FusedRenderer.set_field / set_weights).  Every call keeps its own
     saved state (~115 MB at 8192 rays x 257 fine samples, freed with the graph), so calls compose like any autograd op: several
     forwards before one backward, other renders in between, retain_graph.  A backward after an in-place change of the field or a
@@ -258,6 +276,7 @@ class FusedTrainRender(torch.autograd.Function):
     def forward(ctx, fr, settings, use_gradient_scaling, origins, directions, jitter_coarse, jitter_fine, field, *params):
         out, state = fr.train_forward_saved(origins, directions, settings, jitter_coarse, jitter_fine)
         ctx.fr, ctx.state, ctx.gs = fr, state, bool(use_gradient_scaling)
+        ctx.ray_shapes = (origins.shape, directions.shape)
         ctx.save_for_backward(field, *params)  # their version counters reject a backward after an in-place change
         ctx.mark_non_differentiable(out["depth"], out["ray_mask"])
         return out["rgb"], out["accumulation"], out["depth"], out["ray_mask"]
@@ -267,5 +286,14 @@ class FusedTrainRender(torch.autograd.Function):
         field = ctx.saved_tensors[0]
         if g_rgb is None:
             g_rgb = torch.zeros((ctx.state.R, 3), dtype=torch.float32, device=field.device)
-        gfield, gp = ctx.fr.train_backward_saved(ctx.state, g_rgb, g_acc.reshape(-1) if g_acc is not None else None, field.shape[1], ctx.gs)
-        return (None, None, None, None, None, None, None, gfield) + tuple(gp[n] for n in PARAM_ORDER)
+        want_o, want_d = ctx.needs_input_grad[3], ctx.needs_input_grad[4]
+        g_acc = g_acc.reshape(-1) if g_acc is not None else None
+        go = gd = None
+        if want_o or want_d:
+            gfield, gp, go, gd = ctx.fr.train_backward_saved(ctx.state, g_rgb, g_acc, field.shape[1], ctx.gs, grad_origins=want_o,
+                                                             grad_directions=want_d)
+            go = go.reshape(ctx.ray_shapes[0]) if go is not None else None
+            gd = gd.reshape(ctx.ray_shapes[1]) if gd is not None else None
+        else:
+            gfield, gp = ctx.fr.train_backward_saved(ctx.state, g_rgb, g_acc, field.shape[1], ctx.gs)
+        return (None, None, None, go, gd, None, None, gfield) + tuple(gp[n] for n in PARAM_ORDER)
