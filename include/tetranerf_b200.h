@@ -41,6 +41,18 @@ int tn_synchronize(tn_tracer *h, void *stream);
  * Returns TN_ERR_MESH "A triangle is shared by more than two tetrahedra!" like :64-66.
  * Synchronous (the face table is sized on the host). */
 int tn_load_tetrahedra(tn_tracer *h, const float *d_xyz, uint32_t V, const uint32_t *d_cells, uint32_t T, void *stream);
+/* Moves the loaded mesh's vertices to d_xyz f32[V,3] (same V, same cells; borrowed like load_tetrahedra's) and refits the tracer in
+ * place: the positions in the leaf and walk records, the boxes of both BVHs (the load's Morton order is kept) and the coordinate bound.
+ * Every trace afterwards gives the same bits as the all-hits gather of a fresh tn_load_tetrahedra at d_xyz (the reference's algorithm
+ * on any triangle soup), and while the walk stays on, the same bits as its walk.  (A fresh load has no fold test: on a folded mesh it may
+ * still take the walk, whose results there are not covered by this guarantee.)  The adjacency walk stays on iff the mesh was
+ * walkable at load, its hull is still convex and no interior face is folded: *folded_faces (may be NULL) receives the number of interior
+ * faces whose two opposite vertices are not certified (float64 orient3d on the fp32 positions, with a forward error bound) to lie strictly
+ * on opposite sides; *walkable (may be NULL) whether the walk is on.  Otherwise every trace takes the all-hits gather.  TN_ERR_ARG if V
+ * differs from the load's or a coordinate is not finite (the tracer is then unchanged).  Like tn_load_tetrahedra, it starts a new mesh
+ * generation: a pending ray / vertex gradient backward returns TN_ERR_STATE and tn_surface_copy refuses an earlier extraction.
+ * Synchronous (one small read-back).  DESIGN.md §4.9. */
+int tn_update_vertices(tn_tracer *h, const float *d_xyz, uint32_t V, uint32_t *folded_faces, int *walkable, void *stream);
 int tn_num_faces(tn_tracer *h, uint32_t *F);
 /* copies out the unique-face tables in reference numbering: d_tri u32[F,3], d_tt u32[F,2]
  * (triangle_indices / triangle_tetrahedra of src/optix_types.h:4-5) */
@@ -170,6 +182,15 @@ int tn_render_train_backward_saved(tn_tracer *h, const void *d_saved, const floa
 int tn_render_train_backward_saved_rays(tn_tracer *h, const void *d_saved, const float *d_grad_rgb, const float *d_grad_acc,
                                         int use_gradient_scaling, float *d_grad_field, float *const *d_grad_params12, float *d_grad_origins,
                                         float *d_grad_directions, void *stream);
+/* tn_render_train_backward_saved_rays plus the gradient at the mesh vertex positions d_grad_xyz f32[V,3] (any of the three outputs may be
+ * NULL; every element of a non-NULL one is written).  The sample distances and the matched tetrahedra are held fixed; a fine sample's
+ * weights b = E^-1 (x - x_v0) move with the vertices: dL/dx_vj += -b_j dL/dx (b_0 = 1 - b_1 - b_2 - b_3), the vertex half of the
+ * reference's add_barycentrics_grad.  Default mode: float reductions; deterministic mode: per-vertex sums in a fixed order, bitwise
+ * reproducible.  The other outputs are those of tn_render_train_backward_saved_rays.  TN_ERR_STATE if tn_load_tetrahedra or
+ * tn_update_vertices ran since the forward.  DESIGN.md §4.9. */
+int tn_render_train_backward_saved_geometry(tn_tracer *h, const void *d_saved, const float *d_grad_rgb, const float *d_grad_acc,
+                                            int use_gradient_scaling, float *d_grad_field, float *const *d_grad_params12, float *d_grad_origins,
+                                            float *d_grad_directions, float *d_grad_xyz, void *stream);
 /* Deterministic mode of the fused training step (enable != 0; initial value: 1 if the environment variable TETRANERF_B200_DETERMINISTIC
  * is 1, else 0).  Read by tn_render_train_forward; tn_render_train_backward continues in the mode of the forward it belongs to.  With
  * identical inputs, on the same build and GPU model, forward outputs and every gradient are then bitwise identical from run to run and
@@ -239,7 +260,7 @@ int tn_render_debug_buffers(tn_tracer *h, void **ptrs16);
 /* device pointer of the per-sample density gradient of the last tn_render_normals call: float4 (x, y, z, 0) per sample, in the
  * slot order of the pass that gives the colours (vi_f / bary_f; vi_c / bary_c when num_fine_samples = 0) */
 int tn_render_debug_normals_grad(tn_tracer *h, void **ptr);
-/* device pointer of dL/dx per fine sample of the last tn_render_train_backward_saved_rays call: float4 (x, y, z, 0) per sample, in the
+/* device pointer of dL/dx per fine sample of the last tn_render_train_backward_saved_rays / _geometry call: float4 (x, y, z, 0) per sample, in the
  * slot order of its forward (0 for unmatched samples and flat tetrahedra) */
 int tn_render_debug_ray_grads(tn_tracer *h, void **ptr);
 /* one 128x128 tile out = A[128,K] * W[128,K]^T through the wgmma bf16x3 path (A from registers); K in {64,128}; synchronous */

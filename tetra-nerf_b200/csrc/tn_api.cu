@@ -62,6 +62,7 @@ int tn_destroy(tn_tracer *h) {
     cudaFree(h->d_flags);
     cudaFree(h->d_ovf_list);
     cudaFree(h->d_walk_keys);
+    cudaFree(h->d_refit);
     delete h;
     return TN_OK;
 }
@@ -85,6 +86,13 @@ int tn_load_tetrahedra(tn_tracer *h, const float *d_xyz, uint32_t V, const uint3
     tn::DeviceGuard g(h->device);
     h->mesh_gen = tn::next_generation();  // any earlier surface extraction is stale from here on, even if the build fails
     return tn::build_mesh(h, d_xyz, V, d_cells, T, (cudaStream_t)stream);
+}
+
+int tn_update_vertices(tn_tracer *h, const float *d_xyz, uint32_t V, uint32_t *folded_faces, int *walkable, void *stream) {
+    if (!h) return tn::fail(TN_ERR_ARG, "null tracer");
+    if (!d_xyz) return tn::fail(TN_ERR_ARG, "update_vertices: null pointer");
+    tn::DeviceGuard g(h->device);
+    return tn::refit_mesh(h, d_xyz, V, (cudaStream_t)stream, folded_faces, walkable);
 }
 
 int tn_num_faces(tn_tracer *h, uint32_t *F) {

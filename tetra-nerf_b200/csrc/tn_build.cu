@@ -182,10 +182,62 @@ __global__ void k_level(const float4 *__restrict__ child, uint32_t nchild, float
     parent[2 * (size_t)i + 1] = make_float4(hi[1], hi[2], 0.f, 0.f);
 }
 
+// ---- refit (tn_update_vertices): the position fields of the records, rewritten in place --------------------------------------------
+__global__ void k_nonfinite(const float *__restrict__ xyz, uint32_t n, uint32_t *__restrict__ flag) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n && !isfinite(xyz[i])) atomicOr(flag, 1u);
+}
+// sorted position p -> leaf record positions + level-0 node (the face bits in .w are topological and stay); the boxes as k_leaves.
+// Nothing is written while *bad is set (non-finite input): k_level then recomputes the unchanged boxes, so the tracer stays as it was.
+__global__ void k_refit_leaves(const float *__restrict__ xyz, const uint4 *__restrict__ cells, const uint32_t *__restrict__ order, uint32_t T,
+                               const uint32_t *__restrict__ bad, LeafRec *__restrict__ leaves, float4 *__restrict__ nodes0) {
+    const uint32_t p = blockIdx.x * blockDim.x + threadIdx.x;
+    if (p >= T || *bad) return;
+    const uint4 c = cells[order[p]];
+    const uint32_t id[4] = {c.x, c.y, c.z, c.w};
+    float lo[3] = {3e38f, 3e38f, 3e38f}, hi[3] = {-3e38f, -3e38f, -3e38f};
+    LeafRec rec = leaves[p];
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+        const float x = xyz[3 * (size_t)id[k]], y = xyz[3 * (size_t)id[k] + 1], z = xyz[3 * (size_t)id[k] + 2];
+        rec.v[k] = make_float4(x, y, z, rec.v[k].w);
+        lo[0] = fminf(lo[0], x); hi[0] = fmaxf(hi[0], x);
+        lo[1] = fminf(lo[1], y); hi[1] = fmaxf(hi[1], y);
+        lo[2] = fminf(lo[2], z); hi[2] = fmaxf(hi[2], z);
+    }
+    leaves[p] = rec;
+    nodes0[2 * (size_t)p] = make_float4(lo[0], lo[1], lo[2], hi[0]);
+    nodes0[2 * (size_t)p + 1] = make_float4(hi[1], hi[2], 0.f, 0.f);
+}
+// WalkRec v[k].xyz of tetrahedron i (nbr, vid, map, wind, perm and the face bits are topological and stay); nothing while *bad is set
+__global__ void k_refit_walk(const float *__restrict__ xyz, const uint4 *__restrict__ cells, uint32_t T, const uint32_t *__restrict__ bad,
+                             WalkRec *__restrict__ walk) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= T || *bad) return;
+    const uint4 c = cells[i];
+    const uint32_t id[4] = {c.x, c.y, c.z, c.w};
+    float4 *v = walk[i].v;
+#pragma unroll
+    for (int k = 0; k < 4; ++k)
+        v[k] = make_float4(xyz[3 * (size_t)id[k]], xyz[3 * (size_t)id[k] + 1], xyz[3 * (size_t)id[k] + 2], v[k].w);
+}
+
+static float absmax_of(const int *hbounds) {  // max |coordinate| from the ordered-int bounds of k_bounds
+    float amax = 0.f;
+    for (int a = 0; a < 6; ++a) {
+        int i = hbounds[a];
+        i = i >= 0 ? i : i ^ 0x7FFFFFFF;
+        float f;
+        memcpy(&f, &i, 4);
+        amax = std::max(amax, std::fabs(f));
+    }
+    return amax;
+}
+
 void free_mesh(tn_tracer *h) {
     Mesh &m = h->mesh;
     cudaFree(m.tri); cudaFree(m.tt); cudaFree(m.nodes); cudaFree(m.leaves); cudaFree(m.leaf_tet);
-    cudaFree(m.walk); cudaFree(m.hull_nodes); cudaFree(m.hull_leaves); cudaFree(m.hull_tet);
+    cudaFree(m.walk); cudaFree(m.hull_nodes); cudaFree(m.hull_leaves); cudaFree(m.hull_tet); cudaFree(m.hull_ekey); cudaFree(m.hull_eface);
     m = Mesh();
 }
 
@@ -206,6 +258,7 @@ int build_mesh(tn_tracer *h, const float *d_xyz, uint32_t V, const uint32_t *d_c
     const uint32_t F = ft.F, H = ft.H;
     const bool walkable = ft.walkable;
     m.tri = reinterpret_cast<uint32_t *>(ft.tri); m.tt = reinterpret_cast<uint32_t *>(ft.tt);  // owned by the mesh from here on (free_mesh)
+    m.hull_ekey = ft.hull_ekey; m.hull_eface = ft.hull_eface; m.hull_ne = ft.hull_ne;
     uint4 *d_tet_faces = ft.tet_faces;
     uint4 *d_nbr = ft.nbr;
     uint32_t *d_wind = ft.wind, *d_hull_list = ft.hull_list;
@@ -298,18 +351,60 @@ int build_mesh(tn_tracer *h, const float *d_xyz, uint32_t V, const uint32_t *d_c
     int hbounds[6];
     TN_CUDA_B(cudaMemcpyAsync(hbounds, bounds, sizeof(hbounds), cudaMemcpyDeviceToHost, s));
     TN_CUDA_B(cudaStreamSynchronize(s));
-    float amax = 0.f;
-    for (int a = 0; a < 6; ++a) {
-        int i = hbounds[a];
-        i = i >= 0 ? i : i ^ 0x7FFFFFFF;
-        float f;
-        memcpy(&f, &i, 4);
-        amax = std::max(amax, std::fabs(f));
-    }
+    const float amax = absmax_of(hbounds);
     cleanup();
 #undef TN_CUDA_B
     m.xyz = d_xyz; m.cells = d_cells; m.V = V; m.T = T; m.F = F; m.lv = lv; m.absmax = amax;
     m.walkable = walkable; m.H = walkable ? H : 0; m.hull_lv = hlv;
+    return TN_OK;
+}
+
+// Moves the vertices of the loaded mesh to d_xyz and rewrites every position-dependent field in place (same cells, same Morton order):
+// leaf records and level-0 boxes of both BVHs, the upper levels by k_level, the walk records, absmax; then the hull convexity test on the
+// load's hull edges and the fold test.  The non-finite check runs first on the device and the record kernels skip their writes when it
+// fires, so non-finite input leaves the tracer unchanged with a single read-back at the end.
+int refit_mesh(tn_tracer *h, const float *d_xyz, uint32_t V, cudaStream_t s, uint32_t *folded_faces, int *walkable) {
+    Mesh &m = h->mesh;
+    if (!m.nodes) return fail(TN_ERR_STATE, "update_vertices: no tetrahedra loaded");
+    if (V != m.V) return fail(TN_ERR_ARG, "update_vertices: " + std::to_string(V) + " vertices, the loaded mesh has " + std::to_string(m.V));
+    if (!h->d_refit) TN_CUDA(cudaMalloc(&h->d_refit, 64));
+    uint32_t *d_small = h->d_refit;  // [0] non-finite flag, [2] hull error bits, [3] folded faces, [4..9] bounds (ordered ints)
+    int *bounds = reinterpret_cast<int *>(d_small + 4);
+    // ordered-int encodings (f2ord) of +FLT_MAX for the min slots and -FLT_MAX for the max slots, after four zeroed words
+    const int init[10] = {0, 0, 0, 0, 0x7F7FFFFF, 0x7F7FFFFF, 0x7F7FFFFF, (int)0x80800000, (int)0x80800000, (int)0x80800000};
+    TN_CUDA(cudaMemcpyAsync(d_small, init, sizeof(init), cudaMemcpyHostToDevice, s));
+    const uint32_t n = 3 * V;
+    k_nonfinite<<<(n + 255) / 256, 256, 0, s>>>(d_xyz, n, d_small);
+    k_bounds<<<std::min<uint32_t>((V + 255) / 256, 1184u), 256, 0, s>>>(d_xyz, V, bounds);
+    const uint32_t T = m.T;
+    k_refit_leaves<<<(T + 255) / 256, 256, 0, s>>>(d_xyz, (const uint4 *)m.cells, m.leaf_tet, T, d_small, m.leaves, m.nodes);
+    for (int l = 1; l < m.lv.nlevels; ++l)
+        k_level<<<(m.lv.count[l] + 127) / 128, 128, 0, s>>>(m.nodes + 2 * (size_t)m.lv.offset[l - 1], m.lv.count[l - 1],
+                                                             m.nodes + 2 * (size_t)m.lv.offset[l], m.lv.count[l]);
+    h->launches += 3 + (m.lv.nlevels - 1);
+    if (m.walk) {
+        k_refit_walk<<<(T + 127) / 128, 128, 0, s>>>(d_xyz, (const uint4 *)m.cells, T, d_small, m.walk);
+        const uint32_t H = m.hull_lv.count[0];
+        k_refit_leaves<<<(H + 255) / 256, 256, 0, s>>>(d_xyz, (const uint4 *)m.cells, m.hull_tet, H, d_small, m.hull_leaves, m.hull_nodes);
+        for (int l = 1; l < m.hull_lv.nlevels; ++l)
+            k_level<<<(m.hull_lv.count[l] + 127) / 128, 128, 0, s>>>(m.hull_nodes + 2 * (size_t)m.hull_lv.offset[l - 1], m.hull_lv.count[l - 1],
+                                                                      m.hull_nodes + 2 * (size_t)m.hull_lv.offset[l], m.hull_lv.count[l]);
+        h->launches += 2 + (m.hull_lv.nlevels - 1);
+    }
+    int rc = launch_refit_checks(h, d_xyz, d_small + 2, s);
+    if (rc) return rc;
+    h->launches += 2;
+    uint32_t hs[10];
+    TN_CUDA(cudaMemcpyAsync(hs, d_small, sizeof(hs), cudaMemcpyDeviceToHost, s));
+    TN_CUDA(cudaStreamSynchronize(s));
+    TN_CUDA(cudaGetLastError());
+    if (hs[0]) return fail(TN_ERR_ARG, "update_vertices: a vertex coordinate is not finite");
+    h->mesh_gen = next_generation();  // the positions changed
+    m.xyz = d_xyz;
+    m.absmax = absmax_of(reinterpret_cast<const int *>(hs + 4));
+    m.walkable = m.walk != nullptr && (hs[2] & 4u) == 0 && hs[3] == 0;
+    if (folded_faces) *folded_faces = hs[3];
+    if (walkable) *walkable = m.walkable ? 1 : 0;
     return TN_OK;
 }
 

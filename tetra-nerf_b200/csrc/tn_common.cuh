@@ -86,7 +86,12 @@ struct Mesh {
     uint32_t *hull_tet = nullptr;    // [H] sorted position -> tetrahedron id
     BvhLevels hull_lv{};
     uint32_t H = 0;
-    bool walkable = false;           // conforming mesh with a convex hull (always true for a Delaunay triangulation)
+    bool walkable = false;           // conforming mesh with a convex hull (always true for a Delaunay triangulation), and after a
+                                     // refit (tn_update_vertices) still convex and unfolded
+    // hull edges of a mesh that was walkable at load (walk != nullptr), sorted by (a, b): what the convexity test of a refit reads
+    unsigned long long *hull_ekey = nullptr;  // [hull_ne] (a << 32 | b), a < b
+    uint32_t *hull_eface = nullptr;           // [hull_ne] the hull face of each edge entry
+    uint32_t hull_ne = 0;
     BvhLevels lv{};
     float absmax = 0.f;              // max |coordinate| over the vertices
 };
@@ -116,7 +121,8 @@ struct tn_tracer {
     uint32_t walk_quad_min_rays = 3584, walk_quad_max_rays = 0xFFFFFFFFu;
     uint32_t walk_quad_spec_max_rays = 65536;  // quad walk: batches up to this size load the candidate next records speculatively (tn_walk.cu)
     uint64_t launches = 0;
-    uint64_t mesh_gen = 0;  // a fresh next_generation() on every tn_load_tetrahedra (a surface extraction records it)
+    uint64_t mesh_gen = 0;  // a fresh next_generation() on every tn_load_tetrahedra / tn_update_vertices (a surface extraction records it)
+    uint32_t *d_refit = nullptr;  // 64 bytes of tn_update_vertices scratch: flags, counts and bounds, read back once per refit
     tn::RenderState *render = nullptr;
     tn::SurfaceState *surface = nullptr;
 };
@@ -133,8 +139,16 @@ struct FaceTables {
     uint32_t *hull_list = nullptr;  // [H] tetrahedra owning a hull face, ascending
     uint32_t F = 0, H = 0;
     bool walkable = false;       // the hull is a closed convex surface
+    unsigned long long *hull_ekey = nullptr;  // walkable: the sorted hull edges (Mesh::hull_ekey / hull_eface), owned by the caller
+    uint32_t *hull_eface = nullptr;
+    uint32_t hull_ne = 0;
 };
 int build_faces_device(const float *d_xyz, uint32_t V, const uint32_t *d_cells, uint32_t T, cudaStream_t s, FaceTables &out, int *launches);
+// position-dependent tests of a refit (tn_faces.cu), on the loaded mesh's kept tables at positions d_xyz; stream-ordered.
+// d_counts[0] |= 4 if the hull is not convex (the load's test, on its sorted hull edges); d_counts[1] += number of folded interior faces
+int launch_refit_checks(const tn_tracer *h, const float *d_xyz, uint32_t *d_counts, cudaStream_t s);
+// tn_update_vertices (tn_build.cu)
+int refit_mesh(tn_tracer *h, const float *d_xyz, uint32_t V, cudaStream_t s, uint32_t *folded_faces, int *walkable);
 void free_mesh(tn_tracer *h);
 void free_render(tn_tracer *h);
 void free_surface(tn_tracer *h);
@@ -182,6 +196,18 @@ struct RayGradsLaunch {
     float *grad_o, *grad_d;               // out: [R,3] each, or nullptr
 };
 int launch_ray_grads(const RayGradsLaunch &a, cudaStream_t s);
+// gradient of a training step at the mesh vertex positions (tn_vertex_grads.cu), launched after k_ray_grads on its per-sample dL/dx
+struct VertexGradsLaunch {
+    const uint32_t *n_active;             // active rays
+    uint32_t S, R, V;                     // fine samples per ray, rays of the forward, mesh vertices
+    const uint4 *vi;                      // [n_active*S] matched vertex ids
+    const float *bary;                    // [n_active*S,3] their weights on v1..v3
+    const float4 *gx;                     // [n_active*S] dL/dx per sample (k_ray_grads)
+    const uint32_t *keys, *vals;          // deterministic mode: the (vertex, row * 4 + k) pairs stably sorted by vertex, n of them;
+    uint32_t n;                           //   nullptr = default mode (float reductions)
+    float *grad_xyz;                      // out: [V,3]
+};
+int launch_vertex_grads(const VertexGradsLaunch &a, cudaStream_t s);
 int launch_walk(tn_tracer *h, const float *o, const float *d, uint32_t R, uint32_t M, uint32_t *num, uint32_t *cells, float *bary,
                 float *dist, uint32_t *verts, unsigned long long *keys, uint32_t *list, uint32_t *list_count, int kind, cudaStream_t s);
 int launch_tail_fill(tn_tracer *h, uint32_t R, uint32_t M, const uint32_t *num, uint32_t *cells, float *bary, float *dist, uint32_t *verts,

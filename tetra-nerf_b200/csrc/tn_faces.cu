@@ -172,6 +172,58 @@ __global__ void k_iota(uint32_t *__restrict__ v, uint32_t n) {
     if (i < n) v[i] = i;
 }
 
+// ---- fold test of a refit: for every interior face (a, b, c), the opposite vertices p, q of its two tetrahedra must lie strictly on
+// opposite sides of its plane.  orient3d(a, b, c, x) = det[a - x; b - x; c - x] in float64 on the fp32 positions, with every operation
+// rounded individually (no FMA contraction, the op order of oracle/vertex_grads.py's restatement) and Shewchuk's forward error bound
+// (7 + 56 eps) eps * permanent, eps = 2^-53: a sign the bound cannot certify counts as folded, so rounding can only turn the walk off.
+__device__ __forceinline__ bool orient3d_sign(const float *__restrict__ xyz, uint32_t ia, uint32_t ib, uint32_t ic, uint32_t ix, int &sign) {
+    auto P = [&](uint32_t v, int a) { return (double)__ldg(xyz + 3 * (size_t)v + a); };
+    const double adx = __dsub_rn(P(ia, 0), P(ix, 0)), ady = __dsub_rn(P(ia, 1), P(ix, 1)), adz = __dsub_rn(P(ia, 2), P(ix, 2));
+    const double bdx = __dsub_rn(P(ib, 0), P(ix, 0)), bdy = __dsub_rn(P(ib, 1), P(ix, 1)), bdz = __dsub_rn(P(ib, 2), P(ix, 2));
+    const double cdx = __dsub_rn(P(ic, 0), P(ix, 0)), cdy = __dsub_rn(P(ic, 1), P(ix, 1)), cdz = __dsub_rn(P(ic, 2), P(ix, 2));
+    const double bdxcdy = __dmul_rn(bdx, cdy), cdxbdy = __dmul_rn(cdx, bdy);
+    const double cdxady = __dmul_rn(cdx, ady), adxcdy = __dmul_rn(adx, cdy);
+    const double adxbdy = __dmul_rn(adx, bdy), bdxady = __dmul_rn(bdx, ady);
+    const double det = __dadd_rn(__dadd_rn(__dmul_rn(adz, __dsub_rn(bdxcdy, cdxbdy)), __dmul_rn(bdz, __dsub_rn(cdxady, adxcdy))),
+                                 __dmul_rn(cdz, __dsub_rn(adxbdy, bdxady)));
+    const double perm = __dadd_rn(__dadd_rn(__dmul_rn(__dadd_rn(fabs(bdxcdy), fabs(cdxbdy)), fabs(adz)),
+                                            __dmul_rn(__dadd_rn(fabs(cdxady), fabs(adxcdy)), fabs(bdz))),
+                                  __dmul_rn(__dadd_rn(fabs(adxbdy), fabs(bdxady)), fabs(cdz)));
+    const double eps = 1.1102230246251565e-16;  // 2^-53
+    const double bound = __dmul_rn(__dmul_rn(__dadd_rn(7.0, __dmul_rn(56.0, eps)), eps), perm);
+    sign = det > bound ? 1 : (-det > bound ? -1 : 0);
+    return sign != 0;
+}
+__device__ __forceinline__ uint32_t opposite_vertex(const uint4 c, const uint4 f) {
+    const uint32_t cv[4] = {c.x, c.y, c.z, c.w};
+    uint32_t o = cv[0];
+    for (int q = 0; q < 4; ++q)
+        if (cv[q] != f.x && cv[q] != f.y && cv[q] != f.z) o = cv[q];
+    return o;
+}
+__global__ void k_fold_faces(const float *__restrict__ xyz, const uint4 *__restrict__ cells, const uint4 *__restrict__ tri, const uint2 *__restrict__ tt,
+                             uint32_t F, uint32_t *__restrict__ folded) {
+    const uint32_t f = blockIdx.x * blockDim.x + threadIdx.x;
+    if (f >= F) return;
+    const uint2 o = tt[f];
+    if (o.y == TN_EMPTY) return;
+    const uint4 t = tri[f];
+    int sp = 0, sq = 0;
+    const bool cp = orient3d_sign(xyz, t.x, t.y, t.z, opposite_vertex(cells[o.x], t), sp);
+    const bool cq = orient3d_sign(xyz, t.x, t.y, t.z, opposite_vertex(cells[o.y], t), sq);
+    if (!(cp && cq && sp == -sq)) atomicAdd(folded, 1u);
+}
+
+int launch_refit_checks(const tn_tracer *h, const float *d_xyz, uint32_t *d_counts, cudaStream_t s) {
+    const Mesh &m = h->mesh;
+    if (m.hull_ne > 0)
+        k_hull_check<<<(m.hull_ne + 255) / 256, 256, 0, s>>>(d_xyz, (const uint4 *)m.cells, (const uint4 *)m.tri, (const uint2 *)m.tt, m.hull_ekey,
+                                                            m.hull_eface, m.hull_ne, d_counts);
+    k_fold_faces<<<(m.F + 255) / 256, 256, 0, s>>>(d_xyz, (const uint4 *)m.cells, (const uint4 *)m.tri, (const uint2 *)m.tt, m.F, d_counts + 1);
+    TN_CUDA(cudaGetLastError());
+    return TN_OK;
+}
+
 // Builds the face / adjacency tables of the mesh on the device.  On success the arrays of `out` are allocated (owned by the
 // caller: tri, tt go into the Mesh; tet_faces, nbr, wind, hull_list are build-time temporaries).
 int build_faces_device(const float *d_xyz, uint32_t V, const uint32_t *d_cells, uint32_t T, cudaStream_t s, FaceTables &out, int *launches) {
@@ -188,6 +240,7 @@ int build_faces_device(const float *d_xyz, uint32_t V, const uint32_t *d_cells, 
     auto fail_free = [&](int code, const std::string &msg) {
         cleanup();
         cudaFree(out.tri); cudaFree(out.tt); cudaFree(out.tet_faces); cudaFree(out.nbr); cudaFree(out.wind); cudaFree(out.hull_list);
+        cudaFree(out.hull_ekey); cudaFree(out.hull_eface);
         out = FaceTables();
         return fail(code, msg);
     };
@@ -259,6 +312,12 @@ int build_faces_device(const float *d_xyz, uint32_t V, const uint32_t *d_cells, 
         TN_CUDA_F(cudaStreamSynchronize(s));
         walkable = (h_small[0] & 4u) == 0;
         if (launches) *launches += 2;
+        if (walkable) {  // kept for the convexity test of a refit (tn_update_vertices)
+            TN_CUDA_F(cudaMalloc(&out.hull_ekey, 8 * (size_t)ne)); TN_CUDA_F(cudaMalloc(&out.hull_eface, 4 * (size_t)ne));
+            TN_CUDA_F(cudaMemcpyAsync(out.hull_ekey, kab2, 8 * (size_t)ne, cudaMemcpyDeviceToDevice, s));
+            TN_CUDA_F(cudaMemcpyAsync(out.hull_eface, eface2, 4 * (size_t)ne, cudaMemcpyDeviceToDevice, s));
+            out.hull_ne = ne;
+        }
     }
     out.walkable = walkable;
     if (launches) *launches += 8;

@@ -1079,9 +1079,10 @@ extern "C" int tn_render_train_forward(tn_tracer *h, const tn_render_config *cfg
 // parameter gradients (same order / layouts as tn_render_set_weights); every output element is written.  Reads `b` and the field /
 // weights; writes only the tracer's gradient scratch.  The coarse pass carries no gradient (PDFSampler detaches its bins).  No
 // [samples,128] tensor touches HBM.
-// rays != nullptr: also the gradients at the ray origins / directions (tn_ray_grads.cu); either output may be null
+// rays != nullptr: also the gradients at the ray origins / directions (tn_ray_grads.cu) and at the mesh vertex positions
+// (tn_vertex_grads.cu); any of the three outputs may be null
 struct RayGradOut {
-    float *grad_o, *grad_d;
+    float *grad_o, *grad_d, *grad_xyz;
 };
 static int train_backward_impl(tn_tracer *h, const TrainBufs &b, uint32_t R, uint32_t S2, bool det, const float *bg, const float *d_grad_rgb,
                                const float *d_grad_acc, int use_gradient_scaling, float *d_grad_field, float *const *d_grad_params12, cudaStream_t s,
@@ -1172,6 +1173,9 @@ static int train_backward_impl(tn_tracer *h, const TrainBufs &b, uint32_t R, uin
         k_det_field_grad<<<(uint32_t)(((uint64_t)V * 32 + 255) / 256), 256, 0, s>>>(V, n, k1, v1, b.bary_f, r->det_dx, r->gshadow);
         h->launches += 9;
     }
+    const uint32_t *sorted_keys = nullptr, *sorted_vals = nullptr;  // deterministic mode: the field gradient's sorted pairs
+    const uint32_t npairs = (uint32_t)(4 * (uint64_t)R * S2);
+    if (det) { sorted_keys = r->det_keys + npairs; sorted_vals = r->det_vals + npairs; }
     GradOut go{};
     for (int i = 0; i < 12; ++i) {
         if (!d_grad_params12[i]) return fail(TN_ERR_ARG, "tn_render_train_backward: null parameter gradient pointer");
@@ -1182,9 +1186,17 @@ static int train_backward_impl(tn_tracer *h, const TrainBufs &b, uint32_t R, uin
         rl.n_active = b.n_active; rl.ray_list = b.ray_list; rl.S = S2; rl.R = R; rl.ebins = b.ebins_f; rl.vi = b.vi_f;
         rl.dx = det ? r->det_dx : r->ray_dx; rl.fshadow = r->fshadow; rl.xyz = h->mesh.xyz; rl.enc = b.enc; rl.g_dirbias = r->g_dirbias;
         rl.w4dir = r->w4dir; rl.gx = r->ray_gx; rl.grad_o = rays->grad_o; rl.grad_d = rays->grad_d;
-        const int rc = launch_ray_grads(rl, s);
+        int rc = launch_ray_grads(rl, s);
         if (rc) return rc;
         h->launches += 1;
+        if (rays->grad_xyz != nullptr) {  // after the per-sample dL/dx is complete
+            VertexGradsLaunch vl{};
+            vl.n_active = b.n_active; vl.S = S2; vl.R = R; vl.V = h->mesh.V; vl.vi = b.vi_f; vl.bary = b.bary_f; vl.gx = r->ray_gx;
+            vl.keys = sorted_keys; vl.vals = sorted_vals; vl.n = npairs; vl.grad_xyz = rays->grad_xyz;
+            rc = launch_vertex_grads(vl, s);
+            if (rc) return rc;
+            h->launches += 1;
+        }
     }
     k_scatter_grads<<<(128 * 155 + 255) / 256, 256, 0, s>>>(r->gw, go);
     k_transpose_v64<<<(V + 31) / 32, dim3(32, 8), 0, s>>>(r->gshadow, d_grad_field, V);
@@ -1264,8 +1276,8 @@ static int backward_saved(tn_tracer *h, const void *d_saved, const float *d_grad
         return fail(TN_ERR_STATE, "tn_render_train_backward_saved: the field or the weights changed (tn_render_set_field / "
                                   "tn_render_set_weights) since the forward, or the forward ran on another tracer");
     if (rays != nullptr && hd.mesh_gen != h->mesh_gen)
-        return fail(TN_ERR_STATE, "tn_render_train_backward_saved_rays: tn_load_tetrahedra ran since the forward (the ray gradients read "
-                                  "the mesh positions)");
+        return fail(TN_ERR_STATE, "tn_render_train_backward_saved_geometry: tn_load_tetrahedra or tn_update_vertices ran since the forward "
+                                  "(the ray and vertex gradients read the mesh positions)");
     TrainBufs b{};
     saved_layout(hd.R, hd.S2, (uint8_t *)d_saved, &b);
     return train_backward_impl(h, b, hd.R, hd.S2, hd.det != 0, hd.bg, d_grad_rgb, d_grad_acc, use_gradient_scaling, d_grad_field,
@@ -1282,7 +1294,15 @@ extern "C" int tn_render_train_backward_saved(tn_tracer *h, const void *d_saved,
 extern "C" int tn_render_train_backward_saved_rays(tn_tracer *h, const void *d_saved, const float *d_grad_rgb, const float *d_grad_acc,
                                                    int use_gradient_scaling, float *d_grad_field, float *const *d_grad_params12,
                                                    float *d_grad_origins, float *d_grad_directions, void *stream) {
-    const RayGradOut rays{d_grad_origins, d_grad_directions};
+    return tn_render_train_backward_saved_geometry(h, d_saved, d_grad_rgb, d_grad_acc, use_gradient_scaling, d_grad_field, d_grad_params12,
+                                                   d_grad_origins, d_grad_directions, nullptr, stream);
+}
+
+// ... plus the gradient at the mesh vertex positions, f32[V,3] (NULL = none); DESIGN.md §4.9
+extern "C" int tn_render_train_backward_saved_geometry(tn_tracer *h, const void *d_saved, const float *d_grad_rgb, const float *d_grad_acc,
+                                                       int use_gradient_scaling, float *d_grad_field, float *const *d_grad_params12,
+                                                       float *d_grad_origins, float *d_grad_directions, float *d_grad_xyz, void *stream) {
+    const RayGradOut rays{d_grad_origins, d_grad_directions, d_grad_xyz};
     return backward_saved(h, d_saved, d_grad_rgb, d_grad_acc, use_gradient_scaling, d_grad_field, d_grad_params12, &rays, stream);
 }
 
@@ -1362,7 +1382,7 @@ extern "C" int tn_render_debug_normals_grad(tn_tracer *h, void **ptr) {
     return TN_OK;
 }
 
-// test hook: device pointer of dL/dx per fine sample of the last tn_render_train_backward_saved_rays call, float4 (x, y, z, 0) per sample
+// test hook: device pointer of dL/dx per fine sample of the last tn_render_train_backward_saved_rays / _geometry call, float4 (x, y, z, 0) per sample
 // in the slot order of that call's forward (0 for unmatched samples and flat tetrahedra)
 extern "C" int tn_render_debug_ray_grads(tn_tracer *h, void **ptr) {
     if (!h || !h->render || !h->render->ray_gx) return fail(TN_ERR_STATE, "no backward with ray gradients");

@@ -175,24 +175,28 @@ class FusedRenderer:
         return out, TrainState(blob, R)
 
     def train_backward_saved(self, state: "TrainState", grad_rgb: torch.Tensor, grad_acc: Optional[torch.Tensor], num_vertices: int,
-                             use_gradient_scaling: bool = False, grad_origins: bool = False, grad_directions: bool = False):
+                             use_gradient_scaling: bool = False, grad_origins: bool = False, grad_directions: bool = False,
+                             grad_vertices: bool = False):
         """backward of the train_forward_saved call that returned `state`; outputs as train_backward.  Raises RuntimeError if
         set_field / set_weights ran since that forward.  Waits until the stream has reached it (it reads the call's shape back).
         grad_origins / grad_directions: also the gradients at the forward's ray origins / directions (the sample distances held fixed;
         DESIGN §4.8) -> (grad_field, grads, grad_origins f32[R,3] or None, grad_directions f32[R,3] or None), 0 on empty rays; then it
-        also raises RuntimeError if load_tetrahedra ran since that forward."""
+        also raises RuntimeError if load_tetrahedra ran since that forward.  grad_vertices: also the gradient at the mesh vertex positions
+        (the matched tetrahedra held fixed as well; DESIGN §4.9) -> (grad_field, grads, grad_origins or None, grad_directions or None,
+        grad_vertices f32[V,3]); then it raises RuntimeError if load_tetrahedra or update_vertices ran since that forward."""
         if tuple(grad_rgb.shape) != (state.R, 3) or (grad_acc is not None and grad_acc.numel() != state.R):
             raise RuntimeError(f"the forward rendered {state.R} rays: grad_rgb must be [{state.R}, 3] and grad_acc [{state.R}], got "
                                f"{tuple(grad_rgb.shape)} and {None if grad_acc is None else tuple(grad_acc.shape)}")
         lead = [self.tracer.handle, state.blob.data_ptr()]
-        if not (grad_origins or grad_directions):
+        if not (grad_origins or grad_directions or grad_vertices):
             return self._train_backward(_lib.tn_render_train_backward_saved, lead, grad_rgb, grad_acc, num_vertices, use_gradient_scaling)
         go = torch.empty((state.R, 3), dtype=torch.float32, device=self.device) if grad_origins else None
         gd = torch.empty((state.R, 3), dtype=torch.float32, device=self.device) if grad_directions else None
-        tail = (go.data_ptr() if go is not None else None, gd.data_ptr() if gd is not None else None)
-        gfield, gp = self._train_backward(_lib.tn_render_train_backward_saved_rays, lead, grad_rgb, grad_acc, num_vertices,
+        gv = torch.empty((num_vertices, 3), dtype=torch.float32, device=self.device) if grad_vertices else None
+        tail = tuple(t.data_ptr() if t is not None else None for t in (go, gd, gv))
+        gfield, gp = self._train_backward(_lib.tn_render_train_backward_saved_geometry, lead, grad_rgb, grad_acc, num_vertices,
                                           use_gradient_scaling, tail)
-        return gfield, gp, go, gd
+        return (gfield, gp, go, gd, gv) if grad_vertices else (gfield, gp, go, gd)
 
     # ---- surface extraction ---------------------------------------------------------------------------------------------------------
     def extract_surface(self, level: float) -> Dict[str, torch.Tensor]:
@@ -270,10 +274,25 @@ class FusedTrainRender(torch.autograd.Function):
     The renderer must already hold the current field / weights (FusedRenderer.set_field / set_weights).  Every call keeps its own
     saved state (~115 MB at 8192 rays x 257 fine samples, freed with the graph), so calls compose like any autograd op: several
     forwards before one backward, other renders in between, retain_graph.  A backward after an in-place change of the field or a
-    parameter, or after set_field / set_weights on the renderer, raises RuntimeError."""
+    parameter, or after set_field / set_weights on the renderer, raises RuntimeError.
+
+    An optional 13th tensor after the twelve parameters is the mesh's vertex positions f32[V,3], the very tensor the tracer borrowed
+    (load_tetrahedra / update_vertices); when it requires grad the backward returns its gradient too (DESIGN §4.9: the sample distances
+    and the matched tetrahedra held fixed), so an optimizer can move the points.  It raises if the tensor changed in place since the
+    tracer was loaded or refit (the trace would be stale), and an in-place change of it before the backward raises, as for the field."""
 
     @staticmethod
     def forward(ctx, fr, settings, use_gradient_scaling, origins, directions, jitter_coarse, jitter_fine, field, *params):
+        if len(params) == len(PARAM_ORDER) + 1:
+            xyz, borrowed = params[-1], fr.tracer._vertices
+            if borrowed is None or xyz.data_ptr() != borrowed.data_ptr() or xyz.shape != borrowed.shape:
+                raise RuntimeError("FusedTrainRender: the vertex positions must be the tensor the tracer borrowed (load_tetrahedra / "
+                                   "update_vertices), with the same number of vertices")
+            if xyz._version != fr.tracer._vertices_version:  # (a detached view shares the parameter's version counter)
+                raise RuntimeError("FusedTrainRender: the vertex positions changed in place since the tracer was loaded or refit; call "
+                                   "update_vertices first")
+        elif len(params) != len(PARAM_ORDER):
+            raise RuntimeError(f"FusedTrainRender takes the {len(PARAM_ORDER)} MLP parameters and optionally the vertex positions")
         out, state = fr.train_forward_saved(origins, directions, settings, jitter_coarse, jitter_fine)
         ctx.fr, ctx.state, ctx.gs = fr, state, bool(use_gradient_scaling)
         ctx.ray_shapes = (origins.shape, directions.shape)
@@ -287,13 +306,18 @@ class FusedTrainRender(torch.autograd.Function):
         if g_rgb is None:
             g_rgb = torch.zeros((ctx.state.R, 3), dtype=torch.float32, device=field.device)
         want_o, want_d = ctx.needs_input_grad[3], ctx.needs_input_grad[4]
+        has_xyz = len(ctx.needs_input_grad) == 8 + len(PARAM_ORDER) + 1
+        want_v = has_xyz and ctx.needs_input_grad[-1]
         g_acc = g_acc.reshape(-1) if g_acc is not None else None
-        go = gd = None
-        if want_o or want_d:
+        go = gd = gv = None
+        if want_v:
+            gfield, gp, go, gd, gv = ctx.fr.train_backward_saved(ctx.state, g_rgb, g_acc, field.shape[1], ctx.gs, grad_origins=want_o,
+                                                                 grad_directions=want_d, grad_vertices=True)
+        elif want_o or want_d:
             gfield, gp, go, gd = ctx.fr.train_backward_saved(ctx.state, g_rgb, g_acc, field.shape[1], ctx.gs, grad_origins=want_o,
                                                              grad_directions=want_d)
-            go = go.reshape(ctx.ray_shapes[0]) if go is not None else None
-            gd = gd.reshape(ctx.ray_shapes[1]) if gd is not None else None
         else:
             gfield, gp = ctx.fr.train_backward_saved(ctx.state, g_rgb, g_acc, field.shape[1], ctx.gs)
-        return (None, None, None, go, gd, None, None, gfield) + tuple(gp[n] for n in PARAM_ORDER)
+        go = go.reshape(ctx.ray_shapes[0]) if go is not None else None
+        gd = gd.reshape(ctx.ray_shapes[1]) if gd is not None else None
+        return (None, None, None, go, gd, None, None, gfield) + tuple(gp[n] for n in PARAM_ORDER) + ((gv,) if has_xyz else ())

@@ -21,6 +21,7 @@ from __future__ import annotations
 
 import dataclasses
 import os
+import warnings
 from dataclasses import dataclass
 from pathlib import Path
 from typing import Any, Dict, List, Literal, Optional
@@ -74,6 +75,9 @@ class TetrahedraNerfConfig(ModelConfig):
     use_occupancy_field: bool = False
     render_normals: bool = False
     """eval renders also return "normals" f32[R,3], the composited normal of the density field (fused path only; training ignores it)"""
+    optimize_vertices: bool = False
+    """train the mesh vertex positions too: `tetrahedra_vertices` becomes a parameter in its own param group "vertices" (same state-dict
+    key and shape), the tracer is refit after every optimizer step (topology fixed), training runs on the fused path only (DESIGN §4.9)"""
 
     def __post_init__(self):
         if self.tetrahedra_path is not None and self.num_tetrahedra_vertices is None:
@@ -165,7 +169,7 @@ class TetrahedraNerf(Model):
             if self.config.num_tetrahedra_vertices is None or self.config.num_tetrahedra_cells is None:
                 raise RuntimeError("The tetrahedra_path must be specified.")
             V, T = self.config.num_tetrahedra_vertices, self.config.num_tetrahedra_cells
-            self.register_buffer("tetrahedra_vertices", torch.empty((V, 3), dtype=torch.float32))
+            self._register_vertices(torch.empty((V, 3), dtype=torch.float32))
             self.register_buffer("tetrahedra_cells", torch.empty((T, 4), dtype=torch.int32))
             self.register_parameter("tetrahedra_field", nn.Parameter(torch.empty((self.config.field_dim, V), dtype=torch.float32)))
             self._tetrahedra_initialized = False
@@ -181,14 +185,22 @@ class TetrahedraNerf(Model):
         if complete:
             self._tetrahedra_initialized = True
 
+    def _register_vertices(self, vertices: torch.Tensor):
+        """`tetrahedra_vertices`: a buffer, or with optimize_vertices a parameter (the same state-dict key either way)"""
+        if self.config.optimize_vertices:
+            self.register_parameter("tetrahedra_vertices", nn.Parameter(vertices))
+        else:
+            self.register_buffer("tetrahedra_vertices", vertices)
+
     def _install_mesh(self, vertices: torch.Tensor, cells: torch.Tensor, colors: Optional[torch.Tensor], alpha: Optional[torch.Tensor]):
         V = len(vertices)
         self.config.num_tetrahedra_vertices, self.config.num_tetrahedra_cells = V, len(cells)
         if hasattr(self, "tetrahedra_vertices"):
-            self.tetrahedra_vertices.copy_(vertices.to(self.tetrahedra_vertices.device))
+            with torch.no_grad():
+                self.tetrahedra_vertices.copy_(vertices.to(self.tetrahedra_vertices.device))
             self.tetrahedra_cells.copy_(cells.to(torch.int32).to(self.tetrahedra_cells.device))
         else:
-            self.register_buffer("tetrahedra_vertices", vertices.float())
+            self._register_vertices(vertices.float())
             self.register_buffer("tetrahedra_cells", cells.to(torch.int32))
             self.register_parameter("tetrahedra_field", nn.Parameter(torch.empty((self.config.field_dim, V), dtype=torch.float32)))
         self._init_tetrahedra_field(self.tetrahedra_field.data)
@@ -225,11 +237,25 @@ class TetrahedraNerf(Model):
             raise RuntimeError("Tetrahedra tracer is only supported on a CUDA device")  # reference :396-397
         if self._tetrahedra_tracer is not None and self._tetrahedra_tracer.device != device:
             self._tetrahedra_tracer = self._fused = self._fused_versions = None
+        xyz = self.tetrahedra_vertices.detach()
+        if self._tetrahedra_tracer is not None and self.config.optimize_vertices:
+            ptr, V, version = self._tracer_vertices
+            if (xyz.data_ptr(), len(xyz)) != (ptr, V):  # another tensor: a fresh load
+                self._tetrahedra_tracer.load_tetrahedra(xyz, self.tetrahedra_cells)
+            elif self.tetrahedra_vertices._version != version:  # moved in place (an optimizer step): refit, same topology
+                folded, _ = self._tetrahedra_tracer.update_vertices(xyz)
+                if folded and not self._fold_warned:
+                    warnings.warn(f"optimize_vertices: {folded} mesh faces are folded; tracing continues on the all-hits gather (exact, slower)")
+                    self._fold_warned = True
+            self._tracer_vertices = (xyz.data_ptr(), len(xyz), self.tetrahedra_vertices._version)
         if self._tetrahedra_tracer is None:
             if not self._tetrahedra_initialized:
                 self._init_tetrahedra()
+            xyz = self.tetrahedra_vertices.detach()
             self._tetrahedra_tracer = TetrahedraTracer(device)
-            self._tetrahedra_tracer.load_tetrahedra(self.tetrahedra_vertices, self.tetrahedra_cells)
+            self._tetrahedra_tracer.load_tetrahedra(xyz, self.tetrahedra_cells)
+            self._tracer_vertices = (xyz.data_ptr(), len(xyz), self.tetrahedra_vertices._version)
+            self._fold_warned = False
         return self._tetrahedra_tracer
 
     # ---- modules (reference :409-477) ----------------------------------------------------------------
@@ -263,7 +289,9 @@ class TetrahedraNerf(Model):
         self.rgb_loss = MSELoss()
 
     def get_param_groups(self) -> Dict[str, List[Parameter]]:
-        return {"fields": list(self.parameters())}
+        if not self.config.optimize_vertices:
+            return {"fields": list(self.parameters())}
+        return {"fields": [p for n, p in self.named_parameters() if n != "tetrahedra_vertices"], "vertices": [self.tetrahedra_vertices]}
 
     def get_background_color(self, shape, device):
         return self.renderer_rgb.get_background_color(self.renderer_rgb.background_color, shape, device)
@@ -310,8 +338,13 @@ class TetrahedraNerf(Model):
                                 self.config.use_biased_sampler, float(self.collider.far_plane), bg)
             with torch.no_grad():
                 return self._fused_renderer().render(origins, directions, st, normals=normals)
-        if self.training and torch.is_grad_enabled() and self._fused_supported() and self.config.num_fine_samples > 0 \
-                and os.environ.get("TETRANERF_B200_UNFUSED_TRAIN", "0") != "1":
+        unfused_train = os.environ.get("TETRANERF_B200_UNFUSED_TRAIN", "0") == "1"
+        if self.training and torch.is_grad_enabled() and self.config.optimize_vertices:
+            causes = self._fused_unsupported() + (["num_fine_samples=0"] if self.config.num_fine_samples == 0 else []) \
+                + (["TETRANERF_B200_UNFUSED_TRAIN=1"] if unfused_train else [])
+            if causes:
+                raise RuntimeError(f"optimize_vertices trains on the fused CUDA pipeline, which does not support {', '.join(causes)}")
+        if self.training and torch.is_grad_enabled() and self._fused_supported() and self.config.num_fine_samples > 0 and not unfused_train:
             return self._get_outputs_fused_train(origins, directions)
         return self._get_outputs_unfused(ray_bundle, origins, directions)
 
@@ -328,8 +361,9 @@ class TetrahedraNerf(Model):
         jc = torch.rand((R, c.num_samples + 1), dtype=torch.float32, device=dev) if getattr(self.sampler_uniform, "train_stratified", True) else None
         jf = torch.rand((R, c.num_fine_samples + 1), dtype=torch.float32, device=dev) if getattr(self.sampler_pdf, "train_stratified", True) else None
         named = dict(self.named_parameters())
+        xyz = (self.tetrahedra_vertices,) if c.optimize_vertices else ()  # the tensor the tracer borrowed (get_tetrahedra_tracer)
         rgb, acc, depth, mask = FusedTrainRender.apply(fr, st, c.use_gradient_scaling, origins, directions, jc, jf, self.tetrahedra_field,
-                                                       *[named[n] for n in PARAM_ORDER])
+                                                       *[named[n] for n in PARAM_ORDER], *xyz)
         return {"rgb": rgb, "accumulation": acc, "depth": depth, "ray_mask": mask}
 
     def _field_at(self, tracer, traced, ray_mask, distances):

@@ -32,7 +32,11 @@ def _trainer(name: str, model: TetrahedraNerfConfig) -> TrainerConfig:
         ),
         max_num_iterations=300000, steps_per_save=25000, steps_per_eval_batch=1000, steps_per_eval_image=2000, steps_per_eval_all_images=50000,
         optimizers={"fields": {"optimizer": RAdamOptimizerConfig(lr=0.001),
-                               "scheduler": ExponentialDecaySchedulerConfig(lr_final=0.0001, max_steps=300_000)}},
+                               "scheduler": ExponentialDecaySchedulerConfig(lr_final=0.0001, max_steps=300_000)},
+                    # the param group of TetrahedraNerfConfig.optimize_vertices; nerfstudio's Optimizers builds one optimizer per param
+                    # group the model returns, so this entry is inert while the option is off.  The rate is a placeholder, not tuned.
+                    "vertices": {"optimizer": RAdamOptimizerConfig(lr=1e-5),
+                                 "scheduler": ExponentialDecaySchedulerConfig(lr_final=1e-6, max_steps=300_000)}},
     )
 
 

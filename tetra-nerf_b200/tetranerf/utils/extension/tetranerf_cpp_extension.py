@@ -29,6 +29,7 @@ _lib.tn_create.argtypes = [_i, C.POINTER(_vp)]
 _lib.tn_destroy.argtypes = [_vp]
 _lib.tn_synchronize.argtypes = [_vp, _vp]
 _lib.tn_load_tetrahedra.argtypes = [_vp, _vp, _u32, _vp, _u32, _vp]
+_lib.tn_update_vertices.argtypes = [_vp, _vp, _u32, C.POINTER(_u32), C.POINTER(_i), _vp]
 _lib.tn_num_faces.argtypes = [_vp, C.POINTER(_u32)]
 _lib.tn_get_faces.argtypes = [_vp, _vp, _vp, _vp]
 _lib.tn_trace_rays.argtypes = [_vp, _vp, _vp, _u32, _u32, _vp, _vp, _vp, _vp, _vp, _i, _vp]
@@ -65,6 +66,7 @@ _lib.tn_render_train_saved_bytes.argtypes = [_vp, C.POINTER(_Cfg), _u32, C.POINT
 _lib.tn_render_train_forward_saved.argtypes = [_vp, C.POINTER(_Cfg), _vp, _vp, _u32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, C.c_size_t, _vp]
 _lib.tn_render_train_backward_saved.argtypes = [_vp, _vp, _vp, _vp, _i, _vp, C.POINTER(_vp), _vp]
 _lib.tn_render_train_backward_saved_rays.argtypes = [_vp, _vp, _vp, _vp, _i, _vp, C.POINTER(_vp), _vp, _vp, _vp]
+_lib.tn_render_train_backward_saved_geometry.argtypes = [_vp, _vp, _vp, _vp, _i, _vp, C.POINTER(_vp), _vp, _vp, _vp, _vp]
 _lib.tn_render_debug_buffers.argtypes = [_vp, C.POINTER(_vp)]
 _lib.tn_render_set_profiling.argtypes = [_vp, _i]
 _lib.tn_render_set_mlp_precision.argtypes = [_vp, _i]
@@ -115,6 +117,7 @@ class TetrahedraTracer:
         self._device = device
         self._h = _vp()
         self._vertices = None
+        self._vertices_version = None
         self._cells = None
         _check(_lib.tn_create(device.index, C.byref(self._h)))
 
@@ -155,9 +158,24 @@ class TetrahedraTracer:
         _require(cells.size(-1) == 4, "indices must have last dimension with size 4")
         _require(cells.dtype == torch.int32, "indices must have int32 type")
         self._cells, self._vertices = cells, xyz  # borrowed by the tracer: keep them alive (:154-155)
+        self._vertices_version = xyz._version  # the positions the tracer holds (FusedTrainRender rejects a stale tracer)
         with torch.cuda.device(self._device):
             _check(_lib.tn_load_tetrahedra(self._h, xyz.data_ptr(), xyz.numel() // 3, cells.data_ptr(), cells.numel() // 4,
                                            _stream(self._device)))
+
+    def update_vertices(self, xyz: torch.Tensor):
+        """moves the loaded mesh's vertices to `xyz` f32[V,3] (same V; borrowed like load_tetrahedra's) and refits the tracer in place:
+        every trace afterwards equals one after a fresh load_tetrahedra(xyz, cells).  -> (folded_faces, walkable): the number of interior
+        faces that are folded or not certified unfolded, and whether the adjacency walk stays on (otherwise every trace takes the
+        all-hits gather).  Raises RuntimeError on a different V or a non-finite coordinate (the tracer is then unchanged).  Waits until the
+        stream has reached it.  DESIGN §4.9"""
+        self._check_float_dim3(xyz, "xyz")
+        _require(self._cells is not None, "load_tetrahedra must be called first")
+        folded, walkable = _u32(0), _i(0)
+        with torch.cuda.device(self._device):
+            _check(_lib.tn_update_vertices(self._h, xyz.data_ptr(), xyz.numel() // 3, C.byref(folded), C.byref(walkable), _stream(self._device)))
+        self._vertices, self._vertices_version = xyz, xyz._version
+        return int(folded.value), bool(walkable.value)
 
     def num_faces(self) -> int:
         n = _u32(0)
