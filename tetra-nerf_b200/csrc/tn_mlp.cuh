@@ -39,10 +39,13 @@ constexpr uint32_t MLP_THREADS = 128 * MLP_WGS;
 constexpr uint32_t MLP_TILE = 64;                          // samples per tile
 constexpr uint32_t MLP_W_BYTES = 32768 + 3 * 65536;        // weight image: L1 32K | L2 64K | L3 64K | L4 (base part) 64K
 constexpr uint32_t MLP_W_COARSE = 32768 + 2 * 65536;       // the coarse pass stops after L3
-constexpr uint32_t MLP_OFF_HEAD = MLP_W_BYTES;             // wd[128] wc[3][128] bd bc[3]
-constexpr uint32_t MLP_OFF_BARS = MLP_OFF_HEAD + 520 * 4;  // weight barrier, then the per-warpgroup tile slots [MLP_WGS][2]
-constexpr uint32_t MLP_SMEM_BYTES = MLP_OFF_BARS + 8 + 8 * MLP_WGS;
-static_assert(MLP_SMEM_BYTES <= 232448, "k_mlp shared memory exceeds 227 KB");
+// shared memory of one pass: its own weight bytes, then wd[128] wc[3][128] bd bc[3], the weight barrier and the per-warpgroup
+// tile slots [MLP_WGS][2].  The coarse pass asks for only what it uses (162 KB), which leaves its SM ~92 KB of L1 for the
+// gathered field rows instead of the fine pass's ~28 KB.
+__host__ __device__ constexpr uint32_t mlp_off_head(bool fine) { return fine ? MLP_W_BYTES : MLP_W_COARSE; }
+__host__ __device__ constexpr uint32_t mlp_off_bars(bool fine) { return mlp_off_head(fine) + 520 * 4; }
+__host__ __device__ constexpr uint32_t mlp_smem_bytes(bool fine) { return mlp_off_bars(fine) + 8 + 8 * MLP_WGS; }
+static_assert(mlp_smem_bytes(true) <= 232448, "k_mlp shared memory exceeds 227 KB");
 __host__ __device__ constexpr uint32_t mlp_off_layer(int l) { return l == 0 ? 0u : 32768u + 65536u * (uint32_t)(l - 1); }
 
 struct MlpParams {
@@ -68,6 +71,12 @@ __device__ __forceinline__ float sigmoid_f(float x) { return 1.0f / (1.0f + expf
 __device__ __forceinline__ float2 ldg_stream2(const float *p) {
     float2 v;
     asm volatile("ld.global.nc.L1::no_allocate.v2.f32 {%0, %1}, [%2];" : "=f"(v.x), "=f"(v.y) : "l"(p));
+    return v;
+}
+// 8-byte read-only load that allocates in L1
+__device__ __forceinline__ float2 ldg_l1_2(const float *p) {
+    float2 v;
+    asm volatile("ld.global.nc.v2.f32 {%0, %1}, [%2];" : "=f"(v.x), "=f"(v.y) : "l"(p));
     return v;
 }
 // 16-byte variant
@@ -126,7 +135,10 @@ __device__ __forceinline__ void prefetch_gather_rows(const uint4 *vi, const floa
 // All 64 field loads of the two rows are issued before the first one is consumed, so a thread has its whole gather in flight at
 // once instead of one L2 round trip per column pair.  The loads are unconditional: an unmatched row reads vertex 0's features and
 // its result is replaced by 0 (a branch around the loads would keep the compiler from hoisting them over the FMAs).
-template <int PREC>
+// L1_ROWS: the loads allocate in L1 (k_mlp).  Samples next to each other along a ray lie in the same or adjacent tetrahedra, so
+// most of a row's four vertices are among its neighbours' and the repeats of a field row, within a warp and across the warpgroups
+// of an SM, are served from L1 instead of L2.  Otherwise they stream past L1 (k_mlp_bwd, k_mlp_normals).
+template <int PREC, bool L1_ROWS = false>
 __device__ __forceinline__ void gather_rows(const GatherRows &r, const float *__restrict__ fshadow, uint32_t t, uint32_t (&xh)[16], uint32_t (&xl)[16]) {
     float2 a[2][4][8];  // [row][vertex][column pair]
 #pragma unroll
@@ -137,7 +149,7 @@ __device__ __forceinline__ void gather_rows(const GatherRows &r, const float *__
         for (int k = 0; k < 4; ++k) {
             const float *f = fshadow + (size_t)vs[k] * 64 + 2 * t;
 #pragma unroll
-            for (int c = 0; c < 8; ++c) a[rr][k][c] = ldg_stream2(f + 8 * c);
+            for (int c = 0; c < 8; ++c) a[rr][k][c] = L1_ROWS ? ldg_l1_2(f + 8 * c) : ldg_stream2(f + 8 * c);
         }
     }
 #pragma unroll
@@ -185,14 +197,15 @@ __device__ __forceinline__ void layer_mma(float (&d)[64], const uint32_t (&ah)[4
     reg_fence(d);
 }
 
-template <bool FINE, int PREC>
+// L1_ROWS: the field gather allocates in L1 (the default, tn_set_mlp_gather); the results are bit-identical either way
+template <bool FINE, int PREC, bool L1_ROWS>
 __global__ void __launch_bounds__(MLP_THREADS, 1) k_mlp(const MlpParams p) {
     using namespace tc;
     extern __shared__ __align__(1024) uint8_t tn_mlp_smem[];
     uint8_t *smem = tn_mlp_smem;
-    const float *head_s = reinterpret_cast<const float *>(smem + MLP_OFF_HEAD);
-    uint64_t *w_bar = reinterpret_cast<uint64_t *>(smem + MLP_OFF_BARS);
-    volatile uint32_t *slots = reinterpret_cast<volatile uint32_t *>(smem + MLP_OFF_BARS + 8);  // [wg][2] tile of the next / this round
+    const float *head_s = reinterpret_cast<const float *>(smem + mlp_off_head(FINE));
+    uint64_t *w_bar = reinterpret_cast<uint64_t *>(smem + mlp_off_bars(FINE));
+    volatile uint32_t *slots = reinterpret_cast<volatile uint32_t *>(smem + mlp_off_bars(FINE) + 8);  // [wg][2] tile of the next / this round
 
     constexpr int L = FINE ? 4 : 3;
     constexpr uint32_t WBYTES = FINE ? MLP_W_BYTES : MLP_W_COARSE;
@@ -243,7 +256,7 @@ __global__ void __launch_bounds__(MLP_THREADS, 1) k_mlp(const MlpParams p) {
         uint32_t ah[32], al[32];
         {
             uint32_t xh[16], xl[16];
-            gather_rows<PREC>(load_gather_rows(p.vi, p.bary, row0, total_rows), p.fshadow, t, xh, xl);
+            gather_rows<PREC, L1_ROWS>(load_gather_rows(p.vi, p.bary, row0, total_rows), p.fshadow, t, xh, xl);
             // Into L1 while this tile's MMAs run: the next tile's indices, so its gather starts with the field loads, and (FINE) this
             // tile's bias rows of layer 4, read right after that layer's MMA wait.  Prefetches hold no registers: keeping the 14
             // index words of the next tile in registers instead spills k_mlp<true, 3> at its 168-register limit.
@@ -339,6 +352,15 @@ __global__ void __launch_bounds__(MLP_THREADS, 1) k_mlp(const MlpParams p) {
         tile = next;
     }
     if (!weights_ready) mbar_wait(w_bar, 0);  // a warpgroup without a tile still lets the weight copy land before the CTA exits
+}
+
+// launches one k_mlp pass with the shared memory of that pass; l1_rows selects the field gather (tn_set_mlp_gather)
+template <bool FINE, int PREC>
+inline int launch_mlp(const MlpParams &p, uint32_t grid, bool l1_rows, cudaStream_t s) {
+    auto k = l1_rows ? k_mlp<FINE, PREC, true> : k_mlp<FINE, PREC, false>;
+    TN_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)mlp_smem_bytes(FINE)));
+    k<<<grid, MLP_THREADS, mlp_smem_bytes(FINE), s>>>(p);
+    return TN_OK;
 }
 
 }  // namespace tn

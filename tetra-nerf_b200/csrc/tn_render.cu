@@ -970,10 +970,9 @@ static int render_impl(tn_tracer *h, const tn_render_config *cfg, const float *d
     TN_CUDA(cudaFuncSetAttribute(k_coarse_sample, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_sc));
     TN_CUDA(cudaFuncSetAttribute(k_sample_fine, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_sf));
     TN_CUDA(cudaFuncSetAttribute(k_composite, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_c));
-    auto k_coarse = prec == 2 ? k_mlp<false, 2> : k_mlp<false, 3>;
-    auto k_fine = prec == 2 ? k_mlp<true, 2> : k_mlp<true, 3>;
-    TN_CUDA(cudaFuncSetAttribute(k_coarse, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)MLP_SMEM_BYTES));
-    TN_CUDA(cudaFuncSetAttribute(k_fine, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)MLP_SMEM_BYTES));
+    auto launch_coarse = prec == 2 ? launch_mlp<false, 2> : launch_mlp<false, 3>;
+    auto launch_fine = prec == 2 ? launch_mlp<true, 2> : launch_mlp<true, 3>;
+    const bool l1_rows = h->mlp_gather == 1;
     const uint32_t gridR = (R + SAMPLE_WARPS - 1) / SAMPLE_WARPS;
 
     if (det) {
@@ -994,7 +993,10 @@ static int render_impl(tn_tracer *h, const tn_render_config *cfg, const float *d
     const uint64_t tiles_c = ((uint64_t)R * Sc + MLP_TILE - 1) / MLP_TILE, tiles_f = ((uint64_t)R * S2 + MLP_TILE - 1) / MLP_TILE;
     const uint32_t grid_c = (uint32_t)std::min<uint64_t>((tiles_c + MLP_WGS - 1) / MLP_WGS, (uint64_t)sms);
     const uint32_t grid_f = (uint32_t)std::min<uint64_t>((tiles_f + MLP_WGS - 1) / MLP_WGS, (uint64_t)sms);
-    if (!single) k_coarse<<<grid_c, MLP_THREADS, MLP_SMEM_BYTES, s>>>(mc);
+    if (!single) {
+        rc = launch_coarse(mc, grid_c, l1_rows, s);
+        if (rc) return rc;
+    }
     TN_EV(3);
     if (!single) k_sample_fine<<<gridR, SAMPLE_WARPS * 32, smem_sf, s>>>(p);
     else k_dirbias_only<<<gridR, SAMPLE_WARPS * 32, 0, s>>>(p);
@@ -1004,7 +1006,8 @@ static int render_impl(tn_tracer *h, const tn_render_config *cfg, const float *d
     if (!single) { mf.vi = b.vi_f; mf.bary = b.bary_f; }
     else p.ebins_f = r->ebins_c;  // k_composite integrates over the coarse bins
     mf.tile_ctr = b.n_active + 2;
-    k_fine<<<grid_f, MLP_THREADS, MLP_SMEM_BYTES, s>>>(mf);
+    rc = launch_fine(mf, grid_f, l1_rows, s);
+    if (rc) return rc;
     TN_EV(5);
     k_composite<<<gridR, SAMPLE_WARPS * 32, smem_c, s>>>(p);
     TN_EV(6);

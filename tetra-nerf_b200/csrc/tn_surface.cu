@@ -301,15 +301,13 @@ int run_mlp(tn_tracer *h, const RenderInputs &in, const uint32_t *d_count, uint6
             const float *dirbias, float *out, uint32_t *tile_ctr, cudaStream_t s) {
     int sms = 132;
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, h->device);
-    TN_CUDA(cudaFuncSetAttribute(k_mlp<FINE, 3>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)MLP_SMEM_BYTES));
     MlpParams p{};
     p.n_active = d_count; p.S = S; p.vi = vi; p.bary = bary; p.fshadow = in.fshadow; p.wimg = in.wimg; p.bias = in.bias;
     p.head = in.head; p.dirbias = dirbias; p.out = out; p.tile_ctr = tile_ctr;
     const uint64_t tiles = (rows + MLP_TILE - 1) / MLP_TILE;
     const uint32_t grid = (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>((tiles + MLP_WGS - 1) / MLP_WGS, (uint64_t)sms));
-    k_mlp<FINE, 3><<<grid, MLP_THREADS, MLP_SMEM_BYTES, s>>>(p);
     h->launches += 1;
-    return TN_OK;
+    return launch_mlp<FINE, 3>(p, grid, h->mlp_gather == 1, s);
 }
 
 uint32_t blocks(uint64_t n, uint32_t per) { return (uint32_t)((n + per - 1) / per); }
