@@ -238,19 +238,16 @@ int tn_render_get_timings(tn_tracer *h, float *ms6);
 int tn_render_get_backward_timings(tn_tracer *h, float *ms3);
 /* trace_rays picks between bit-identical implementations by batch size:
  * >= walk_min_rays (default 2^20): adjacency walk, 32 rays per warp (throughput);
- * solo range [lo, hi] below that (default empty): adjacency walk, one ray per warp with cooperating lanes;
+ * solo range [lo, hi] below that (default empty): adjacency walk, one ray per warp, 4 cooperating lanes (the quad walk's kernel
+ * with one quad per warp);
  * otherwise, for meshes that cannot be walked, and as the exact stage the walks fall back to: warp-per-ray all-hits BVH gather. */
 int tn_set_walk_min_rays(tn_tracer *h, uint32_t n);
 int tn_set_walk_solo_range(tn_tracer *h, uint32_t lo, uint32_t hi);
 /* [lo, hi] below walk_min_rays (checked before the solo range): adjacency walk with 8 rays per warp, 4 cooperating lanes per ray */
 int tn_set_walk_quad_range(tn_tracer *h, uint32_t lo, uint32_t hi);
-/* the quad walk of batches of up to n rays (default 65536) loads the records of all candidate next tetrahedra while the current one
- * is intersected instead of prefetching them (latency-bound regime); 0 = never.  Results are identical. */
+/* the quad and solo walks of batches of up to n rays (default 65536) load the records of all candidate next tetrahedra while the
+ * current one is intersected instead of prefetching them (latency-bound regime); 0 = never.  Results are identical. */
 int tn_set_walk_quad_spec_max_rays(tn_tracer *h, uint32_t n);
-/* field gather of the fused MLP passes (render, training forward, surface extraction); results are bit-identical either way.
- * 1 (default): the gathered field rows allocate in L1, so the rows that neighbouring samples share are mostly read from L2 once;
- * 0: they stream past L1.  The initial value of a new tracer is TETRANERF_B200_MLP_GATHER (read once), else 1. */
-int tn_set_mlp_gather(tn_tracer *h, int mode);
 /* test hook: number of CTAs of the backward MLP kernel of tn_render_train_backward (0 = default, one per SM) */
 int tn_render_set_backward_grid(tn_tracer *h, uint32_t ctas);
 /* out2[0] = 1 if the loaded mesh takes the adjacency-walk fast path (conforming, convex hull); out2[1] = rays of the last

@@ -43,17 +43,18 @@ def setup(V, C, field_kind="normal", prec=3, field=None, params=None):
 # per-sample error is relative to the activations (~4.9e-4 sigma, 1.8e-4 colour on a trained-NeRF-like network: tests/test_gpu_opaque.py,
 # DESIGN 4.2); its pixels stay within 1e-4 there too.
 @pytest.mark.parametrize("prec", [3, 2])
-@pytest.mark.parametrize("cfgname", ["tetra_nerf", "tetra_nerf_original", "small_uniform", "small_biased"])
+@pytest.mark.parametrize("cfgname", ["tetra_nerf", "tetra_nerf_original", "small_uniform", "small_biased", "tetra_nerf_cube"])
 @pytest.mark.parametrize("field_kind", ["normal", "init"])
-def test_fused_render_vs_oracle(small_mesh, cfgname, field_kind, prec):
+def test_fused_render_vs_oracle(small_mesh, cube_mesh, cfgname, field_kind, prec):
     from tetranerf.b200.render import RenderSettings
 
-    V, C = small_mesh
+    # tetra_nerf_cube: the 12-tetrahedra cube, so whole MLP tiles read the same few field rows
+    V, C = cube_mesh if cfgname == "tetra_nerf_cube" else small_mesh
     tr, fr, field, params = setup(V, C, field_kind, prec)
     o, d = syn.camera_rays(300)
     o[5] = [5, 5, 5]; d[5] = [1, 0, 0]       # empty ray
     o[17] = [0.5, 0.5, 0.5]                   # origin inside the mesh
-    if cfgname == "tetra_nerf":
+    if cfgname in ("tetra_nerf", "tetra_nerf_cube"):
         st, oc = RenderSettings.tetra_nerf(), orc.RenderConfig.tetra_nerf()
     elif cfgname == "tetra_nerf_original":
         st, oc = RenderSettings.tetra_nerf_original(), orc.RenderConfig.tetra_nerf_original()
@@ -79,6 +80,7 @@ def test_fused_render_vs_oracle(small_mesh, cfgname, field_kind, prec):
     inv[active] = torch.arange(n_act)
     order = inv[ray_list]  # row of the oracle's compacted arrays for each slot
     Sc, S2 = st.num_samples, st.num_samples + st.num_fine_samples + 1
+    assert (n_act * S2) % 64 != 0  # the fine pass ends in a partly filled 64-row MLP tile
     aux = ref["aux"]
     eb_c = _from_ptr(bufs["ebins_c"], (n_act, Sc + 1), torch.float32).cpu()
     torch.testing.assert_close(eb_c, aux["coarse_euclid"][order], rtol=2e-6, atol=2e-6)

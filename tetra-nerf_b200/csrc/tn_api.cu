@@ -42,8 +42,6 @@ int tn_create(int device, tn_tracer **out) {
                                          std::to_string(minor));
     tn_tracer *h = new tn_tracer();
     h->device = device;
-    static const int gather_env = [] { const char *e = getenv("TETRANERF_B200_MLP_GATHER"); return e ? atoi(e) : 1; }();  // A/B switch
-    h->mlp_gather = gather_env == 0 ? 0 : 1;
     cudaError_t e = cudaMalloc(&h->d_flags, sizeof(int) * 4);
     if (e == cudaSuccess) e = cudaMemset(h->d_flags, 0, sizeof(int) * 4);
     if (e != cudaSuccess) {
@@ -170,17 +168,10 @@ extern "C" int tn_set_walk_quad_range(tn_tracer *h, uint32_t lo, uint32_t hi) {
     h->walk_quad_max_rays = hi;
     return TN_OK;
 }
-// quad walk: batches of up to n rays load the records of all candidate next tetrahedra while the current one is intersected (0 = never)
+// quad and solo walks: batches of up to n rays load the records of all candidate next tetrahedra while the current one is intersected (0 = never)
 extern "C" int tn_set_walk_quad_spec_max_rays(tn_tracer *h, uint32_t n) {
     if (!h) return tn::fail(TN_ERR_ARG, "null tracer");
     h->walk_quad_spec_max_rays = n;
-    return TN_OK;
-}
-// field gather of the fused MLP passes: 1 = field rows cached in L1, 0 = streamed past it; results are identical
-extern "C" int tn_set_mlp_gather(tn_tracer *h, int mode) {
-    if (!h) return tn::fail(TN_ERR_ARG, "null tracer");
-    if (mode != 0 && mode != 1) return tn::fail(TN_ERR_ARG, "tn_set_mlp_gather: 0 (rows streamed past L1) or 1 (rows cached in L1)");
-    h->mlp_gather = mode;
     return TN_OK;
 }
 static uint32_t g_last_exact = 0;

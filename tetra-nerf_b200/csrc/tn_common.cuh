@@ -113,17 +113,13 @@ struct tn_tracer {
     //   warp-per-ray all-hits BVH gather   <- below walk_quad_min_rays (latency of the few rays in flight dominates)
     //   walk, 8 rays per warp ("quad")     <- [walk_quad_min_rays, walk_min_rays)  (speculative record loads up to walk_quad_spec_max_rays,
     //                                         prefetches above)
-    //   walk, 1 ray per warp ("solo")      (kept for tests / experiments: range empty by default)
+    //   walk, 1 ray per warp ("solo")      (the quad walk launched with one quad per warp; range empty by default, for tests)
     //   walk, 32 rays per warp             <- >= walk_min_rays (fewest instructions per ray: only pays off once the machine is full
     //                                         several times over)
     uint32_t walk_min_rays = 1u << 20;
     uint32_t walk_solo_min_rays = 1, walk_solo_max_rays = 0;
     uint32_t walk_quad_min_rays = 3584, walk_quad_max_rays = 0xFFFFFFFFu;
-    uint32_t walk_quad_spec_max_rays = 65536;  // quad walk: batches up to this size load the candidate next records speculatively (tn_walk.cu)
-    // field gather of the fused MLP passes (k_mlp, tn_mlp.cuh), bit-identical either way: 1 = the field rows allocate in L1, so
-    // rows that neighbouring samples share are read from L2 about once; 0 = they stream past L1.  Initial value:
-    // TETRANERF_B200_MLP_GATHER (default 1)
-    int mlp_gather = 1;
+    uint32_t walk_quad_spec_max_rays = 65536;  // quad and solo walks: batches up to this size load the candidate next records speculatively (tn_walk.cu)
     uint64_t launches = 0;
     uint64_t mesh_gen = 0;  // a fresh next_generation() on every tn_load_tetrahedra / tn_update_vertices (a surface extraction records it)
     uint32_t *d_refit = nullptr;  // 64 bytes of tn_update_vertices scratch: flags, counts and bounds, read back once per refit

@@ -135,10 +135,10 @@ __device__ __forceinline__ void prefetch_gather_rows(const uint4 *vi, const floa
 // All 64 field loads of the two rows are issued before the first one is consumed, so a thread has its whole gather in flight at
 // once instead of one L2 round trip per column pair.  The loads are unconditional: an unmatched row reads vertex 0's features and
 // its result is replaced by 0 (a branch around the loads would keep the compiler from hoisting them over the FMAs).
-// L1_ROWS: the loads allocate in L1 (k_mlp).  Samples next to each other along a ray lie in the same or adjacent tetrahedra, so
+// ALLOC_L1: the loads allocate in L1 (k_mlp).  Samples next to each other along a ray lie in the same or adjacent tetrahedra, so
 // most of a row's four vertices are among its neighbours' and the repeats of a field row, within a warp and across the warpgroups
 // of an SM, are served from L1 instead of L2.  Otherwise they stream past L1 (k_mlp_bwd, k_mlp_normals).
-template <int PREC, bool L1_ROWS = false>
+template <int PREC, bool ALLOC_L1 = false>
 __device__ __forceinline__ void gather_rows(const GatherRows &r, const float *__restrict__ fshadow, uint32_t t, uint32_t (&xh)[16], uint32_t (&xl)[16]) {
     float2 a[2][4][8];  // [row][vertex][column pair]
 #pragma unroll
@@ -149,7 +149,7 @@ __device__ __forceinline__ void gather_rows(const GatherRows &r, const float *__
         for (int k = 0; k < 4; ++k) {
             const float *f = fshadow + (size_t)vs[k] * 64 + 2 * t;
 #pragma unroll
-            for (int c = 0; c < 8; ++c) a[rr][k][c] = L1_ROWS ? ldg_l1_2(f + 8 * c) : ldg_stream2(f + 8 * c);
+            for (int c = 0; c < 8; ++c) a[rr][k][c] = ALLOC_L1 ? ldg_l1_2(f + 8 * c) : ldg_stream2(f + 8 * c);
         }
     }
 #pragma unroll
@@ -197,8 +197,7 @@ __device__ __forceinline__ void layer_mma(float (&d)[64], const uint32_t (&ah)[4
     reg_fence(d);
 }
 
-// L1_ROWS: the field gather allocates in L1 (the default, tn_set_mlp_gather); the results are bit-identical either way
-template <bool FINE, int PREC, bool L1_ROWS>
+template <bool FINE, int PREC>
 __global__ void __launch_bounds__(MLP_THREADS, 1) k_mlp(const MlpParams p) {
     using namespace tc;
     extern __shared__ __align__(1024) uint8_t tn_mlp_smem[];
@@ -256,7 +255,7 @@ __global__ void __launch_bounds__(MLP_THREADS, 1) k_mlp(const MlpParams p) {
         uint32_t ah[32], al[32];
         {
             uint32_t xh[16], xl[16];
-            gather_rows<PREC, L1_ROWS>(load_gather_rows(p.vi, p.bary, row0, total_rows), p.fshadow, t, xh, xl);
+            gather_rows<PREC, true>(load_gather_rows(p.vi, p.bary, row0, total_rows), p.fshadow, t, xh, xl);
             // Into L1 while this tile's MMAs run: the next tile's indices, so its gather starts with the field loads, and (FINE) this
             // tile's bias rows of layer 4, read right after that layer's MMA wait.  Prefetches hold no registers: keeping the 14
             // index words of the next tile in registers instead spills k_mlp<true, 3> at its 168-register limit.
@@ -354,10 +353,10 @@ __global__ void __launch_bounds__(MLP_THREADS, 1) k_mlp(const MlpParams p) {
     if (!weights_ready) mbar_wait(w_bar, 0);  // a warpgroup without a tile still lets the weight copy land before the CTA exits
 }
 
-// launches one k_mlp pass with the shared memory of that pass; l1_rows selects the field gather (tn_set_mlp_gather)
+// launches one k_mlp pass with the shared memory of that pass
 template <bool FINE, int PREC>
-inline int launch_mlp(const MlpParams &p, uint32_t grid, bool l1_rows, cudaStream_t s) {
-    auto k = l1_rows ? k_mlp<FINE, PREC, true> : k_mlp<FINE, PREC, false>;
+inline int launch_mlp(const MlpParams &p, uint32_t grid, cudaStream_t s) {
+    auto k = k_mlp<FINE, PREC>;
     TN_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)mlp_smem_bytes(FINE)));
     k<<<grid, MLP_THREADS, mlp_smem_bytes(FINE), s>>>(p);
     return TN_OK;

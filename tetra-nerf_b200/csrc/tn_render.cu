@@ -972,7 +972,6 @@ static int render_impl(tn_tracer *h, const tn_render_config *cfg, const float *d
     TN_CUDA(cudaFuncSetAttribute(k_composite, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_c));
     auto launch_coarse = prec == 2 ? launch_mlp<false, 2> : launch_mlp<false, 3>;
     auto launch_fine = prec == 2 ? launch_mlp<true, 2> : launch_mlp<true, 3>;
-    const bool l1_rows = h->mlp_gather == 1;
     const uint32_t gridR = (R + SAMPLE_WARPS - 1) / SAMPLE_WARPS;
 
     if (det) {
@@ -994,7 +993,7 @@ static int render_impl(tn_tracer *h, const tn_render_config *cfg, const float *d
     const uint32_t grid_c = (uint32_t)std::min<uint64_t>((tiles_c + MLP_WGS - 1) / MLP_WGS, (uint64_t)sms);
     const uint32_t grid_f = (uint32_t)std::min<uint64_t>((tiles_f + MLP_WGS - 1) / MLP_WGS, (uint64_t)sms);
     if (!single) {
-        rc = launch_coarse(mc, grid_c, l1_rows, s);
+        rc = launch_coarse(mc, grid_c, s);
         if (rc) return rc;
     }
     TN_EV(3);
@@ -1006,7 +1005,7 @@ static int render_impl(tn_tracer *h, const tn_render_config *cfg, const float *d
     if (!single) { mf.vi = b.vi_f; mf.bary = b.bary_f; }
     else p.ebins_f = r->ebins_c;  // k_composite integrates over the coarse bins
     mf.tile_ctr = b.n_active + 2;
-    rc = launch_fine(mf, grid_f, l1_rows, s);
+    rc = launch_fine(mf, grid_f, s);
     if (rc) return rc;
     TN_EV(5);
     k_composite<<<gridR, SAMPLE_WARPS * 32, smem_c, s>>>(p);

@@ -307,7 +307,7 @@ int run_mlp(tn_tracer *h, const RenderInputs &in, const uint32_t *d_count, uint6
     const uint64_t tiles = (rows + MLP_TILE - 1) / MLP_TILE;
     const uint32_t grid = (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>((tiles + MLP_WGS - 1) / MLP_WGS, (uint64_t)sms));
     h->launches += 1;
-    return launch_mlp<FINE, 3>(p, grid, h->mlp_gather == 1, s);
+    return launch_mlp<FINE, 3>(p, grid, s);
 }
 
 uint32_t blocks(uint64_t n, uint32_t per) { return (uint32_t)((n + per - 1) / per); }

@@ -52,7 +52,6 @@ struct TraceParams {
     // list entries with bit 31 set carry their face hits already (written by the adjacency walk, tn_walk.cu):
     // num[ray] keys at keys_in[ray*M ..]; the gather is skipped and only sort + pairing + emit run
     const u64 *keys_in;
-    int windowed;  // literal pairing restricted to the windows around eps-ties (post_process_windows); 0 = over the whole array (A/B)
 };
 
 __device__ __forceinline__ uint32_t warp_incl_scan(uint32_t v, int lane) {
@@ -251,7 +250,7 @@ __global__ void __launch_bounds__(TRACE_WARPS * 32, 7) k_trace(const TraceParams
             uint2 *tts = reinterpret_cast<uint2 *>(stack);
             uint16_t *emit = reinterpret_cast<uint16_t *>(leafq);
             const uint32_t nw = (nh + 31u) >> 5;  // mask words of the windowed pairing: behind tts[] in the work-list region when it has room
-            uint32_t *mask = (p.windowed && (size_t)nh * 8 + (size_t)nw * 12 <= (size_t)p.scap * 4) ? reinterpret_cast<uint32_t *>(tts + nh) : nullptr;
+            uint32_t *mask = (size_t)nh * 8 + (size_t)nw * 12 <= (size_t)p.scap * 4 ? reinterpret_cast<uint32_t *>(tts + nh) : nullptr;
             const pairing::PairOut po{p.cells, p.verts, p.bary, p.dist};
             jc = pairing::pair_and_emit(hits, tts, emit, mask, nh, p.tt, p.tri, p.xyz, rs, row, po, lane);
             if (p.dense) {
@@ -332,8 +331,6 @@ static int launch_trace(tn_tracer *h, int mode, const float *o, const float *d, 
     p.o = o; p.d = d; p.R = R; p.M = M; p.num = num; p.cells = cells; p.bary = bary; p.dist = dist; p.verts = verts;
     p.nodes = h->mesh.nodes; p.leaves = h->mesh.leaves; p.tri = (const uint4 *)h->mesh.tri; p.tt = (const uint2 *)h->mesh.tt;
     p.xyz = h->mesh.xyz; p.lv = h->mesh.lv; p.absmax = h->mesh.absmax; p.dense = dense; p.flags = h->d_flags;
-    static const int windowed_env = [] { const char *e = getenv("TETRANERF_B200_WINDOWED_PAIRING"); return e ? atoi(e) : 1; }();  // A/B switch
-    p.windowed = windowed_env;
     auto kern = mode == 0 ? k_trace<0> : k_trace<1>;
     int sms = 132;
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, h->device);
@@ -351,14 +348,12 @@ static int launch_trace(tn_tracer *h, int mode, const float *o, const float *d, 
     };
     const uint32_t want = (R + TRACE_WARPS - 1) / TRACE_WARPS;
     // path choice.  The adjacency walk needs ~40x fewer instructions per ray than the all-hits gather but is a serial chain
-    // of L2 round trips per ray: with >= walk_min_rays rays it runs 32 rays per warp (throughput); smaller batches up to
-    // walk_solo_max_rays run ONE ray per warp (latency: no divergence, no scattered 32-way accesses); anything else, and
-    // meshes that cannot be walked, take the warp-per-ray BVH gather.  TETRANERF_B200_WALK=0/1/2 forces BVH / 32-per-warp
-    // walk / solo walk (the tests exercise all three through the setters).
-    static const int walk_env = [] { const char *e = getenv("TETRANERF_B200_WALK"); return e ? atoi(e) : -1; }();
-    const bool thread_walk = walk_env >= 0 ? walk_env == 1 : R >= h->walk_min_rays;
-    const bool quad_walk = walk_env >= 0 ? walk_env == 3 : (!thread_walk && R >= h->walk_quad_min_rays && R <= h->walk_quad_max_rays);
-    const bool solo_walk = walk_env >= 0 ? walk_env == 2 : (!thread_walk && !quad_walk && R >= h->walk_solo_min_rays && R <= h->walk_solo_max_rays);
+    // of L2 round trips per ray: with >= walk_min_rays rays it runs 32 rays per warp (throughput); smaller batches in the quad
+    // range run 4 lanes per ray, 8 rays per warp (latency: no divergence, no scattered 32-way accesses), and those in the solo
+    // range 4 lanes per ray, one ray per warp; anything else, and meshes that cannot be walked, take the warp-per-ray BVH gather.
+    const bool thread_walk = R >= h->walk_min_rays;
+    const bool quad_walk = !thread_walk && R >= h->walk_quad_min_rays && R <= h->walk_quad_max_rays;
+    const bool solo_walk = !thread_walk && !quad_walk && R >= h->walk_solo_min_rays && R <= h->walk_solo_max_rays;
     if (mode == 0 && h->mesh.walkable && M >= 4 && (thread_walk || solo_walk || quad_walk)) {
         // fast path: adjacency walk (tn_walk.cu); rays it cannot certify are listed for the exact stage below
         const size_t need = (size_t)R * M;

@@ -45,7 +45,6 @@ _lib.tn_set_walk_min_rays.argtypes = [_vp, _u32]
 _lib.tn_set_walk_solo_range.argtypes = [_vp, _u32, _u32]
 _lib.tn_set_walk_quad_range.argtypes = [_vp, _u32, _u32]
 _lib.tn_set_walk_quad_spec_max_rays.argtypes = [_vp, _u32]
-_lib.tn_set_mlp_gather.argtypes = [_vp, _i]
 _lib.tn_launch_count.restype = C.c_uint64
 _lib.tn_launch_count.argtypes = [_vp]
 
@@ -210,12 +209,8 @@ class TetrahedraTracer:
         _check(_lib.tn_set_walk_quad_range(self._h, int(lo), int(hi)))
 
     def set_walk_quad_spec_max_rays(self, n: int) -> None:
-        """quad walk: batches of up to n rays load all candidate next records speculatively instead of prefetching them (0 = never)"""
+        """quad and solo walks: batches of up to n rays load all candidate next records speculatively instead of prefetching them (0 = never)"""
         _check(_lib.tn_set_walk_quad_spec_max_rays(self._h, int(n)))
-
-    def set_mlp_gather(self, mode: int) -> None:
-        """field gather of the fused MLP passes: 1 (default) = field rows cached in L1, 0 = streamed past it; bit-identical results"""
-        _check(_lib.tn_set_mlp_gather(self._h, int(mode)))
 
     def trace_stats(self):
         """(walkable mesh?, rays of the last trace_rays that took the exact stage) -- test/diagnostic hook"""

@@ -1,18 +1,28 @@
-"""trace-only sweep: warp-per-ray BVH gather vs adjacency walk, through the fused renderer's per-kernel timings"""
-import os, sys, subprocess, json
+"""trace-only sweep: warp-per-ray BVH gather vs adjacency walks, through the fused renderer's per-kernel timings"""
+import os, sys, json
 R = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-if len(sys.argv) > 1:
-    sys.path[:0] = [R, R + "/tetra-nerf_b200"]
-    import numpy as np, torch, bench
-    from tetranerf import cpp
-    from tetranerf.b200 import synthetic as syn
-    from tetranerf.b200.render import FusedRenderer, RenderSettings
-    dev = torch.device("cuda:0")
-    V, C, field = bench.make_workload()
-    tr = cpp.TetrahedraTracer(dev); dV, dC = torch.from_numpy(V).to(dev), torch.from_numpy(C).to(dev); tr.load_tetrahedra(dV, dC)
-    if "TN_SWEEP_SPEC" in os.environ: tr.set_walk_quad_spec_max_rays(int(os.environ["TN_SWEEP_SPEC"]))
-    fr = FusedRenderer(tr); fr.set_field(torch.from_numpy(field).to(dev)); fr.set_weights(bench.mlp_params()); fr.set_profiling(True)
-    st = RenderSettings.tetra_nerf()
+sys.path[:0] = [R, R + "/tetra-nerf_b200"]
+import numpy as np, torch, bench
+from tetranerf import cpp
+from tetranerf.b200 import synthetic as syn
+from tetranerf.b200.render import FusedRenderer, RenderSettings
+
+# each implementation of trace_rays forced through the setters: (walk_min_rays, solo range, quad range, spec max rays)
+NEVER, ALWAYS = (1, 0), (0, 2**32 - 1)
+FORMS = {
+    "bvh": (2**32 - 1, NEVER, NEVER, 0),                       # warp-per-ray all-hits BVH gather
+    "walk": (0, NEVER, NEVER, 0),                              # 32 rays per warp
+    "walk_solo": (2**32 - 1, ALWAYS, NEVER, 2**32 - 1),        # 1 ray per warp, speculative record loads
+    "walk_quad_pf": (2**32 - 1, NEVER, ALWAYS, 0),             # 8 rays per warp, prefetched record loads
+    "walk_quad": (2**32 - 1, NEVER, ALWAYS, 2**32 - 1),        # 8 rays per warp, speculative record loads
+}
+dev = torch.device("cuda:0")
+V, C, field = bench.make_workload()
+tr = cpp.TetrahedraTracer(dev); dV, dC = torch.from_numpy(V).to(dev), torch.from_numpy(C).to(dev); tr.load_tetrahedra(dV, dC)
+fr = FusedRenderer(tr); fr.set_field(torch.from_numpy(field).to(dev)); fr.set_weights(bench.mlp_params()); fr.set_profiling(True)
+st = RenderSettings.tetra_nerf()
+for name, (min_rays, solo, quad, spec) in FORMS.items():
+    tr.set_walk_min_rays(min_rays); tr.set_walk_solo_range(*solo); tr.set_walk_quad_range(*quad); tr.set_walk_quad_spec_max_rays(spec)
     res = {}
     for n in (1024, 2048, 4096, 8192, 16384, 32768, 65536):
         o, d = syn.camera_rays(n, seed=3); o, d = torch.from_numpy(o).to(dev), torch.from_numpy(d).to(dev)
@@ -21,11 +31,4 @@ if len(sys.argv) > 1:
         for _ in range(4):
             fr.render(o, d, st); t.append(fr.kernel_timings_ms())
         res[n] = {k: round(float(np.median([x[k] for x in t])), 4) for k in t[0]}
-    print(json.dumps(res))
-else:
-    # BVH gather, walk 32 rays/warp, walk 1 ray/warp, walk 8 rays/warp (prefetching / speculative record loads)
-    for mode, spec in (("0", None), ("1", None), ("2", None), ("3", "0"), ("3", str(2**32 - 1))):
-        env = dict(os.environ, TETRANERF_B200_WALK=mode)
-        if spec is not None: env["TN_SWEEP_SPEC"] = spec
-        out = subprocess.run([sys.executable, __file__, "child"], env=env, capture_output=True, text=True)
-        print("WALK=" + mode + ("" if spec is None else "/spec=" + spec), out.stdout.strip().splitlines()[-1] if out.stdout.strip() else out.stderr[-500:])
+    print(name, json.dumps(res), flush=True)
