@@ -141,6 +141,15 @@ int tn_render(tn_tracer *h, const tn_render_config *cfg, const float *d_origins,
  * (tn_render_set_gather).  DESIGN.md §4.7. */
 int tn_render_normals(tn_tracer *h, const tn_render_config *cfg, const float *d_origins, const float *d_directions, uint32_t R,
                       float *d_rgb, float *d_acc, float *d_depth, uint8_t *d_mask, float *d_normals, void *stream);
+/* tn_render plus the expected depth d_expected_depth f32[R] (every element written; nerfstudio DepthRenderer(method="expected")) and,
+ * if d_normals is not NULL, the normal map of tn_render_normals.  Over the samples that give rgb (the fine pass; the coarse one when
+ * num_fine_samples = 0), t_i the bin midpoints and w_i the weights of rgb, A = sum w_i: D_raw = sum w_i t_i / (A + 1e-10), and
+ * D = clip(D_raw, t_min, t_max) with t_min / t_max the smallest / largest midpoint over every active ray of the call; far_plane on empty
+ * rays.  rgb, acc, depth, mask and normals are the same bits as without it.  TN_ERR_ARG while a fused pixel gather is set.
+ * DESIGN.md §4.10. */
+int tn_render_expected_depth(tn_tracer *h, const tn_render_config *cfg, const float *d_origins, const float *d_directions, uint32_t R,
+                             float *d_rgb, float *d_acc, float *d_depth, uint8_t *d_mask, float *d_expected_depth, float *d_normals,
+                             void *stream);
 /* ---- fused training step (SURVEY.md §8f-1): TetrahedraNerf.get_outputs in training mode (model.py:520-662) + its autograd backward.
  * Forward = the fused pipeline with the stratified bins of training (model.py:169-174 for the coarse pass, PDFSampler train_stratified
  * for the fine pass; the uniform [0,1) draws come from the caller, d_jitter_coarse f32[R,S_c+1] / d_jitter_fine f32[R,S_f+1] indexed by
@@ -191,6 +200,22 @@ int tn_render_train_backward_saved_rays(tn_tracer *h, const void *d_saved, const
 int tn_render_train_backward_saved_geometry(tn_tracer *h, const void *d_saved, const float *d_grad_rgb, const float *d_grad_acc,
                                             int use_gradient_scaling, float *d_grad_field, float *const *d_grad_params12, float *d_grad_origins,
                                             float *d_grad_directions, float *d_grad_xyz, void *stream);
+/* The saved training pair with the expected depth (DESIGN.md §4.10).  tn_render_train_forward_saved_depth is
+ * tn_render_train_forward_saved plus d_expected_depth f32[R], defined as for tn_render_expected_depth (training mode: no nan_to_num, no
+ * clamp; the same saved-state size: the two clip bounds sit in the slot of the active count, and the header records that the forward
+ * produced them).  tn_render_train_backward_saved_depth takes the arguments of tn_render_train_backward_saved_geometry plus
+ * d_grad_expected_depth f32[R] (NULL: none, and then every output is that of the existing entry point with the same ray / vertex
+ * outputs; all three of those NULL: tn_render_train_backward_saved's path).  The bins and midpoints are constants; where
+ * t_min <= D_raw <= t_max, dL/dw_i gains dL/dD (t_i - D_raw) / (A + 1e-10), before the transmittance sums and GradientScaler, so the
+ * depth loss reaches the field, the MLP, the rays and the vertices.  TN_ERR_STATE if d_grad_expected_depth is given and the forward was
+ * not a _depth one.  The forward returns TN_ERR_ARG while a fused pixel gather is set, as tn_render_normals does. */
+int tn_render_train_forward_saved_depth(tn_tracer *h, const tn_render_config *cfg, const float *d_origins, const float *d_directions, uint32_t R,
+                                        const float *d_jitter_coarse, const float *d_jitter_fine, float *d_rgb, float *d_acc, float *d_depth,
+                                        uint8_t *d_mask, float *d_expected_depth, void *d_saved, size_t saved_bytes, void *stream);
+int tn_render_train_backward_saved_depth(tn_tracer *h, const void *d_saved, const float *d_grad_rgb, const float *d_grad_acc,
+                                         const float *d_grad_expected_depth, int use_gradient_scaling, float *d_grad_field,
+                                         float *const *d_grad_params12, float *d_grad_origins, float *d_grad_directions, float *d_grad_xyz,
+                                         void *stream);
 /* Deterministic mode of the fused training step (enable != 0; initial value: 1 if the environment variable TETRANERF_B200_DETERMINISTIC
  * is 1, else 0).  Read by tn_render_train_forward; tn_render_train_backward continues in the mode of the forward it belongs to.  With
  * identical inputs, on the same build and GPU model, forward outputs and every gradient are then bitwise identical from run to run and

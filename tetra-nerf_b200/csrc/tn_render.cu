@@ -204,6 +204,10 @@ struct SampleParams {
     float *peer[8];
     uint32_t gather_world, gather_rank, gather_stride;
     const uint32_t *ray_slot;     // deterministic mode: slot of every ray with hits (exclusive scan of num > 0)
+    // expected depth (k_composite<true>): unclipped depth per active ray [R]; ordered keys of the smallest / largest sample midpoint
+    // of the call (DESIGN §4.10)
+    float *edepth;
+    uint32_t *dbounds;
 };
 
 // lane 0 writes the local outputs; lanes < gather_world each post the pixel to one rank's gathered buffer (three 8-byte stores)
@@ -454,6 +458,17 @@ __global__ void __launch_bounds__(SAMPLE_WARPS * 32) k_sample_fine(const SampleP
     dir_bias(p, ray, slot, lane);
 }
 
+// expected depth (DESIGN §4.10): the clip bounds are the smallest / largest sample midpoint over every active ray of the call, reduced
+// with atomicMin / atomicMax on an order-preserving unsigned key of the float (exact and order-independent)
+__device__ __forceinline__ uint32_t depth_key(float f) {
+    const uint32_t b = __float_as_uint(f);
+    return (b & 0x80000000u) ? ~b : (b | 0x80000000u);
+}
+__device__ __forceinline__ float depth_unkey(uint32_t k) { return __uint_as_float((k & 0x80000000u) ? (k & 0x7fffffffu) : ~k); }
+
+// DEPTH: also the unclipped expected depth sum_j w_j t_j / (sum_j w_j + 1e-10) of the ray (-> p.edepth) and its midpoints' share of the
+// call's clip bounds (-> p.dbounds); k_expected_depth_finalize clips.  The other outputs are the same bits either way.
+template <bool DEPTH>
 __global__ void __launch_bounds__(SAMPLE_WARPS * 32) k_composite(const SampleParams p) {
     extern __shared__ float sm[];
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -468,13 +483,32 @@ __global__ void __launch_bounds__(SAMPLE_WARPS * 32) k_composite(const SamplePar
     __syncwarp();
     weights_from_density(w, tr, S2, lane);  // model.py:632
     float r = 0.f, g = 0.f, b = 0.f, a = 0.f;
+    float dt = 0.f, tlo = 3.4028234663852886e38f, thi = -3.4028234663852886e38f;  // (DEPTH only)
     for (uint32_t j = lane; j < S2; j += 32) {
         const float4 c = of[j];
         const float wj = w[j];
         if (p.train) { r += wj * c.y; g += wj * c.z; b += wj * c.w; a += wj; }  // RGBRenderer in training: no nan_to_num, no clamp
         else { r += wj * nan_to_num_f(c.y); g += wj * nan_to_num_f(c.z); b += wj * nan_to_num_f(c.w); a += wj; }
+        if constexpr (DEPTH) {  // DepthRenderer("expected"): steps = (starts + ends) / 2
+            const float t = (eb[j] + eb[j + 1]) / 2.f;
+            dt += wj * t;
+            tlo = fminf(tlo, t); thi = fmaxf(thi, t);
+        }
     }
     r = warp_sum_f(r); g = warp_sum_f(g); b = warp_sum_f(b); a = warp_sum_f(a);
+    if constexpr (DEPTH) {
+        dt = warp_sum_f(dt);
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) {
+            tlo = fminf(tlo, __shfl_xor_sync(0xffffffffu, tlo, o));
+            thi = fmaxf(thi, __shfl_xor_sync(0xffffffffu, thi, o));
+        }
+        if (lane == 0) {
+            p.edepth[ray] = dt / (a + 1e-10f);
+            atomicMin(p.dbounds, depth_key(tlo));
+            atomicMax(p.dbounds + 1, depth_key(thi));
+        }
+    }
     // DepthRenderer("median"): first sample whose cumulative weight reaches 0.5
     for (uint32_t j = lane; j < S2; j += 32) tr[j] = w[j];
     __syncwarp();
@@ -488,6 +522,16 @@ __global__ void __launch_bounds__(SAMPLE_WARPS * 32) k_composite(const SamplePar
     float pr = r + p.bg0 * (1.f - a), pg = g + p.bg1 * (1.f - a), pb = b + p.bg2 * (1.f - a);
     if (!p.train) { pr = fminf(fmaxf(pr, 0.f), 1.f); pg = fminf(fmaxf(pg, 0.f), 1.f); pb = fminf(fmaxf(pb, 0.f), 1.f); }
     store_pixel(p, ray, lane, pr, pg, pb, a, (eb[mi] + eb[mi + 1]) / 2.f, 1);
+}
+
+// after k_composite<true>: D = clip(D_raw, t_min, t_max) on active rays (NaN passes through, as torch.clip), far_plane on empty ones
+__global__ void k_expected_depth_finalize(uint32_t R, const uint32_t *__restrict__ num, const uint32_t *__restrict__ dbounds, float far_plane,
+                                          float *__restrict__ edepth) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= R) return;
+    if (num[i] == 0) { edepth[i] = far_plane; return; }
+    const float lo = depth_unkey(dbounds[0]), hi = depth_unkey(dbounds[1]), x = edepth[i];
+    edepth[i] = x < lo ? lo : (x > hi ? hi : x);
 }
 
 // ---- backward of the compositing + field heads of the fine pass (model.py:621-637; RaySamples.get_weights, RGBRenderer and
@@ -504,8 +548,12 @@ struct CompositeBwdParams {
     float4 *dout;                      // [slot * S2 + j]
     float *sums;                       // 4 floats: sum d sigma_pre, sum d z_r, d z_g, d z_b (bias gradients of the two heads);
                                        // deterministic mode: [n_active] float4, one per slot (summed in slot order by k_det_sum_slots)
+    const float *grad_ed;              // DEPTH: [R] dL/d expected depth
+    const uint32_t *dbounds;           // DEPTH: the forward's clip bounds (ordered keys, k_composite<true>)
 };
-template <bool DET>
+// DEPTH: g_j also gets the expected depth's term grad_ed (t_j - D_raw) / (A + 1e-10), 0 where the forward's clip binds (DESIGN §4.10);
+// A and D_raw are recomputed from the saved bins and densities exactly as k_composite<true> formed them
+template <bool DET, bool DEPTH = false>
 __global__ void __launch_bounds__(SAMPLE_WARPS * 32) k_composite_bwd(const CompositeBwdParams p) {
     extern __shared__ float sm[];
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -521,6 +569,22 @@ __global__ void __launch_bounds__(SAMPLE_WARPS * 32) k_composite_bwd(const Compo
     for (uint32_t j = lane; j < S2; j += 32) tr[j] = (eb[j + 1] - eb[j]) * of[j].x;  // x_j
     __syncwarp();
     smem_scan_add(tr, S2, lane);  // inclusive cumsum of x
+    float gd = 0.f, draw = 0.f, den = 1.f;
+    if constexpr (DEPTH) {
+        float a = 0.f, dt = 0.f;
+        for (uint32_t j = lane; j < S2; j += 32) {
+            const float excl = j == 0 ? 0.f : tr[j - 1];
+            const float x = (eb[j + 1] - eb[j]) * of[j].x;
+            const float wj = nan_to_num_f((1.f - expf(-x)) * expf(-excl));
+            a += wj;
+            dt += wj * ((eb[j] + eb[j + 1]) / 2.f);
+        }
+        a = warp_sum_f(a); dt = warp_sum_f(dt);
+        den = a + 1e-10f;
+        draw = dt / den;
+        const float lo = depth_unkey(p.dbounds[0]), hi = depth_unkey(p.dbounds[1]);
+        gd = (draw >= lo && draw <= hi) ? p.grad_ed[ray] : 0.f;  // torch.clip's backward: inclusive bounds
+    }
     for (uint32_t j = lane; j < S2; j += 32) {
         const float excl = j == 0 ? 0.f : tr[j - 1];
         const float x = (eb[j + 1] - eb[j]) * of[j].x;
@@ -529,7 +593,9 @@ __global__ void __launch_bounds__(SAMPLE_WARPS * 32) k_composite_bwd(const Compo
         const bool fin = isfinite(wj);  // nan_to_num in the forward: a replaced weight carries no gradient
         wj = fin ? wj : nan_to_num_f(wj);
         const float4 c = of[j];
-        const float g = fin ? (gr * (c.y - p.bg0) + gg * (c.z - p.bg1) + gb * (c.w - p.bg2) + ga) : 0.f;
+        float g;
+        if constexpr (DEPTH) g = fin ? (gr * (c.y - p.bg0) + gg * (c.z - p.bg1) + gb * (c.w - p.bg2) + ga + gd * (((eb[j] + eb[j + 1]) / 2.f - draw) / den)) : 0.f;
+        else g = fin ? (gr * (c.y - p.bg0) + gg * (c.z - p.bg1) + gb * (c.w - p.bg2) + ga) : 0.f;
         w[j] = wj;
         gw[j] = g * wj;
         fx[j] = fin ? g * (T - wj) : 0.f;  // first term of dL/dx_j
@@ -739,7 +805,7 @@ static int ensure_ws(RenderState *r, size_t R, size_t M, size_t Sc, size_t S2) {
     R = std::max(R, r->cap_R); M = std::max(M, r->cap_M); Sc = std::max(Sc, r->cap_Sc); S2 = std::max(S2, r->cap_S2);
 #define A(ptr, bytes) TN_CUDA(cudaMalloc((void **)&(ptr), (bytes)))
     A(r->num, 4 * R); A(r->cells, 4 * R * M); A(r->verts, 16 * R * M); A(r->bary, 24 * R * M); A(r->dist, 8 * R * M);
-    A(r->n_active, 16); A(r->ray_list, 4 * R);
+    A(r->n_active, 32); A(r->ray_list, 4 * R);  // words 4, 5: clip bounds of the expected depth
     A(r->ebins_c, 4 * R * (Sc + 1)); A(r->sbins_c, 4 * R * (Sc + 1)); A(r->bary_c, 12 * R * Sc); A(r->dens_c, 4 * R * Sc); A(r->vi_c, 16 * R * Sc);
     A(r->ebins_f, 4 * R * (S2 + 1)); A(r->bary_f, 12 * R * S2); A(r->out_f, 16 * R * S2); A(r->dirbias, 512 * R); A(r->vi_f, 16 * R * S2);
 #undef A
@@ -855,7 +921,8 @@ extern "C" int tn_render_set_weights(tn_tracer *h, const float *const *P, void *
 // the buffers a training forward leaves for its backward: the tracer's own (tn_render_train_forward, the "last call") or those of a
 // caller's saved-state blob (tn_render_train_forward_saved)
 struct TrainBufs {
-    uint32_t *n_active;        // 16-byte block: active rays | tile counter of the coarse pass | of the fine pass | (unused)
+    uint32_t *n_active;        // 16-byte block: active rays | tile counter of the coarse pass | of the fine pass | (unused); then words
+                               // 4, 5: the clip bounds of the expected depth (in the slot the saved state reserves for the block)
     uint32_t *ray_list;        // [R] slot -> ray
     float *ebins_f, *sbins_f;  // [R,S2+1] euclidean / spacing bins of the fine pass
     uint4 *vi_f;               // [R*S2] matched vertices
@@ -870,7 +937,8 @@ static TrainBufs own_bufs(RenderState *r) {
 // saved-state blob of tn_render_train_forward_saved: this header, then the TrainBufs arrays, each 256-byte aligned
 constexpr uint32_t SAVED_MAGIC = 0x53564e54u;  // "TNVS"
 struct SavedHeader {
-    uint32_t magic, R, M, Sc, Sf, S2, det, pad;
+    uint32_t magic, R, M, Sc, Sf, S2, det;
+    uint32_t edepth;           // 1: the forward produced the expected depth (its clip bounds are in words 4, 5 of the n_active slot)
     float bg[3];
     uint32_t pad2;
     uint64_t gen;              // RenderState::gen at the forward
@@ -883,7 +951,7 @@ static size_t saved_layout(size_t R, size_t S2, uint8_t *base, TrainBufs *b) {
     size_t off = SAVED_ALIGN;  // header
     auto take = [&](size_t bytes) { uint8_t *p = base ? base + off : nullptr; off += (bytes + SAVED_ALIGN - 1) / SAVED_ALIGN * SAVED_ALIGN; return p; };
     TrainBufs t{};
-    t.n_active = (uint32_t *)take(16);
+    t.n_active = (uint32_t *)take(24);  // (one 256-byte slot either way)
     t.ray_list = (uint32_t *)take(4 * R);
     t.ebins_f = (float *)take(4 * R * (S2 + 1));
     t.sbins_f = (float *)take(4 * R * (S2 + 1));
@@ -904,7 +972,8 @@ struct TrainFwd {
 static int ensure_train_ws(RenderState *r, size_t R, size_t S2, uint32_t V);
 
 static int render_impl(tn_tracer *h, const tn_render_config *cfg, const float *d_origins, const float *d_directions, uint32_t R,
-                       float *d_rgb, float *d_acc, float *d_depth, uint8_t *d_mask, const TrainFwd *tf, float *d_normals, void *stream) {
+                       float *d_rgb, float *d_acc, float *d_depth, uint8_t *d_mask, const TrainFwd *tf, float *d_normals, float *d_edepth,
+                       void *stream) {
     if (!h || !cfg) return fail(TN_ERR_ARG, "null argument");
     RenderState *r = h->render;
     if (!r || !r->fshadow || !r->have_weights) return fail(TN_ERR_STATE, "tn_render: call tn_render_set_field and tn_render_set_weights first");
@@ -937,6 +1006,10 @@ static int render_impl(tn_tracer *h, const tn_render_config *cfg, const float *d
     const TrainBufs b = tf != nullptr && tf->saved != nullptr ? *tf->saved : own_bufs(r);
     const int prec = tf != nullptr ? 3 : r->mlp_prec;  // the training forward keeps bf16x3 (its backward recomputes in bf16x3)
     TN_CUDA(cudaMemsetAsync(b.n_active, 0, 16, s));
+    if (d_edepth != nullptr) {  // clip bounds: min starts at the largest key, max at the smallest
+        TN_CUDA(cudaMemsetAsync(b.n_active + 4, 0xff, 4, s));
+        TN_CUDA(cudaMemsetAsync(b.n_active + 5, 0, 4, s));
+    }
 #define TN_EV(i) do { if (r->profile) cudaEventRecord(r->ev[i], s); } while (0)
     TN_EV(0);  // the "trace" interval includes the L2 warm-up it exists for
     {   // L2 warm-up of everything read-only that the step gathers from (mesh tables, field shadow, weight image)
@@ -957,6 +1030,7 @@ static int render_impl(tn_tracer *h, const tn_render_config *cfg, const float *d
     p.rgb = d_rgb; p.acc = d_acc; p.depth = d_depth; p.mask = d_mask;
     p.far_plane = cfg->far_plane; p.bg0 = cfg->background[0]; p.bg1 = cfg->background[1]; p.bg2 = cfg->background[2];
     if (tf != nullptr) { p.train = 1; p.jit_c = tf->jit_c; p.jit_f = tf->jit_f; p.sbins_f = b.sbins_f; p.enc = b.enc; }
+    p.edepth = d_edepth; p.dbounds = b.n_active + 4;
     if (r->gather_world) {
         if (R > r->gather_stride) return fail(TN_ERR_ARG, "tn_render: more rays than the gathered-pixel buffers were sized for (tn_render_set_gather)");
         for (int k = 0; k < 8; ++k) p.peer[k] = r->peer[k];
@@ -969,7 +1043,8 @@ static int render_impl(tn_tracer *h, const tn_render_config *cfg, const float *d
     auto k_coarse_sample = det ? k_sample_coarse<true> : k_sample_coarse<false>;
     TN_CUDA(cudaFuncSetAttribute(k_coarse_sample, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_sc));
     TN_CUDA(cudaFuncSetAttribute(k_sample_fine, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_sf));
-    TN_CUDA(cudaFuncSetAttribute(k_composite, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_c));
+    auto k_comp = d_edepth != nullptr ? k_composite<true> : k_composite<false>;
+    TN_CUDA(cudaFuncSetAttribute(k_comp, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_c));
     auto launch_coarse = prec == 2 ? launch_mlp<false, 2> : launch_mlp<false, 3>;
     auto launch_fine = prec == 2 ? launch_mlp<true, 2> : launch_mlp<true, 3>;
     const uint32_t gridR = (R + SAMPLE_WARPS - 1) / SAMPLE_WARPS;
@@ -1008,11 +1083,16 @@ static int render_impl(tn_tracer *h, const tn_render_config *cfg, const float *d
     rc = launch_fine(mf, grid_f, s);
     if (rc) return rc;
     TN_EV(5);
-    k_composite<<<gridR, SAMPLE_WARPS * 32, smem_c, s>>>(p);
+    k_comp<<<gridR, SAMPLE_WARPS * 32, smem_c, s>>>(p);
     TN_EV(6);
 #undef TN_EV
     h->launches += 5;
     TN_CUDA(cudaGetLastError());
+    if (d_edepth != nullptr) {  // after the six timed intervals, as the normals
+        k_expected_depth_finalize<<<(R + 255) / 256, 256, 0, s>>>(R, r->num, p.dbounds, cfg->far_plane, d_edepth);
+        h->launches += 1;
+        TN_CUDA(cudaGetLastError());
+    }
     if (d_normals != nullptr) {  // after the six timed intervals: the density gradient at the samples that give the colours, composited
         NormalsLaunch nl{};
         nl.n_active = b.n_active; nl.ray_list = b.ray_list; nl.tile_ctr = b.n_active + 3;  // word 3 of the zeroed block
@@ -1054,7 +1134,7 @@ static int ensure_train_ws(RenderState *r, size_t R, size_t S2, uint32_t V) {
 
 extern "C" int tn_render(tn_tracer *h, const tn_render_config *cfg, const float *d_origins, const float *d_directions, uint32_t R,
                          float *d_rgb, float *d_acc, float *d_depth, uint8_t *d_mask, void *stream) {
-    return render_impl(h, cfg, d_origins, d_directions, R, d_rgb, d_acc, d_depth, d_mask, nullptr, nullptr, stream);
+    return render_impl(h, cfg, d_origins, d_directions, R, d_rgb, d_acc, d_depth, d_mask, nullptr, nullptr, nullptr, stream);
 }
 
 // tn_render plus the normal map d_normals f32[R,3] (DESIGN.md §4.7; tn_normals.cu)
@@ -1063,7 +1143,17 @@ extern "C" int tn_render_normals(tn_tracer *h, const tn_render_config *cfg, cons
     if (!h || !d_normals) return fail(TN_ERR_ARG, "null argument");
     if (h->render && h->render->gather_world)
         return fail(TN_ERR_ARG, "tn_render_normals: the fused pixel gather (tn_render_set_gather) carries no normals; switch it off first");
-    return render_impl(h, cfg, d_origins, d_directions, R, d_rgb, d_acc, d_depth, d_mask, nullptr, d_normals, stream);
+    return render_impl(h, cfg, d_origins, d_directions, R, d_rgb, d_acc, d_depth, d_mask, nullptr, d_normals, nullptr, stream);
+}
+
+// tn_render plus the expected depth d_expected_depth f32[R] and optionally the normal map d_normals f32[R,3] (DESIGN.md §4.10)
+extern "C" int tn_render_expected_depth(tn_tracer *h, const tn_render_config *cfg, const float *d_origins, const float *d_directions, uint32_t R,
+                                        float *d_rgb, float *d_acc, float *d_depth, uint8_t *d_mask, float *d_expected_depth, float *d_normals,
+                                        void *stream) {
+    if (!h || !d_expected_depth) return fail(TN_ERR_ARG, "null argument");
+    if (h->render && h->render->gather_world)
+        return fail(TN_ERR_ARG, "tn_render_expected_depth: the fused pixel gather (tn_render_set_gather) carries no expected depth; switch it off first");
+    return render_impl(h, cfg, d_origins, d_directions, R, d_rgb, d_acc, d_depth, d_mask, nullptr, d_normals, d_expected_depth, stream);
 }
 
 // ---- fused training step (SURVEY §8f-1; model.py:520-662 in training mode + autograd) ------------------------------------------------
@@ -1073,7 +1163,7 @@ extern "C" int tn_render_train_forward(tn_tracer *h, const tn_render_config *cfg
                                        const float *d_jitter_coarse, const float *d_jitter_fine, float *d_rgb, float *d_acc, float *d_depth,
                                        uint8_t *d_mask, void *stream) {
     TrainFwd tf{d_jitter_coarse, d_jitter_fine, nullptr};
-    return render_impl(h, cfg, d_origins, d_directions, R, d_rgb, d_acc, d_depth, d_mask, &tf, nullptr, stream);
+    return render_impl(h, cfg, d_origins, d_directions, R, d_rgb, d_acc, d_depth, d_mask, &tf, nullptr, nullptr, stream);
 }
 
 // backward of a training forward of R rays x S2 fine samples whose buffers are `b`, in the mode (det) and with the background it ran
@@ -1086,9 +1176,10 @@ extern "C" int tn_render_train_forward(tn_tracer *h, const tn_render_config *cfg
 struct RayGradOut {
     float *grad_o, *grad_d, *grad_xyz;
 };
+// d_grad_ed != nullptr: dL/d expected depth f32[R] of a forward that produced it (its clip bounds in b.n_active[4, 5])
 static int train_backward_impl(tn_tracer *h, const TrainBufs &b, uint32_t R, uint32_t S2, bool det, const float *bg, const float *d_grad_rgb,
                                const float *d_grad_acc, int use_gradient_scaling, float *d_grad_field, float *const *d_grad_params12, cudaStream_t s,
-                               const RayGradOut *rays = nullptr) {
+                               const RayGradOut *rays = nullptr, const float *d_grad_ed = nullptr) {
     RenderState *r = h->render;
     int sms = 132;
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, h->device);
@@ -1121,8 +1212,10 @@ static int train_backward_impl(tn_tracer *h, const TrainBufs &b, uint32_t R, uin
     cb.S2 = S2; cb.use_gradient_scaling = use_gradient_scaling ? 1u : 0u; cb.n_active = b.n_active; cb.ray_list = b.ray_list;
     cb.ebins_f = b.ebins_f; cb.sbins_f = b.sbins_f; cb.out_f = b.out_f; cb.grad_rgb = d_grad_rgb; cb.grad_acc = d_grad_acc;
     cb.bg0 = bg[0]; cb.bg1 = bg[1]; cb.bg2 = bg[2]; cb.dout = r->dout; cb.sums = det ? (float *)r->det_sums : r->gw + GW_SUMS;
+    cb.grad_ed = d_grad_ed; cb.dbounds = b.n_active + 4;
     const size_t smem_cb = SAMPLE_WARPS * sizeof(float) * 4 * ((size_t)S2 + 2);
-    auto k_cbwd = det ? k_composite_bwd<true> : k_composite_bwd<false>;
+    auto k_cbwd = d_grad_ed != nullptr ? (det ? k_composite_bwd<true, true> : k_composite_bwd<false, true>)
+                                       : (det ? k_composite_bwd<true> : k_composite_bwd<false>);
     TN_CUDA(cudaFuncSetAttribute(k_cbwd, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_cb));
     const uint32_t gridR = (R + SAMPLE_WARPS - 1) / SAMPLE_WARPS;
     if (r->profile) cudaEventRecord(r->evb[0], s);
@@ -1239,9 +1332,9 @@ extern "C" int tn_render_train_saved_bytes(tn_tracer *h, const tn_render_config 
     return TN_OK;
 }
 
-extern "C" int tn_render_train_forward_saved(tn_tracer *h, const tn_render_config *cfg, const float *d_origins, const float *d_directions,
-                                             uint32_t R, const float *d_jitter_coarse, const float *d_jitter_fine, float *d_rgb, float *d_acc,
-                                             float *d_depth, uint8_t *d_mask, void *d_saved, size_t saved_bytes, void *stream) {
+static int forward_saved(tn_tracer *h, const tn_render_config *cfg, const float *d_origins, const float *d_directions, uint32_t R,
+                         const float *d_jitter_coarse, const float *d_jitter_fine, float *d_rgb, float *d_acc, float *d_depth, uint8_t *d_mask,
+                         float *d_edepth, void *d_saved, size_t saved_bytes, void *stream) {
     if (!h || !d_saved) return fail(TN_ERR_ARG, "null argument");
     uint32_t S2 = 0;
     int rc = saved_shape(cfg, R, &S2);
@@ -1251,19 +1344,40 @@ extern "C" int tn_render_train_forward_saved(tn_tracer *h, const tn_render_confi
     if (saved_bytes < saved_layout(R, S2, (uint8_t *)d_saved, &b))
         return fail(TN_ERR_ARG, "tn_render_train_forward_saved: saved_bytes is smaller than tn_render_train_saved_bytes");
     TrainFwd tf{d_jitter_coarse, d_jitter_fine, &b};
-    rc = render_impl(h, cfg, d_origins, d_directions, R, d_rgb, d_acc, d_depth, d_mask, &tf, nullptr, stream);
+    rc = render_impl(h, cfg, d_origins, d_directions, R, d_rgb, d_acc, d_depth, d_mask, &tf, nullptr, d_edepth, stream);
     if (rc) return rc;
     RenderState *r = h->render;
-    const SavedHeader hd{SAVED_MAGIC, R, cfg->max_ray_triangles, cfg->num_samples, cfg->num_fine_samples, S2, r->det ? 1u : 0u, 0,
-                         {cfg->background[0], cfg->background[1], cfg->background[2]}, 0, r->gen, h->mesh_gen};
+    const SavedHeader hd{SAVED_MAGIC, R, cfg->max_ray_triangles, cfg->num_samples, cfg->num_fine_samples, S2, r->det ? 1u : 0u,
+                         d_edepth != nullptr ? 1u : 0u, {cfg->background[0], cfg->background[1], cfg->background[2]}, 0, r->gen, h->mesh_gen};
     DeviceGuard g(h->device);
     // pageable source: staged before the call returns, so `hd` may go out of scope
     TN_CUDA(cudaMemcpyAsync(d_saved, &hd, sizeof(hd), cudaMemcpyHostToDevice, (cudaStream_t)stream));
     return TN_OK;
 }
 
+extern "C" int tn_render_train_forward_saved(tn_tracer *h, const tn_render_config *cfg, const float *d_origins, const float *d_directions,
+                                             uint32_t R, const float *d_jitter_coarse, const float *d_jitter_fine, float *d_rgb, float *d_acc,
+                                             float *d_depth, uint8_t *d_mask, void *d_saved, size_t saved_bytes, void *stream) {
+    return forward_saved(h, cfg, d_origins, d_directions, R, d_jitter_coarse, d_jitter_fine, d_rgb, d_acc, d_depth, d_mask, nullptr, d_saved,
+                         saved_bytes, stream);
+}
+
+// tn_render_train_forward_saved plus the expected depth d_expected_depth f32[R] (DESIGN.md §4.10)
+extern "C" int tn_render_train_forward_saved_depth(tn_tracer *h, const tn_render_config *cfg, const float *d_origins, const float *d_directions,
+                                                   uint32_t R, const float *d_jitter_coarse, const float *d_jitter_fine, float *d_rgb, float *d_acc,
+                                                   float *d_depth, uint8_t *d_mask, float *d_expected_depth, void *d_saved, size_t saved_bytes,
+                                                   void *stream) {
+    if (!h || !d_expected_depth) return fail(TN_ERR_ARG, "null argument");
+    if (h->render && h->render->gather_world)
+        return fail(TN_ERR_ARG, "tn_render_train_forward_saved_depth: the fused pixel gather (tn_render_set_gather) carries no expected depth; "
+                                "switch it off first");
+    return forward_saved(h, cfg, d_origins, d_directions, R, d_jitter_coarse, d_jitter_fine, d_rgb, d_acc, d_depth, d_mask, d_expected_depth,
+                         d_saved, saved_bytes, stream);
+}
+
 static int backward_saved(tn_tracer *h, const void *d_saved, const float *d_grad_rgb, const float *d_grad_acc, int use_gradient_scaling,
-                          float *d_grad_field, float *const *d_grad_params12, const RayGradOut *rays, void *stream) {
+                          float *d_grad_field, float *const *d_grad_params12, const RayGradOut *rays, void *stream,
+                          const float *d_grad_ed = nullptr) {
     if (!h || !d_saved || !d_grad_rgb || !d_grad_field || !d_grad_params12) return fail(TN_ERR_ARG, "null argument");
     RenderState *r = h->render;
     if (!r || !r->n_active) return fail(TN_ERR_STATE, "tn_render_train_backward_saved: no training forward on this tracer");
@@ -1280,10 +1394,13 @@ static int backward_saved(tn_tracer *h, const void *d_saved, const float *d_grad
     if (rays != nullptr && hd.mesh_gen != h->mesh_gen)
         return fail(TN_ERR_STATE, "tn_render_train_backward_saved_geometry: tn_load_tetrahedra or tn_update_vertices ran since the forward "
                                   "(the ray and vertex gradients read the mesh positions)");
+    if (d_grad_ed != nullptr && hd.edepth == 0)
+        return fail(TN_ERR_STATE, "tn_render_train_backward_saved_depth: the forward produced no expected depth (use "
+                                  "tn_render_train_forward_saved_depth)");
     TrainBufs b{};
     saved_layout(hd.R, hd.S2, (uint8_t *)d_saved, &b);
     return train_backward_impl(h, b, hd.R, hd.S2, hd.det != 0, hd.bg, d_grad_rgb, d_grad_acc, use_gradient_scaling, d_grad_field,
-                               d_grad_params12, s, rays);
+                               d_grad_params12, s, rays, d_grad_ed);
 }
 
 extern "C" int tn_render_train_backward_saved(tn_tracer *h, const void *d_saved, const float *d_grad_rgb, const float *d_grad_acc,
@@ -1306,6 +1423,18 @@ extern "C" int tn_render_train_backward_saved_geometry(tn_tracer *h, const void 
                                                        float *d_grad_origins, float *d_grad_directions, float *d_grad_xyz, void *stream) {
     const RayGradOut rays{d_grad_origins, d_grad_directions, d_grad_xyz};
     return backward_saved(h, d_saved, d_grad_rgb, d_grad_acc, use_gradient_scaling, d_grad_field, d_grad_params12, &rays, stream);
+}
+
+// tn_render_train_backward_saved with the gradient of the expected depth d_grad_expected_depth f32[R] (NULL: none) and the optional ray /
+// vertex gradients of _geometry (all three NULL: tn_render_train_backward_saved's path, else _geometry's); DESIGN.md §4.10
+extern "C" int tn_render_train_backward_saved_depth(tn_tracer *h, const void *d_saved, const float *d_grad_rgb, const float *d_grad_acc,
+                                                    const float *d_grad_expected_depth, int use_gradient_scaling, float *d_grad_field,
+                                                    float *const *d_grad_params12, float *d_grad_origins, float *d_grad_directions,
+                                                    float *d_grad_xyz, void *stream) {
+    const RayGradOut rays{d_grad_origins, d_grad_directions, d_grad_xyz};
+    const bool any = d_grad_origins != nullptr || d_grad_directions != nullptr || d_grad_xyz != nullptr;
+    return backward_saved(h, d_saved, d_grad_rgb, d_grad_acc, use_gradient_scaling, d_grad_field, d_grad_params12, any ? &rays : nullptr,
+                          stream, d_grad_expected_depth);
 }
 
 // deterministic mode of the fused training step (see the header): applies from the next tn_render_train_forward on

@@ -86,10 +86,13 @@ class FusedRenderer:
         ext._check(_lib.tn_render_set_weights(self.tracer.handle, arr, self._stream()))
         self._keep = ts  # repacked on the stream; keep sources alive until then
 
-    def render(self, origins: torch.Tensor, directions: torch.Tensor, settings: RenderSettings, out: Optional[dict] = None, normals: bool = False):
+    def render(self, origins: torch.Tensor, directions: torch.Tensor, settings: RenderSettings, out: Optional[dict] = None, normals: bool = False,
+               expected_depth: bool = False):
         """eval-mode render -> `rgb` f32[R,3], `accumulation` / `depth` f32[R,1], `ray_mask` bool[R]; normals=True adds `normals`
         f32[R,3]: the composited unit normal of the density field (nerfstudio's "normals" output, (0, 0, 0) on empty rays; DESIGN §4.7).
-        The other outputs are the same bits as without normals.  Not available while a fused pixel gather is set."""
+        expected_depth=True adds `expected_depth` f32[R,1]: nerfstudio's DepthRenderer(method="expected"), clipped to the call's smallest
+        and largest sample midpoint, far_plane on empty rays (DESIGN §4.10).  The two combine; the other outputs are the same bits as
+        without them.  Neither is available while a fused pixel gather is set."""
         tr = self.tracer
         tr._check_float_dim3(origins, "ray_origins")
         tr._check_float_dim3(directions, "ray_directions")
@@ -105,9 +108,14 @@ class FusedRenderer:
         cfg = _config(settings)
         args = [tr.handle, C.byref(cfg), origins.data_ptr(), directions.data_ptr(), R, out["rgb"].data_ptr(), out["accumulation"].data_ptr(),
                 out["depth"].data_ptr(), out["ray_mask"].data_ptr()]
-        if normals:
-            if "normals" not in out:
-                out["normals"] = torch.empty((R, 3), dtype=torch.float32, device=dev)
+        if normals and "normals" not in out:
+            out["normals"] = torch.empty((R, 3), dtype=torch.float32, device=dev)
+        if expected_depth:
+            if "expected_depth" not in out:
+                out["expected_depth"] = torch.empty((R, 1), dtype=torch.float32, device=dev)
+            ext._check(_lib.tn_render_expected_depth(*args, out["expected_depth"].data_ptr(), out["normals"].data_ptr() if normals else None,
+                                                     self._stream()))
+        elif normals:
             ext._check(_lib.tn_render_normals(*args, out["normals"].data_ptr(), self._stream()))
         else:
             ext._check(_lib.tn_render(*args, self._stream()))
@@ -132,16 +140,18 @@ class FusedRenderer:
                 out["rgb"].data_ptr(), out["accumulation"].data_ptr(), out["depth"].data_ptr(), out["ray_mask"].data_ptr()]
         return R, out, args
 
-    def _train_backward(self, entry, lead, grad_rgb, grad_acc, num_vertices, use_gradient_scaling, tail=()):
-        """runs a training backward, entry(*lead, grads in, gradients out, *tail, stream) -> (grad_field, {name: gradient})"""
+    def _train_backward(self, entry, lead, grad_rgb, grad_acc, num_vertices, use_gradient_scaling, tail=(), grad_ed=()):
+        """runs a training backward, entry(*lead, grads in, gradients out, *tail, stream) -> (grad_field, {name: gradient}); grad_ed: () or
+        (the expected depth's gradient tensor or None,), passed after grad_acc"""
         grad_rgb = grad_rgb.contiguous()
         if grad_acc is not None:
             grad_acc = grad_acc.contiguous()
+        grad_ed = tuple(t.contiguous() if t is not None else None for t in grad_ed)
         gfield = torch.empty((64, num_vertices), dtype=torch.float32, device=self.device)
         gps = [torch.empty(sh, dtype=torch.float32, device=self.device) for sh in _SHAPES]
         arr = (_vp * 12)(*[t.data_ptr() for t in gps])
-        ext._check(entry(*lead, grad_rgb.data_ptr(), grad_acc.data_ptr() if grad_acc is not None else None, int(use_gradient_scaling),
-                         gfield.data_ptr(), arr, *tail, self._stream()))
+        ext._check(entry(*lead, grad_rgb.data_ptr(), grad_acc.data_ptr() if grad_acc is not None else None, *[t.data_ptr() if t is not None else None for t in grad_ed],
+                         int(use_gradient_scaling), gfield.data_ptr(), arr, *tail, self._stream()))
         return gfield, dict(zip(PARAM_ORDER, gps))
 
     def train_forward(self, origins: torch.Tensor, directions: torch.Tensor, settings: RenderSettings, jitter_coarse: Optional[torch.Tensor] = None,
@@ -166,36 +176,55 @@ class FusedRenderer:
         return n.value
 
     def train_forward_saved(self, origins: torch.Tensor, directions: torch.Tensor, settings: RenderSettings,
-                            jitter_coarse: Optional[torch.Tensor] = None, jitter_fine: Optional[torch.Tensor] = None):
+                            jitter_coarse: Optional[torch.Tensor] = None, jitter_fine: Optional[torch.Tensor] = None, expected_depth: bool = False):
         """train_forward whose backward state goes to a blob of its own instead of the tracer -> (outputs, TrainState).  Any number of
-        these can be in flight; train_backward_saved(state, ...) continues from the one it is given."""
+        these can be in flight; train_backward_saved(state, ...) continues from the one it is given.  expected_depth=True adds
+        `expected_depth` f32[R,1] to the outputs (as render's, in training mode; DESIGN §4.10), and its backward then accepts a gradient
+        for it; the other outputs are the same bits either way."""
         R, out, args = self._train_args(origins, directions, settings, jitter_coarse, jitter_fine)
         blob = torch.empty((self.train_saved_bytes(R, settings),), dtype=torch.uint8, device=self.device)
-        ext._check(_lib.tn_render_train_forward_saved(*args, blob.data_ptr(), blob.numel(), self._stream()))
+        if expected_depth:
+            out["expected_depth"] = torch.empty((R, 1), dtype=torch.float32, device=self.device)
+            ext._check(_lib.tn_render_train_forward_saved_depth(*args, out["expected_depth"].data_ptr(), blob.data_ptr(), blob.numel(),
+                                                                self._stream()))
+        else:
+            ext._check(_lib.tn_render_train_forward_saved(*args, blob.data_ptr(), blob.numel(), self._stream()))
         return out, TrainState(blob, R)
 
     def train_backward_saved(self, state: "TrainState", grad_rgb: torch.Tensor, grad_acc: Optional[torch.Tensor], num_vertices: int,
                              use_gradient_scaling: bool = False, grad_origins: bool = False, grad_directions: bool = False,
-                             grad_vertices: bool = False):
+                             grad_vertices: bool = False, grad_expected_depth: Optional[torch.Tensor] = None):
         """backward of the train_forward_saved call that returned `state`; outputs as train_backward.  Raises RuntimeError if
         set_field / set_weights ran since that forward.  Waits until the stream has reached it (it reads the call's shape back).
         grad_origins / grad_directions: also the gradients at the forward's ray origins / directions (the sample distances held fixed;
         DESIGN §4.8) -> (grad_field, grads, grad_origins f32[R,3] or None, grad_directions f32[R,3] or None), 0 on empty rays; then it
         also raises RuntimeError if load_tetrahedra ran since that forward.  grad_vertices: also the gradient at the mesh vertex positions
         (the matched tetrahedra held fixed as well; DESIGN §4.9) -> (grad_field, grads, grad_origins or None, grad_directions or None,
-        grad_vertices f32[V,3]); then it raises RuntimeError if load_tetrahedra or update_vertices ran since that forward."""
+        grad_vertices f32[V,3]); then it raises RuntimeError if load_tetrahedra or update_vertices ran since that forward.
+        grad_expected_depth f32[R] or [R,1]: dL/d expected_depth of a forward with expected_depth=True (RuntimeError otherwise); the
+        outputs keep the form above."""
         if tuple(grad_rgb.shape) != (state.R, 3) or (grad_acc is not None and grad_acc.numel() != state.R):
             raise RuntimeError(f"the forward rendered {state.R} rays: grad_rgb must be [{state.R}, 3] and grad_acc [{state.R}], got "
                                f"{tuple(grad_rgb.shape)} and {None if grad_acc is None else tuple(grad_acc.shape)}")
         lead = [self.tracer.handle, state.blob.data_ptr()]
-        if not (grad_origins or grad_directions or grad_vertices):
-            return self._train_backward(_lib.tn_render_train_backward_saved, lead, grad_rgb, grad_acc, num_vertices, use_gradient_scaling)
+        rays = grad_origins or grad_directions or grad_vertices
         go = torch.empty((state.R, 3), dtype=torch.float32, device=self.device) if grad_origins else None
         gd = torch.empty((state.R, 3), dtype=torch.float32, device=self.device) if grad_directions else None
         gv = torch.empty((num_vertices, 3), dtype=torch.float32, device=self.device) if grad_vertices else None
         tail = tuple(t.data_ptr() if t is not None else None for t in (go, gd, gv))
-        gfield, gp = self._train_backward(_lib.tn_render_train_backward_saved_geometry, lead, grad_rgb, grad_acc, num_vertices,
-                                          use_gradient_scaling, tail)
+        if grad_expected_depth is not None:
+            g = grad_expected_depth
+            if g.numel() != state.R or g.device != self.device or g.dtype != torch.float32:
+                raise RuntimeError(f"grad_expected_depth must be a float32 [{state.R}] tensor on the tracer's device, got {tuple(g.shape)}")
+            gfield, gp = self._train_backward(_lib.tn_render_train_backward_saved_depth, lead, grad_rgb, grad_acc, num_vertices,
+                                              use_gradient_scaling, tail, grad_ed=(g.reshape(-1),))
+        elif not rays:
+            return self._train_backward(_lib.tn_render_train_backward_saved, lead, grad_rgb, grad_acc, num_vertices, use_gradient_scaling)
+        else:
+            gfield, gp = self._train_backward(_lib.tn_render_train_backward_saved_geometry, lead, grad_rgb, grad_acc, num_vertices,
+                                              use_gradient_scaling, tail)
+        if not rays:
+            return gfield, gp
         return (gfield, gp, go, gd, gv) if grad_vertices else (gfield, gp, go, gd)
 
     # ---- surface extraction ---------------------------------------------------------------------------------------------------------
@@ -283,41 +312,74 @@ class FusedTrainRender(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, fr, settings, use_gradient_scaling, origins, directions, jitter_coarse, jitter_fine, field, *params):
-        if len(params) == len(PARAM_ORDER) + 1:
-            xyz, borrowed = params[-1], fr.tracer._vertices
-            if borrowed is None or xyz.data_ptr() != borrowed.data_ptr() or xyz.shape != borrowed.shape:
-                raise RuntimeError("FusedTrainRender: the vertex positions must be the tensor the tracer borrowed (load_tetrahedra / "
-                                   "update_vertices), with the same number of vertices")
-            if xyz._version != fr.tracer._vertices_version:  # (a detached view shares the parameter's version counter)
-                raise RuntimeError("FusedTrainRender: the vertex positions changed in place since the tracer was loaded or refit; call "
-                                   "update_vertices first")
-        elif len(params) != len(PARAM_ORDER):
-            raise RuntimeError(f"FusedTrainRender takes the {len(PARAM_ORDER)} MLP parameters and optionally the vertex positions")
-        out, state = fr.train_forward_saved(origins, directions, settings, jitter_coarse, jitter_fine)
-        ctx.fr, ctx.state, ctx.gs = fr, state, bool(use_gradient_scaling)
-        ctx.ray_shapes = (origins.shape, directions.shape)
-        ctx.save_for_backward(field, *params)  # their version counters reject a backward after an in-place change
-        ctx.mark_non_differentiable(out["depth"], out["ray_mask"])
+        out = _fused_forward(ctx, "FusedTrainRender", False, fr, settings, use_gradient_scaling, origins, directions, jitter_coarse,
+                             jitter_fine, field, params)
         return out["rgb"], out["accumulation"], out["depth"], out["ray_mask"]
 
     @staticmethod
     def backward(ctx, g_rgb, g_acc, _g_depth, _g_mask):
-        field = ctx.saved_tensors[0]
-        if g_rgb is None:
-            g_rgb = torch.zeros((ctx.state.R, 3), dtype=torch.float32, device=field.device)
-        want_o, want_d = ctx.needs_input_grad[3], ctx.needs_input_grad[4]
-        has_xyz = len(ctx.needs_input_grad) == 8 + len(PARAM_ORDER) + 1
-        want_v = has_xyz and ctx.needs_input_grad[-1]
-        g_acc = g_acc.reshape(-1) if g_acc is not None else None
-        go = gd = gv = None
-        if want_v:
-            gfield, gp, go, gd, gv = ctx.fr.train_backward_saved(ctx.state, g_rgb, g_acc, field.shape[1], ctx.gs, grad_origins=want_o,
-                                                                 grad_directions=want_d, grad_vertices=True)
-        elif want_o or want_d:
-            gfield, gp, go, gd = ctx.fr.train_backward_saved(ctx.state, g_rgb, g_acc, field.shape[1], ctx.gs, grad_origins=want_o,
-                                                             grad_directions=want_d)
-        else:
-            gfield, gp = ctx.fr.train_backward_saved(ctx.state, g_rgb, g_acc, field.shape[1], ctx.gs)
-        go = go.reshape(ctx.ray_shapes[0]) if go is not None else None
-        gd = gd.reshape(ctx.ray_shapes[1]) if gd is not None else None
-        return (None, None, None, go, gd, None, None, gfield) + tuple(gp[n] for n in PARAM_ORDER) + ((gv,) if has_xyz else ())
+        return _fused_backward(ctx, g_rgb, g_acc, None)
+
+
+class FusedTrainRenderDepth(torch.autograd.Function):
+    """FusedTrainRender with the expected depth (DESIGN §4.10): the same arguments (the optional vertex positions included), outputs
+    (rgb, accumulation, depth, expected_depth, ray_mask) with expected_depth f32[R,1] nerfstudio's DepthRenderer(method="expected") over
+    the fine samples (clipped to the call's smallest / largest sample midpoint, far_plane on empty rays).  rgb, accumulation and
+    expected_depth are differentiable: a depth loss reaches the field, the MLP and, when they require grad, the ray origins / directions
+    and the vertex positions (tn_render_train_forward_saved_depth / tn_render_train_backward_saved_depth).  The other outputs are the
+    same bits as FusedTrainRender's."""
+
+    @staticmethod
+    def forward(ctx, fr, settings, use_gradient_scaling, origins, directions, jitter_coarse, jitter_fine, field, *params):
+        out = _fused_forward(ctx, "FusedTrainRenderDepth", True, fr, settings, use_gradient_scaling, origins, directions, jitter_coarse,
+                             jitter_fine, field, params)
+        return out["rgb"], out["accumulation"], out["depth"], out["expected_depth"], out["ray_mask"]
+
+    @staticmethod
+    def backward(ctx, g_rgb, g_acc, _g_depth, g_ed, _g_mask):
+        return _fused_backward(ctx, g_rgb, g_acc, g_ed)
+
+
+def _fused_forward(ctx, name, expected_depth, fr, settings, use_gradient_scaling, origins, directions, jitter_coarse, jitter_fine, field, params):
+    """forward of FusedTrainRender / FusedTrainRenderDepth: checks the optional vertex positions, runs the saved training forward and
+    keeps what the backward needs in ctx -> the forward's outputs"""
+    if len(params) == len(PARAM_ORDER) + 1:
+        xyz, borrowed = params[-1], fr.tracer._vertices
+        if borrowed is None or xyz.data_ptr() != borrowed.data_ptr() or xyz.shape != borrowed.shape:
+            raise RuntimeError(f"{name}: the vertex positions must be the tensor the tracer borrowed (load_tetrahedra / "
+                               "update_vertices), with the same number of vertices")
+        if xyz._version != fr.tracer._vertices_version:  # (a detached view shares the parameter's version counter)
+            raise RuntimeError(f"{name}: the vertex positions changed in place since the tracer was loaded or refit; call "
+                               "update_vertices first")
+    elif len(params) != len(PARAM_ORDER):
+        raise RuntimeError(f"{name} takes the {len(PARAM_ORDER)} MLP parameters and optionally the vertex positions")
+    out, state = fr.train_forward_saved(origins, directions, settings, jitter_coarse, jitter_fine, expected_depth=expected_depth)
+    ctx.fr, ctx.state, ctx.gs = fr, state, bool(use_gradient_scaling)
+    ctx.ray_shapes = (origins.shape, directions.shape)
+    ctx.save_for_backward(field, *params)  # their version counters reject a backward after an in-place change
+    ctx.mark_non_differentiable(out["depth"], out["ray_mask"])
+    return out
+
+
+def _fused_backward(ctx, g_rgb, g_acc, g_ed):
+    """backward of FusedTrainRender / FusedTrainRenderDepth (g_ed: the expected depth's gradient, or None)"""
+    field = ctx.saved_tensors[0]
+    if g_rgb is None:
+        g_rgb = torch.zeros((ctx.state.R, 3), dtype=torch.float32, device=field.device)
+    want_o, want_d = ctx.needs_input_grad[3], ctx.needs_input_grad[4]
+    has_xyz = len(ctx.needs_input_grad) == 8 + len(PARAM_ORDER) + 1
+    want_v = has_xyz and ctx.needs_input_grad[-1]
+    g_acc = g_acc.reshape(-1) if g_acc is not None else None
+    g_ed = g_ed.reshape(-1) if g_ed is not None else None
+    go = gd = gv = None
+    if want_v:
+        gfield, gp, go, gd, gv = ctx.fr.train_backward_saved(ctx.state, g_rgb, g_acc, field.shape[1], ctx.gs, grad_origins=want_o,
+                                                             grad_directions=want_d, grad_vertices=True, grad_expected_depth=g_ed)
+    elif want_o or want_d:
+        gfield, gp, go, gd = ctx.fr.train_backward_saved(ctx.state, g_rgb, g_acc, field.shape[1], ctx.gs, grad_origins=want_o,
+                                                         grad_directions=want_d, grad_expected_depth=g_ed)
+    else:
+        gfield, gp = ctx.fr.train_backward_saved(ctx.state, g_rgb, g_acc, field.shape[1], ctx.gs, grad_expected_depth=g_ed)
+    go = go.reshape(ctx.ray_shapes[0]) if go is not None else None
+    gd = gd.reshape(ctx.ray_shapes[1]) if gd is not None else None
+    return (None, None, None, go, gd, None, None, gfield) + tuple(gp[n] for n in PARAM_ORDER) + ((gv,) if has_xyz else ())

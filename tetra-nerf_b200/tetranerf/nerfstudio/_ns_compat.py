@@ -247,8 +247,18 @@ class AccumulationRenderer(nn.Module):
 
 
 class DepthRenderer(nn.Module):
+    def __init__(self, method="median"):
+        super().__init__()
+        if method not in ("median", "expected"):
+            raise NotImplementedError(f"DepthRenderer method {method!r}")
+        self.method = method
+
     def forward(self, weights, ray_samples):
         steps = (ray_samples.frustums.starts + ray_samples.frustums.ends) / 2
+        if self.method == "expected":  # clipped to the smallest / largest midpoint of the whole batch (DESIGN §4.10)
+            eps = 1e-10
+            depth = torch.sum(weights * steps, dim=-2) / (torch.sum(weights, -2) + eps)
+            return torch.clip(depth, steps.min(), steps.max())
         cum = torch.cumsum(weights[..., 0], dim=-1)
         split = torch.ones((*weights.shape[:-2], 1), device=weights.device) * 0.5
         idx = torch.clamp(torch.searchsorted(cum, split, side="left"), 0, steps.shape[-2] - 1)

@@ -78,6 +78,15 @@ class TetrahedraNerfConfig(ModelConfig):
     optimize_vertices: bool = False
     """train the mesh vertex positions too: `tetrahedra_vertices` becomes a parameter in its own param group "vertices" (same state-dict
     key and shape), the tracer is refit after every optimizer step (topology fixed), training runs on the fused path only (DESIGN §4.9)"""
+    render_expected_depth: bool = False
+    """every path (fused eval, fused training, unfused) also returns "expected_depth" f32[R,1], nerfstudio's
+    DepthRenderer(method="expected") clipped to the batch's smallest / largest sample midpoint, far plane on empty rays (DESIGN §4.10);
+    differentiable in training"""
+    depth_loss_mult: float = 0.0
+    """> 0: implies render_expected_depth and adds depth_loss = depth_loss_mult * mean over rays with hits and a finite target > 0 of
+    (expected_depth - target)^2, the target batch["depth_image"] [R,1] in the model's frame"""
+    is_euclidean_depth: bool = False
+    """the depth target is the distance along the ray; False: z-depth, multiplied by the ray bundle's metadata["directions_norm"]"""
 
     def __post_init__(self):
         if self.tetrahedra_path is not None and self.num_tetrahedra_vertices is None:
@@ -286,6 +295,7 @@ class TetrahedraNerf(Model):
         self.renderer_rgb = RGBRenderer(background_color=self.config.background_color)
         self.renderer_accumulation = AccumulationRenderer()
         self.renderer_depth = DepthRenderer()
+        self.renderer_expected_depth = DepthRenderer(method="expected")
         self.rgb_loss = MSELoss()
 
     def get_param_groups(self) -> Dict[str, List[Parameter]]:
@@ -324,7 +334,20 @@ class TetrahedraNerf(Model):
         return self._fused
 
     # ---- forward (reference :520-662) ---------------------------------------------------------------------
+    def _expected_depth_on(self) -> bool:
+        return self.config.render_expected_depth or self.config.depth_loss_mult > 0
+
     def get_outputs(self, ray_bundle: RayBundle):
+        outputs = self._get_outputs(ray_bundle)
+        # the z-depth target's conversion to a distance along the ray, for get_loss_dict only: in training, and in nerfstudio's eval
+        # loss (get_eval_loss_dict renders in eval mode and calls get_loss_dict too)
+        if self.config.depth_loss_mult > 0 and not self.config.is_euclidean_depth:
+            dn = (getattr(ray_bundle, "metadata", None) or {}).get("directions_norm")
+            if dn is not None:
+                outputs["directions_norm"] = dn
+        return outputs
+
+    def _get_outputs(self, ray_bundle: RayBundle):
         assert self.collider is not None
         origins, directions = ray_bundle.origins.contiguous(), ray_bundle.directions.contiguous()
         normals = self.config.render_normals and not self.training
@@ -337,7 +360,7 @@ class TetrahedraNerf(Model):
             st = RenderSettings(self.config.max_intersected_triangles, self.config.num_samples, self.config.num_fine_samples,
                                 self.config.use_biased_sampler, float(self.collider.far_plane), bg)
             with torch.no_grad():
-                return self._fused_renderer().render(origins, directions, st, normals=normals)
+                return self._fused_renderer().render(origins, directions, st, normals=normals, expected_depth=self._expected_depth_on())
         unfused_train = os.environ.get("TETRANERF_B200_UNFUSED_TRAIN", "0") == "1"
         if self.training and torch.is_grad_enabled() and self.config.optimize_vertices:
             causes = self._fused_unsupported() + (["num_fine_samples=0"] if self.config.num_fine_samples == 0 else []) \
@@ -351,7 +374,7 @@ class TetrahedraNerf(Model):
     def _get_outputs_fused_train(self, origins, directions):
         """training step on the fused CUDA pipeline: ONE differentiable op (forward + wgmma backward) instead of the reference's op
         sequence; the stratified draws are the same two torch.rand calls the reference makes (model.py:169-174, PDFSampler)."""
-        from ..b200.render import PARAM_ORDER, FusedTrainRender, RenderSettings
+        from ..b200.render import PARAM_ORDER, FusedTrainRender, FusedTrainRenderDepth, RenderSettings
 
         c = self.config
         bg = (1.0, 1.0, 1.0) if c.background_color == "white" else (0.0, 0.0, 0.0)
@@ -362,8 +385,11 @@ class TetrahedraNerf(Model):
         jf = torch.rand((R, c.num_fine_samples + 1), dtype=torch.float32, device=dev) if getattr(self.sampler_pdf, "train_stratified", True) else None
         named = dict(self.named_parameters())
         xyz = (self.tetrahedra_vertices,) if c.optimize_vertices else ()  # the tensor the tracer borrowed (get_tetrahedra_tracer)
-        rgb, acc, depth, mask = FusedTrainRender.apply(fr, st, c.use_gradient_scaling, origins, directions, jc, jf, self.tetrahedra_field,
-                                                       *[named[n] for n in PARAM_ORDER], *xyz)
+        args = (fr, st, c.use_gradient_scaling, origins, directions, jc, jf, self.tetrahedra_field, *[named[n] for n in PARAM_ORDER], *xyz)
+        if self._expected_depth_on():
+            rgb, acc, depth, ed, mask = FusedTrainRenderDepth.apply(*args)
+            return {"rgb": rgb, "accumulation": acc, "depth": depth, "expected_depth": ed, "ray_mask": mask}
+        rgb, acc, depth, mask = FusedTrainRender.apply(*args)
         return {"rgb": rgb, "accumulation": acc, "depth": depth, "ray_mask": mask}
 
     def _field_at(self, tracer, traced, ray_mask, distances):
@@ -384,6 +410,9 @@ class TetrahedraNerf(Model):
         rgb = self.get_background_color((R, 3), device=device)
         accumulation = torch.zeros((R, 1), dtype=torch.float32, device=device)
         depth = torch.full((R, 1), self.collider.far_plane, dtype=torch.float32, device=device)
+        outputs = {"rgb": rgb, "accumulation": accumulation, "depth": depth, "ray_mask": ray_mask}
+        if self._expected_depth_on():
+            outputs["expected_depth"] = depth.clone()
         if bool(ray_mask.any()):
             bundle = dataclasses.replace(ray_bundle[ray_mask], nears=nears[ray_mask], fars=fars[ray_mask])
             if isinstance(self.sampler_uniform, TetrahedraSampler):
@@ -411,7 +440,9 @@ class TetrahedraNerf(Model):
             rgb[ray_mask] = self.renderer_rgb(rgb=colors, weights=weights)
             accumulation[ray_mask] = self.renderer_accumulation(weights)
             depth[ray_mask] = self.renderer_depth(weights, samples)
-        return {"rgb": rgb, "accumulation": accumulation, "depth": depth, "ray_mask": ray_mask}
+            if self._expected_depth_on():
+                outputs["expected_depth"][ray_mask] = self.renderer_expected_depth(weights, samples)
+        return outputs
 
     # ---- geometry export -----------------------------------------------------------------------------------------------------------------
     def extract_surface(self, level: float) -> Dict[str, torch.Tensor]:
@@ -427,7 +458,24 @@ class TetrahedraNerf(Model):
 
     def get_loss_dict(self, outputs, batch, metrics_dict=None) -> Dict[str, torch.Tensor]:
         image = batch["image"].to(outputs["rgb"].device)
-        return scale_dict({"rgb_loss": self.rgb_loss(image, outputs["rgb"])}, self.config.loss_coefficients)
+        losses = {"rgb_loss": self.rgb_loss(image, outputs["rgb"])}
+        if self.config.depth_loss_mult > 0:
+            losses["depth_loss"] = self.config.depth_loss_mult * self._depth_loss(outputs, batch)
+        return scale_dict(losses, self.config.loss_coefficients)
+
+    def _depth_loss(self, outputs, batch) -> torch.Tensor:
+        """mean over rays with hits and a finite target > 0 of (expected_depth - target)^2; the target batch["depth_image"] [R,1] is a
+        distance along the ray (is_euclidean_depth) or a z-depth, converted with outputs["directions_norm"]"""
+        ed = outputs["expected_depth"]
+        target = batch["depth_image"].to(ed.device).reshape(ed.shape).to(ed.dtype)
+        if not self.config.is_euclidean_depth:
+            if "directions_norm" not in outputs:
+                raise RuntimeError("depth_loss_mult > 0 with a z-depth target (is_euclidean_depth=False) needs the ray bundle's "
+                                   'metadata["directions_norm"] to turn z-depth into a distance along the ray')
+            target = target * outputs["directions_norm"].to(ed.device).reshape(ed.shape)
+        valid = outputs["ray_mask"].reshape(-1, 1) & torch.isfinite(target) & (target > 0)
+        sq = torch.where(valid, ed - torch.where(valid, target, torch.zeros_like(target)), torch.zeros_like(ed)) ** 2
+        return sq.sum() / valid.sum().clamp_min(1)
 
     # ---- evaluation images and metrics (reference :676-713) --------------------------------------------------------------------------
     def get_image_metrics_and_images(self, outputs: Dict[str, torch.Tensor], batch: Dict[str, torch.Tensor]):
@@ -436,6 +484,8 @@ class TetrahedraNerf(Model):
         acc = _apply_colormap(outputs["accumulation"])
         depth = _apply_depth_colormap(outputs["depth"], accumulation=outputs["accumulation"])
         images = {"img": torch.cat([image, rgb], dim=1), "accumulation": torch.cat([acc], dim=1), "depth": torch.cat([depth], dim=1)}
+        if "expected_depth" in outputs:
+            images["expected_depth"] = _apply_depth_colormap(outputs["expected_depth"], accumulation=outputs["accumulation"])
         if "normals" in outputs:  # unit normals in [-1, 1] shown as colours in [0, 1]
             images["normals"] = (outputs["normals"] + 1.0) / 2.0
         # [H, W, C] -> [1, C, H, W]
