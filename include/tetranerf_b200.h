@@ -113,9 +113,13 @@ int tn_interpolate_values_backward_deterministic(int device, uint32_t D, uint32_
  * Weights are passed once (tn_render_set_weights) in nerfstudio state-dict layout and repacked on
  * the device.  See DESIGN.md §"fused render". */
 typedef struct tn_render_config {
-    uint32_t max_ray_triangles; /* M, power of two                      model.py:77  */
-    uint32_t num_samples;       /* S_c                                  model.py:78  */
-    uint32_t num_fine_samples;  /* S_f (0 = single pass)                model.py:79  */
+    uint32_t max_ray_triangles; /* M, power of two in [2, 2048]         model.py:77  */
+    uint32_t num_samples;       /* S_c in [1, 4096]                     model.py:78  */
+    uint32_t num_fine_samples;  /* S_f in [0, 4096] (0 = single pass)   model.py:79  */
+    /* With S_f > 0 the per-ray fine sampler stages 16 (M + 4 S2 + 10) bytes of shared memory per block, S2 = S_c + S_f + 1, and the
+     * training backward's composite stage 64 (S2 + 2): a call whose largest staging exceeds the device's opt-in shared memory per
+     * block (cudaDevAttrMaxSharedMemoryPerBlockOptin; 232,448 B on an H100) returns TN_ERR_ARG before anything runs.  On an H100
+     * that is S_c + S_f > 3500 at M = 512 and > 3116 at M = 2048.  Single-pass settings (S_f = 0) always fit. */
     uint32_t use_biased_sampler;/*                                      model.py:80  */
     float far_plane;            /* collider far plane: depth of empty rays (model.py:645-650) */
     float background[3];        /* renderer background colour (white = 1,1,1; model.py:93) */

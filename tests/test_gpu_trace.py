@@ -131,8 +131,10 @@ def test_cube_edge_and_vertex_rays(cube_mesh):
     assert_same(gpu_trace(tr, o, d, 32), orc.OracleMesh(V, C).trace_rays(o, d, 32))
 
 
-@pytest.mark.parametrize("gen,M", [(syn.camera_rays, 512), (syn.sphere_rays, 256), (syn.camera_rays, 64), (syn.camera_rays, 16)])
+@pytest.mark.parametrize("gen,M", [(syn.camera_rays, 512), (syn.sphere_rays, 256), (syn.camera_rays, 64), (syn.camera_rays, 16),
+                                   (syn.camera_rays, 2), (syn.camera_rays, 4), (syn.camera_rays, 2048)])
 def test_random_mesh_bit_exact(small_mesh, gen, M):
+    """M = 2 keeps no cell on any ray, M = 4 truncates nearly every ray, M = 2048 is the largest hit cap"""
     V, C = small_mesh
     tr = make_tracer(V, C)
     o, d = gen(700)
@@ -142,6 +144,19 @@ def test_random_mesh_bit_exact(small_mesh, gen, M):
         assert g["num_visited_cells"].max() > 40
     else:
         assert g["num_visited_cells"].max() <= M - 2
+    if M == 4:
+        assert (g["num_visited_cells"] == 2).mean() > 0.9
+
+
+@pytest.mark.parametrize("R", [1, 3, 9])
+def test_tiny_batches_bit_exact(small_mesh, R):
+    """batches below the 4-warp blocks and not a multiple of the quad walk's 8 rays per warp"""
+    V, C = small_mesh
+    tr = make_tracer(V, C)
+    o, d = syn.camera_rays(R, seed=30 + R)
+    g = gpu_trace(tr, o, d, 512)
+    assert_same(g, orc.OracleMesh(V, C).trace_rays(o, d, 512), f"R={R} ")
+    assert g["num_visited_cells"].min() > 0
 
 
 def test_medium_mesh_bit_exact(medium_mesh):

@@ -72,6 +72,7 @@ struct RenderState {
     bool det = false;                  // mode of the next training forward (initial value: TETRANERF_B200_DETERMINISTIC)
     bool t_det = false;                // mode the last training forward ran in: its backward continues in it
     uint32_t bwd_grid = 0;             // CTAs of the backward MLP kernel (test hook; 0 = default)
+    int smem_optin = 0;                // the device's opt-in dynamic shared memory per block (read on the first render call)
     uint32_t *ray_flag = nullptr, *ray_slot = nullptr;  // [R] ray has hits, its slot (exclusive scan)
     size_t cap_slot_R = 0;
     void *cub_tmp = nullptr;           // CUB scan / sort temporary storage
@@ -991,6 +992,24 @@ static int render_impl(tn_tracer *h, const tn_render_config *cfg, const float *d
     const uint32_t S2 = single ? Sc : Sc + Sf + 1;     // PDFSampler include_original (model.py:463)
     DeviceGuard g(h->device);
     cudaStream_t s = (cudaStream_t)stream;
+    // dynamic shared memory of the per-ray kernels (4 warps per block, one ray per warp): checked before anything is allocated or
+    // launched, so a setting that cannot run fails as an argument error and leaves no CUDA error behind
+    const size_t smem_sc = SAMPLE_WARPS * sizeof(float) * coarse_floats(M, Sc, cfg->use_biased_sampler);
+    const size_t smem_sf = SAMPLE_WARPS * sizeof(float) * fine_floats(M, std::max(Sc, S2));
+    const size_t smem_c = SAMPLE_WARPS * sizeof(float) * 2 * ((size_t)S2 + 2);
+    const size_t smem_cb = SAMPLE_WARPS * sizeof(float) * 4 * ((size_t)S2 + 2);  // k_composite_bwd, which the backward launches
+    if (!r->smem_optin) TN_CUDA(cudaDeviceGetAttribute(&r->smem_optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, h->device));
+    {
+        size_t need = std::max(smem_sc, smem_c);
+        const char *kern = smem_sc >= smem_c ? "k_sample_coarse" : "k_composite";
+        if (!single && smem_sf > need) { need = smem_sf; kern = "k_sample_fine"; }
+        if (tf != nullptr && smem_cb > need) { need = smem_cb; kern = "k_composite_bwd"; }
+        if (need > (size_t)r->smem_optin)
+            return fail(TN_ERR_ARG, "tn_render: num_samples + num_fine_samples = " + std::to_string(Sc + Sf) + " at max_ray_triangles = " +
+                                        std::to_string(M) + " needs " + std::to_string(need) + " bytes of shared memory per block in " + kern +
+                                        ", above the device's shared-memory limit of " + std::to_string(r->smem_optin) +
+                                        " bytes (fewer samples or a smaller max_ray_triangles)");
+    }
     int rc = ensure_ws(r, R, M, Sc, S2);
     if (rc) return rc;
     if (d_normals != nullptr && (size_t)R * S2 > r->cap_grad_n) {
@@ -1036,13 +1055,10 @@ static int render_impl(tn_tracer *h, const tn_render_config *cfg, const float *d
         for (int k = 0; k < 8; ++k) p.peer[k] = r->peer[k];
         p.gather_world = r->gather_world; p.gather_rank = r->gather_rank; p.gather_stride = r->gather_stride;
     }
-    const uint32_t Smax = std::max(Sc, S2);
-    const size_t smem_sc = SAMPLE_WARPS * sizeof(float) * coarse_floats(M, Sc, p.biased);
-    const size_t smem_sf = SAMPLE_WARPS * sizeof(float) * fine_floats(M, Smax);
-    const size_t smem_c = SAMPLE_WARPS * sizeof(float) * 2 * ((size_t)S2 + 2);
     auto k_coarse_sample = det ? k_sample_coarse<true> : k_sample_coarse<false>;
     TN_CUDA(cudaFuncSetAttribute(k_coarse_sample, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_sc));
-    TN_CUDA(cudaFuncSetAttribute(k_sample_fine, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_sf));
+    // (single pass: k_sample_fine is not launched, and its staging at S2 = Sc can exceed the limit where the call itself fits)
+    if (!single) TN_CUDA(cudaFuncSetAttribute(k_sample_fine, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_sf));
     auto k_comp = d_edepth != nullptr ? k_composite<true> : k_composite<false>;
     TN_CUDA(cudaFuncSetAttribute(k_comp, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_c));
     auto launch_coarse = prec == 2 ? launch_mlp<false, 2> : launch_mlp<false, 3>;

@@ -27,7 +27,11 @@ _SHAPES = [(128, 64), (128,), (128, 128), (128,), (128, 128), (128,), (128, 155)
 
 @dataclass
 class RenderSettings:
-    """hot-path subset of TetrahedraNerfConfig (model.py:70-107)"""
+    """hot-path subset of TetrahedraNerfConfig (model.py:70-107).  max_intersected_triangles (M) is a power of two in [2, 2048],
+    num_samples in [1, 4096], num_fine_samples in [0, 4096] (0 = single pass).  Two-pass settings must also fit the per-ray kernels'
+    shared memory: 16 (M + 4 S2 + 10) bytes per block with S2 = num_samples + num_fine_samples + 1, at most the device's opt-in limit
+    (232,448 B on an H100: num_samples + num_fine_samples <= 3500 at M = 512, <= 3116 at M = 2048); beyond it render and the
+    training forwards raise RuntimeError before anything runs."""
 
     max_intersected_triangles: int = 512
     num_samples: int = 256
