@@ -135,25 +135,18 @@ int tn_render_set_mlp_precision(tn_tracer *h, int prec);
 /* mlp_base.layers.{0,1,2}.{weight,bias}, mlp_head.layers.0.{weight,bias}, field_output_color.net.*,
  * field_output_density.net.* as 12 device pointers in that order (torch nn.Linear [out,in] layout). */
 int tn_render_set_weights(tn_tracer *h, const float *const *d_params12, void *stream);
-/* d_rgb f32[R,3], d_acc f32[R,1], d_depth f32[R,1], d_mask u8[R] */
+/* d_rgb f32[R,3], d_acc f32[R,1], d_depth f32[R,1], d_mask u8[R].  Two optional outputs (NULL: not computed; every element of a
+ * non-NULL one is written); the other outputs are the same bits with or without them:
+ *   d_expected_depth f32[R], nerfstudio DepthRenderer(method="expected"): over the samples that give rgb (the fine pass; the coarse one
+ *     when num_fine_samples = 0), t_i the bin midpoints and w_i the weights of rgb, A = sum w_i: D_raw = sum w_i t_i / (A + 1e-10), and
+ *     D = clip(D_raw, t_min, t_max) with t_min / t_max the smallest / largest midpoint over every active ray of the call; far_plane on
+ *     empty rays.  DESIGN.md §4.10.
+ *   d_normals f32[R,3]: per sample the exact gradient of the density pre-activation (reverse pass through mlp_base in the render's
+ *     operand precision, then grad = cof(E) q / det(E) on the matched tetrahedron), n = -grad / |grad|, composited with the weights of
+ *     rgb and normalised (nerfstudio NormalsRenderer(normalize=True)); (0,0,0) on empty rays.  DESIGN.md §4.7.
+ * TN_ERR_ARG if either is given while a fused pixel gather is set (tn_render_set_gather). */
 int tn_render(tn_tracer *h, const tn_render_config *cfg, const float *d_origins, const float *d_directions, uint32_t R,
-              float *d_rgb, float *d_acc, float *d_depth, uint8_t *d_mask, void *stream);
-/* tn_render plus the normal map d_normals f32[R,3] (every element written): per sample the exact gradient of the density
- * pre-activation (reverse pass through mlp_base in the render's operand precision, then grad = cof(E) q / det(E) on the matched
- * tetrahedron), n = -grad / |grad|, composited with the weights of rgb and normalised (nerfstudio NormalsRenderer(normalize=True));
- * (0,0,0) on empty rays.  rgb, acc, depth and mask are the same bits as tn_render's.  TN_ERR_ARG while a fused pixel gather is set
- * (tn_render_set_gather).  DESIGN.md §4.7. */
-int tn_render_normals(tn_tracer *h, const tn_render_config *cfg, const float *d_origins, const float *d_directions, uint32_t R,
-                      float *d_rgb, float *d_acc, float *d_depth, uint8_t *d_mask, float *d_normals, void *stream);
-/* tn_render plus the expected depth d_expected_depth f32[R] (every element written; nerfstudio DepthRenderer(method="expected")) and,
- * if d_normals is not NULL, the normal map of tn_render_normals.  Over the samples that give rgb (the fine pass; the coarse one when
- * num_fine_samples = 0), t_i the bin midpoints and w_i the weights of rgb, A = sum w_i: D_raw = sum w_i t_i / (A + 1e-10), and
- * D = clip(D_raw, t_min, t_max) with t_min / t_max the smallest / largest midpoint over every active ray of the call; far_plane on empty
- * rays.  rgb, acc, depth, mask and normals are the same bits as without it.  TN_ERR_ARG while a fused pixel gather is set.
- * DESIGN.md §4.10. */
-int tn_render_expected_depth(tn_tracer *h, const tn_render_config *cfg, const float *d_origins, const float *d_directions, uint32_t R,
-                             float *d_rgb, float *d_acc, float *d_depth, uint8_t *d_mask, float *d_expected_depth, float *d_normals,
-                             void *stream);
+              float *d_rgb, float *d_acc, float *d_depth, uint8_t *d_mask, float *d_expected_depth, float *d_normals, void *stream);
 /* ---- fused training step (SURVEY.md §8f-1): TetrahedraNerf.get_outputs in training mode (model.py:520-662) + its autograd backward.
  * Forward = the fused pipeline with the stratified bins of training (model.py:169-174 for the coarse pass, PDFSampler train_stratified
  * for the fine pass; the uniform [0,1) draws come from the caller, d_jitter_coarse f32[R,S_c+1] / d_jitter_fine f32[R,S_f+1] indexed by
@@ -174,52 +167,37 @@ int tn_render_train_backward(tn_tracer *h, const float *d_grad_rgb, const float 
  * tn_render_train_forward plus d_saved (256-byte aligned, saved_bytes >= that size) and writes into it everything its backward reads that
  * a later call could overwrite: a header (R, M, S_c, S_f, S2, background, deterministic mode, generations of field and weights and of the mesh), the
  * slot -> ray map and active count, the fine-pass samples (matched vertices, weights, (sigma, rgb) pre-activations, bins, spacing bins),
- * the per-ray direction bias and encoding.  tn_render_train_backward_saved computes the gradients of that forward (outputs as
- * tn_render_train_backward, d_grad_rgb f32[R,3] of the forward's R).  It reads d_saved, the field and the weights, and uses the tracer's
- * gradient scratch, so calls on one tracer must be stream-ordered.  It reads the header back to the host, so it waits until the stream
- * has reached it.  Returns TN_ERR_STATE if tn_render_set_field or tn_render_set_weights ran since the forward (or the forward ran on
- * another tracer).  The caller frees d_saved whenever it likes; the library keeps no reference to it. */
+ * the per-ray direction bias and encoding.  Its optional d_expected_depth f32[R] (NULL: none) is tn_render's, in training mode (no
+ * nan_to_num, no clamp); the saved state has the same size with it (the two clip bounds sit in the slot of the active count, and the
+ * header records that the forward produced them).  TN_ERR_ARG if it is given while a fused pixel gather is set.
+ * tn_render_train_backward_saved computes the gradients of that forward (outputs as tn_render_train_backward, d_grad_rgb f32[R,3] of the
+ * forward's R).  It reads d_saved, the field and the weights, and uses the tracer's gradient scratch, so calls on one tracer must be
+ * stream-ordered.  It reads the header back to the host, so it waits until the stream has reached it.  Returns TN_ERR_STATE if
+ * tn_render_set_field or tn_render_set_weights ran since the forward (or the forward ran on another tracer).  The caller frees d_saved
+ * whenever it likes; the library keeps no reference to it.  Optional input and outputs (NULL: none; every element of a non-NULL output
+ * is written); with all four NULL the backward runs the same kernels as tn_render_train_backward, and given or not, the ray and vertex
+ * gradients leave the other outputs as they are (bitwise in the deterministic mode):
+ *   d_grad_expected_depth f32[R]: dL/d expected depth, for a forward that produced it (TN_ERR_STATE otherwise).  The bins and midpoints
+ *     are constants; where t_min <= D_raw <= t_max, dL/dw_i gains dL/dD (t_i - D_raw) / (A + 1e-10), before the transmittance sums and
+ *     GradientScaler, so the depth loss reaches the field, the MLP, the rays and the vertices.  DESIGN.md §4.10.
+ *   d_grad_origins / d_grad_directions f32[R,3]: the gradients at the forward's ray origins and directions, 0 on empty rays.  The sample
+ *     distances are constants: a fine sample sits at x = o + t d, t the midpoint of its bin; dL/dx = E^-T q on its tetrahedron
+ *     (q_k = dL/df . (F_vk - F_v0), solved in float64 from the fp32 mesh positions), dL/do = sum dL/dx, dL/dd = sum t dL/dx + the
+ *     direction encoding's term.  dL/do is bitwise reproducible in both modes, dL/dd in the deterministic mode.  DESIGN.md §4.8.
+ *   d_grad_xyz f32[V,3]: the gradient at the mesh vertex positions.  The sample distances and the matched tetrahedra are held fixed; a
+ *     fine sample's weights b = E^-1 (x - x_v0) move with the vertices: dL/dx_vj += -b_j dL/dx (b_0 = 1 - b_1 - b_2 - b_3), the vertex
+ *     half of the reference's add_barycentrics_grad.  Default mode: float reductions; deterministic mode: per-vertex sums in a fixed
+ *     order, bitwise reproducible.  DESIGN.md §4.9.
+ * With any of the last three: TN_ERR_STATE if tn_load_tetrahedra or tn_update_vertices ran since the forward (they read the mesh
+ * positions), and the default mode keeps the [samples,64] feature gradient for them (0.54 GB at 8192 rays x 257 fine samples). */
 int tn_render_train_saved_bytes(tn_tracer *h, const tn_render_config *cfg, uint32_t R, size_t *bytes);
 int tn_render_train_forward_saved(tn_tracer *h, const tn_render_config *cfg, const float *d_origins, const float *d_directions, uint32_t R,
                                   const float *d_jitter_coarse, const float *d_jitter_fine, float *d_rgb, float *d_acc, float *d_depth,
-                                  uint8_t *d_mask, void *d_saved, size_t saved_bytes, void *stream);
+                                  uint8_t *d_mask, float *d_expected_depth, void *d_saved, size_t saved_bytes, void *stream);
 int tn_render_train_backward_saved(tn_tracer *h, const void *d_saved, const float *d_grad_rgb, const float *d_grad_acc,
-                                   int use_gradient_scaling, float *d_grad_field, float *const *d_grad_params12, void *stream);
-/* tn_render_train_backward_saved plus the gradients at the forward's ray origins and directions, d_grad_origins / d_grad_directions
- * f32[R,3] (either may be NULL; every element of a non-NULL one is written, 0 on empty rays).  The sample distances are constants:
- * a fine sample sits at x = o + t d, t the midpoint of its bin; dL/dx = E^-T q on its tetrahedron (q_k = dL/df . (F_vk - F_v0), solved in
- * float64 from the fp32 mesh positions), dL/do = sum dL/dx, dL/dd = sum t dL/dx + the direction encoding's term.  The other outputs are
- * those of tn_render_train_backward_saved (bitwise in the deterministic mode).  dL/do is bitwise reproducible in both modes, dL/dd in
- * the deterministic mode.  Also returns TN_ERR_STATE if tn_load_tetrahedra ran since the forward (it reads the mesh positions).  The
- * default mode keeps the [samples,64] feature gradient for it (0.54 GB at 8192 rays x 257 fine samples).  DESIGN.md §4.8. */
-int tn_render_train_backward_saved_rays(tn_tracer *h, const void *d_saved, const float *d_grad_rgb, const float *d_grad_acc,
-                                        int use_gradient_scaling, float *d_grad_field, float *const *d_grad_params12, float *d_grad_origins,
-                                        float *d_grad_directions, void *stream);
-/* tn_render_train_backward_saved_rays plus the gradient at the mesh vertex positions d_grad_xyz f32[V,3] (any of the three outputs may be
- * NULL; every element of a non-NULL one is written).  The sample distances and the matched tetrahedra are held fixed; a fine sample's
- * weights b = E^-1 (x - x_v0) move with the vertices: dL/dx_vj += -b_j dL/dx (b_0 = 1 - b_1 - b_2 - b_3), the vertex half of the
- * reference's add_barycentrics_grad.  Default mode: float reductions; deterministic mode: per-vertex sums in a fixed order, bitwise
- * reproducible.  The other outputs are those of tn_render_train_backward_saved_rays.  TN_ERR_STATE if tn_load_tetrahedra or
- * tn_update_vertices ran since the forward.  DESIGN.md §4.9. */
-int tn_render_train_backward_saved_geometry(tn_tracer *h, const void *d_saved, const float *d_grad_rgb, const float *d_grad_acc,
-                                            int use_gradient_scaling, float *d_grad_field, float *const *d_grad_params12, float *d_grad_origins,
-                                            float *d_grad_directions, float *d_grad_xyz, void *stream);
-/* The saved training pair with the expected depth (DESIGN.md §4.10).  tn_render_train_forward_saved_depth is
- * tn_render_train_forward_saved plus d_expected_depth f32[R], defined as for tn_render_expected_depth (training mode: no nan_to_num, no
- * clamp; the same saved-state size: the two clip bounds sit in the slot of the active count, and the header records that the forward
- * produced them).  tn_render_train_backward_saved_depth takes the arguments of tn_render_train_backward_saved_geometry plus
- * d_grad_expected_depth f32[R] (NULL: none, and then every output is that of the existing entry point with the same ray / vertex
- * outputs; all three of those NULL: tn_render_train_backward_saved's path).  The bins and midpoints are constants; where
- * t_min <= D_raw <= t_max, dL/dw_i gains dL/dD (t_i - D_raw) / (A + 1e-10), before the transmittance sums and GradientScaler, so the
- * depth loss reaches the field, the MLP, the rays and the vertices.  TN_ERR_STATE if d_grad_expected_depth is given and the forward was
- * not a _depth one.  The forward returns TN_ERR_ARG while a fused pixel gather is set, as tn_render_normals does. */
-int tn_render_train_forward_saved_depth(tn_tracer *h, const tn_render_config *cfg, const float *d_origins, const float *d_directions, uint32_t R,
-                                        const float *d_jitter_coarse, const float *d_jitter_fine, float *d_rgb, float *d_acc, float *d_depth,
-                                        uint8_t *d_mask, float *d_expected_depth, void *d_saved, size_t saved_bytes, void *stream);
-int tn_render_train_backward_saved_depth(tn_tracer *h, const void *d_saved, const float *d_grad_rgb, const float *d_grad_acc,
-                                         const float *d_grad_expected_depth, int use_gradient_scaling, float *d_grad_field,
-                                         float *const *d_grad_params12, float *d_grad_origins, float *d_grad_directions, float *d_grad_xyz,
-                                         void *stream);
+                                   const float *d_grad_expected_depth, int use_gradient_scaling, float *d_grad_field,
+                                   float *const *d_grad_params12, float *d_grad_origins, float *d_grad_directions, float *d_grad_xyz,
+                                   void *stream);
 /* Deterministic mode of the fused training step (enable != 0; initial value: 1 if the environment variable TETRANERF_B200_DETERMINISTIC
  * is 1, else 0).  Read by tn_render_train_forward; tn_render_train_backward continues in the mode of the forward it belongs to.  With
  * identical inputs, on the same build and GPU model, forward outputs and every gradient are then bitwise identical from run to run and
@@ -263,7 +241,7 @@ int tn_render_set_gather(tn_tracer *h, uint32_t world, uint32_t rank, void *cons
  * mlp_fine, composite (used by bench.py for the roofline of the dominant kernel) */
 int tn_render_set_profiling(tn_tracer *h, int enable);
 int tn_render_get_timings(tn_tracer *h, float *ms6);
-/* the same for the last tn_render_train_backward: ms3 = composite_bwd, mlp_bwd, finalize */
+/* the same for the last tn_render_train_backward or tn_render_train_backward_saved: ms3 = composite_bwd, mlp_bwd, finalize */
 int tn_render_get_backward_timings(tn_tracer *h, float *ms3);
 /* trace_rays picks between bit-identical implementations by batch size:
  * >= walk_min_rays (default 2^20): adjacency walk, 32 rays per warp (throughput);
@@ -287,11 +265,11 @@ int tn_debug_trace_stats(tn_tracer *h, uint32_t *out2);
  * num, dist, n_active, ray_list, ebins_c, sbins_c, vi_c, bary_c, dens_c, ebins_f, vi_f, bary_f, out_f,
  * dirbias, field shadow, weight image */
 int tn_render_debug_buffers(tn_tracer *h, void **ptrs16);
-/* device pointer of the per-sample density gradient of the last tn_render_normals call: float4 (x, y, z, 0) per sample, in the
+/* device pointer of the per-sample density gradient of the last tn_render call with d_normals: float4 (x, y, z, 0) per sample, in the
  * slot order of the pass that gives the colours (vi_f / bary_f; vi_c / bary_c when num_fine_samples = 0) */
 int tn_render_debug_normals_grad(tn_tracer *h, void **ptr);
-/* device pointer of dL/dx per fine sample of the last tn_render_train_backward_saved_rays / _geometry call: float4 (x, y, z, 0) per sample, in the
- * slot order of its forward (0 for unmatched samples and flat tetrahedra) */
+/* device pointer of dL/dx per fine sample of the last tn_render_train_backward_saved call with ray or vertex gradients: float4
+ * (x, y, z, 0) per sample, in the slot order of its forward (0 for unmatched samples and flat tetrahedra) */
 int tn_render_debug_ray_grads(tn_tracer *h, void **ptr);
 /* one 128x128 tile out = A[128,K] * W[128,K]^T through the wgmma bf16x3 path (A from registers); K in {64,128}; synchronous */
 int tn_debug_gemm_bf16x3(int device, const float *d_A, const float *d_W, uint32_t K, float *d_out, void *stream);

@@ -61,9 +61,9 @@ def test_eval_outputs_unchanged(small_mesh, prec):
             assert b["expected_depth"][5, 0].item() == st.far_plane
 
 
-def test_training_outputs_and_gradients_unchanged(small_mesh, monkeypatch):
-    """deterministic mode: a _depth forward gives the same rgb / accumulation / depth / mask, and its backward without a depth gradient
-    the same gradients as the existing entry points, with and without the ray and vertex gradients"""
+def test_training_outputs_and_gradients_unchanged_by_expected_depth(small_mesh, monkeypatch):
+    """deterministic mode: a forward with the expected depth gives the same rgb / accumulation / depth / mask, and its backward without
+    a depth gradient the same gradients as a forward without it, with and without the ray and vertex gradients"""
     monkeypatch.setenv("TETRANERF_B200_DETERMINISTIC", "1")
     V, C = small_mesh
     field, params = _field(V, None)
@@ -81,10 +81,12 @@ def test_training_outputs_and_gradients_unchanged(small_mesh, monkeypatch):
     for kw in ({}, {"grad_origins": True, "grad_directions": True, "grad_vertices": True}):
         ra = fr.train_backward_saved(sa, g_rgb, g_acc, len(V), True, **kw)
         rb = fr.train_backward_saved(sb, g_rgb, g_acc, len(V), True, **kw)
-        # the depth entry point itself with a NULL depth gradient
+        # the backward entry point itself with a NULL depth gradient
         outs = [torch.empty((n, 3), device=DEV) if kw else None for n in (len(o), len(o), len(V))]
-        rc = fr._train_backward(_lib.tn_render_train_backward_saved_depth, [fr.tracer.handle, sb.blob.data_ptr()], g_rgb, g_acc, len(V), True,
-                                tuple(t.data_ptr() if t is not None else None for t in outs), grad_ed=(None,))
+        rc = fr._grad_outputs(len(V))
+        assert _lib.tn_render_train_backward_saved(fr.tracer.handle, sb.blob.data_ptr(), g_rgb.data_ptr(), g_acc.data_ptr(), None, 1,
+                                                   rc[0].data_ptr(), rc[2], *(t.data_ptr() if t is not None else None for t in outs),
+                                                   fr._stream()) == 0
         torch.cuda.synchronize()
         assert torch.equal(ra[0], rb[0])
         for n in ra[1]:

@@ -1,4 +1,4 @@
-"""GPU: the normal map of the fused render (tn_render_normals, DESIGN §4.7) against the float64 oracle (oracle/normals.py).
+"""GPU: the normal map of the fused render (tn_render's d_normals, DESIGN §4.7) against the float64 oracle (oracle/normals.py).
 
 Per sample, at the kernel's own samples: |grad_kernel - grad_64| <= tol |cof E|_F |q_64| / |det E|, tol = 1e-3 (bf16x3) and 5e-2
 (f16w2).  The operand-rounding emulation of the reverse chain (oracle.normals.emulate_grad_pre) puts the maximum of this measure in a

@@ -1,4 +1,4 @@
-"""GPU: gradients of the fused training step at the ray origins and directions (tn_render_train_backward_saved_rays, DESIGN §4.8) against
+"""GPU: gradients of the fused training step at the ray origins and directions (tn_render_train_backward_saved, DESIGN §4.8) against
 float64 autograd of oracle/ray_grads.render_train_rays, with the bars of test_gpu_train.py: (A) at the kernel's own fine bins and (B) end to
 end, max |g - g64| <= max(2e-4, 6 max |g_torch_f32 - g64|) in units of the largest entry.  Also: dL/dx per sample against float64 at the
 kernel's positions, isolation of the other outputs and gradients, determinism, saved state, the autograd op, and recovery of a perturbed

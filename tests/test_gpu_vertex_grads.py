@@ -1,4 +1,4 @@
-"""GPU: gradient of the fused training step at the mesh vertex positions (tn_render_train_backward_saved_geometry, DESIGN §4.9) and the
+"""GPU: gradient of the fused training step at the mesh vertex positions (tn_render_train_backward_saved, DESIGN §4.9) and the
 in-place refit of the tracer (tn_update_vertices).
 
 Gradients: against float64 autograd of oracle/vertex_grads.render_train_geometry with the bars of test_gpu_train.py, (A) at the kernel's

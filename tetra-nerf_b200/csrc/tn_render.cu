@@ -84,10 +84,10 @@ struct RenderState {
     float *det_dbg = nullptr;          // [R/64][128*28] partial W4dir / b4 gradients per block of k_dirbias_grads
     uint32_t *det_keys = nullptr, *det_vals = nullptr;  // [2][R*S2*4] (vertex, sample row * 4 + k) pairs, sort input | output
     size_t cap_det_R = 0, cap_det_S2 = 0;
-    // normal map (tn_render_normals): density gradient per sample of the last normals render
+    // normal map (tn_render with d_normals): density gradient per sample of the last normals render
     float4 *grad_n = nullptr;
     size_t cap_grad_n = 0;
-    // ray gradients (tn_render_train_backward_saved_rays): dX rows of the default mode (the deterministic mode keeps them in det_dx),
+    // ray gradients (tn_render_train_backward_saved with ray or vertex outputs): dX rows of the default mode (the deterministic mode keeps them in det_dx),
     // dL/dx per sample of the last such backward
     float *ray_dx = nullptr;
     float4 *ray_gx = nullptr;
@@ -977,6 +977,10 @@ static int render_impl(tn_tracer *h, const tn_render_config *cfg, const float *d
                        void *stream) {
     if (!h || !cfg) return fail(TN_ERR_ARG, "null argument");
     RenderState *r = h->render;
+    if (r && r->gather_world && d_edepth != nullptr)
+        return fail(TN_ERR_ARG, "tn_render: the fused pixel gather (tn_render_set_gather) carries no expected depth; switch it off first");
+    if (r && r->gather_world && d_normals != nullptr)
+        return fail(TN_ERR_ARG, "tn_render: the fused pixel gather (tn_render_set_gather) carries no normals; switch it off first");
     if (!r || !r->fshadow || !r->have_weights) return fail(TN_ERR_STATE, "tn_render: call tn_render_set_field and tn_render_set_weights first");
     if (!h->mesh.nodes) return fail(TN_ERR_STATE, "tn_render: no tetrahedra loaded");
     if (r->V != h->mesh.V) return fail(TN_ERR_ARG, "tn_render: field has a different vertex count than the mesh");
@@ -1148,27 +1152,10 @@ static int ensure_train_ws(RenderState *r, size_t R, size_t S2, uint32_t V) {
     return TN_OK;
 }
 
+// optional outputs: the expected depth d_expected_depth f32[R] (DESIGN.md §4.10) and the normal map d_normals f32[R,3] (§4.7;
+// tn_normals.cu)
 extern "C" int tn_render(tn_tracer *h, const tn_render_config *cfg, const float *d_origins, const float *d_directions, uint32_t R,
-                         float *d_rgb, float *d_acc, float *d_depth, uint8_t *d_mask, void *stream) {
-    return render_impl(h, cfg, d_origins, d_directions, R, d_rgb, d_acc, d_depth, d_mask, nullptr, nullptr, nullptr, stream);
-}
-
-// tn_render plus the normal map d_normals f32[R,3] (DESIGN.md §4.7; tn_normals.cu)
-extern "C" int tn_render_normals(tn_tracer *h, const tn_render_config *cfg, const float *d_origins, const float *d_directions, uint32_t R,
-                                 float *d_rgb, float *d_acc, float *d_depth, uint8_t *d_mask, float *d_normals, void *stream) {
-    if (!h || !d_normals) return fail(TN_ERR_ARG, "null argument");
-    if (h->render && h->render->gather_world)
-        return fail(TN_ERR_ARG, "tn_render_normals: the fused pixel gather (tn_render_set_gather) carries no normals; switch it off first");
-    return render_impl(h, cfg, d_origins, d_directions, R, d_rgb, d_acc, d_depth, d_mask, nullptr, d_normals, nullptr, stream);
-}
-
-// tn_render plus the expected depth d_expected_depth f32[R] and optionally the normal map d_normals f32[R,3] (DESIGN.md §4.10)
-extern "C" int tn_render_expected_depth(tn_tracer *h, const tn_render_config *cfg, const float *d_origins, const float *d_directions, uint32_t R,
-                                        float *d_rgb, float *d_acc, float *d_depth, uint8_t *d_mask, float *d_expected_depth, float *d_normals,
-                                        void *stream) {
-    if (!h || !d_expected_depth) return fail(TN_ERR_ARG, "null argument");
-    if (h->render && h->render->gather_world)
-        return fail(TN_ERR_ARG, "tn_render_expected_depth: the fused pixel gather (tn_render_set_gather) carries no expected depth; switch it off first");
+                         float *d_rgb, float *d_acc, float *d_depth, uint8_t *d_mask, float *d_expected_depth, float *d_normals, void *stream) {
     return render_impl(h, cfg, d_origins, d_directions, R, d_rgb, d_acc, d_depth, d_mask, nullptr, d_normals, d_expected_depth, stream);
 }
 
@@ -1187,15 +1174,12 @@ extern "C" int tn_render_train_forward(tn_tracer *h, const tn_render_config *cfg
 // parameter gradients (same order / layouts as tn_render_set_weights); every output element is written.  Reads `b` and the field /
 // weights; writes only the tracer's gradient scratch.  The coarse pass carries no gradient (PDFSampler detaches its bins).  No
 // [samples,128] tensor touches HBM.
-// rays != nullptr: also the gradients at the ray origins / directions (tn_ray_grads.cu) and at the mesh vertex positions
-// (tn_vertex_grads.cu); any of the three outputs may be null
-struct RayGradOut {
-    float *grad_o, *grad_d, *grad_xyz;
-};
-// d_grad_ed != nullptr: dL/d expected depth f32[R] of a forward that produced it (its clip bounds in b.n_active[4, 5])
+// d_grad_ed != nullptr: dL/d expected depth f32[R] of a forward that produced it (its clip bounds in b.n_active[4, 5]).
+// Any of d_grad_o / d_grad_d / d_grad_xyz != nullptr: also the gradients at the ray origins / directions (tn_ray_grads.cu) and at the
+// mesh vertex positions (tn_vertex_grads.cu), into the non-null ones.
 static int train_backward_impl(tn_tracer *h, const TrainBufs &b, uint32_t R, uint32_t S2, bool det, const float *bg, const float *d_grad_rgb,
-                               const float *d_grad_acc, int use_gradient_scaling, float *d_grad_field, float *const *d_grad_params12, cudaStream_t s,
-                               const RayGradOut *rays = nullptr, const float *d_grad_ed = nullptr) {
+                               const float *d_grad_acc, const float *d_grad_ed, int use_gradient_scaling, float *d_grad_field,
+                               float *const *d_grad_params12, float *d_grad_o, float *d_grad_d, float *d_grad_xyz, cudaStream_t s) {
     RenderState *r = h->render;
     int sms = 132;
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, h->device);
@@ -1204,8 +1188,9 @@ static int train_backward_impl(tn_tracer *h, const TrainBufs &b, uint32_t R, uin
         const int rc = ensure_det_ws(r, R, S2);
         if (rc) return rc;
     }
+    const bool rays = d_grad_o != nullptr || d_grad_d != nullptr || d_grad_xyz != nullptr;
     const size_t rows = (size_t)R * S2;
-    if (rays != nullptr) {
+    if (rays) {
         if (!det && rows > r->cap_ray_dx) {
             cudaFree(r->ray_dx); r->ray_dx = nullptr; r->cap_ray_dx = 0;
             TN_CUDA(cudaMalloc((void **)&r->ray_dx, sizeof(float) * 64 * rows));
@@ -1244,7 +1229,7 @@ static int train_backward_impl(tn_tracer *h, const TrainBufs &b, uint32_t R, uin
     const uint64_t tiles = ((uint64_t)R * S2 + BWD_TILE - 1) / BWD_TILE;
     if (!det) {
         const uint32_t grid = r->bwd_grid ? r->bwd_grid : (uint32_t)std::min<uint64_t>(tiles, (uint64_t)sms);
-        if (rays == nullptr) {
+        if (!rays) {
             TN_CUDA(cudaFuncSetAttribute(k_mlp_bwd<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)BWD_SMEM_BYTES));
             k_mlp_bwd<false><<<grid, BWD_THREADS, BWD_SMEM_BYTES, s>>>(bp);
         } else {  // the same backward, storing the dX rows for k_ray_grads as well
@@ -1292,18 +1277,18 @@ static int train_backward_impl(tn_tracer *h, const TrainBufs &b, uint32_t R, uin
         if (!d_grad_params12[i]) return fail(TN_ERR_ARG, "tn_render_train_backward: null parameter gradient pointer");
         go.p[i] = d_grad_params12[i];
     }
-    if (rays != nullptr) {  // after the direction-bias gradient is complete
+    if (rays) {  // after the direction-bias gradient is complete
         RayGradsLaunch rl{};
         rl.n_active = b.n_active; rl.ray_list = b.ray_list; rl.S = S2; rl.R = R; rl.ebins = b.ebins_f; rl.vi = b.vi_f;
         rl.dx = det ? r->det_dx : r->ray_dx; rl.fshadow = r->fshadow; rl.xyz = h->mesh.xyz; rl.enc = b.enc; rl.g_dirbias = r->g_dirbias;
-        rl.w4dir = r->w4dir; rl.gx = r->ray_gx; rl.grad_o = rays->grad_o; rl.grad_d = rays->grad_d;
+        rl.w4dir = r->w4dir; rl.gx = r->ray_gx; rl.grad_o = d_grad_o; rl.grad_d = d_grad_d;
         int rc = launch_ray_grads(rl, s);
         if (rc) return rc;
         h->launches += 1;
-        if (rays->grad_xyz != nullptr) {  // after the per-sample dL/dx is complete
+        if (d_grad_xyz != nullptr) {  // after the per-sample dL/dx is complete
             VertexGradsLaunch vl{};
             vl.n_active = b.n_active; vl.S = S2; vl.R = R; vl.V = h->mesh.V; vl.vi = b.vi_f; vl.bary = b.bary_f; vl.gx = r->ray_gx;
-            vl.keys = sorted_keys; vl.vals = sorted_vals; vl.n = npairs; vl.grad_xyz = rays->grad_xyz;
+            vl.keys = sorted_keys; vl.vals = sorted_vals; vl.n = npairs; vl.grad_xyz = d_grad_xyz;
             rc = launch_vertex_grads(vl, s);
             if (rc) return rc;
             h->launches += 1;
@@ -1324,8 +1309,8 @@ extern "C" int tn_render_train_backward(tn_tracer *h, const float *d_grad_rgb, c
     RenderState *r = h->render;
     if (!r || !r->train_valid) return fail(TN_ERR_STATE, "tn_render_train_backward: no training forward to continue from");
     DeviceGuard g(h->device);
-    return train_backward_impl(h, own_bufs(r), r->t_R, r->t_S2, r->t_det, r->t_bg, d_grad_rgb, d_grad_acc, use_gradient_scaling, d_grad_field,
-                               d_grad_params12, (cudaStream_t)stream);
+    return train_backward_impl(h, own_bufs(r), r->t_R, r->t_S2, r->t_det, r->t_bg, d_grad_rgb, d_grad_acc, nullptr, use_gradient_scaling,
+                               d_grad_field, d_grad_params12, nullptr, nullptr, nullptr, (cudaStream_t)stream);
 }
 
 // ---- the training pair with per-call saved state: everything the backward reads that a later call could overwrite goes to the
@@ -1348,9 +1333,11 @@ extern "C" int tn_render_train_saved_bytes(tn_tracer *h, const tn_render_config 
     return TN_OK;
 }
 
-static int forward_saved(tn_tracer *h, const tn_render_config *cfg, const float *d_origins, const float *d_directions, uint32_t R,
-                         const float *d_jitter_coarse, const float *d_jitter_fine, float *d_rgb, float *d_acc, float *d_depth, uint8_t *d_mask,
-                         float *d_edepth, void *d_saved, size_t saved_bytes, void *stream) {
+// optional output: the expected depth d_expected_depth f32[R] (DESIGN.md §4.10)
+extern "C" int tn_render_train_forward_saved(tn_tracer *h, const tn_render_config *cfg, const float *d_origins, const float *d_directions,
+                                             uint32_t R, const float *d_jitter_coarse, const float *d_jitter_fine, float *d_rgb, float *d_acc,
+                                             float *d_depth, uint8_t *d_mask, float *d_expected_depth, void *d_saved, size_t saved_bytes,
+                                             void *stream) {
     if (!h || !d_saved) return fail(TN_ERR_ARG, "null argument");
     uint32_t S2 = 0;
     int rc = saved_shape(cfg, R, &S2);
@@ -1360,40 +1347,24 @@ static int forward_saved(tn_tracer *h, const tn_render_config *cfg, const float 
     if (saved_bytes < saved_layout(R, S2, (uint8_t *)d_saved, &b))
         return fail(TN_ERR_ARG, "tn_render_train_forward_saved: saved_bytes is smaller than tn_render_train_saved_bytes");
     TrainFwd tf{d_jitter_coarse, d_jitter_fine, &b};
-    rc = render_impl(h, cfg, d_origins, d_directions, R, d_rgb, d_acc, d_depth, d_mask, &tf, nullptr, d_edepth, stream);
+    rc = render_impl(h, cfg, d_origins, d_directions, R, d_rgb, d_acc, d_depth, d_mask, &tf, nullptr, d_expected_depth, stream);
     if (rc) return rc;
     RenderState *r = h->render;
     const SavedHeader hd{SAVED_MAGIC, R, cfg->max_ray_triangles, cfg->num_samples, cfg->num_fine_samples, S2, r->det ? 1u : 0u,
-                         d_edepth != nullptr ? 1u : 0u, {cfg->background[0], cfg->background[1], cfg->background[2]}, 0, r->gen, h->mesh_gen};
+                         d_expected_depth != nullptr ? 1u : 0u, {cfg->background[0], cfg->background[1], cfg->background[2]}, 0, r->gen,
+                         h->mesh_gen};
     DeviceGuard g(h->device);
     // pageable source: staged before the call returns, so `hd` may go out of scope
     TN_CUDA(cudaMemcpyAsync(d_saved, &hd, sizeof(hd), cudaMemcpyHostToDevice, (cudaStream_t)stream));
     return TN_OK;
 }
 
-extern "C" int tn_render_train_forward_saved(tn_tracer *h, const tn_render_config *cfg, const float *d_origins, const float *d_directions,
-                                             uint32_t R, const float *d_jitter_coarse, const float *d_jitter_fine, float *d_rgb, float *d_acc,
-                                             float *d_depth, uint8_t *d_mask, void *d_saved, size_t saved_bytes, void *stream) {
-    return forward_saved(h, cfg, d_origins, d_directions, R, d_jitter_coarse, d_jitter_fine, d_rgb, d_acc, d_depth, d_mask, nullptr, d_saved,
-                         saved_bytes, stream);
-}
-
-// tn_render_train_forward_saved plus the expected depth d_expected_depth f32[R] (DESIGN.md §4.10)
-extern "C" int tn_render_train_forward_saved_depth(tn_tracer *h, const tn_render_config *cfg, const float *d_origins, const float *d_directions,
-                                                   uint32_t R, const float *d_jitter_coarse, const float *d_jitter_fine, float *d_rgb, float *d_acc,
-                                                   float *d_depth, uint8_t *d_mask, float *d_expected_depth, void *d_saved, size_t saved_bytes,
-                                                   void *stream) {
-    if (!h || !d_expected_depth) return fail(TN_ERR_ARG, "null argument");
-    if (h->render && h->render->gather_world)
-        return fail(TN_ERR_ARG, "tn_render_train_forward_saved_depth: the fused pixel gather (tn_render_set_gather) carries no expected depth; "
-                                "switch it off first");
-    return forward_saved(h, cfg, d_origins, d_directions, R, d_jitter_coarse, d_jitter_fine, d_rgb, d_acc, d_depth, d_mask, d_expected_depth,
-                         d_saved, saved_bytes, stream);
-}
-
-static int backward_saved(tn_tracer *h, const void *d_saved, const float *d_grad_rgb, const float *d_grad_acc, int use_gradient_scaling,
-                          float *d_grad_field, float *const *d_grad_params12, const RayGradOut *rays, void *stream,
-                          const float *d_grad_ed = nullptr) {
+// optional input: the gradient of the expected depth d_grad_expected_depth f32[R] (DESIGN.md §4.10); optional outputs: the gradients at
+// the ray origins / directions of the forward, f32[R,3] each (0 on empty rays; §4.8), and at the mesh vertex positions, f32[V,3] (§4.9)
+extern "C" int tn_render_train_backward_saved(tn_tracer *h, const void *d_saved, const float *d_grad_rgb, const float *d_grad_acc,
+                                              const float *d_grad_expected_depth, int use_gradient_scaling, float *d_grad_field,
+                                              float *const *d_grad_params12, float *d_grad_origins, float *d_grad_directions, float *d_grad_xyz,
+                                              void *stream) {
     if (!h || !d_saved || !d_grad_rgb || !d_grad_field || !d_grad_params12) return fail(TN_ERR_ARG, "null argument");
     RenderState *r = h->render;
     if (!r || !r->n_active) return fail(TN_ERR_STATE, "tn_render_train_backward_saved: no training forward on this tracer");
@@ -1407,50 +1378,17 @@ static int backward_saved(tn_tracer *h, const void *d_saved, const float *d_grad
     if (hd.gen != r->gen)
         return fail(TN_ERR_STATE, "tn_render_train_backward_saved: the field or the weights changed (tn_render_set_field / "
                                   "tn_render_set_weights) since the forward, or the forward ran on another tracer");
-    if (rays != nullptr && hd.mesh_gen != h->mesh_gen)
-        return fail(TN_ERR_STATE, "tn_render_train_backward_saved_geometry: tn_load_tetrahedra or tn_update_vertices ran since the forward "
+    const bool rays = d_grad_origins != nullptr || d_grad_directions != nullptr || d_grad_xyz != nullptr;
+    if (rays && hd.mesh_gen != h->mesh_gen)
+        return fail(TN_ERR_STATE, "tn_render_train_backward_saved: tn_load_tetrahedra or tn_update_vertices ran since the forward "
                                   "(the ray and vertex gradients read the mesh positions)");
-    if (d_grad_ed != nullptr && hd.edepth == 0)
-        return fail(TN_ERR_STATE, "tn_render_train_backward_saved_depth: the forward produced no expected depth (use "
-                                  "tn_render_train_forward_saved_depth)");
+    if (d_grad_expected_depth != nullptr && hd.edepth == 0)
+        return fail(TN_ERR_STATE, "tn_render_train_backward_saved: the forward produced no expected depth (pass d_expected_depth to "
+                                  "tn_render_train_forward_saved)");
     TrainBufs b{};
     saved_layout(hd.R, hd.S2, (uint8_t *)d_saved, &b);
-    return train_backward_impl(h, b, hd.R, hd.S2, hd.det != 0, hd.bg, d_grad_rgb, d_grad_acc, use_gradient_scaling, d_grad_field,
-                               d_grad_params12, s, rays, d_grad_ed);
-}
-
-extern "C" int tn_render_train_backward_saved(tn_tracer *h, const void *d_saved, const float *d_grad_rgb, const float *d_grad_acc,
-                                              int use_gradient_scaling, float *d_grad_field, float *const *d_grad_params12, void *stream) {
-    return backward_saved(h, d_saved, d_grad_rgb, d_grad_acc, use_gradient_scaling, d_grad_field, d_grad_params12, nullptr, stream);
-}
-
-// tn_render_train_backward_saved plus the gradients at the ray origins / directions of the forward, f32[R,3] each (either may be NULL;
-// 0 on empty rays); DESIGN.md §4.8
-extern "C" int tn_render_train_backward_saved_rays(tn_tracer *h, const void *d_saved, const float *d_grad_rgb, const float *d_grad_acc,
-                                                   int use_gradient_scaling, float *d_grad_field, float *const *d_grad_params12,
-                                                   float *d_grad_origins, float *d_grad_directions, void *stream) {
-    return tn_render_train_backward_saved_geometry(h, d_saved, d_grad_rgb, d_grad_acc, use_gradient_scaling, d_grad_field, d_grad_params12,
-                                                   d_grad_origins, d_grad_directions, nullptr, stream);
-}
-
-// ... plus the gradient at the mesh vertex positions, f32[V,3] (NULL = none); DESIGN.md §4.9
-extern "C" int tn_render_train_backward_saved_geometry(tn_tracer *h, const void *d_saved, const float *d_grad_rgb, const float *d_grad_acc,
-                                                       int use_gradient_scaling, float *d_grad_field, float *const *d_grad_params12,
-                                                       float *d_grad_origins, float *d_grad_directions, float *d_grad_xyz, void *stream) {
-    const RayGradOut rays{d_grad_origins, d_grad_directions, d_grad_xyz};
-    return backward_saved(h, d_saved, d_grad_rgb, d_grad_acc, use_gradient_scaling, d_grad_field, d_grad_params12, &rays, stream);
-}
-
-// tn_render_train_backward_saved with the gradient of the expected depth d_grad_expected_depth f32[R] (NULL: none) and the optional ray /
-// vertex gradients of _geometry (all three NULL: tn_render_train_backward_saved's path, else _geometry's); DESIGN.md §4.10
-extern "C" int tn_render_train_backward_saved_depth(tn_tracer *h, const void *d_saved, const float *d_grad_rgb, const float *d_grad_acc,
-                                                    const float *d_grad_expected_depth, int use_gradient_scaling, float *d_grad_field,
-                                                    float *const *d_grad_params12, float *d_grad_origins, float *d_grad_directions,
-                                                    float *d_grad_xyz, void *stream) {
-    const RayGradOut rays{d_grad_origins, d_grad_directions, d_grad_xyz};
-    const bool any = d_grad_origins != nullptr || d_grad_directions != nullptr || d_grad_xyz != nullptr;
-    return backward_saved(h, d_saved, d_grad_rgb, d_grad_acc, use_gradient_scaling, d_grad_field, d_grad_params12, any ? &rays : nullptr,
-                          stream, d_grad_expected_depth);
+    return train_backward_impl(h, b, hd.R, hd.S2, hd.det != 0, hd.bg, d_grad_rgb, d_grad_acc, d_grad_expected_depth, use_gradient_scaling,
+                               d_grad_field, d_grad_params12, d_grad_origins, d_grad_directions, d_grad_xyz, s);
 }
 
 // deterministic mode of the fused training step (see the header): applies from the next tn_render_train_forward on
@@ -1501,7 +1439,7 @@ extern "C" int tn_render_get_timings(tn_tracer *h, float *ms6) {
     return TN_OK;
 }
 
-// per-kernel timing of the LAST tn_render_train_backward call: ms3 = composite_bwd, mlp_bwd, finalize (memsets excluded)
+// per-kernel timing of the LAST tn_render_train_backward or tn_render_train_backward_saved call: ms3 = composite_bwd, mlp_bwd, finalize (memsets excluded)
 extern "C" int tn_render_get_backward_timings(tn_tracer *h, float *ms3) {
     if (!h || !h->render || !h->render->profile) return fail(TN_ERR_STATE, "profiling is not enabled");
     DeviceGuard g(h->device);
@@ -1521,7 +1459,7 @@ extern "C" int tn_render_debug_buffers(tn_tracer *h, void **ptrs16) {
     return TN_OK;
 }
 
-// test hook: device pointer of the per-sample density gradient of the last tn_render_normals call, float4 (x, y, z, 0) per sample in
+// test hook: device pointer of the per-sample density gradient of the last tn_render call with normals, float4 (x, y, z, 0) per sample in
 // the slot order of the pass that gives the colours (vi_f / bary_f, or vi_c / bary_c in single-pass configurations)
 extern "C" int tn_render_debug_normals_grad(tn_tracer *h, void **ptr) {
     if (!h || !h->render || !h->render->grad_n) return fail(TN_ERR_STATE, "no normals render");
@@ -1529,7 +1467,7 @@ extern "C" int tn_render_debug_normals_grad(tn_tracer *h, void **ptr) {
     return TN_OK;
 }
 
-// test hook: device pointer of dL/dx per fine sample of the last tn_render_train_backward_saved_rays / _geometry call, float4 (x, y, z, 0) per sample
+// test hook: device pointer of dL/dx per fine sample of the last tn_render_train_backward_saved call with ray or vertex gradients, float4 (x, y, z, 0) per sample
 // in the slot order of that call's forward (0 for unmatched samples and flat tetrahedra)
 extern "C" int tn_render_debug_ray_grads(tn_tracer *h, void **ptr) {
     if (!h || !h->render || !h->render->ray_gx) return fail(TN_ERR_STATE, "no backward with ray gradients");

@@ -49,6 +49,11 @@ class RenderSettings:
         return RenderSettings()
 
 
+def _ptr(t: Optional[torch.Tensor]):
+    """device pointer of an optional tensor (None: NULL)"""
+    return t.data_ptr() if t is not None else None
+
+
 def _config(settings: RenderSettings) -> "ext._Cfg":
     return ext._Cfg(settings.max_intersected_triangles, settings.num_samples, settings.num_fine_samples, int(settings.use_biased_sampler),
                     float(settings.far_plane), (C.c_float * 3)(*settings.background))
@@ -109,20 +114,14 @@ class FusedRenderer:
                 "depth": torch.empty((R, 1), dtype=torch.float32, device=dev),
                 "ray_mask": torch.empty((R,), dtype=torch.bool, device=dev),
             }
-        cfg = _config(settings)
-        args = [tr.handle, C.byref(cfg), origins.data_ptr(), directions.data_ptr(), R, out["rgb"].data_ptr(), out["accumulation"].data_ptr(),
-                out["depth"].data_ptr(), out["ray_mask"].data_ptr()]
         if normals and "normals" not in out:
             out["normals"] = torch.empty((R, 3), dtype=torch.float32, device=dev)
-        if expected_depth:
-            if "expected_depth" not in out:
-                out["expected_depth"] = torch.empty((R, 1), dtype=torch.float32, device=dev)
-            ext._check(_lib.tn_render_expected_depth(*args, out["expected_depth"].data_ptr(), out["normals"].data_ptr() if normals else None,
-                                                     self._stream()))
-        elif normals:
-            ext._check(_lib.tn_render_normals(*args, out["normals"].data_ptr(), self._stream()))
-        else:
-            ext._check(_lib.tn_render(*args, self._stream()))
+        if expected_depth and "expected_depth" not in out:
+            out["expected_depth"] = torch.empty((R, 1), dtype=torch.float32, device=dev)
+        ext._check(_lib.tn_render(tr.handle, C.byref(_config(settings)), origins.data_ptr(), directions.data_ptr(), R, out["rgb"].data_ptr(),
+                                  out["accumulation"].data_ptr(), out["depth"].data_ptr(), out["ray_mask"].data_ptr(),
+                                  out["expected_depth"].data_ptr() if expected_depth else None, out["normals"].data_ptr() if normals else None,
+                                  self._stream()))
         return out
 
     # ---- fused training step ------------------------------------------------------------------------------------------------------
@@ -144,19 +143,12 @@ class FusedRenderer:
                 out["rgb"].data_ptr(), out["accumulation"].data_ptr(), out["depth"].data_ptr(), out["ray_mask"].data_ptr()]
         return R, out, args
 
-    def _train_backward(self, entry, lead, grad_rgb, grad_acc, num_vertices, use_gradient_scaling, tail=(), grad_ed=()):
-        """runs a training backward, entry(*lead, grads in, gradients out, *tail, stream) -> (grad_field, {name: gradient}); grad_ed: () or
-        (the expected depth's gradient tensor or None,), passed after grad_acc"""
-        grad_rgb = grad_rgb.contiguous()
-        if grad_acc is not None:
-            grad_acc = grad_acc.contiguous()
-        grad_ed = tuple(t.contiguous() if t is not None else None for t in grad_ed)
+    def _grad_outputs(self, num_vertices):
+        """the outputs of a training backward -> (grad_field f32[64,V], {state-dict name: gradient} for the twelve MLP parameters, the
+        twelve as the C pointer array the backward writes through)"""
         gfield = torch.empty((64, num_vertices), dtype=torch.float32, device=self.device)
         gps = [torch.empty(sh, dtype=torch.float32, device=self.device) for sh in _SHAPES]
-        arr = (_vp * 12)(*[t.data_ptr() for t in gps])
-        ext._check(entry(*lead, grad_rgb.data_ptr(), grad_acc.data_ptr() if grad_acc is not None else None, *[t.data_ptr() if t is not None else None for t in grad_ed],
-                         int(use_gradient_scaling), gfield.data_ptr(), arr, *tail, self._stream()))
-        return gfield, dict(zip(PARAM_ORDER, gps))
+        return gfield, dict(zip(PARAM_ORDER, gps)), (_vp * 12)(*[t.data_ptr() for t in gps])
 
     def train_forward(self, origins: torch.Tensor, directions: torch.Tensor, settings: RenderSettings, jitter_coarse: Optional[torch.Tensor] = None,
                       jitter_fine: Optional[torch.Tensor] = None):
@@ -171,7 +163,12 @@ class FusedRenderer:
 
     def train_backward(self, grad_rgb: torch.Tensor, grad_acc: Optional[torch.Tensor], num_vertices: int, use_gradient_scaling: bool = False):
         """backward of the last train_forward: -> (grad_field f32[64,V], {state-dict name: gradient} for the twelve MLP parameters)"""
-        return self._train_backward(_lib.tn_render_train_backward, [self.tracer.handle], grad_rgb, grad_acc, num_vertices, use_gradient_scaling)
+        grad_rgb = grad_rgb.contiguous()
+        grad_acc = grad_acc.contiguous() if grad_acc is not None else None
+        gfield, gp, arr = self._grad_outputs(num_vertices)
+        ext._check(_lib.tn_render_train_backward(self.tracer.handle, grad_rgb.data_ptr(), _ptr(grad_acc), int(use_gradient_scaling),
+                                                 gfield.data_ptr(), arr, self._stream()))
+        return gfield, gp
 
     def train_saved_bytes(self, R: int, settings: RenderSettings) -> int:
         """device bytes of the saved state of one training forward of R rays"""
@@ -189,10 +186,7 @@ class FusedRenderer:
         blob = torch.empty((self.train_saved_bytes(R, settings),), dtype=torch.uint8, device=self.device)
         if expected_depth:
             out["expected_depth"] = torch.empty((R, 1), dtype=torch.float32, device=self.device)
-            ext._check(_lib.tn_render_train_forward_saved_depth(*args, out["expected_depth"].data_ptr(), blob.data_ptr(), blob.numel(),
-                                                                self._stream()))
-        else:
-            ext._check(_lib.tn_render_train_forward_saved(*args, blob.data_ptr(), blob.numel(), self._stream()))
+        ext._check(_lib.tn_render_train_forward_saved(*args, _ptr(out.get("expected_depth")), blob.data_ptr(), blob.numel(), self._stream()))
         return out, TrainState(blob, R)
 
     def train_backward_saved(self, state: "TrainState", grad_rgb: torch.Tensor, grad_acc: Optional[torch.Tensor], num_vertices: int,
@@ -210,26 +204,23 @@ class FusedRenderer:
         if tuple(grad_rgb.shape) != (state.R, 3) or (grad_acc is not None and grad_acc.numel() != state.R):
             raise RuntimeError(f"the forward rendered {state.R} rays: grad_rgb must be [{state.R}, 3] and grad_acc [{state.R}], got "
                                f"{tuple(grad_rgb.shape)} and {None if grad_acc is None else tuple(grad_acc.shape)}")
-        lead = [self.tracer.handle, state.blob.data_ptr()]
-        rays = grad_origins or grad_directions or grad_vertices
+        g_ed = grad_expected_depth
+        if g_ed is not None:
+            if g_ed.numel() != state.R or g_ed.device != self.device or g_ed.dtype != torch.float32:
+                raise RuntimeError(f"grad_expected_depth must be a float32 [{state.R}] tensor on the tracer's device, got {tuple(g_ed.shape)}")
+            g_ed = g_ed.reshape(-1).contiguous()
+        grad_rgb = grad_rgb.contiguous()
+        grad_acc = grad_acc.contiguous() if grad_acc is not None else None
         go = torch.empty((state.R, 3), dtype=torch.float32, device=self.device) if grad_origins else None
         gd = torch.empty((state.R, 3), dtype=torch.float32, device=self.device) if grad_directions else None
         gv = torch.empty((num_vertices, 3), dtype=torch.float32, device=self.device) if grad_vertices else None
-        tail = tuple(t.data_ptr() if t is not None else None for t in (go, gd, gv))
-        if grad_expected_depth is not None:
-            g = grad_expected_depth
-            if g.numel() != state.R or g.device != self.device or g.dtype != torch.float32:
-                raise RuntimeError(f"grad_expected_depth must be a float32 [{state.R}] tensor on the tracer's device, got {tuple(g.shape)}")
-            gfield, gp = self._train_backward(_lib.tn_render_train_backward_saved_depth, lead, grad_rgb, grad_acc, num_vertices,
-                                              use_gradient_scaling, tail, grad_ed=(g.reshape(-1),))
-        elif not rays:
-            return self._train_backward(_lib.tn_render_train_backward_saved, lead, grad_rgb, grad_acc, num_vertices, use_gradient_scaling)
-        else:
-            gfield, gp = self._train_backward(_lib.tn_render_train_backward_saved_geometry, lead, grad_rgb, grad_acc, num_vertices,
-                                              use_gradient_scaling, tail)
-        if not rays:
-            return gfield, gp
-        return (gfield, gp, go, gd, gv) if grad_vertices else (gfield, gp, go, gd)
+        gfield, gp, arr = self._grad_outputs(num_vertices)
+        ext._check(_lib.tn_render_train_backward_saved(self.tracer.handle, state.blob.data_ptr(), grad_rgb.data_ptr(), _ptr(grad_acc),
+                                                       _ptr(g_ed), int(use_gradient_scaling), gfield.data_ptr(), arr, _ptr(go), _ptr(gd),
+                                                       _ptr(gv), self._stream()))
+        if grad_vertices:
+            return gfield, gp, go, gd, gv
+        return (gfield, gp, go, gd) if grad_origins or grad_directions else (gfield, gp)
 
     # ---- surface extraction ---------------------------------------------------------------------------------------------------------
     def extract_surface(self, level: float) -> Dict[str, torch.Tensor]:
@@ -302,7 +293,7 @@ class FusedRenderer:
 class FusedTrainRender(torch.autograd.Function):
     """TetrahedraNerf.get_outputs in training mode as ONE differentiable op: forward = tn_render_train_forward_saved, backward =
     tn_render_train_backward_saved (gradients for `tetrahedra_field` and the twelve MLP parameters; none for the jitter).  When
-    `origins` / `directions` require grad, the backward also returns their gradients (tn_render_train_backward_saved_rays, DESIGN §4.8:
+    `origins` / `directions` require grad, the backward also returns their gradients (tn_render_train_backward_saved, DESIGN §4.8:
     the sample distances held fixed, as nerfstudio's samplers feed a camera optimizer), so a pose correction upstream of the rays learns.
     The renderer must already hold the current field / weights (FusedRenderer.set_field / set_weights).  Every call keeps its own
     saved state (~115 MB at 8192 rays x 257 fine samples, freed with the graph), so calls compose like any autograd op: several
@@ -330,7 +321,7 @@ class FusedTrainRenderDepth(torch.autograd.Function):
     (rgb, accumulation, depth, expected_depth, ray_mask) with expected_depth f32[R,1] nerfstudio's DepthRenderer(method="expected") over
     the fine samples (clipped to the call's smallest / largest sample midpoint, far_plane on empty rays).  rgb, accumulation and
     expected_depth are differentiable: a depth loss reaches the field, the MLP and, when they require grad, the ray origins / directions
-    and the vertex positions (tn_render_train_forward_saved_depth / tn_render_train_backward_saved_depth).  The other outputs are the
+    and the vertex positions (tn_render_train_forward_saved / tn_render_train_backward_saved).  The other outputs are the
     same bits as FusedTrainRender's."""
 
     @staticmethod
@@ -375,15 +366,9 @@ def _fused_backward(ctx, g_rgb, g_acc, g_ed):
     want_v = has_xyz and ctx.needs_input_grad[-1]
     g_acc = g_acc.reshape(-1) if g_acc is not None else None
     g_ed = g_ed.reshape(-1) if g_ed is not None else None
-    go = gd = gv = None
-    if want_v:
-        gfield, gp, go, gd, gv = ctx.fr.train_backward_saved(ctx.state, g_rgb, g_acc, field.shape[1], ctx.gs, grad_origins=want_o,
-                                                             grad_directions=want_d, grad_vertices=True, grad_expected_depth=g_ed)
-    elif want_o or want_d:
-        gfield, gp, go, gd = ctx.fr.train_backward_saved(ctx.state, g_rgb, g_acc, field.shape[1], ctx.gs, grad_origins=want_o,
-                                                         grad_directions=want_d, grad_expected_depth=g_ed)
-    else:
-        gfield, gp = ctx.fr.train_backward_saved(ctx.state, g_rgb, g_acc, field.shape[1], ctx.gs, grad_expected_depth=g_ed)
+    res = ctx.fr.train_backward_saved(ctx.state, g_rgb, g_acc, field.shape[1], ctx.gs, grad_origins=want_o, grad_directions=want_d,
+                                      grad_vertices=want_v, grad_expected_depth=g_ed)
+    gfield, gp, go, gd, gv = res + (None,) * (5 - len(res))
     go = go.reshape(ctx.ray_shapes[0]) if go is not None else None
     gd = gd.reshape(ctx.ray_shapes[1]) if gd is not None else None
     return (None, None, None, go, gd, None, None, gfield) + tuple(gp[n] for n in PARAM_ORDER) + ((gv,) if has_xyz else ())
