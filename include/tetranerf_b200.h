@@ -280,6 +280,8 @@ int tn_debug_gemm_modes(int device, int mode, uint32_t N, uint32_t lbo, uint32_t
                         const float *d_Q, float *d_out, void *stream);
 /* rays of the last tn_debug_trace_stats call that needed the all-hits gather (subset of out2[1]) */
 uint32_t tn_debug_last_exact_count(void);
+/* bytes of device memory the library's own buffers hold in this process, over every tracer (peer buffers excluded) */
+uint64_t tn_debug_device_bytes(void);
 
 /* number of kernels launched by this library on this tracer since creation (bench "gpu_launches") */
 uint64_t tn_launch_count(tn_tracer *h);

@@ -1,5 +1,6 @@
 // tn_api.cu -- C-ABI entry points: tracer lifetime, errors, mesh load, face export, sync.
 #include <cstring>
+#include <memory>
 
 #include "tn_common.cuh"
 
@@ -40,15 +41,11 @@ int tn_create(int device, tn_tracer **out) {
     if (major != 9 || minor != 0)
         return tn::fail(TN_ERR_CUDA, "tetranerf_b200 is built for sm_90a (H100) only; device has compute capability " + std::to_string(major) + "." +
                                          std::to_string(minor));
-    tn_tracer *h = new tn_tracer();
+    std::unique_ptr<tn_tracer> h(new tn_tracer());
     h->device = device;
-    cudaError_t e = cudaMalloc(&h->d_flags, sizeof(int) * 4);
-    if (e == cudaSuccess) e = cudaMemset(h->d_flags, 0, sizeof(int) * 4);
-    if (e != cudaSuccess) {
-        delete h;
-        return tn::fail(TN_ERR_CUDA, std::string("tn_create: ") + cudaGetErrorString(e));
-    }
-    *out = h;
+    TN_TRY(h->d_flags.grow(4));
+    TN_CUDA(cudaMemset(h->d_flags.p, 0, sizeof(int) * 4));
+    *out = h.release();
     return TN_OK;
 }
 
@@ -58,11 +55,6 @@ int tn_destroy(tn_tracer *h) {
     cudaDeviceSynchronize();
     tn::free_render(h);
     tn::free_surface(h);
-    tn::free_mesh(h);
-    cudaFree(h->d_flags);
-    cudaFree(h->d_ovf_list);
-    cudaFree(h->d_walk_keys);
-    cudaFree(h->d_refit);
     delete h;
     return TN_OK;
 }
@@ -72,9 +64,9 @@ int tn_synchronize(tn_tracer *h, void *stream) {
     tn::DeviceGuard g(h->device);
     TN_CUDA(cudaStreamSynchronize((cudaStream_t)stream));
     int flags[4] = {0, 0, 0, 0};
-    TN_CUDA(cudaMemcpy(flags, h->d_flags, sizeof(flags), cudaMemcpyDeviceToHost));
+    TN_CUDA(cudaMemcpy(flags, h->d_flags.p, sizeof(flags), cudaMemcpyDeviceToHost));
     if (flags[0] != 0) {
-        cudaMemset(h->d_flags, 0, sizeof(flags));
+        cudaMemset(h->d_flags.p, 0, sizeof(flags));
         return tn::fail(TN_ERR_OVERFLOW, "trace_rays: BVH work list overflow on " + std::to_string(flags[0]) + " ray(s); their results were dropped");
     }
     return TN_OK;
@@ -97,23 +89,26 @@ int tn_update_vertices(tn_tracer *h, const float *d_xyz, uint32_t V, uint32_t *f
 
 int tn_num_faces(tn_tracer *h, uint32_t *F) {
     if (!h || !F) return tn::fail(TN_ERR_ARG, "null argument");
-    if (!h->mesh.nodes) return tn::fail(TN_ERR_STATE, "no tetrahedra loaded");
+    if (!h->mesh.nodes.p) return tn::fail(TN_ERR_STATE, "no tetrahedra loaded");
     *F = h->mesh.F;
     return TN_OK;
 }
 
 int tn_get_faces(tn_tracer *h, uint32_t *d_tri, uint32_t *d_tt, void *stream) {
     if (!h) return tn::fail(TN_ERR_ARG, "null tracer");
-    if (!h->mesh.nodes) return tn::fail(TN_ERR_STATE, "no tetrahedra loaded");
+    if (!h->mesh.nodes.p) return tn::fail(TN_ERR_STATE, "no tetrahedra loaded");
     tn::DeviceGuard g(h->device);
     const uint32_t F = h->mesh.F;
-    tn::k_export_faces<<<(F + 255) / 256, 256, 0, (cudaStream_t)stream>>>((const uint4 *)h->mesh.tri, (const uint2 *)h->mesh.tt, F, d_tri, d_tt);
+    tn::k_export_faces<<<(F + 255) / 256, 256, 0, (cudaStream_t)stream>>>(h->mesh.tri.p, h->mesh.tt.p, F, d_tri, d_tt);
     h->launches += 1;
     TN_CUDA(cudaGetLastError());
     return TN_OK;
 }
 
 uint64_t tn_launch_count(tn_tracer *h) { return h ? h->launches : 0; }
+
+// test hook: bytes held by the library's own device buffers (every DevArray of the process; peer buffers excluded)
+uint64_t tn_debug_device_bytes(void) { return tn::g_device_bytes.load(); }
 
 // ---- peer-mapped buffers (one process per GPU): cudaMalloc + CUDA IPC, so that a kernel of rank a can store into rank b's
 // memory over NVLink (fused pixel gather, tn_render_set_gather) ----
@@ -182,7 +177,7 @@ int tn_debug_trace_stats(tn_tracer *h, uint32_t *out2) {
     tn::DeviceGuard g(h->device);
     TN_CUDA(cudaDeviceSynchronize());
     int flags[4];
-    TN_CUDA(cudaMemcpy(flags, h->d_flags, sizeof(flags), cudaMemcpyDeviceToHost));
+    TN_CUDA(cudaMemcpy(flags, h->d_flags.p, sizeof(flags), cudaMemcpyDeviceToHost));
     out2[0] = h->mesh.walkable ? 1u : 0u;
     out2[1] = (uint32_t)flags[2];
     g_last_exact = (uint32_t)flags[3];

@@ -8,6 +8,7 @@
 
 #include <algorithm>
 #include <cmath>
+#include <utility>
 #include <vector>
 
 #include "tn_common.cuh"
@@ -234,54 +235,35 @@ static float absmax_of(const int *hbounds) {  // max |coordinate| from the order
     return amax;
 }
 
-void free_mesh(tn_tracer *h) {
-    Mesh &m = h->mesh;
-    cudaFree(m.tri); cudaFree(m.tt); cudaFree(m.nodes); cudaFree(m.leaves); cudaFree(m.leaf_tet);
-    cudaFree(m.walk); cudaFree(m.hull_nodes); cudaFree(m.hull_leaves); cudaFree(m.hull_tet); cudaFree(m.hull_ekey); cudaFree(m.hull_eface);
-    m = Mesh();
-}
-
 int build_mesh(tn_tracer *h, const float *d_xyz, uint32_t V, const uint32_t *d_cells, uint32_t T, cudaStream_t s) {
-    free_mesh(h);
+    h->mesh = Mesh();  // the old mesh goes first (it is not needed to build the new one), and a failed load leaves none
     if (T == 0 || V == 0) return fail(TN_ERR_ARG, "load_tetrahedra: empty mesh");
     if (T >= (1u << 28)) return fail(TN_ERR_ARG, "load_tetrahedra: more than 2^28 tetrahedra are not supported");
-    Mesh &m = h->mesh;
+    Mesh m;  // moved into h->mesh once complete
 
     // ---- faces, adjacency tables, hull convexity: all on the device (tn_faces.cu) ----
     FaceTables ft;
     {
         int extra = 0;
-        const int rc = build_faces_device(d_xyz, V, d_cells, T, s, ft, &extra);
-        if (rc != TN_OK) return rc;
+        TN_TRY(build_faces_device(d_xyz, V, d_cells, T, s, ft, &extra));
         h->launches += extra;
     }
     const uint32_t F = ft.F, H = ft.H;
     const bool walkable = ft.walkable;
-    m.tri = reinterpret_cast<uint32_t *>(ft.tri); m.tt = reinterpret_cast<uint32_t *>(ft.tt);  // owned by the mesh from here on (free_mesh)
-    m.hull_ekey = ft.hull_ekey; m.hull_eface = ft.hull_eface; m.hull_ne = ft.hull_ne;
-    uint4 *d_tet_faces = ft.tet_faces;
-    uint4 *d_nbr = ft.nbr;
-    uint32_t *d_wind = ft.wind, *d_hull_list = ft.hull_list;
-    uint32_t *keys = nullptr, *keys2 = nullptr, *vals = nullptr;
-    int *bounds = nullptr;
-    void *tmp = nullptr;
-    auto cleanup = [&]() { cudaFree(d_nbr); cudaFree(d_wind); cudaFree(d_hull_list); cudaFree(d_tet_faces); cudaFree(keys); cudaFree(keys2); cudaFree(vals); cudaFree(bounds); cudaFree(tmp); };
-#define TN_CUDA_B(expr)                                                                      \
-    do {                                                                                     \
-        cudaError_t _e = (expr);                                                             \
-        if (_e != cudaSuccess) {                                                             \
-            cleanup();                                                                       \
-            free_mesh(h);                                                                    \
-            return fail(TN_ERR_CUDA, std::string(#expr) + " failed: " + cudaGetErrorString(_e)); \
-        }                                                                                    \
-    } while (0)
+    m.tri = std::move(ft.tri); m.tt = std::move(ft.tt);
+    m.hull_ekey = std::move(ft.hull_ekey); m.hull_eface = std::move(ft.hull_eface); m.hull_ne = ft.hull_ne;
+    const uint4 *d_tet_faces = ft.tet_faces.p, *d_nbr = ft.nbr.p;
+    const uint32_t *d_wind = ft.wind.p, *d_hull_list = ft.hull_list.p;
+    DevArray<uint32_t> keys, keys2, vals;
+    DevArray<int> bounds;
+    DevArray<uint8_t> tmp;
 
     // ---- levels ----
     BvhLevels lv{};
     uint32_t cnt = T, off = 0;
     int L = 0;
     for (;;) {
-        if (L >= TN_MAX_LEVELS) { cleanup(); free_mesh(h); return fail(TN_ERR_ARG, "load_tetrahedra: too many BVH levels"); }
+        if (L >= TN_MAX_LEVELS) return fail(TN_ERR_ARG, "load_tetrahedra: too many BVH levels");
         lv.count[L] = cnt; lv.offset[L] = off;
         off += (cnt + TN_FAN - 1) & ~(TN_FAN - 1);  // keep every level's base a multiple of TN_FAN nodes (256 B)
         ++L;
@@ -294,36 +276,36 @@ int build_mesh(tn_tracer *h, const float *d_xyz, uint32_t V, const uint32_t *d_c
     lv.nlevels = L;
     const uint32_t total_nodes = off;
 
-    TN_CUDA_B(cudaMalloc(&m.nodes, sizeof(float4) * 2 * (size_t)total_nodes));
-    TN_CUDA_B(cudaMalloc(&m.leaves, sizeof(LeafRec) * (size_t)T));
-    TN_CUDA_B(cudaMalloc(&m.leaf_tet, sizeof(uint32_t) * (size_t)T));
-    TN_CUDA_B(cudaMalloc(&keys, sizeof(uint32_t) * (size_t)T));
-    TN_CUDA_B(cudaMalloc(&keys2, sizeof(uint32_t) * (size_t)T));
-    TN_CUDA_B(cudaMalloc(&vals, sizeof(uint32_t) * (size_t)T));
-    TN_CUDA_B(cudaMalloc(&bounds, sizeof(int) * 6));
+    TN_TRY(m.nodes.grow(2 * (size_t)total_nodes));
+    TN_TRY(m.leaves.grow(T));
+    TN_TRY(m.leaf_tet.grow(T));
+    TN_TRY(keys.grow(T));
+    TN_TRY(keys2.grow(T));
+    TN_TRY(vals.grow(T));
+    TN_TRY(bounds.grow(6));
 
     // ordered-int encodings (f2ord) of +FLT_MAX for the min slots and -FLT_MAX for the max slots
     const int hb_enc[6] = {0x7F7FFFFF, 0x7F7FFFFF, 0x7F7FFFFF, (int)0x80800000, (int)0x80800000, (int)0x80800000};
-    TN_CUDA_B(cudaMemcpyAsync(bounds, hb_enc, sizeof(hb_enc), cudaMemcpyHostToDevice, s));
-    k_bounds<<<std::min<uint32_t>((V + 255) / 256, 1184u), 256, 0, s>>>(d_xyz, V, bounds);
-    k_morton<<<(T + 255) / 256, 256, 0, s>>>(d_xyz, (const uint4 *)d_cells, T, bounds, keys, vals);
+    TN_CUDA(cudaMemcpyAsync(bounds.p, hb_enc, sizeof(hb_enc), cudaMemcpyHostToDevice, s));
+    k_bounds<<<std::min<uint32_t>((V + 255) / 256, 1184u), 256, 0, s>>>(d_xyz, V, bounds.p);
+    k_morton<<<(T + 255) / 256, 256, 0, s>>>(d_xyz, (const uint4 *)d_cells, T, bounds.p, keys.p, vals.p);
     size_t tmp_bytes = 0;
-    TN_CUDA_B(cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, keys, keys2, vals, m.leaf_tet, (int)T, 0, 30, s));
-    TN_CUDA_B(cudaMalloc(&tmp, tmp_bytes));
-    TN_CUDA_B(cub::DeviceRadixSort::SortPairs(tmp, tmp_bytes, keys, keys2, vals, m.leaf_tet, (int)T, 0, 30, s));
-    k_leaves<<<(T + 255) / 256, 256, 0, s>>>(d_xyz, (const uint4 *)d_cells, d_tet_faces, m.leaf_tet, T, m.leaves, m.nodes);
+    TN_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, keys.p, keys2.p, vals.p, m.leaf_tet.p, (int)T, 0, 30, s));
+    TN_TRY(tmp.grow(tmp_bytes));
+    TN_CUDA(cub::DeviceRadixSort::SortPairs(tmp.p, tmp_bytes, keys.p, keys2.p, vals.p, m.leaf_tet.p, (int)T, 0, 30, s));
+    k_leaves<<<(T + 255) / 256, 256, 0, s>>>(d_xyz, (const uint4 *)d_cells, d_tet_faces, m.leaf_tet.p, T, m.leaves.p, m.nodes.p);
     for (int l = 1; l < L; ++l) {
         const uint32_t np = lv.count[l], nc = lv.count[l - 1];
-        k_level<<<(np + 127) / 128, 128, 0, s>>>(m.nodes + 2 * (size_t)lv.offset[l - 1], nc, m.nodes + 2 * (size_t)lv.offset[l], np);
+        k_level<<<(np + 127) / 128, 128, 0, s>>>(m.nodes.p + 2 * (size_t)lv.offset[l - 1], nc, m.nodes.p + 2 * (size_t)lv.offset[l], np);
     }
     h->launches += 4 + (L - 1);
-    TN_CUDA_B(cudaGetLastError());
+    TN_CUDA(cudaGetLastError());
 
     // ---- adjacency walk: per-tetrahedron records + a small BVH over the tetrahedra that own a hull face ----
     BvhLevels hlv{};
     if (walkable) {
-        TN_CUDA_B(cudaMalloc(&m.walk, sizeof(WalkRec) * (size_t)T));
-        k_walk_records<<<(T + 127) / 128, 128, 0, s>>>(d_xyz, (const uint4 *)d_cells, d_tet_faces, d_nbr, d_wind, T, m.walk);
+        TN_TRY(m.walk.grow(T));
+        k_walk_records<<<(T + 127) / 128, 128, 0, s>>>(d_xyz, (const uint4 *)d_cells, d_tet_faces, d_nbr, d_wind, T, m.walk.p);
         uint32_t hc_ = H, hoff = 0;
         int HL = 0;
         for (;;) {
@@ -335,27 +317,25 @@ int build_mesh(tn_tracer *h, const float *d_xyz, uint32_t V, const uint32_t *d_c
         }
         if (HL == 1) { hlv.count[1] = 1; hlv.offset[1] = hoff; hoff += TN_FAN; HL = 2; }
         hlv.nlevels = HL;
-        TN_CUDA_B(cudaMalloc(&m.hull_nodes, sizeof(float4) * 2 * (size_t)hoff));
-        TN_CUDA_B(cudaMalloc(&m.hull_leaves, sizeof(LeafRec) * (size_t)H));
-        TN_CUDA_B(cudaMalloc(&m.hull_tet, sizeof(uint32_t) * (size_t)H));
-        k_morton_subset<<<(H + 255) / 256, 256, 0, s>>>(d_xyz, (const uint4 *)d_cells, d_hull_list, H, bounds, keys, vals);
-        TN_CUDA_B(cub::DeviceRadixSort::SortPairs(tmp, tmp_bytes, keys, keys2, vals, m.hull_tet, (int)H, 0, 30, s));
-        k_leaves<<<(H + 255) / 256, 256, 0, s>>>(d_xyz, (const uint4 *)d_cells, d_tet_faces, m.hull_tet, H, m.hull_leaves, m.hull_nodes);
+        TN_TRY(m.hull_nodes.grow(2 * (size_t)hoff));
+        TN_TRY(m.hull_leaves.grow(H));
+        TN_TRY(m.hull_tet.grow(H));
+        k_morton_subset<<<(H + 255) / 256, 256, 0, s>>>(d_xyz, (const uint4 *)d_cells, d_hull_list, H, bounds.p, keys.p, vals.p);
+        TN_CUDA(cub::DeviceRadixSort::SortPairs(tmp.p, tmp_bytes, keys.p, keys2.p, vals.p, m.hull_tet.p, (int)H, 0, 30, s));
+        k_leaves<<<(H + 255) / 256, 256, 0, s>>>(d_xyz, (const uint4 *)d_cells, d_tet_faces, m.hull_tet.p, H, m.hull_leaves.p, m.hull_nodes.p);
         for (int l = 1; l < HL; ++l) {
             const uint32_t np = hlv.count[l], nc = hlv.count[l - 1];
-            k_level<<<(np + 127) / 128, 128, 0, s>>>(m.hull_nodes + 2 * (size_t)hlv.offset[l - 1], nc, m.hull_nodes + 2 * (size_t)hlv.offset[l], np);
+            k_level<<<(np + 127) / 128, 128, 0, s>>>(m.hull_nodes.p + 2 * (size_t)hlv.offset[l - 1], nc, m.hull_nodes.p + 2 * (size_t)hlv.offset[l], np);
         }
         h->launches += 3 + HL;
-        TN_CUDA_B(cudaGetLastError());
+        TN_CUDA(cudaGetLastError());
     }
     int hbounds[6];
-    TN_CUDA_B(cudaMemcpyAsync(hbounds, bounds, sizeof(hbounds), cudaMemcpyDeviceToHost, s));
-    TN_CUDA_B(cudaStreamSynchronize(s));
-    const float amax = absmax_of(hbounds);
-    cleanup();
-#undef TN_CUDA_B
-    m.xyz = d_xyz; m.cells = d_cells; m.V = V; m.T = T; m.F = F; m.lv = lv; m.absmax = amax;
+    TN_CUDA(cudaMemcpyAsync(hbounds, bounds.p, sizeof(hbounds), cudaMemcpyDeviceToHost, s));
+    TN_CUDA(cudaStreamSynchronize(s));
+    m.xyz = d_xyz; m.cells = d_cells; m.V = V; m.T = T; m.F = F; m.lv = lv; m.absmax = absmax_of(hbounds);
     m.walkable = walkable; m.H = walkable ? H : 0; m.hull_lv = hlv;
+    h->mesh = std::move(m);
     return TN_OK;
 }
 
@@ -365,10 +345,10 @@ int build_mesh(tn_tracer *h, const float *d_xyz, uint32_t V, const uint32_t *d_c
 // fires, so non-finite input leaves the tracer unchanged with a single read-back at the end.
 int refit_mesh(tn_tracer *h, const float *d_xyz, uint32_t V, cudaStream_t s, uint32_t *folded_faces, int *walkable) {
     Mesh &m = h->mesh;
-    if (!m.nodes) return fail(TN_ERR_STATE, "update_vertices: no tetrahedra loaded");
+    if (!m.nodes.p) return fail(TN_ERR_STATE, "update_vertices: no tetrahedra loaded");
     if (V != m.V) return fail(TN_ERR_ARG, "update_vertices: " + std::to_string(V) + " vertices, the loaded mesh has " + std::to_string(m.V));
-    if (!h->d_refit) TN_CUDA(cudaMalloc(&h->d_refit, 64));
-    uint32_t *d_small = h->d_refit;  // [0] non-finite flag, [2] hull error bits, [3] folded faces, [4..9] bounds (ordered ints)
+    TN_TRY(h->d_refit.grow(16));
+    uint32_t *d_small = h->d_refit.p;  // [0] non-finite flag, [2] hull error bits, [3] folded faces, [4..9] bounds (ordered ints)
     int *bounds = reinterpret_cast<int *>(d_small + 4);
     // ordered-int encodings (f2ord) of +FLT_MAX for the min slots and -FLT_MAX for the max slots, after four zeroed words
     const int init[10] = {0, 0, 0, 0, 0x7F7FFFFF, 0x7F7FFFFF, 0x7F7FFFFF, (int)0x80800000, (int)0x80800000, (int)0x80800000};
@@ -377,18 +357,18 @@ int refit_mesh(tn_tracer *h, const float *d_xyz, uint32_t V, cudaStream_t s, uin
     k_nonfinite<<<(n + 255) / 256, 256, 0, s>>>(d_xyz, n, d_small);
     k_bounds<<<std::min<uint32_t>((V + 255) / 256, 1184u), 256, 0, s>>>(d_xyz, V, bounds);
     const uint32_t T = m.T;
-    k_refit_leaves<<<(T + 255) / 256, 256, 0, s>>>(d_xyz, (const uint4 *)m.cells, m.leaf_tet, T, d_small, m.leaves, m.nodes);
+    k_refit_leaves<<<(T + 255) / 256, 256, 0, s>>>(d_xyz, (const uint4 *)m.cells, m.leaf_tet.p, T, d_small, m.leaves.p, m.nodes.p);
     for (int l = 1; l < m.lv.nlevels; ++l)
-        k_level<<<(m.lv.count[l] + 127) / 128, 128, 0, s>>>(m.nodes + 2 * (size_t)m.lv.offset[l - 1], m.lv.count[l - 1],
-                                                             m.nodes + 2 * (size_t)m.lv.offset[l], m.lv.count[l]);
+        k_level<<<(m.lv.count[l] + 127) / 128, 128, 0, s>>>(m.nodes.p + 2 * (size_t)m.lv.offset[l - 1], m.lv.count[l - 1],
+                                                             m.nodes.p + 2 * (size_t)m.lv.offset[l], m.lv.count[l]);
     h->launches += 3 + (m.lv.nlevels - 1);
-    if (m.walk) {
-        k_refit_walk<<<(T + 127) / 128, 128, 0, s>>>(d_xyz, (const uint4 *)m.cells, T, d_small, m.walk);
+    if (m.walk.p) {
+        k_refit_walk<<<(T + 127) / 128, 128, 0, s>>>(d_xyz, (const uint4 *)m.cells, T, d_small, m.walk.p);
         const uint32_t H = m.hull_lv.count[0];
-        k_refit_leaves<<<(H + 255) / 256, 256, 0, s>>>(d_xyz, (const uint4 *)m.cells, m.hull_tet, H, d_small, m.hull_leaves, m.hull_nodes);
+        k_refit_leaves<<<(H + 255) / 256, 256, 0, s>>>(d_xyz, (const uint4 *)m.cells, m.hull_tet.p, H, d_small, m.hull_leaves.p, m.hull_nodes.p);
         for (int l = 1; l < m.hull_lv.nlevels; ++l)
-            k_level<<<(m.hull_lv.count[l] + 127) / 128, 128, 0, s>>>(m.hull_nodes + 2 * (size_t)m.hull_lv.offset[l - 1], m.hull_lv.count[l - 1],
-                                                                      m.hull_nodes + 2 * (size_t)m.hull_lv.offset[l], m.hull_lv.count[l]);
+            k_level<<<(m.hull_lv.count[l] + 127) / 128, 128, 0, s>>>(m.hull_nodes.p + 2 * (size_t)m.hull_lv.offset[l - 1], m.hull_lv.count[l - 1],
+                                                                      m.hull_nodes.p + 2 * (size_t)m.hull_lv.offset[l], m.hull_lv.count[l]);
         h->launches += 2 + (m.hull_lv.nlevels - 1);
     }
     int rc = launch_refit_checks(h, d_xyz, d_small + 2, s);
@@ -402,7 +382,7 @@ int refit_mesh(tn_tracer *h, const float *d_xyz, uint32_t V, cudaStream_t s, uin
     h->mesh_gen = next_generation();  // the positions changed
     m.xyz = d_xyz;
     m.absmax = absmax_of(reinterpret_cast<const int *>(hs + 4));
-    m.walkable = m.walk != nullptr && (hs[2] & 4u) == 0 && hs[3] == 0;
+    m.walkable = m.walk.p != nullptr && (hs[2] & 4u) == 0 && hs[3] == 0;
     if (folded_faces) *folded_faces = hs[3];
     if (walkable) *walkable = m.walkable ? 1 : 0;
     return TN_OK;

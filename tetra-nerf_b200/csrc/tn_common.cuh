@@ -3,6 +3,7 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <atomic>
 #include <string>
 
 #include "../../include/tetranerf_b200.h"
@@ -21,6 +22,61 @@ int fail(int code, const std::string &msg);
             return tn::fail(TN_ERR_CUDA, std::string(#expr) + " failed: " + cudaGetErrorString(_e) + " (" + \
                                              __FILE__ + ":" + std::to_string(__LINE__) + ")");              \
     } while (0)
+
+// returns a non-zero TN_* code of expr to the caller
+#define TN_TRY(...)                              \
+    do {                                         \
+        const int _rc = (__VA_ARGS__);           \
+        if (_rc != TN_OK) return _rc;            \
+    } while (0)
+
+// bytes held by every DevArray of the process (tn_debug_device_bytes)
+inline std::atomic<uint64_t> g_device_bytes{0};
+
+// The owner of every device buffer of the library (DESIGN.md §3): grow-only, freed by its destructor.  `cap` (elements) is set only
+// after a successful allocation, so a failed grow leaves {nullptr, 0} and the next call allocates again.  No device is recorded: every
+// owner is destroyed, and every grow runs, under the tracer's DeviceGuard.  No conversion to T *: call sites write `.p`.
+template <typename T>
+struct DevArray {
+    T *p = nullptr;
+    size_t cap = 0;
+
+    DevArray() = default;
+    DevArray(const DevArray &) = delete;
+    DevArray &operator=(const DevArray &) = delete;
+    DevArray(DevArray &&o) noexcept : p(o.p), cap(o.cap) { o.p = nullptr; o.cap = 0; }
+    DevArray &operator=(DevArray &&o) noexcept {
+        if (this != &o) {
+            release();
+            p = o.p; cap = o.cap;
+            o.p = nullptr; o.cap = 0;
+        }
+        return *this;
+    }
+    ~DevArray() { release(); }
+
+    // at least n elements (rounded up to 256 bytes); the contents are not kept.  The old allocation is freed first, so the peak is the
+    // larger of the two, never their sum.
+    int grow(size_t n) {
+        if (n <= cap) return TN_OK;
+        release();
+        const size_t bytes = (n * sizeof(T) + 255) / 256 * 256;
+        void *q = nullptr;
+        TN_CUDA(cudaMalloc(&q, bytes));
+        p = static_cast<T *>(q);
+        cap = bytes / sizeof(T);
+        g_device_bytes += cap * sizeof(T);
+        return TN_OK;
+    }
+
+  private:
+    void release() {
+        if (!p) return;
+        cudaFree(p);
+        g_device_bytes -= cap * sizeof(T);
+        p = nullptr; cap = 0;
+    }
+};
 
 struct DeviceGuard {
     int prev = -1;
@@ -74,23 +130,23 @@ struct Mesh {
     const float *xyz = nullptr;      // borrowed, [V,3]
     const uint32_t *cells = nullptr; // borrowed, [T,4]
     uint32_t V = 0, T = 0, F = 0;
-    uint32_t *tri = nullptr;         // [F,4]: stored winding (v0,v1,v2, 0)   (triangle_indices)
-    uint32_t *tt = nullptr;          // [F,2]: (first owner, second owner|E)   (triangle_tetrahedra)
-    float4 *nodes = nullptr;         // BVH nodes, 2 float4 per node
-    LeafRec *leaves = nullptr;       // [T]
-    uint32_t *leaf_tet = nullptr;    // [T] sorted position -> tetrahedron id
+    DevArray<uint4> tri;             // [F]: stored winding (v0,v1,v2, 0)   (triangle_indices)
+    DevArray<uint2> tt;              // [F]: (first owner, second owner|E)   (triangle_tetrahedra)
+    DevArray<float4> nodes;          // BVH nodes, 2 float4 per node
+    DevArray<LeafRec> leaves;        // [T]
+    DevArray<uint32_t> leaf_tet;     // [T] sorted position -> tetrahedron id
     // adjacency walk (fast path of trace_rays): valid when `walkable`
-    WalkRec *walk = nullptr;         // [T]
-    float4 *hull_nodes = nullptr;    // BVH over the tetrahedra that own a hull face
-    LeafRec *hull_leaves = nullptr;  // [H]
-    uint32_t *hull_tet = nullptr;    // [H] sorted position -> tetrahedron id
+    DevArray<WalkRec> walk;          // [T]
+    DevArray<float4> hull_nodes;     // BVH over the tetrahedra that own a hull face
+    DevArray<LeafRec> hull_leaves;   // [H]
+    DevArray<uint32_t> hull_tet;     // [H] sorted position -> tetrahedron id
     BvhLevels hull_lv{};
     uint32_t H = 0;
     bool walkable = false;           // conforming mesh with a convex hull (always true for a Delaunay triangulation), and after a
                                      // refit (tn_update_vertices) still convex and unfolded
-    // hull edges of a mesh that was walkable at load (walk != nullptr), sorted by (a, b): what the convexity test of a refit reads
-    unsigned long long *hull_ekey = nullptr;  // [hull_ne] (a << 32 | b), a < b
-    uint32_t *hull_eface = nullptr;           // [hull_ne] the hull face of each edge entry
+    // hull edges of a mesh that was walkable at load (walk.p != nullptr), sorted by (a, b): what the convexity test of a refit reads
+    DevArray<unsigned long long> hull_ekey;  // [hull_ne] (a << 32 | b), a < b
+    DevArray<uint32_t> hull_eface;           // [hull_ne] the hull face of each edge entry
     uint32_t hull_ne = 0;
     BvhLevels lv{};
     float absmax = 0.f;              // max |coordinate| over the vertices
@@ -104,11 +160,9 @@ struct SurfaceState;
 struct tn_tracer {
     int device = 0;
     tn::Mesh mesh;
-    int *d_flags = nullptr;  // [0] traversal-stack overflow count, [2] number of rays deferred to the large-buffer pass
-    uint32_t *d_ovf_list = nullptr;  // rays deferred by phase 1 of trace_rays / listed by the walk for the exact stage
-    uint32_t ovf_cap = 0;
-    unsigned long long *d_walk_keys = nullptr;  // [R, M] (t, face) keys written by the adjacency walk
-    size_t walk_keys_cap = 0;
+    tn::DevArray<int> d_flags;  // [0] traversal-stack overflow count, [2] number of rays deferred to the large-buffer pass
+    tn::DevArray<uint32_t> d_ovf_list;  // rays deferred by phase 1 of trace_rays / listed by the walk for the exact stage
+    tn::DevArray<unsigned long long> d_walk_keys;  // [R, M] (t, face) keys written by the adjacency walk
     // trace_rays picks between bit-identical implementations by batch size:
     //   warp-per-ray all-hits BVH gather   <- below walk_quad_min_rays (latency of the few rays in flight dominates)
     //   walk, 8 rays per warp ("quad")     <- [walk_quad_min_rays, walk_min_rays)  (speculative record loads up to walk_quad_spec_max_rays,
@@ -122,25 +176,25 @@ struct tn_tracer {
     uint32_t walk_quad_spec_max_rays = 65536;  // quad and solo walks: batches up to this size load the candidate next records speculatively (tn_walk.cu)
     uint64_t launches = 0;
     uint64_t mesh_gen = 0;  // a fresh next_generation() on every tn_load_tetrahedra / tn_update_vertices (a surface extraction records it)
-    uint32_t *d_refit = nullptr;  // 64 bytes of tn_update_vertices scratch: flags, counts and bounds, read back once per refit
+    tn::DevArray<uint32_t> d_refit;  // 16 words of tn_update_vertices scratch: flags, counts and bounds, read back once per refit
     tn::RenderState *render = nullptr;
     tn::SurfaceState *surface = nullptr;
 };
 
 namespace tn {
 int build_mesh(tn_tracer *h, const float *d_xyz, uint32_t V, const uint32_t *d_cells, uint32_t T, cudaStream_t s);
-// device-built face / adjacency tables (tn_faces.cu); all pointers are device allocations handed to the caller
+// device-built face / adjacency tables (tn_faces.cu)
 struct FaceTables {
-    uint4 *tri = nullptr;        // [F] stored winding (reference numbering), padded
-    uint2 *tt = nullptr;         // [F] (first owner, second owner or TN_EMPTY)
-    uint4 *tet_faces = nullptr;  // [T] face id | TN_FACE_OWNER | TN_FACE_HULL of the face opposite local vertex j
-    uint4 *nbr = nullptr;        // [T] neighbour across each face
-    uint32_t *wind = nullptr;    // [T] stored windings as local vertex indices (2 bits x 3 x 4)
-    uint32_t *hull_list = nullptr;  // [H] tetrahedra owning a hull face, ascending
+    DevArray<uint4> tri;         // [F] stored winding (reference numbering), padded
+    DevArray<uint2> tt;          // [F] (first owner, second owner or TN_EMPTY)
+    DevArray<uint4> tet_faces;   // [T] face id | TN_FACE_OWNER | TN_FACE_HULL of the face opposite local vertex j
+    DevArray<uint4> nbr;         // [T] neighbour across each face
+    DevArray<uint32_t> wind;     // [T] stored windings as local vertex indices (2 bits x 3 x 4)
+    DevArray<uint32_t> hull_list;  // [H] tetrahedra owning a hull face, ascending
     uint32_t F = 0, H = 0;
     bool walkable = false;       // the hull is a closed convex surface
-    unsigned long long *hull_ekey = nullptr;  // walkable: the sorted hull edges (Mesh::hull_ekey / hull_eface), owned by the caller
-    uint32_t *hull_eface = nullptr;
+    DevArray<unsigned long long> hull_ekey;  // walkable: the sorted hull edges (Mesh::hull_ekey / hull_eface)
+    DevArray<uint32_t> hull_eface;
     uint32_t hull_ne = 0;
 };
 int build_faces_device(const float *d_xyz, uint32_t V, const uint32_t *d_cells, uint32_t T, cudaStream_t s, FaceTables &out, int *launches);
@@ -149,7 +203,6 @@ int build_faces_device(const float *d_xyz, uint32_t V, const uint32_t *d_cells, 
 int launch_refit_checks(const tn_tracer *h, const float *d_xyz, uint32_t *d_counts, cudaStream_t s);
 // tn_update_vertices (tn_build.cu)
 int refit_mesh(tn_tracer *h, const float *d_xyz, uint32_t V, cudaStream_t s, uint32_t *folded_faces, int *walkable);
-void free_mesh(tn_tracer *h);
 void free_render(tn_tracer *h);
 void free_surface(tn_tracer *h);
 // a value no earlier call returned (tn_render.cu): the generation of a field, weights or mesh

@@ -95,12 +95,12 @@ __global__ void k_find(const FindParams p) {
 extern "C" int tn_find_tetrahedra(tn_tracer *h, const float *d_positions, uint32_t N, uint32_t *d_tet, float *d_bary, uint32_t *d_verts,
                                   void *stream) {
     if (!h) return tn::fail(TN_ERR_ARG, "null tracer");
-    if (!h->mesh.nodes) return tn::fail(TN_ERR_STATE, "find_tetrahedra: no tetrahedra loaded");
+    if (!h->mesh.nodes.p) return tn::fail(TN_ERR_STATE, "find_tetrahedra: no tetrahedra loaded");
     if (N == 0) return TN_OK;
     tn::DeviceGuard g(h->device);
     tn::FindParams p;
     p.pos = d_positions; p.N = N; p.tet = d_tet; p.bary = d_bary; p.verts = d_verts;
-    p.nodes = h->mesh.nodes; p.leaves = h->mesh.leaves; p.tri = (const uint4 *)h->mesh.tri; p.tt = (const uint2 *)h->mesh.tt;
+    p.nodes = h->mesh.nodes.p; p.leaves = h->mesh.leaves.p; p.tri = h->mesh.tri.p; p.tt = h->mesh.tt.p;
     p.lv = h->mesh.lv; p.absmax = h->mesh.absmax;
     tn::k_find<<<(N + 63) / 64, 64, 0, (cudaStream_t)stream>>>(p);
     h->launches += 1;

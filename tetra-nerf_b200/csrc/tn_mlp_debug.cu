@@ -59,15 +59,14 @@ extern "C" int tn_debug_gemm_bf16x3(int device, const float *d_A, const float *d
     if (K != 64 && K != 128) return tn::fail(TN_ERR_ARG, "tn_debug_gemm_bf16x3: K must be 64 or 128");
     tn::DeviceGuard g(device);
     cudaStream_t s = (cudaStream_t)stream;
-    uint8_t *img = nullptr;
-    TN_CUDA(cudaMalloc(&img, (K / 64) * 32768));
-    tn::launch_pack_weights(d_W, K, 0, K, img, s);
+    tn::DevArray<uint8_t> img;
+    TN_TRY(img.grow((K / 64) * 32768));
+    tn::launch_pack_weights(d_W, K, 0, K, img.p, s);
     const int smem = 65536 + 128;
     TN_CUDA(cudaFuncSetAttribute(tn::k_debug_gemm, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    tn::k_debug_gemm<<<1, 256, smem, s>>>(d_A, img, K, d_out);
+    tn::k_debug_gemm<<<1, 256, smem, s>>>(d_A, img.p, K, d_out);
     TN_CUDA(cudaGetLastError());
     TN_CUDA(cudaStreamSynchronize(s));
-    cudaFree(img);
     return TN_OK;
 }
 

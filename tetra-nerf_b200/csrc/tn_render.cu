@@ -30,33 +30,30 @@ int launch_trace_internal(tn_tracer *h, const float *o, const float *d, uint32_t
 
 struct RenderState {
     // field
-    float *fshadow = nullptr;  // [V,64]
+    DevArray<float> fshadow;   // [V,64]
     uint32_t V = 0;
     // weights
-    uint8_t *wimg = nullptr;   // L1 32K | L2 64K | L3 64K | L4(base part) 64K  (bf16 hi/lo)
-    uint8_t *wimg16 = nullptr; // the same image with fp16 hi/lo halves (mlp_prec == 2)
+    DevArray<uint8_t> wimg;    // L1 32K | L2 64K | L3 64K | L4(base part) 64K  (bf16 hi/lo)
+    DevArray<uint8_t> wimg16;  // the same image with fp16 hi/lo halves (mlp_prec == 2)
     int mlp_prec = 2;          // operand precision of the inference MLP: 2 = f16w2 (default), 3 = bf16x3 (tn_mlp.cuh); training always runs 3
-    float *bias = nullptr;     // b1 b2 b3 [3][128]
-    float *head = nullptr;     // wd[128] wc[3][128] bd bc[3]
-    float *w4dir = nullptr;    // [128][27] + b4[128]
+    DevArray<float> bias;      // b1 b2 b3 [3][128]
+    DevArray<float> head;      // wd[128] wc[3][128] bd bc[3]
+    DevArray<float> w4dir;     // [128][27] + b4[128]
     bool have_weights = false;
     uint64_t gen = 0;          // generation of field + weights: a fresh value from next_generation() on every set_field / set_weights
     // workspace
-    size_t cap_R = 0, cap_M = 0, cap_Sc = 0, cap_S2 = 0;
-    uint32_t *num = nullptr, *cells = nullptr, *verts = nullptr;
-    float *bary = nullptr, *dist = nullptr;
-    uint32_t *n_active = nullptr, *ray_list = nullptr;
-    float *ebins_c = nullptr, *sbins_c = nullptr, *bary_c = nullptr, *dens_c = nullptr;
-    uint4 *vi_c = nullptr;
-    float *ebins_f = nullptr, *bary_f = nullptr, *out_f = nullptr, *dirbias = nullptr;
-    uint4 *vi_f = nullptr;
+    DevArray<uint32_t> num, cells, verts;  // trace output: [R], [R,M], [R,M,4]
+    DevArray<float> bary, dist;            // [R,M,6], [R,M,2]
+    DevArray<uint32_t> n_active, ray_list; // 8 words (see TrainBufs), [R] slot -> ray
+    DevArray<float> ebins_c, sbins_c, bary_c, dens_c;  // [R,Sc+1], [R,Sc+1], [R*Sc,3], [R*Sc]
+    DevArray<uint4> vi_c;                  // [R*Sc]
+    DevArray<float> ebins_f, bary_f, out_f, dirbias;   // [R,S2+1], [R*S2,3], [R*S2,4], [R,128]
+    DevArray<uint4> vi_f;                  // [R*S2]
     // training: backward weight image, per-sample head gradients, accumulators (scratch of every backward, saved state or not)
-    uint8_t *wimg_bwd = nullptr;       // 7 stages of 32 KB (tn_mlp_bwd.cuh)
-    float *sbins_f = nullptr, *enc = nullptr;   // tn_render_train_forward: [R,S2+1] spacing bins of the fine pass, [R,27] encoded directions (per slot)
-    float4 *dout = nullptr;            // [R*S2] gradients at the head pre-activations
-    float *gshadow = nullptr, *gw = nullptr, *g_dirbias = nullptr;
-    size_t cap_train_R = 0, cap_train_S2 = 0;
-    uint32_t gshadow_V = 0;
+    DevArray<uint8_t> wimg_bwd;        // 7 stages of 32 KB (tn_mlp_bwd.cuh)
+    DevArray<float> sbins_f, enc;      // tn_render_train_forward: [R,S2+1] spacing bins of the fine pass, [R,27] encoded directions (per slot)
+    DevArray<float4> dout;             // [R*S2] gradients at the head pre-activations
+    DevArray<float> gshadow, gw, g_dirbias;  // [V,64], [GW_TOTAL], [R,128]
     // what the last training forward ran with (the backward continues from its buffers)
     bool train_valid = false;
     uint32_t t_R = 0, t_M = 0, t_Sc = 0, t_Sf = 0, t_S2 = 0;
@@ -73,46 +70,25 @@ struct RenderState {
     bool t_det = false;                // mode the last training forward ran in: its backward continues in it
     uint32_t bwd_grid = 0;             // CTAs of the backward MLP kernel (test hook; 0 = default)
     int smem_optin = 0;                // the device's opt-in dynamic shared memory per block (read on the first render call)
-    uint32_t *ray_flag = nullptr, *ray_slot = nullptr;  // [R] ray has hits, its slot (exclusive scan)
-    size_t cap_slot_R = 0;
-    void *cub_tmp = nullptr;           // CUB scan / sort temporary storage
-    size_t cub_tmp_bytes = 0;
-    float *det_part = nullptr;         // [BWD_PARTS][BWD_PART_STRIDE] per-partition dW / column sums
-    float *det_gdb = nullptr;          // [4 (ntiles + R)][128] direction-bias gradient partials
-    float *det_dx = nullptr;           // [R*S2,64] feature gradient per sample
-    float4 *det_sums = nullptr;        // [R] head-bias gradient per slot
-    float *det_dbg = nullptr;          // [R/64][128*28] partial W4dir / b4 gradients per block of k_dirbias_grads
-    uint32_t *det_keys = nullptr, *det_vals = nullptr;  // [2][R*S2*4] (vertex, sample row * 4 + k) pairs, sort input | output
-    size_t cap_det_R = 0, cap_det_S2 = 0;
+    DevArray<uint32_t> ray_flag, ray_slot;  // [R] ray has hits, its slot (exclusive scan)
+    DevArray<uint8_t> cub_tmp;         // CUB scan / sort temporary storage
+    DevArray<float> det_part;          // [BWD_PARTS][BWD_PART_STRIDE] per-partition dW / column sums
+    DevArray<float> det_gdb;           // [4 (ntiles + R)][128] direction-bias gradient partials
+    DevArray<float> det_dx;            // [R*S2,64] feature gradient per sample
+    DevArray<float4> det_sums;         // [R] head-bias gradient per slot
+    DevArray<float> det_dbg;           // [R/64][128*28] partial W4dir / b4 gradients per block of k_dirbias_grads
+    DevArray<uint32_t> det_keys, det_vals;  // [2][R*S2*4] (vertex, sample row * 4 + k) pairs, sort input | output
     // normal map (tn_render with d_normals): density gradient per sample of the last normals render
-    float4 *grad_n = nullptr;
-    size_t cap_grad_n = 0;
+    DevArray<float4> grad_n;
     // ray gradients (tn_render_train_backward_saved with ray or vertex outputs): dX rows of the default mode (the deterministic mode keeps them in det_dx),
     // dL/dx per sample of the last such backward
-    float *ray_dx = nullptr;
-    float4 *ray_gx = nullptr;
-    size_t cap_ray_dx = 0, cap_ray_gx = 0;
+    DevArray<float> ray_dx;
+    DevArray<float4> ray_gx;
 };
-
-static void free_ws(RenderState *r) {
-    cudaFree(r->num); cudaFree(r->cells); cudaFree(r->verts); cudaFree(r->bary); cudaFree(r->dist);
-    cudaFree(r->n_active); cudaFree(r->ray_list); cudaFree(r->ebins_c); cudaFree(r->sbins_c); cudaFree(r->bary_c); cudaFree(r->dens_c);
-    cudaFree(r->vi_c); cudaFree(r->ebins_f); cudaFree(r->bary_f); cudaFree(r->out_f); cudaFree(r->dirbias); cudaFree(r->vi_f);
-    r->num = r->cells = r->verts = nullptr; r->bary = r->dist = nullptr; r->n_active = r->ray_list = nullptr;
-    r->ebins_c = r->sbins_c = r->bary_c = r->dens_c = nullptr; r->vi_c = nullptr;
-    r->ebins_f = r->bary_f = r->out_f = r->dirbias = nullptr; r->vi_f = nullptr;
-    r->cap_R = r->cap_M = r->cap_Sc = r->cap_S2 = 0;
-}
 
 void free_render(tn_tracer *h) {
     if (!h->render) return;
     RenderState *r = h->render;
-    free_ws(r);
-    cudaFree(r->fshadow); cudaFree(r->wimg); cudaFree(r->wimg16); cudaFree(r->bias); cudaFree(r->head); cudaFree(r->w4dir);
-    cudaFree(r->wimg_bwd); cudaFree(r->sbins_f); cudaFree(r->enc); cudaFree(r->dout); cudaFree(r->gshadow); cudaFree(r->gw); cudaFree(r->g_dirbias);
-    cudaFree(r->ray_flag); cudaFree(r->ray_slot); cudaFree(r->cub_tmp); cudaFree(r->det_part); cudaFree(r->det_gdb); cudaFree(r->det_dx);
-    cudaFree(r->det_sums); cudaFree(r->det_dbg); cudaFree(r->det_keys); cudaFree(r->det_vals);
-    cudaFree(r->grad_n); cudaFree(r->ray_dx); cudaFree(r->ray_gx);
     for (auto &e : r->ev) if (e) cudaEventDestroy(e);
     for (auto &e : r->evb) if (e) cudaEventDestroy(e);
     delete r;
@@ -127,8 +103,8 @@ uint64_t next_generation() {
 
 int render_inputs(tn_tracer *h, RenderInputs *out) {
     const RenderState *r = h->render;
-    if (!r || !r->fshadow || !r->have_weights) return TN_ERR_STATE;
-    *out = RenderInputs{r->fshadow, r->V, r->wimg, r->bias, r->head, r->w4dir, r->gen};
+    if (!r || !r->fshadow.p || !r->have_weights) return TN_ERR_STATE;
+    *out = RenderInputs{r->fshadow.p, r->V, r->wimg.p, r->bias.p, r->head.p, r->w4dir.p, r->gen};
     return TN_OK;
 }
 
@@ -801,60 +777,45 @@ __global__ void __launch_bounds__(SAMPLE_WARPS * 32) k_dirbias_only(const Sample
 }
 
 static int ensure_ws(RenderState *r, size_t R, size_t M, size_t Sc, size_t S2) {
-    if (R <= r->cap_R && M <= r->cap_M && Sc <= r->cap_Sc && S2 <= r->cap_S2) return TN_OK;
-    free_ws(r);
-    R = std::max(R, r->cap_R); M = std::max(M, r->cap_M); Sc = std::max(Sc, r->cap_Sc); S2 = std::max(S2, r->cap_S2);
-#define A(ptr, bytes) TN_CUDA(cudaMalloc((void **)&(ptr), (bytes)))
-    A(r->num, 4 * R); A(r->cells, 4 * R * M); A(r->verts, 16 * R * M); A(r->bary, 24 * R * M); A(r->dist, 8 * R * M);
-    A(r->n_active, 32); A(r->ray_list, 4 * R);  // words 4, 5: clip bounds of the expected depth
-    A(r->ebins_c, 4 * R * (Sc + 1)); A(r->sbins_c, 4 * R * (Sc + 1)); A(r->bary_c, 12 * R * Sc); A(r->dens_c, 4 * R * Sc); A(r->vi_c, 16 * R * Sc);
-    A(r->ebins_f, 4 * R * (S2 + 1)); A(r->bary_f, 12 * R * S2); A(r->out_f, 16 * R * S2); A(r->dirbias, 512 * R); A(r->vi_f, 16 * R * S2);
-#undef A
-    r->cap_R = R; r->cap_M = M; r->cap_Sc = Sc; r->cap_S2 = S2;
+    TN_TRY(r->num.grow(R)); TN_TRY(r->cells.grow(R * M)); TN_TRY(r->verts.grow(4 * R * M)); TN_TRY(r->bary.grow(6 * R * M));
+    TN_TRY(r->dist.grow(2 * R * M));
+    TN_TRY(r->n_active.grow(8)); TN_TRY(r->ray_list.grow(R));  // n_active words 4, 5: clip bounds of the expected depth
+    TN_TRY(r->ebins_c.grow(R * (Sc + 1))); TN_TRY(r->sbins_c.grow(R * (Sc + 1))); TN_TRY(r->bary_c.grow(3 * R * Sc));
+    TN_TRY(r->dens_c.grow(R * Sc)); TN_TRY(r->vi_c.grow(R * Sc));
+    TN_TRY(r->ebins_f.grow(R * (S2 + 1))); TN_TRY(r->bary_f.grow(3 * R * S2)); TN_TRY(r->out_f.grow(4 * R * S2));
+    TN_TRY(r->dirbias.grow(128 * R)); TN_TRY(r->vi_f.grow(R * S2));
     return TN_OK;
 }
 
-static int ensure_cub_tmp(RenderState *r, size_t bytes) {
-    if (bytes <= r->cub_tmp_bytes) return TN_OK;
-    cudaFree(r->cub_tmp); r->cub_tmp = nullptr; r->cub_tmp_bytes = 0;
-    TN_CUDA(cudaMalloc(&r->cub_tmp, bytes));
-    r->cub_tmp_bytes = bytes;
+// training forward: the tracer-held pair's fine bins and encodings, and the gradient scratch of every backward
+static int ensure_train_ws(RenderState *r, size_t R, size_t S2, uint32_t V) {
+    TN_TRY(r->sbins_f.grow(R * (S2 + 1))); TN_TRY(r->enc.grow(27 * R)); TN_TRY(r->dout.grow(R * S2)); TN_TRY(r->g_dirbias.grow(128 * R));
+    TN_TRY(r->gw.grow(GW_TOTAL));
+    TN_TRY(r->gshadow.grow(64 * (size_t)V));
     return TN_OK;
 }
 
 // deterministic mode, forward: slot of every ray = number of rays with hits before it (exclusive scan)
 static int ordered_slots(RenderState *r, uint32_t R, cudaStream_t s) {
-    if (R > r->cap_slot_R) {
-        cudaFree(r->ray_flag); cudaFree(r->ray_slot); r->ray_flag = r->ray_slot = nullptr; r->cap_slot_R = 0;
-        TN_CUDA(cudaMalloc((void **)&r->ray_flag, 4 * (size_t)R));
-        TN_CUDA(cudaMalloc((void **)&r->ray_slot, 4 * (size_t)R));
-        r->cap_slot_R = R;
-    }
+    TN_TRY(r->ray_flag.grow(R)); TN_TRY(r->ray_slot.grow(R));
     size_t bytes = 0;
-    TN_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, bytes, r->ray_flag, r->ray_slot, (int)R, s));
-    int rc = ensure_cub_tmp(r, bytes);
-    if (rc) return rc;
-    k_ray_flags<<<(R + 255) / 256, 256, 0, s>>>(R, r->num, r->ray_flag);
-    TN_CUDA(cub::DeviceScan::ExclusiveSum(r->cub_tmp, bytes, r->ray_flag, r->ray_slot, (int)R, s));
+    TN_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, bytes, r->ray_flag.p, r->ray_slot.p, (int)R, s));
+    TN_TRY(r->cub_tmp.grow(bytes));
+    k_ray_flags<<<(R + 255) / 256, 256, 0, s>>>(R, r->num.p, r->ray_flag.p);
+    TN_CUDA(cub::DeviceScan::ExclusiveSum(r->cub_tmp.p, bytes, r->ray_flag.p, r->ray_slot.p, (int)R, s));
     return TN_OK;
 }
 
 // deterministic mode, backward workspace for R rays of S2 fine samples
 static int ensure_det_ws(RenderState *r, size_t R, size_t S2) {
-    if (!r->det_part) TN_CUDA(cudaMalloc((void **)&r->det_part, sizeof(float) * BWD_PARTS * (size_t)BWD_PART_STRIDE));
-    if (R <= r->cap_det_R && S2 <= r->cap_det_S2) return TN_OK;
-    cudaFree(r->det_gdb); cudaFree(r->det_dx); cudaFree(r->det_sums); cudaFree(r->det_dbg); cudaFree(r->det_keys); cudaFree(r->det_vals);
-    r->det_gdb = r->det_dx = r->det_dbg = nullptr; r->det_sums = nullptr; r->det_keys = r->det_vals = nullptr;
-    r->cap_det_R = r->cap_det_S2 = 0;
-    R = std::max(R, r->cap_det_R); S2 = std::max(S2, r->cap_det_S2);
     const size_t rows = R * S2, ntiles = (rows + BWD_TILE - 1) / BWD_TILE;
-    TN_CUDA(cudaMalloc((void **)&r->det_gdb, sizeof(float) * 4 * (ntiles + R) * 128));
-    TN_CUDA(cudaMalloc((void **)&r->det_dx, sizeof(float) * 64 * rows));
-    TN_CUDA(cudaMalloc((void **)&r->det_sums, sizeof(float4) * R));
-    TN_CUDA(cudaMalloc((void **)&r->det_dbg, sizeof(float) * DBG_PART * ((R + DBG_SLOTS - 1) / DBG_SLOTS)));
-    TN_CUDA(cudaMalloc((void **)&r->det_keys, sizeof(uint32_t) * 2 * 4 * rows));
-    TN_CUDA(cudaMalloc((void **)&r->det_vals, sizeof(uint32_t) * 2 * 4 * rows));
-    r->cap_det_R = R; r->cap_det_S2 = S2;
+    TN_TRY(r->det_part.grow((size_t)BWD_PARTS * BWD_PART_STRIDE));
+    TN_TRY(r->det_gdb.grow(4 * (ntiles + R) * 128));
+    TN_TRY(r->det_dx.grow(64 * rows));
+    TN_TRY(r->det_sums.grow(R));
+    TN_TRY(r->det_dbg.grow((size_t)DBG_PART * ((R + DBG_SLOTS - 1) / DBG_SLOTS)));
+    TN_TRY(r->det_keys.grow(2 * 4 * rows));
+    TN_TRY(r->det_vals.grow(2 * 4 * rows));
     return TN_OK;
 }
 
@@ -867,8 +828,9 @@ extern "C" int tn_render_set_field(tn_tracer *h, const float *d_field, uint32_t 
     if (C != 64) return fail(TN_ERR_ARG, "tn_render: field_dim must be 64 (model.py:81)");
     DeviceGuard g(h->device);
     RenderState *r = state(h);
-    if (r->V != V) { cudaFree(r->fshadow); r->fshadow = nullptr; TN_CUDA(cudaMalloc((void **)&r->fshadow, sizeof(float) * 64 * (size_t)V)); r->V = V; }
-    k_transpose64<<<(V + 31) / 32, dim3(32, 8), 0, (cudaStream_t)stream>>>(d_field, r->fshadow, V);
+    TN_TRY(r->fshadow.grow(64 * (size_t)V));
+    r->V = V;
+    k_transpose64<<<(V + 31) / 32, dim3(32, 8), 0, (cudaStream_t)stream>>>(d_field, r->fshadow.p, V);
     h->launches += 1;
     r->gen = next_generation();
     TN_CUDA(cudaGetLastError());
@@ -890,28 +852,23 @@ extern "C" int tn_render_set_weights(tn_tracer *h, const float *const *P, void *
     DeviceGuard g(h->device);
     RenderState *r = state(h);
     cudaStream_t s = (cudaStream_t)stream;
-    if (!r->wimg) {
-        TN_CUDA(cudaMalloc((void **)&r->wimg, 32768 + 3 * 65536));
-        TN_CUDA(cudaMalloc((void **)&r->wimg16, 32768 + 3 * 65536));
-        TN_CUDA(cudaMalloc((void **)&r->bias, sizeof(float) * 384));
-        TN_CUDA(cudaMalloc((void **)&r->head, sizeof(float) * 520));
-        TN_CUDA(cudaMalloc((void **)&r->w4dir, sizeof(float) * (128 * 27 + 128)));
-    }
-    launch_pack_weights(P[0], 64, 0, 64, r->wimg, s);                     // mlp_base.layers.0.weight [128,64]
-    launch_pack_weights(P[2], 128, 0, 128, r->wimg + 32768, s);           // mlp_base.layers.1.weight [128,128]
-    launch_pack_weights(P[4], 128, 0, 128, r->wimg + 32768 + 65536, s);   // mlp_base.layers.2.weight
-    launch_pack_weights(P[6], 155, 27, 128, r->wimg + 32768 + 131072, s); // mlp_head.layers.0.weight [128,155], base part
-    launch_pack_weights(P[0], 64, 0, 64, r->wimg16, s, 32768u, 16384u, 1);
-    launch_pack_weights(P[2], 128, 0, 128, r->wimg16 + 32768, s, 32768u, 16384u, 1);
-    launch_pack_weights(P[4], 128, 0, 128, r->wimg16 + 32768 + 65536, s, 32768u, 16384u, 1);
-    launch_pack_weights(P[6], 155, 27, 128, r->wimg16 + 32768 + 131072, s, 32768u, 16384u, 1);
-    k_pack_small<<<1, 128, 0, s>>>(P[1], P[3], P[5], P[6], P[7], P[8], P[9], P[10], P[11], r->bias, r->head, r->w4dir);
+    TN_TRY(r->wimg.grow(32768 + 3 * 65536)); TN_TRY(r->wimg16.grow(32768 + 3 * 65536));
+    TN_TRY(r->bias.grow(384)); TN_TRY(r->head.grow(520)); TN_TRY(r->w4dir.grow(128 * 27 + 128));
+    TN_TRY(r->wimg_bwd.grow(BWD_WIMG_BYTES));
+    launch_pack_weights(P[0], 64, 0, 64, r->wimg.p, s);                     // mlp_base.layers.0.weight [128,64]
+    launch_pack_weights(P[2], 128, 0, 128, r->wimg.p + 32768, s);           // mlp_base.layers.1.weight [128,128]
+    launch_pack_weights(P[4], 128, 0, 128, r->wimg.p + 32768 + 65536, s);   // mlp_base.layers.2.weight
+    launch_pack_weights(P[6], 155, 27, 128, r->wimg.p + 32768 + 131072, s); // mlp_head.layers.0.weight [128,155], base part
+    launch_pack_weights(P[0], 64, 0, 64, r->wimg16.p, s, 32768u, 16384u, 1);
+    launch_pack_weights(P[2], 128, 0, 128, r->wimg16.p + 32768, s, 32768u, 16384u, 1);
+    launch_pack_weights(P[4], 128, 0, 128, r->wimg16.p + 32768 + 65536, s, 32768u, 16384u, 1);
+    launch_pack_weights(P[6], 155, 27, 128, r->wimg16.p + 32768 + 131072, s, 32768u, 16384u, 1);
+    k_pack_small<<<1, 128, 0, s>>>(P[1], P[3], P[5], P[6], P[7], P[8], P[9], P[10], P[11], r->bias.p, r->head.p, r->w4dir.p);
     // backward image (tn_mlp_bwd.cuh): stage 0 = [W1 hi | W1 lo]; then per 128-wide layer [hi kb0 | hi kb1][lo kb0 | lo kb1]
-    if (!r->wimg_bwd) TN_CUDA(cudaMalloc((void **)&r->wimg_bwd, BWD_WIMG_BYTES));
-    launch_pack_weights(P[0], 64, 0, 64, r->wimg_bwd, s, 16384u, 16384u);
-    launch_pack_weights(P[2], 128, 0, 128, r->wimg_bwd + 1 * BWD_STAGE, s, 16384u, 32768u);
-    launch_pack_weights(P[4], 128, 0, 128, r->wimg_bwd + 3 * BWD_STAGE, s, 16384u, 32768u);
-    launch_pack_weights(P[6], 155, 27, 128, r->wimg_bwd + 5 * BWD_STAGE, s, 16384u, 32768u);
+    launch_pack_weights(P[0], 64, 0, 64, r->wimg_bwd.p, s, 16384u, 16384u);
+    launch_pack_weights(P[2], 128, 0, 128, r->wimg_bwd.p + 1 * BWD_STAGE, s, 16384u, 32768u);
+    launch_pack_weights(P[4], 128, 0, 128, r->wimg_bwd.p + 3 * BWD_STAGE, s, 16384u, 32768u);
+    launch_pack_weights(P[6], 155, 27, 128, r->wimg_bwd.p + 5 * BWD_STAGE, s, 16384u, 32768u);
     h->launches += 13;
     r->gen = next_generation();
     TN_CUDA(cudaGetLastError());
@@ -932,7 +889,7 @@ struct TrainBufs {
     float *dirbias, *enc;      // [R,128] direction bias, [R,27] encoded direction
 };
 static TrainBufs own_bufs(RenderState *r) {
-    return TrainBufs{r->n_active, r->ray_list, r->ebins_f, r->sbins_f, r->vi_f, r->bary_f, r->out_f, r->dirbias, r->enc};
+    return TrainBufs{r->n_active.p, r->ray_list.p, r->ebins_f.p, r->sbins_f.p, r->vi_f.p, r->bary_f.p, r->out_f.p, r->dirbias.p, r->enc.p};
 }
 
 // saved-state blob of tn_render_train_forward_saved: this header, then the TrainBufs arrays, each 256-byte aligned
@@ -970,7 +927,6 @@ struct TrainFwd {
     const float *jit_c, *jit_f;
     const TrainBufs *saved;
 };
-static int ensure_train_ws(RenderState *r, size_t R, size_t S2, uint32_t V);
 
 static int render_impl(tn_tracer *h, const tn_render_config *cfg, const float *d_origins, const float *d_directions, uint32_t R,
                        float *d_rgb, float *d_acc, float *d_depth, uint8_t *d_mask, const TrainFwd *tf, float *d_normals, float *d_edepth,
@@ -981,8 +937,8 @@ static int render_impl(tn_tracer *h, const tn_render_config *cfg, const float *d
         return fail(TN_ERR_ARG, "tn_render: the fused pixel gather (tn_render_set_gather) carries no expected depth; switch it off first");
     if (r && r->gather_world && d_normals != nullptr)
         return fail(TN_ERR_ARG, "tn_render: the fused pixel gather (tn_render_set_gather) carries no normals; switch it off first");
-    if (!r || !r->fshadow || !r->have_weights) return fail(TN_ERR_STATE, "tn_render: call tn_render_set_field and tn_render_set_weights first");
-    if (!h->mesh.nodes) return fail(TN_ERR_STATE, "tn_render: no tetrahedra loaded");
+    if (!r || !r->fshadow.p || !r->have_weights) return fail(TN_ERR_STATE, "tn_render: call tn_render_set_field and tn_render_set_weights first");
+    if (!h->mesh.nodes.p) return fail(TN_ERR_STATE, "tn_render: no tetrahedra loaded");
     if (r->V != h->mesh.V) return fail(TN_ERR_ARG, "tn_render: field has a different vertex count than the mesh");
     const uint32_t M = cfg->max_ray_triangles, Sc = cfg->num_samples, Sf = cfg->num_fine_samples;
     if (Sc == 0 || Sc > 4096 || Sf > 4096) return fail(TN_ERR_ARG, "tn_render: num_samples must be in [1,4096]");
@@ -1014,17 +970,9 @@ static int render_impl(tn_tracer *h, const tn_render_config *cfg, const float *d
                                         ", above the device's shared-memory limit of " + std::to_string(r->smem_optin) +
                                         " bytes (fewer samples or a smaller max_ray_triangles)");
     }
-    int rc = ensure_ws(r, R, M, Sc, S2);
-    if (rc) return rc;
-    if (d_normals != nullptr && (size_t)R * S2 > r->cap_grad_n) {
-        cudaFree(r->grad_n); r->grad_n = nullptr; r->cap_grad_n = 0;
-        TN_CUDA(cudaMalloc((void **)&r->grad_n, sizeof(float4) * (size_t)R * S2));
-        r->cap_grad_n = (size_t)R * S2;
-    }
-    if (tf != nullptr) {
-        rc = ensure_train_ws(r, R, S2, r->V);
-        if (rc) return rc;
-    }
+    TN_TRY(ensure_ws(r, R, M, Sc, S2));
+    if (d_normals != nullptr) TN_TRY(r->grad_n.grow((size_t)R * S2));
+    if (tf != nullptr) TN_TRY(ensure_train_ws(r, R, S2, r->V));
     r->train_valid = false;
     const TrainBufs b = tf != nullptr && tf->saved != nullptr ? *tf->saved : own_bufs(r);
     const int prec = tf != nullptr ? 3 : r->mlp_prec;  // the training forward keeps bf16x3 (its backward recomputes in bf16x3)
@@ -1036,20 +984,20 @@ static int render_impl(tn_tracer *h, const tn_render_config *cfg, const float *d
 #define TN_EV(i) do { if (r->profile) cudaEventRecord(r->ev[i], s); } while (0)
     TN_EV(0);  // the "trace" interval includes the L2 warm-up it exists for
     {   // L2 warm-up of everything read-only that the step gathers from (mesh tables, field shadow, weight image)
-        const void *extra[2] = {r->fshadow, prec == 2 ? r->wimg16 : r->wimg};
+        const void *extra[2] = {r->fshadow.p, prec == 2 ? r->wimg16.p : r->wimg.p};
         const size_t extra_b[2] = {sizeof(float) * 64 * (size_t)r->V, 32768 + 3 * 65536};
-        rc = launch_prefetch(h, extra, extra_b, 2, s);
+        const int rc = launch_prefetch(h, extra, extra_b, 2, s);
         if (rc) return rc;
     }
-    rc = launch_trace_internal(h, d_origins, d_directions, R, M, r->num, r->cells, r->bary, r->dist, r->verts, 0, s);
+    int rc = launch_trace_internal(h, d_origins, d_directions, R, M, r->num.p, r->cells.p, r->bary.p, r->dist.p, r->verts.p, 0, s);
     if (rc) return rc;
     TN_EV(1);
     SampleParams p{};
     p.R = R; p.M = M; p.Sc = Sc; p.Sf = Sf; p.S2 = S2; p.biased = cfg->use_biased_sampler;
-    p.num = r->num; p.dist = (const float2 *)r->dist; p.verts = (const uint4 *)r->verts; p.bary = r->bary;
+    p.num = r->num.p; p.dist = (const float2 *)r->dist.p; p.verts = (const uint4 *)r->verts.p; p.bary = r->bary.p;
     p.o = d_origins; p.d = d_directions; p.n_active = b.n_active; p.ray_list = b.ray_list;
-    p.ebins_c = r->ebins_c; p.sbins_c = r->sbins_c; p.bary_c = r->bary_c; p.vi_c = r->vi_c; p.dens_c = r->dens_c;
-    p.ebins_f = b.ebins_f; p.bary_f = b.bary_f; p.vi_f = b.vi_f; p.dirbias = b.dirbias; p.w4dir = r->w4dir; p.out_f = b.out_f;
+    p.ebins_c = r->ebins_c.p; p.sbins_c = r->sbins_c.p; p.bary_c = r->bary_c.p; p.vi_c = r->vi_c.p; p.dens_c = r->dens_c.p;
+    p.ebins_f = b.ebins_f; p.bary_f = b.bary_f; p.vi_f = b.vi_f; p.dirbias = b.dirbias; p.w4dir = r->w4dir.p; p.out_f = b.out_f;
     p.rgb = d_rgb; p.acc = d_acc; p.depth = d_depth; p.mask = d_mask;
     p.far_plane = cfg->far_plane; p.bg0 = cfg->background[0]; p.bg1 = cfg->background[1]; p.bg2 = cfg->background[2];
     if (tf != nullptr) { p.train = 1; p.jit_c = tf->jit_c; p.jit_f = tf->jit_f; p.sbins_f = b.sbins_f; p.enc = b.enc; }
@@ -1072,14 +1020,14 @@ static int render_impl(tn_tracer *h, const tn_render_config *cfg, const float *d
     if (det) {
         rc = ordered_slots(r, R, s);
         if (rc) return rc;
-        p.ray_slot = r->ray_slot;
+        p.ray_slot = r->ray_slot.p;
         h->launches += 2;
     }
     k_coarse_sample<<<gridR, SAMPLE_WARPS * 32, smem_sc, s>>>(p);
     TN_EV(2);
     MlpParams mc{};
-    mc.n_active = b.n_active; mc.S = Sc; mc.vi = r->vi_c; mc.bary = r->bary_c; mc.fshadow = r->fshadow; mc.wimg = prec == 2 ? r->wimg16 : r->wimg;
-    mc.bias = r->bias; mc.head = r->head; mc.dirbias = nullptr; mc.out = r->dens_c;
+    mc.n_active = b.n_active; mc.S = Sc; mc.vi = r->vi_c.p; mc.bary = r->bary_c.p; mc.fshadow = r->fshadow.p; mc.wimg = prec == 2 ? r->wimg16.p : r->wimg.p;
+    mc.bias = r->bias.p; mc.head = r->head.p; mc.dirbias = nullptr; mc.out = r->dens_c.p;
     mc.tile_ctr = b.n_active + 1;  // words 1, 2 of the zeroed 16-byte block: tile counters of the coarse / fine pass
     // one CTA per SM at most (the weight image fills its shared memory), MLP_WGS tiles of MLP_TILE samples in flight per CTA
     int sms = 132;
@@ -1098,7 +1046,7 @@ static int render_impl(tn_tracer *h, const tn_render_config *cfg, const float *d
     MlpParams mf = mc;
     mf.S = S2; mf.dirbias = b.dirbias; mf.out = b.out_f;
     if (!single) { mf.vi = b.vi_f; mf.bary = b.bary_f; }
-    else p.ebins_f = r->ebins_c;  // k_composite integrates over the coarse bins
+    else p.ebins_f = r->ebins_c.p;  // k_composite integrates over the coarse bins
     mf.tile_ctr = b.n_active + 2;
     rc = launch_fine(mf, grid_f, s);
     if (rc) return rc;
@@ -1109,7 +1057,7 @@ static int render_impl(tn_tracer *h, const tn_render_config *cfg, const float *d
     h->launches += 5;
     TN_CUDA(cudaGetLastError());
     if (d_edepth != nullptr) {  // after the six timed intervals, as the normals
-        k_expected_depth_finalize<<<(R + 255) / 256, 256, 0, s>>>(R, r->num, p.dbounds, cfg->far_plane, d_edepth);
+        k_expected_depth_finalize<<<(R + 255) / 256, 256, 0, s>>>(R, r->num.p, p.dbounds, cfg->far_plane, d_edepth);
         h->launches += 1;
         TN_CUDA(cudaGetLastError());
     }
@@ -1117,7 +1065,7 @@ static int render_impl(tn_tracer *h, const tn_render_config *cfg, const float *d
         NormalsLaunch nl{};
         nl.n_active = b.n_active; nl.ray_list = b.ray_list; nl.tile_ctr = b.n_active + 3;  // word 3 of the zeroed block
         nl.S = S2; nl.R = R; nl.prec = (uint32_t)prec; nl.vi = mf.vi; nl.bary = mf.bary; nl.ebins = p.ebins_f; nl.out_f = b.out_f;
-        nl.fshadow = r->fshadow; nl.wimg = mf.wimg; nl.bias = r->bias; nl.head = r->head; nl.xyz = h->mesh.xyz; nl.grad = r->grad_n;
+        nl.fshadow = r->fshadow.p; nl.wimg = mf.wimg; nl.bias = r->bias.p; nl.head = r->head.p; nl.xyz = h->mesh.xyz; nl.grad = r->grad_n.p;
         nl.normals = d_normals;
         rc = launch_normals(nl, sms, s);
         if (rc) return rc;
@@ -1128,26 +1076,6 @@ static int render_impl(tn_tracer *h, const tn_render_config *cfg, const float *d
         r->t_det = det;
         r->t_R = R; r->t_M = M; r->t_Sc = Sc; r->t_Sf = Sf; r->t_S2 = S2;
         r->t_bg[0] = cfg->background[0]; r->t_bg[1] = cfg->background[1]; r->t_bg[2] = cfg->background[2];
-    }
-    return TN_OK;
-}
-
-static int ensure_train_ws(RenderState *r, size_t R, size_t S2, uint32_t V) {
-    if (R > r->cap_train_R || S2 > r->cap_train_S2) {
-        cudaFree(r->sbins_f); cudaFree(r->enc); cudaFree(r->dout); cudaFree(r->g_dirbias);
-        r->sbins_f = r->enc = r->g_dirbias = nullptr; r->dout = nullptr;
-        R = std::max(R, r->cap_train_R); S2 = std::max(S2, r->cap_train_S2);
-        TN_CUDA(cudaMalloc((void **)&r->sbins_f, 4 * R * (S2 + 1)));
-        TN_CUDA(cudaMalloc((void **)&r->enc, 4 * R * 27));
-        TN_CUDA(cudaMalloc((void **)&r->dout, 16 * R * S2));
-        TN_CUDA(cudaMalloc((void **)&r->g_dirbias, 512 * R));
-        r->cap_train_R = R; r->cap_train_S2 = S2;
-    }
-    if (!r->gw) TN_CUDA(cudaMalloc((void **)&r->gw, sizeof(float) * GW_TOTAL));
-    if (r->gshadow_V != V) {
-        cudaFree(r->gshadow); r->gshadow = nullptr;
-        TN_CUDA(cudaMalloc((void **)&r->gshadow, sizeof(float) * 64 * (size_t)V));
-        r->gshadow_V = V;
     }
     return TN_OK;
 }
@@ -1184,35 +1112,24 @@ static int train_backward_impl(tn_tracer *h, const TrainBufs &b, uint32_t R, uin
     int sms = 132;
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, h->device);
     const uint32_t V = r->V;
-    if (det) {
-        const int rc = ensure_det_ws(r, R, S2);
-        if (rc) return rc;
-    }
+    if (det) TN_TRY(ensure_det_ws(r, R, S2));
     const bool rays = d_grad_o != nullptr || d_grad_d != nullptr || d_grad_xyz != nullptr;
     const size_t rows = (size_t)R * S2;
     if (rays) {
-        if (!det && rows > r->cap_ray_dx) {
-            cudaFree(r->ray_dx); r->ray_dx = nullptr; r->cap_ray_dx = 0;
-            TN_CUDA(cudaMalloc((void **)&r->ray_dx, sizeof(float) * 64 * rows));
-            r->cap_ray_dx = rows;
-        }
-        if (rows > r->cap_ray_gx) {
-            cudaFree(r->ray_gx); r->ray_gx = nullptr; r->cap_ray_gx = 0;
-            TN_CUDA(cudaMalloc((void **)&r->ray_gx, sizeof(float4) * rows));
-            r->cap_ray_gx = rows;
-        }
+        if (!det) TN_TRY(r->ray_dx.grow(64 * rows));
+        TN_TRY(r->ray_gx.grow(rows));
     }
-    TN_CUDA(cudaMemsetAsync(r->gw, 0, sizeof(float) * GW_TOTAL, s));
+    TN_CUDA(cudaMemsetAsync(r->gw.p, 0, sizeof(float) * GW_TOTAL, s));
     if (!det) {  // (deterministic mode writes every element of these)
-        TN_CUDA(cudaMemsetAsync(r->gshadow, 0, sizeof(float) * 64 * (size_t)V, s));
-        TN_CUDA(cudaMemsetAsync(r->g_dirbias, 0, 512 * (size_t)R, s));
+        TN_CUDA(cudaMemsetAsync(r->gshadow.p, 0, sizeof(float) * 64 * (size_t)V, s));
+        TN_CUDA(cudaMemsetAsync(r->g_dirbias.p, 0, 512 * (size_t)R, s));
         // tile counter of the backward kernel: word 3 of the tracer's own 16-byte block (scratch even when `b` is a saved state)
-        TN_CUDA(cudaMemsetAsync(r->n_active + 3, 0, 4, s));
+        TN_CUDA(cudaMemsetAsync(r->n_active.p + 3, 0, 4, s));
     }
     CompositeBwdParams cb{};
     cb.S2 = S2; cb.use_gradient_scaling = use_gradient_scaling ? 1u : 0u; cb.n_active = b.n_active; cb.ray_list = b.ray_list;
     cb.ebins_f = b.ebins_f; cb.sbins_f = b.sbins_f; cb.out_f = b.out_f; cb.grad_rgb = d_grad_rgb; cb.grad_acc = d_grad_acc;
-    cb.bg0 = bg[0]; cb.bg1 = bg[1]; cb.bg2 = bg[2]; cb.dout = r->dout; cb.sums = det ? (float *)r->det_sums : r->gw + GW_SUMS;
+    cb.bg0 = bg[0]; cb.bg1 = bg[1]; cb.bg2 = bg[2]; cb.dout = r->dout.p; cb.sums = det ? (float *)r->det_sums.p : r->gw.p + GW_SUMS;
     cb.grad_ed = d_grad_ed; cb.dbounds = b.n_active + 4;
     const size_t smem_cb = SAMPLE_WARPS * sizeof(float) * 4 * ((size_t)S2 + 2);
     auto k_cbwd = d_grad_ed != nullptr ? (det ? k_composite_bwd<true, true> : k_composite_bwd<false, true>)
@@ -1223,9 +1140,9 @@ static int train_backward_impl(tn_tracer *h, const TrainBufs &b, uint32_t R, uin
     k_cbwd<<<gridR, SAMPLE_WARPS * 32, smem_cb, s>>>(cb);
     if (r->profile) cudaEventRecord(r->evb[1], s);
     MlpBwdParams bp{};
-    bp.n_active = b.n_active; bp.S = S2; bp.vi = b.vi_f; bp.bary = b.bary_f; bp.fshadow = r->fshadow; bp.wimg = r->wimg_bwd;
-    bp.bias = r->bias; bp.head = r->head; bp.dirbias = b.dirbias; bp.dout = r->dout; bp.gshadow = r->gshadow;
-    bp.gw = r->gw; bp.g_dirbias = r->g_dirbias; bp.tile_ctr = r->n_active + 3;
+    bp.n_active = b.n_active; bp.S = S2; bp.vi = b.vi_f; bp.bary = b.bary_f; bp.fshadow = r->fshadow.p; bp.wimg = r->wimg_bwd.p;
+    bp.bias = r->bias.p; bp.head = r->head.p; bp.dirbias = b.dirbias; bp.dout = r->dout.p; bp.gshadow = r->gshadow.p;
+    bp.gw = r->gw.p; bp.g_dirbias = r->g_dirbias.p; bp.tile_ctr = r->n_active.p + 3;
     const uint64_t tiles = ((uint64_t)R * S2 + BWD_TILE - 1) / BWD_TILE;
     if (!det) {
         const uint32_t grid = r->bwd_grid ? r->bwd_grid : (uint32_t)std::min<uint64_t>(tiles, (uint64_t)sms);
@@ -1235,43 +1152,42 @@ static int train_backward_impl(tn_tracer *h, const TrainBufs &b, uint32_t R, uin
         } else {  // the same backward, storing the dX rows for k_ray_grads as well
             MlpBwdDxParams xp{};
             static_cast<MlpBwdParams &>(xp) = bp;
-            xp.dx = r->ray_dx;
+            xp.dx = r->ray_dx.p;
             TN_CUDA(cudaFuncSetAttribute(k_mlp_bwd<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)BWD_SMEM_BYTES));
             k_mlp_bwd<false, true><<<grid, BWD_THREADS, BWD_SMEM_BYTES, s>>>(xp);
         }
         if (r->profile) cudaEventRecord(r->evb[2], s);
-        k_dirbias_grads<false><<<(R + DBG_SLOTS - 1) / DBG_SLOTS, 256, 0, s>>>(b.n_active, r->g_dirbias, b.enc, r->gw, nullptr);
+        k_dirbias_grads<false><<<(R + DBG_SLOTS - 1) / DBG_SLOTS, 256, 0, s>>>(b.n_active, r->g_dirbias.p, b.enc, r->gw.p, nullptr);
     } else {
         // the same stages with every reduction in a fixed order (header of tn_mlp_bwd.cuh); the grid only decides which CTA runs
         // which partition, never what is summed in which order
         MlpBwdDetParams dp{};
         static_cast<MlpBwdParams &>(dp) = bp;
-        dp.part = r->det_part; dp.gdb_part = r->det_gdb; dp.dx = r->det_dx;
+        dp.part = r->det_part.p; dp.gdb_part = r->det_gdb.p; dp.dx = r->det_dx.p;
         TN_CUDA(cudaFuncSetAttribute(k_mlp_bwd<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)BWD_DET_SMEM_BYTES));
         const uint32_t grid = r->bwd_grid ? r->bwd_grid : std::min<uint32_t>(BWD_PARTS, (uint32_t)sms);
         k_mlp_bwd<true><<<grid, BWD_THREADS, BWD_DET_SMEM_BYTES, s>>>(dp);
         if (r->profile) cudaEventRecord(r->evb[2], s);
-        k_det_reduce_parts<<<(BWD_PART_STRIDE + 255) / 256, 256, 0, s>>>(b.n_active, S2, r->det_part, r->gw);
-        k_det_sum_slots<<<1, 256, 0, s>>>(b.n_active, r->det_sums, r->gw + GW_SUMS);
-        k_det_dirbias<<<R, 128, 0, s>>>(b.n_active, S2, r->det_gdb, r->g_dirbias);
-        k_dirbias_grads<true><<<(R + DBG_SLOTS - 1) / DBG_SLOTS, 256, 0, s>>>(b.n_active, r->g_dirbias, b.enc, r->gw, r->det_dbg);
-        k_det_reduce_dbg<<<(DBG_PART + 255) / 256, 256, 0, s>>>(b.n_active, r->det_dbg, r->gw);
+        k_det_reduce_parts<<<(BWD_PART_STRIDE + 255) / 256, 256, 0, s>>>(b.n_active, S2, r->det_part.p, r->gw.p);
+        k_det_sum_slots<<<1, 256, 0, s>>>(b.n_active, r->det_sums.p, r->gw.p + GW_SUMS);
+        k_det_dirbias<<<R, 128, 0, s>>>(b.n_active, S2, r->det_gdb.p, r->g_dirbias.p);
+        k_dirbias_grads<true><<<(R + DBG_SLOTS - 1) / DBG_SLOTS, 256, 0, s>>>(b.n_active, r->g_dirbias.p, b.enc, r->gw.p, r->det_dbg.p);
+        k_det_reduce_dbg<<<(DBG_PART + 255) / 256, 256, 0, s>>>(b.n_active, r->det_dbg.p, r->gw.p);
         // field gradient: stable sort of (vertex, row * 4 + k) by vertex, then per-vertex sums in row order
         const uint32_t n = (uint32_t)(4 * (uint64_t)R * S2);
         const int end_bit = 32 - __builtin_clz(V | 1u);  // keys are <= V
-        uint32_t *k0 = r->det_keys, *k1 = r->det_keys + n, *v0 = r->det_vals, *v1 = r->det_vals + n;
+        uint32_t *k0 = r->det_keys.p, *k1 = r->det_keys.p + n, *v0 = r->det_vals.p, *v1 = r->det_vals.p + n;
         size_t bytes = 0;
         TN_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, bytes, k0, k1, v0, v1, (int)n, 0, end_bit, s));
-        const int rc = ensure_cub_tmp(r, bytes);
-        if (rc) return rc;
+        TN_TRY(r->cub_tmp.grow(bytes));
         k_det_field_keys<<<(n + 255) / 256, 256, 0, s>>>(b.n_active, S2, n, V, b.vi_f, k0, v0);
-        TN_CUDA(cub::DeviceRadixSort::SortPairs(r->cub_tmp, bytes, k0, k1, v0, v1, (int)n, 0, end_bit, s));
-        k_det_field_grad<<<(uint32_t)(((uint64_t)V * 32 + 255) / 256), 256, 0, s>>>(V, n, k1, v1, b.bary_f, r->det_dx, r->gshadow);
+        TN_CUDA(cub::DeviceRadixSort::SortPairs(r->cub_tmp.p, bytes, k0, k1, v0, v1, (int)n, 0, end_bit, s));
+        k_det_field_grad<<<(uint32_t)(((uint64_t)V * 32 + 255) / 256), 256, 0, s>>>(V, n, k1, v1, b.bary_f, r->det_dx.p, r->gshadow.p);
         h->launches += 9;
     }
     const uint32_t *sorted_keys = nullptr, *sorted_vals = nullptr;  // deterministic mode: the field gradient's sorted pairs
     const uint32_t npairs = (uint32_t)(4 * (uint64_t)R * S2);
-    if (det) { sorted_keys = r->det_keys + npairs; sorted_vals = r->det_vals + npairs; }
+    if (det) { sorted_keys = r->det_keys.p + npairs; sorted_vals = r->det_vals.p + npairs; }
     GradOut go{};
     for (int i = 0; i < 12; ++i) {
         if (!d_grad_params12[i]) return fail(TN_ERR_ARG, "tn_render_train_backward: null parameter gradient pointer");
@@ -1280,22 +1196,22 @@ static int train_backward_impl(tn_tracer *h, const TrainBufs &b, uint32_t R, uin
     if (rays) {  // after the direction-bias gradient is complete
         RayGradsLaunch rl{};
         rl.n_active = b.n_active; rl.ray_list = b.ray_list; rl.S = S2; rl.R = R; rl.ebins = b.ebins_f; rl.vi = b.vi_f;
-        rl.dx = det ? r->det_dx : r->ray_dx; rl.fshadow = r->fshadow; rl.xyz = h->mesh.xyz; rl.enc = b.enc; rl.g_dirbias = r->g_dirbias;
-        rl.w4dir = r->w4dir; rl.gx = r->ray_gx; rl.grad_o = d_grad_o; rl.grad_d = d_grad_d;
+        rl.dx = det ? r->det_dx.p : r->ray_dx.p; rl.fshadow = r->fshadow.p; rl.xyz = h->mesh.xyz; rl.enc = b.enc; rl.g_dirbias = r->g_dirbias.p;
+        rl.w4dir = r->w4dir.p; rl.gx = r->ray_gx.p; rl.grad_o = d_grad_o; rl.grad_d = d_grad_d;
         int rc = launch_ray_grads(rl, s);
         if (rc) return rc;
         h->launches += 1;
         if (d_grad_xyz != nullptr) {  // after the per-sample dL/dx is complete
             VertexGradsLaunch vl{};
-            vl.n_active = b.n_active; vl.S = S2; vl.R = R; vl.V = h->mesh.V; vl.vi = b.vi_f; vl.bary = b.bary_f; vl.gx = r->ray_gx;
+            vl.n_active = b.n_active; vl.S = S2; vl.R = R; vl.V = h->mesh.V; vl.vi = b.vi_f; vl.bary = b.bary_f; vl.gx = r->ray_gx.p;
             vl.keys = sorted_keys; vl.vals = sorted_vals; vl.n = npairs; vl.grad_xyz = d_grad_xyz;
             rc = launch_vertex_grads(vl, s);
             if (rc) return rc;
             h->launches += 1;
         }
     }
-    k_scatter_grads<<<(128 * 155 + 255) / 256, 256, 0, s>>>(r->gw, go);
-    k_transpose_v64<<<(V + 31) / 32, dim3(32, 8), 0, s>>>(r->gshadow, d_grad_field, V);
+    k_scatter_grads<<<(128 * 155 + 255) / 256, 256, 0, s>>>(r->gw.p, go);
+    k_transpose_v64<<<(V + 31) / 32, dim3(32, 8), 0, s>>>(r->gshadow.p, d_grad_field, V);
     if (r->profile) cudaEventRecord(r->evb[3], s);
     h->launches += 5;
     TN_CUDA(cudaGetLastError());
@@ -1367,7 +1283,7 @@ extern "C" int tn_render_train_backward_saved(tn_tracer *h, const void *d_saved,
                                               void *stream) {
     if (!h || !d_saved || !d_grad_rgb || !d_grad_field || !d_grad_params12) return fail(TN_ERR_ARG, "null argument");
     RenderState *r = h->render;
-    if (!r || !r->n_active) return fail(TN_ERR_STATE, "tn_render_train_backward_saved: no training forward on this tracer");
+    if (!r || !r->n_active.p) return fail(TN_ERR_STATE, "tn_render_train_backward_saved: no training forward on this tracer");
     DeviceGuard g(h->device);
     cudaStream_t s = (cudaStream_t)stream;
     // the launch shapes depend on the call's R and S2: read the header back (waits until the stream has reached this backward)
@@ -1453,8 +1369,8 @@ extern "C" int tn_render_get_backward_timings(tn_tracer *h, float *ms3) {
 extern "C" int tn_render_debug_buffers(tn_tracer *h, void **ptrs16) {
     if (!h || !h->render) return fail(TN_ERR_STATE, "no render state");
     RenderState *r = h->render;
-    void *v[16] = {r->num, r->dist, r->n_active, r->ray_list, r->ebins_c, r->sbins_c, r->vi_c, r->bary_c,
-                   r->dens_c, r->ebins_f, r->vi_f, r->bary_f, r->out_f, r->dirbias, r->fshadow, r->wimg};
+    void *v[16] = {r->num.p, r->dist.p, r->n_active.p, r->ray_list.p, r->ebins_c.p, r->sbins_c.p, r->vi_c.p, r->bary_c.p,
+                   r->dens_c.p, r->ebins_f.p, r->vi_f.p, r->bary_f.p, r->out_f.p, r->dirbias.p, r->fshadow.p, r->wimg.p};
     for (int i = 0; i < 16; ++i) ptrs16[i] = v[i];
     return TN_OK;
 }
@@ -1462,15 +1378,15 @@ extern "C" int tn_render_debug_buffers(tn_tracer *h, void **ptrs16) {
 // test hook: device pointer of the per-sample density gradient of the last tn_render call with normals, float4 (x, y, z, 0) per sample in
 // the slot order of the pass that gives the colours (vi_f / bary_f, or vi_c / bary_c in single-pass configurations)
 extern "C" int tn_render_debug_normals_grad(tn_tracer *h, void **ptr) {
-    if (!h || !h->render || !h->render->grad_n) return fail(TN_ERR_STATE, "no normals render");
-    *ptr = h->render->grad_n;
+    if (!h || !h->render || !h->render->grad_n.p) return fail(TN_ERR_STATE, "no normals render");
+    *ptr = h->render->grad_n.p;
     return TN_OK;
 }
 
 // test hook: device pointer of dL/dx per fine sample of the last tn_render_train_backward_saved call with ray or vertex gradients, float4 (x, y, z, 0) per sample
 // in the slot order of that call's forward (0 for unmatched samples and flat tetrahedra)
 extern "C" int tn_render_debug_ray_grads(tn_tracer *h, void **ptr) {
-    if (!h || !h->render || !h->render->ray_gx) return fail(TN_ERR_STATE, "no backward with ray gradients");
-    *ptr = h->render->ray_gx;
+    if (!h || !h->render || !h->render->ray_gx.p) return fail(TN_ERR_STATE, "no backward with ray gradients");
+    *ptr = h->render->ray_gx.p;
     return TN_OK;
 }

@@ -28,38 +28,23 @@ struct SurfaceState {
     uint32_t N = 0, F = 0;
     uint64_t gen = 0, mesh_gen = 0;
     // workspace, grown on demand and kept
-    struct Buf {
-        void *p = nullptr;
-        size_t cap = 0;
-    };
-    Buf small;                   // u32[8]: tile counters of the four k_mlp launches | V | E
-    Buf vvi, vbary, vsig;        // [V] (v,v,v,v), [V,3] zeros, [V] vertex densities
-    Buf tcnt, toff;              // u64[T+1] (edges << 32 | triangles) per tetrahedron, its exclusive scan
-    Buf keys, skeys;             // u64[crossing-edge slots]: keys a * V + b as emitted, sorted; `keys` then holds the unique ones
-    Buf evi, ebary, eout;        // [64 E] rows of a refinement round (the colour pass reuses the first E rows; eout as float4 [E])
-    Buf br;                      // float4[E]: (s_lo, sigma_lo, sigma_hi, s) bracket of each edge, final parameter
-    Buf pos, nrm, dirbias;       // [E,3], [E,3], [E,128]
-    Buf faces, ftet, fnrm;       // u32[F,3], u32[F], float[F,3]
-    Buf nk0, nk1, nv0, nv1;      // u32[3F] (vertex, face) pairs and their sorted copies
-    Buf cub;
+    DevArray<uint32_t> small;                  // [8]: tile counters of the four k_mlp launches | V | E
+    DevArray<uint4> vvi;                       // [V] (v,v,v,v)
+    DevArray<float> vbary, vsig;               // [V,3] zeros, [V] vertex densities
+    DevArray<unsigned long long> tcnt, toff;   // [T+1] (edges << 32 | triangles) per tetrahedron, its exclusive scan
+    DevArray<unsigned long long> keys, skeys;  // [crossing-edge slots]: keys a * V + b as emitted, sorted; `keys` then holds the unique ones
+    DevArray<uint4> evi;                       // [64 E] rows of a refinement round (the colour pass reuses the first E rows)
+    DevArray<float> ebary, eout;               // [64 E,3], [64 E] (the colour pass: eout as float4 [E])
+    DevArray<float4> br;                       // [E]: (s_lo, sigma_lo, sigma_hi, s) bracket of each edge, final parameter
+    DevArray<float> pos, nrm, dirbias;         // [E,3], [E,3], [E,128]
+    DevArray<uint32_t> faces, ftet;            // [F,3], [F]
+    DevArray<float> fnrm;                      // [F,3]
+    DevArray<uint32_t> nk0, nk1, nv0, nv1;     // [3F] (vertex, face) pairs and their sorted copies
+    DevArray<uint8_t> cub;
 };
 
-static int grow(SurfaceState::Buf &b, size_t bytes) {
-    if (bytes <= b.cap) return TN_OK;
-    cudaFree(b.p); b.p = nullptr; b.cap = 0;
-    TN_CUDA(cudaMalloc(&b.p, std::max<size_t>(bytes, 256)));
-    b.cap = std::max<size_t>(bytes, 256);
-    return TN_OK;
-}
-
 void free_surface(tn_tracer *h) {
-    SurfaceState *s = h->surface;
-    if (!s) return;
-    for (SurfaceState::Buf *b : {&s->small, &s->vvi, &s->vbary, &s->vsig, &s->tcnt, &s->toff, &s->keys, &s->skeys, &s->evi, &s->ebary,
-                                 &s->eout, &s->br, &s->pos, &s->nrm, &s->dirbias, &s->faces, &s->ftet, &s->fnrm, &s->nk0, &s->nk1,
-                                 &s->nv0, &s->nv1, &s->cub})
-        cudaFree(b->p);
-    delete s;
+    delete h->surface;
     h->surface = nullptr;
 }
 
@@ -317,7 +302,7 @@ int bits_for(uint64_t x) { int b = 1; while (b < 64 && (x >> b) != 0) ++b; retur
 
 extern "C" int tn_surface_extract(tn_tracer *h, float level, uint32_t *n_vertices, uint32_t *n_faces, void *stream) {
     if (!h || !n_vertices || !n_faces) return fail(TN_ERR_ARG, "null argument");
-    if (!h->mesh.nodes) return fail(TN_ERR_STATE, "tn_surface_extract: no tetrahedra loaded");
+    if (!h->mesh.nodes.p) return fail(TN_ERR_STATE, "tn_surface_extract: no tetrahedra loaded");
     RenderInputs in{};
     if (render_inputs(h, &in) != TN_OK) return fail(TN_ERR_STATE, "tn_surface_extract: call tn_render_set_field and tn_render_set_weights first");
     if (!(level > 0.f) || !std::isfinite(level)) return fail(TN_ERR_ARG, "tn_surface_extract: the level must be finite and greater than 0");
@@ -330,25 +315,23 @@ extern "C" int tn_surface_extract(tn_tracer *h, float level, uint32_t *n_vertice
     SurfaceState &S = *h->surface;
     S.valid = false;
     *n_vertices = *n_faces = 0;
-    int rc;
-#define GROW(buf, bytes) do { if ((rc = grow(S.buf, (bytes))) != TN_OK) return rc; } while (0)
-    GROW(small, 8 * sizeof(uint32_t));
-    uint32_t *small = (uint32_t *)S.small.p, *d_V = small + 4, *d_E = small + 5;
+    TN_TRY(S.small.grow(8));
+    uint32_t *small = S.small.p, *d_V = small + 4, *d_E = small + 5;
     TN_CUDA(cudaMemsetAsync(small, 0, 8 * sizeof(uint32_t), s));
     // ---- vertex densities ----
-    GROW(vvi, 16 * (size_t)V); GROW(vbary, 12 * (size_t)V); GROW(vsig, 4 * (size_t)V);
-    const float *vsig = (const float *)S.vsig.p;
+    TN_TRY(S.vvi.grow(V)); TN_TRY(S.vbary.grow(3 * (size_t)V)); TN_TRY(S.vsig.grow(V));
+    const float *vsig = S.vsig.p;
     TN_CUDA(cudaMemsetAsync(S.vbary.p, 0, 12 * (size_t)V, s));
-    k_vertex_rows<<<blocks(V, 256), 256, 0, s>>>(V, (uint4 *)S.vvi.p, d_V);
+    k_vertex_rows<<<blocks(V, 256), 256, 0, s>>>(V, S.vvi.p, d_V);
     h->launches += 1;
-    if ((rc = run_mlp<false>(h, in, d_V, V, 1, (const uint4 *)S.vvi.p, (const float *)S.vbary.p, nullptr, (float *)S.vsig.p, small + 0, s))) return rc;
+    TN_TRY(run_mlp<false>(h, in, d_V, V, 1, S.vvi.p, S.vbary.p, nullptr, S.vsig.p, small + 0, s));
     // ---- cases, crossing edges, faces ----
-    GROW(tcnt, 8 * ((size_t)T + 1)); GROW(toff, 8 * ((size_t)T + 1));
-    unsigned long long *tcnt = (unsigned long long *)S.tcnt.p, *toff = (unsigned long long *)S.toff.p;
+    TN_TRY(S.tcnt.grow((size_t)T + 1)); TN_TRY(S.toff.grow((size_t)T + 1));
+    unsigned long long *tcnt = S.tcnt.p, *toff = S.toff.p;
     k_tet_case<<<blocks((uint64_t)T + 1, 256), 256, 0, s>>>(T, h->mesh.cells, vsig, level, tcnt);
     size_t bytes = 0;
     TN_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, bytes, tcnt, toff, (int64_t)T + 1, s));
-    GROW(cub, bytes);
+    TN_TRY(S.cub.grow(bytes));
     TN_CUDA(cub::DeviceScan::ExclusiveSum(S.cub.p, bytes, tcnt, toff, (int64_t)T + 1, s));
     h->launches += 2;
     unsigned long long total = 0;
@@ -361,15 +344,15 @@ extern "C" int tn_surface_extract(tn_tracer *h, float level, uint32_t *n_vertice
         return TN_OK;
     }
     if (nslots >= (1ull << 31)) return fail(TN_ERR_ARG, "tn_surface_extract: too many crossing tetrahedra");
-    GROW(keys, 8 * nslots); GROW(skeys, 8 * nslots);
-    unsigned long long *keys = (unsigned long long *)S.keys.p, *skeys = (unsigned long long *)S.skeys.p;
+    TN_TRY(S.keys.grow(nslots)); TN_TRY(S.skeys.grow(nslots));
+    unsigned long long *keys = S.keys.p, *skeys = S.skeys.p;
     k_tet_edges<<<blocks(T, 256), 256, 0, s>>>(T, V, h->mesh.cells, vsig, level, toff, keys);
     const int end_bit = bits_for((uint64_t)V * V);
     TN_CUDA(cub::DeviceRadixSort::SortKeys(nullptr, bytes, keys, skeys, (int64_t)nslots, 0, end_bit, s));
-    GROW(cub, bytes);
+    TN_TRY(S.cub.grow(bytes));
     TN_CUDA(cub::DeviceRadixSort::SortKeys(S.cub.p, bytes, keys, skeys, (int64_t)nslots, 0, end_bit, s));
     TN_CUDA(cub::DeviceSelect::Unique(nullptr, bytes, skeys, keys, d_E, (int64_t)nslots, s));
-    GROW(cub, bytes);
+    TN_TRY(S.cub.grow(bytes));
     TN_CUDA(cub::DeviceSelect::Unique(S.cub.p, bytes, skeys, keys, d_E, (int64_t)nslots, s));
     h->launches += 3;
     uint32_t E = 0;
@@ -377,38 +360,36 @@ extern "C" int tn_surface_extract(tn_tracer *h, float level, uint32_t *n_vertice
     TN_CUDA(cudaStreamSynchronize(s));
     if ((uint64_t)E * EDGE_SAMPLES >= (1ull << 32)) return fail(TN_ERR_ARG, "tn_surface_extract: more than 2^26 crossing edges");
     const unsigned long long *ukeys = keys;
-    GROW(faces, 12 * F); GROW(ftet, 4 * F);
-    k_faces<<<blocks(T, 256), 256, 0, s>>>(T, V, E, h->mesh.cells, h->mesh.xyz, vsig, level, toff, ukeys, (uint32_t *)S.faces.p, (uint32_t *)S.ftet.p);
+    TN_TRY(S.faces.grow(3 * F)); TN_TRY(S.ftet.grow(F));
+    k_faces<<<blocks(T, 256), 256, 0, s>>>(T, V, E, h->mesh.cells, h->mesh.xyz, vsig, level, toff, ukeys, S.faces.p, S.ftet.p);
     h->launches += 1;
     // ---- refinement: two rounds of 64 samples per edge ----
     const uint64_t rows = (uint64_t)E * EDGE_SAMPLES;
-    GROW(evi, 16 * rows); GROW(ebary, 12 * rows); GROW(eout, 4 * rows); GROW(br, 16 * (size_t)E); GROW(pos, 12 * (size_t)E);
-    uint4 *evi = (uint4 *)S.evi.p;
-    float *ebary = (float *)S.ebary.p, *eout = (float *)S.eout.p, *pos = (float *)S.pos.p;
-    float4 *br = (float4 *)S.br.p;
+    TN_TRY(S.evi.grow(rows)); TN_TRY(S.ebary.grow(3 * rows)); TN_TRY(S.eout.grow(rows)); TN_TRY(S.br.grow(E)); TN_TRY(S.pos.grow(3 * (size_t)E));
+    uint4 *evi = S.evi.p;
+    float *ebary = S.ebary.p, *eout = S.eout.p, *pos = S.pos.p;
+    float4 *br = S.br.p;
     for (int round = 0; round < 2; ++round) {
         const float step = round == 0 ? 1.f / 64.f : 1.f / 4096.f;
         k_edge_rows<<<blocks(rows, 256), 256, 0, s>>>(E, V, ukeys, round == 0 ? nullptr : br, step, evi, ebary);
-        if ((rc = run_mlp<false>(h, in, d_E, rows, EDGE_SAMPLES, evi, ebary, nullptr, eout, small + 1 + round, s))) return rc;
+        TN_TRY(run_mlp<false>(h, in, d_E, rows, EDGE_SAMPLES, evi, ebary, nullptr, eout, small + 1 + round, s));
         k_bracket<<<blocks((uint64_t)E * 32, 256), 256, 0, s>>>(E, V, ukeys, vsig, level, eout, step, round, br, h->mesh.xyz, pos, evi, ebary);
         h->launches += 2;
     }
     // ---- normals (deterministic segmented sum) and the colour pass's direction bias ----
     const uint64_t n3 = 3 * F;
-    GROW(fnrm, 12 * F); GROW(nk0, 4 * n3); GROW(nk1, 4 * n3); GROW(nv0, 4 * n3); GROW(nv1, 4 * n3); GROW(nrm, 12 * (size_t)E);
-    GROW(dirbias, 512 * (size_t)E);
-    uint32_t *nk0 = (uint32_t *)S.nk0.p, *nk1 = (uint32_t *)S.nk1.p, *nv0 = (uint32_t *)S.nv0.p, *nv1 = (uint32_t *)S.nv1.p;
-    k_face_normals<<<blocks(F, 256), 256, 0, s>>>((uint32_t)F, (const uint32_t *)S.faces.p, pos, (float *)S.fnrm.p, nk0, nv0);
+    TN_TRY(S.fnrm.grow(3 * F)); TN_TRY(S.nk0.grow(n3)); TN_TRY(S.nk1.grow(n3)); TN_TRY(S.nv0.grow(n3)); TN_TRY(S.nv1.grow(n3));
+    TN_TRY(S.nrm.grow(3 * (size_t)E)); TN_TRY(S.dirbias.grow(128 * (size_t)E));
+    uint32_t *nk0 = S.nk0.p, *nk1 = S.nk1.p, *nv0 = S.nv0.p, *nv1 = S.nv1.p;
+    k_face_normals<<<blocks(F, 256), 256, 0, s>>>((uint32_t)F, S.faces.p, pos, S.fnrm.p, nk0, nv0);
     const int vbits = bits_for(E);
     TN_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, bytes, nk0, nk1, nv0, nv1, (int64_t)n3, 0, vbits, s));
-    GROW(cub, bytes);
+    TN_TRY(S.cub.grow(bytes));
     TN_CUDA(cub::DeviceRadixSort::SortPairs(S.cub.p, bytes, nk0, nk1, nv0, nv1, (int64_t)n3, 0, vbits, s));
-    k_vertex_normals<<<blocks((uint64_t)E * 32, 256), 256, 0, s>>>(E, (uint32_t)n3, nk1, nv1, (const float *)S.fnrm.p, in.w4dir, (float *)S.nrm.p,
-                                                                  (float *)S.dirbias.p);
+    k_vertex_normals<<<blocks((uint64_t)E * 32, 256), 256, 0, s>>>(E, (uint32_t)n3, nk1, nv1, S.fnrm.p, in.w4dir, S.nrm.p, S.dirbias.p);
     h->launches += 3;
     // ---- colours: the colour head at the vertex's features, seen along -n ----
-    if ((rc = run_mlp<true>(h, in, d_E, E, 1, evi, ebary, (const float *)S.dirbias.p, eout, small + 3, s))) return rc;
-#undef GROW
+    TN_TRY(run_mlp<true>(h, in, d_E, E, 1, evi, ebary, S.dirbias.p, eout, small + 3, s));
     TN_CUDA(cudaGetLastError());
     S.N = E; S.F = (uint32_t)F; S.gen = in.gen; S.mesh_gen = h->mesh_gen; S.valid = true;
     *n_vertices = E; *n_faces = (uint32_t)F;
@@ -427,8 +408,8 @@ extern "C" int tn_surface_copy(tn_tracer *h, float *d_vertices, float *d_normals
     DeviceGuard g(h->device);
     cudaStream_t s = (cudaStream_t)stream;
     if (S->N > 0 && (d_vertices || d_normals || d_colors)) {
-        k_surface_copy<<<blocks(3 * (uint64_t)S->N, 256), 256, 0, s>>>(S->N, (const float *)S->pos.p, (const float *)S->nrm.p,
-                                                                        (const float4 *)S->eout.p, d_vertices, d_normals, d_colors);
+        k_surface_copy<<<blocks(3 * (uint64_t)S->N, 256), 256, 0, s>>>(S->N, S->pos.p, S->nrm.p, reinterpret_cast<const float4 *>(S->eout.p),
+                                                                        d_vertices, d_normals, d_colors);
         h->launches += 1;
     }
     if (S->F > 0 && d_faces) TN_CUDA(cudaMemcpyAsync(d_faces, S->faces.p, 12 * (size_t)S->F, cudaMemcpyDeviceToDevice, s));

@@ -298,16 +298,16 @@ int launch_prefetch(tn_tracer *h, const void *const *extra, const size_t *extra_
     int n = 0;
     auto add = [&](const void *p, size_t b) { if (p && b && n < 8 && ((uintptr_t)p & 15) == 0) { a.ptr[n] = p; a.bytes[n] = b; ++n; } };
     if (m.walkable) {  // the walk touches one 128-byte record per crossed tetrahedron; the big BVH is only the rare exact path's
-        add(m.walk, sizeof(WalkRec) * (size_t)m.T);
-        add(m.hull_leaves, sizeof(LeafRec) * (size_t)m.H);
-        add(m.hull_nodes, sizeof(float4) * 2 * (size_t)(m.hull_lv.offset[m.hull_lv.nlevels - 1] + TN_FAN));
+        add(m.walk.p, sizeof(WalkRec) * (size_t)m.T);
+        add(m.hull_leaves.p, sizeof(LeafRec) * (size_t)m.H);
+        add(m.hull_nodes.p, sizeof(float4) * 2 * (size_t)(m.hull_lv.offset[m.hull_lv.nlevels - 1] + TN_FAN));
     } else {
         const uint32_t total_nodes = m.lv.offset[m.lv.nlevels - 1] + TN_FAN;
-        add(m.nodes, sizeof(float4) * 2 * (size_t)total_nodes);
-        add(m.leaves, sizeof(LeafRec) * (size_t)m.T);
+        add(m.nodes.p, sizeof(float4) * 2 * (size_t)total_nodes);
+        add(m.leaves.p, sizeof(LeafRec) * (size_t)m.T);
     }
-    add(m.tri, sizeof(uint4) * (size_t)m.F);
-    add(m.tt, sizeof(uint2) * (size_t)m.F);
+    add(m.tri.p, sizeof(uint4) * (size_t)m.F);
+    add(m.tt.p, sizeof(uint2) * (size_t)m.F);
     add(m.xyz, sizeof(float) * 3 * (size_t)m.V);
     for (int i = 0; i < nextra; ++i) add(extra[i], extra_bytes[i]);
     a.n = n;
@@ -324,13 +324,13 @@ static int launch_trace(tn_tracer *h, int mode, const float *o, const float *d, 
     if (!h) return fail(TN_ERR_ARG, "null tracer");
     if (M == 0 || (M & (M - 1)) != 0) return fail(TN_ERR_ARG, "max_ray_triangles must be a power of 2.");  // py_binding.cpp:44-47
     if (M < 2 || M > 2048) return fail(TN_ERR_ARG, "max_ray_triangles must be in [2, 2048]");
-    if (!h->mesh.nodes) return fail(TN_ERR_STATE, "trace_rays: no tetrahedra loaded (call load_tetrahedra first)");
+    if (!h->mesh.nodes.p) return fail(TN_ERR_STATE, "trace_rays: no tetrahedra loaded (call load_tetrahedra first)");
     if (R == 0) return TN_OK;
     DeviceGuard g(h->device);
     TraceParams p{};
     p.o = o; p.d = d; p.R = R; p.M = M; p.num = num; p.cells = cells; p.bary = bary; p.dist = dist; p.verts = verts;
-    p.nodes = h->mesh.nodes; p.leaves = h->mesh.leaves; p.tri = (const uint4 *)h->mesh.tri; p.tt = (const uint2 *)h->mesh.tt;
-    p.xyz = h->mesh.xyz; p.lv = h->mesh.lv; p.absmax = h->mesh.absmax; p.dense = dense; p.flags = h->d_flags;
+    p.nodes = h->mesh.nodes.p; p.leaves = h->mesh.leaves.p; p.tri = h->mesh.tri.p; p.tt = h->mesh.tt.p;
+    p.xyz = h->mesh.xyz; p.lv = h->mesh.lv; p.absmax = h->mesh.absmax; p.dense = dense; p.flags = h->d_flags.p;
     auto kern = mode == 0 ? k_trace<0> : k_trace<1>;
     int sms = 132;
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, h->device);
@@ -357,25 +357,15 @@ static int launch_trace(tn_tracer *h, int mode, const float *o, const float *d, 
     if (mode == 0 && h->mesh.walkable && M >= 4 && (thread_walk || solo_walk || quad_walk)) {
         // fast path: adjacency walk (tn_walk.cu); rays it cannot certify are listed for the exact stage below
         const size_t need = (size_t)R * M;
-        if (h->walk_keys_cap < need) {
-            cudaFree(h->d_walk_keys);
-            h->d_walk_keys = nullptr; h->walk_keys_cap = 0;
-            TN_CUDA(cudaMalloc((void **)&h->d_walk_keys, sizeof(u64) * need));
-            h->walk_keys_cap = need;
-        }
-        if (h->ovf_cap < R) {
-            cudaFree(h->d_ovf_list);
-            h->d_ovf_list = nullptr; h->ovf_cap = 0;
-            TN_CUDA(cudaMalloc((void **)&h->d_ovf_list, sizeof(uint32_t) * (size_t)R));
-            h->ovf_cap = R;
-        }
-        uint32_t *list_count = reinterpret_cast<uint32_t *>(h->d_flags + 2);
+        TN_TRY(h->d_walk_keys.grow(need));
+        TN_TRY(h->d_ovf_list.grow(R));
+        uint32_t *list_count = reinterpret_cast<uint32_t *>(h->d_flags.p + 2);
         TN_CUDA(cudaMemsetAsync(list_count, 0, 2 * sizeof(uint32_t), s));
-        int rc = launch_walk(h, o, d, R, M, num, cells, bary, dist, verts, h->d_walk_keys, h->d_ovf_list, list_count, thread_walk ? 0 : (quad_walk ? 2 : 1), s);
+        int rc = launch_walk(h, o, d, R, M, num, cells, bary, dist, verts, h->d_walk_keys.p, h->d_ovf_list.p, list_count, thread_walk ? 0 : (quad_walk ? 2 : 1), s);
         if (rc) return rc;
         p.dense = 0;
         p.hcap = M + 128; p.scap = 4096; p.lcap = M > 512 ? M / 2 : 320;
-        p.ray_count = list_count; p.ray_list = h->d_ovf_list; p.keys_in = h->d_walk_keys;
+        p.ray_count = list_count; p.ray_list = h->d_ovf_list.p; p.keys_in = h->d_walk_keys.p;
         rc = launch((uint32_t)sms);
         if (rc) return rc;
         if (dense) return launch_tail_fill(h, R, M, num, cells, bary, dist, verts, s);
@@ -383,21 +373,16 @@ static int launch_trace(tn_tracer *h, int mode, const float *o, const float *d, 
     }
     // phase 1: min(M + 128, 512) keys per ray (7.75 KB of shared memory per ray at M = 512 -> 28 rays per SM); rays whose hits
     // or work list do not fit are deferred to phase 2 (never dropped)
-    if (h->ovf_cap < R) {
-        cudaFree(h->d_ovf_list);
-        h->d_ovf_list = nullptr; h->ovf_cap = 0;
-        TN_CUDA(cudaMalloc((void **)&h->d_ovf_list, sizeof(uint32_t) * (size_t)R));
-        h->ovf_cap = R;
-    }
-    uint32_t *ovf_count = reinterpret_cast<uint32_t *>(h->d_flags + 2);
+    TN_TRY(h->d_ovf_list.grow(R));
+    uint32_t *ovf_count = reinterpret_cast<uint32_t *>(h->d_flags.p + 2);
     TN_CUDA(cudaMemsetAsync(ovf_count, 0, sizeof(uint32_t), s));
-    p.hcap = M <= 256 ? M + 128 : M; p.scap = 640; p.lcap = 320; p.ovf_count = ovf_count; p.ovf_list = h->d_ovf_list;
+    p.hcap = M <= 256 ? M + 128 : M; p.scap = 640; p.lcap = 320; p.ovf_count = ovf_count; p.ovf_list = h->d_ovf_list.p;
     int rc = launch(want);
     if (rc) return rc;
     // phase 2: the deferred rays with the full streaming buffer (M + 128 keys) and a 4096-entry work list; exits at once
     // when there are none.  A work list overflow HERE is counted in d_flags[0] and reported by tn_synchronize.
     p.hcap = M + 128; p.scap = 4096; p.lcap = M > 512 ? M / 2 : 320;
-    p.ovf_count = nullptr; p.ovf_list = nullptr; p.ray_count = ovf_count; p.ray_list = h->d_ovf_list;
+    p.ovf_count = nullptr; p.ovf_list = nullptr; p.ray_count = ovf_count; p.ray_list = h->d_ovf_list.p;
     return launch((uint32_t)sms);
 }
 

@@ -434,7 +434,7 @@ int launch_walk(tn_tracer *h, const float *o, const float *d, uint32_t R, uint32
                 float *dist, uint32_t *verts, u64 *keys, uint32_t *list, uint32_t *list_count, int kind, cudaStream_t s) {
     WalkParams p{};
     p.o = o; p.d = d; p.R = R; p.M = M; p.num = num; p.cells = cells; p.bary = bary; p.dist = dist; p.verts = verts;
-    p.walk = h->mesh.walk; p.hull_nodes = h->mesh.hull_nodes; p.hull_leaves = h->mesh.hull_leaves; p.hull_tet = h->mesh.hull_tet;
+    p.walk = h->mesh.walk.p; p.hull_nodes = h->mesh.hull_nodes.p; p.hull_leaves = h->mesh.hull_leaves.p; p.hull_tet = h->mesh.hull_tet.p;
     p.hlv = h->mesh.hull_lv; p.absmax = h->mesh.absmax; p.keys = keys; p.list = list; p.list_count = list_count;
     if (kind == 1 || kind == 2) {  // 4 lanes per ray: kind 2 = 8 rays per warp, kind 1 = one ray per warp
         const bool spec = R <= h->walk_quad_spec_max_rays;  // speculative record loads, else prefetched

@@ -47,6 +47,7 @@ _lib.tn_set_walk_quad_range.argtypes = [_vp, _u32, _u32]
 _lib.tn_set_walk_quad_spec_max_rays.argtypes = [_vp, _u32]
 _lib.tn_launch_count.restype = C.c_uint64
 _lib.tn_launch_count.argtypes = [_vp]
+_lib.tn_debug_device_bytes.restype = C.c_uint64
 
 
 class _Cfg(C.Structure):  # tn_render_config
