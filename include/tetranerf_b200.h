@@ -189,7 +189,17 @@ int tn_render_train_backward(tn_tracer *h, const float *d_grad_rgb, const float 
  *     half of the reference's add_barycentrics_grad.  Default mode: float reductions; deterministic mode: per-vertex sums in a fixed
  *     order, bitwise reproducible.  DESIGN.md §4.9.
  * With any of the last three: TN_ERR_STATE if tn_load_tetrahedra or tn_update_vertices ran since the forward (they read the mesh
- * positions), and the default mode keeps the [samples,64] feature gradient for them (0.54 GB at 8192 rays x 257 fine samples). */
+ * positions), and the default mode keeps the [samples,64] feature gradient for them (0.54 GB at 8192 rays x 257 fine samples).
+ * tn_render_train_backward_saved2 is tn_render_train_backward_saved with one more optional input after d_grad_expected_depth:
+ *   d_grad_distortion f32[R]: dL/d distortion (tn_render_train_distortion).  The spacing bins are constants; dL/dw_j gains
+ *     dL/dd (2 sum_i w_i |u_j - u_i| + 2/3 w_j delta_j), before the transmittance sums and GradientScaler, so the distortion loss
+ *     reaches the field, the MLP, the rays and the vertices.  NULL runs the same kernels as tn_render_train_backward_saved, which is
+ *     tn_render_train_backward_saved2 with NULL here.  DESIGN.md §4.11.
+ * tn_render_train_distortion writes d_distortion f32[R], the distortion loss of mip-NeRF 360 / nerfstudio's distortion_loss per ray of a
+ * saved forward: over its fine samples, with s_0 ... s_S2 the spacing bins, u_i = (s_i + s_{i+1}) / 2, delta_i = s_{i+1} - s_i and w_i the
+ * weights of rgb, d = sum_i sum_j w_i w_j |u_i - u_j| + 1/3 sum_i w_i^2 delta_i, in O(S2) per ray; 0 on empty rays.  It reads d_saved
+ * only, so the forward and its saved state are the same with or without it; like the backward it reads the header back (waits until
+ * the stream has reached it) and returns TN_ERR_STATE if the field or the weights changed since the forward. */
 int tn_render_train_saved_bytes(tn_tracer *h, const tn_render_config *cfg, uint32_t R, size_t *bytes);
 int tn_render_train_forward_saved(tn_tracer *h, const tn_render_config *cfg, const float *d_origins, const float *d_directions, uint32_t R,
                                   const float *d_jitter_coarse, const float *d_jitter_fine, float *d_rgb, float *d_acc, float *d_depth,
@@ -198,6 +208,11 @@ int tn_render_train_backward_saved(tn_tracer *h, const void *d_saved, const floa
                                    const float *d_grad_expected_depth, int use_gradient_scaling, float *d_grad_field,
                                    float *const *d_grad_params12, float *d_grad_origins, float *d_grad_directions, float *d_grad_xyz,
                                    void *stream);
+int tn_render_train_backward_saved2(tn_tracer *h, const void *d_saved, const float *d_grad_rgb, const float *d_grad_acc,
+                                    const float *d_grad_expected_depth, const float *d_grad_distortion, int use_gradient_scaling,
+                                    float *d_grad_field, float *const *d_grad_params12, float *d_grad_origins, float *d_grad_directions,
+                                    float *d_grad_xyz, void *stream);
+int tn_render_train_distortion(tn_tracer *h, const void *d_saved, float *d_distortion, void *stream);
 /* Deterministic mode of the fused training step (enable != 0; initial value: 1 if the environment variable TETRANERF_B200_DETERMINISTIC
  * is 1, else 0).  Read by tn_render_train_forward; tn_render_train_backward continues in the mode of the forward it belongs to.  With
  * identical inputs, on the same build and GPU model, forward outputs and every gradient are then bitwise identical from run to run and

@@ -527,10 +527,54 @@ struct CompositeBwdParams {
                                        // deterministic mode: [n_active] float4, one per slot (summed in slot order by k_det_sum_slots)
     const float *grad_ed;              // DEPTH: [R] dL/d expected depth
     const uint32_t *dbounds;           // DEPTH: the forward's clip bounds (ordered keys, k_composite<true>)
+    const float *grad_dist;            // DIST: [R] dL/d distortion
 };
+
+// ---- distortion loss (DESIGN §4.11; mip-NeRF 360, nerfstudio losses.distortion_loss) over the fine pass of one ray: spacing bins s_0..s_S2,
+// u_i = (s_i + s_{i+1}) / 2, delta_i = s_{i+1} - s_i, w_i the weights of rgb:
+//   d = sum_i sum_j w_i w_j |u_i - u_j| + 1/3 sum_i w_i^2 delta_i = 2 sum_j w_j (u_j W_<j - P_<j) + 1/3 sum_j w_j^2 delta_j
+// with W, P the prefix sums of w and w u (the bins are sorted), in one pass of warp scans.
+struct DistortionParams {
+    uint32_t S2;
+    const uint32_t *n_active, *ray_list;
+    const float *ebins_f, *sbins_f, *out_f;
+    float *dist;                       // [R], zeroed by the caller (empty rays stay 0)
+};
+__global__ void __launch_bounds__(SAMPLE_WARPS * 32) k_distortion(const DistortionParams p) {
+    extern __shared__ float sm[];
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const uint32_t slot = blockIdx.x * SAMPLE_WARPS + warp;
+    if (slot >= *p.n_active) return;
+    const uint32_t S2 = p.S2;
+    float *w = sm + (size_t)warp * (2 * ((size_t)S2 + 2)), *tr = w + S2 + 2;
+    const float *eb = p.ebins_f + (size_t)slot * (S2 + 1);
+    const float *sb = p.sbins_f + (size_t)slot * (S2 + 1);
+    const float4 *of = reinterpret_cast<const float4 *>(p.out_f) + (size_t)slot * S2;
+    for (uint32_t j = lane; j < S2; j += 32) w[j] = (eb[j + 1] - eb[j]) * of[j].x;
+    __syncwarp();
+    weights_from_density(w, tr, S2, lane);  // the weights k_composite composites rgb with
+    float cw = 0.f, cp = 0.f, inter = 0.f, intra = 0.f;  // carries of W and P from the previous 32 samples
+    for (uint32_t base = 0; base < S2; base += 32) {
+        const uint32_t j = base + lane;
+        const float wj = j < S2 ? w[j] : 0.f;
+        const float uj = j < S2 ? (sb[j] + sb[j + 1]) / 2.f : 0.f, dj = j < S2 ? sb[j + 1] - sb[j] : 0.f;
+        const float iw = warp_incl_scan_f(wj, lane), ip = warp_incl_scan_f(wj * uj, lane);
+        float ew = __shfl_up_sync(0xffffffffu, iw, 1), ep = __shfl_up_sync(0xffffffffu, ip, 1);
+        if (lane == 0) ew = ep = 0.f;
+        inter += wj * (uj * (cw + ew) - (cp + ep));
+        intra += wj * wj * dj;
+        cw += __shfl_sync(0xffffffffu, iw, 31); cp += __shfl_sync(0xffffffffu, ip, 31);
+    }
+    inter = warp_sum_f(inter); intra = warp_sum_f(intra);
+    if (lane == 0) p.dist[p.ray_list[slot]] = 2.f * inter + intra / 3.f;
+}
+
 // DEPTH: g_j also gets the expected depth's term grad_ed (t_j - D_raw) / (A + 1e-10), 0 where the forward's clip binds (DESIGN §4.10);
-// A and D_raw are recomputed from the saved bins and densities exactly as k_composite<true> formed them
-template <bool DET, bool DEPTH = false>
+// A and D_raw are recomputed from the saved bins and densities exactly as k_composite<true> formed them.
+// DIST: g_j also gets the distortion's term grad_dist (2 sum_i w_i |u_j - u_i| + 2/3 w_j delta_j) (DESIGN §4.11), with
+// sum_i w_i |u_j - u_i| = u_j W_<j - P_<j + (P - P_<=j) - u_j (W - W_<=j) from two scans.  It is staged in fx[j], which the same lane
+// overwrites only after reading it, so the shared memory per block stays 64 (S2 + 2) bytes.
+template <bool DET, bool DEPTH = false, bool DIST = false>
 __global__ void __launch_bounds__(SAMPLE_WARPS * 32) k_composite_bwd(const CompositeBwdParams p) {
     extern __shared__ float sm[];
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -562,6 +606,31 @@ __global__ void __launch_bounds__(SAMPLE_WARPS * 32) k_composite_bwd(const Compo
         const float lo = depth_unkey(p.dbounds[0]), hi = depth_unkey(p.dbounds[1]);
         gd = (draw >= lo && draw <= hi) ? p.grad_ed[ray] : 0.f;  // torch.clip's backward: inclusive bounds
     }
+    if constexpr (DIST) {
+        const float *sb = p.sbins_f + (size_t)slot * (S2 + 1);
+        const float gdist = p.grad_dist[ray];
+        float tw = 0.f, tp = 0.f;  // W, P
+        for (uint32_t j = lane; j < S2; j += 32) {
+            const float excl = j == 0 ? 0.f : tr[j - 1];
+            const float x = (eb[j + 1] - eb[j]) * of[j].x;
+            const float wj = nan_to_num_f((1.f - expf(-x)) * expf(-excl));  // the forward's weights
+            w[j] = wj;
+            tw += wj; tp += wj * ((sb[j] + sb[j + 1]) / 2.f);
+        }
+        tw = warp_sum_f(tw); tp = warp_sum_f(tp);
+        float cw = 0.f, cp = 0.f;  // carries of W and P from the previous 32 samples
+        for (uint32_t base = 0; base < S2; base += 32) {
+            const uint32_t j = base + lane;
+            const float wj = j < S2 ? w[j] : 0.f;
+            const float uj = j < S2 ? (sb[j] + sb[j + 1]) / 2.f : 0.f, dj = j < S2 ? sb[j + 1] - sb[j] : 0.f;
+            const float iw = warp_incl_scan_f(wj, lane), ip = warp_incl_scan_f(wj * uj, lane);
+            float ew = __shfl_up_sync(0xffffffffu, iw, 1), ep = __shfl_up_sync(0xffffffffu, ip, 1);
+            if (lane == 0) ew = ep = 0.f;
+            const float wl = cw + ew, pl = cp + ep, wle = cw + iw, ple = cp + ip;  // W_<j, P_<j, W_<=j, P_<=j
+            if (j < S2) fx[j] = gdist * (2.f * (uj * wl - pl + (tp - ple) - uj * (tw - wle)) + (2.f / 3.f) * wj * dj);
+            cw += __shfl_sync(0xffffffffu, iw, 31); cp += __shfl_sync(0xffffffffu, ip, 31);
+        }
+    }
     for (uint32_t j = lane; j < S2; j += 32) {
         const float excl = j == 0 ? 0.f : tr[j - 1];
         const float x = (eb[j + 1] - eb[j]) * of[j].x;
@@ -573,6 +642,7 @@ __global__ void __launch_bounds__(SAMPLE_WARPS * 32) k_composite_bwd(const Compo
         float g;
         if constexpr (DEPTH) g = fin ? (gr * (c.y - p.bg0) + gg * (c.z - p.bg1) + gb * (c.w - p.bg2) + ga + gd * (((eb[j] + eb[j + 1]) / 2.f - draw) / den)) : 0.f;
         else g = fin ? (gr * (c.y - p.bg0) + gg * (c.z - p.bg1) + gb * (c.w - p.bg2) + ga) : 0.f;
+        if constexpr (DIST) g = fin ? g + fx[j] : 0.f;  // (read before this lane overwrites fx[j] below)
         w[j] = wj;
         gw[j] = g * wj;
         fx[j] = fin ? g * (T - wj) : 0.f;  // first term of dL/dx_j
@@ -1103,10 +1173,11 @@ extern "C" int tn_render_train_forward(tn_tracer *h, const tn_render_config *cfg
 // weights; writes only the tracer's gradient scratch.  The coarse pass carries no gradient (PDFSampler detaches its bins).  No
 // [samples,128] tensor touches HBM.
 // d_grad_ed != nullptr: dL/d expected depth f32[R] of a forward that produced it (its clip bounds in b.n_active[4, 5]).
+// d_grad_dist != nullptr: dL/d distortion f32[R] (k_distortion).
 // Any of d_grad_o / d_grad_d / d_grad_xyz != nullptr: also the gradients at the ray origins / directions (tn_ray_grads.cu) and at the
 // mesh vertex positions (tn_vertex_grads.cu), into the non-null ones.
 static int train_backward_impl(tn_tracer *h, const TrainBufs &b, uint32_t R, uint32_t S2, bool det, const float *bg, const float *d_grad_rgb,
-                               const float *d_grad_acc, const float *d_grad_ed, int use_gradient_scaling, float *d_grad_field,
+                               const float *d_grad_acc, const float *d_grad_ed, const float *d_grad_dist, int use_gradient_scaling, float *d_grad_field,
                                float *const *d_grad_params12, float *d_grad_o, float *d_grad_d, float *d_grad_xyz, cudaStream_t s) {
     RenderState *r = h->render;
     int sms = 132;
@@ -1130,10 +1201,13 @@ static int train_backward_impl(tn_tracer *h, const TrainBufs &b, uint32_t R, uin
     cb.S2 = S2; cb.use_gradient_scaling = use_gradient_scaling ? 1u : 0u; cb.n_active = b.n_active; cb.ray_list = b.ray_list;
     cb.ebins_f = b.ebins_f; cb.sbins_f = b.sbins_f; cb.out_f = b.out_f; cb.grad_rgb = d_grad_rgb; cb.grad_acc = d_grad_acc;
     cb.bg0 = bg[0]; cb.bg1 = bg[1]; cb.bg2 = bg[2]; cb.dout = r->dout.p; cb.sums = det ? (float *)r->det_sums.p : r->gw.p + GW_SUMS;
-    cb.grad_ed = d_grad_ed; cb.dbounds = b.n_active + 4;
+    cb.grad_ed = d_grad_ed; cb.dbounds = b.n_active + 4; cb.grad_dist = d_grad_dist;
     const size_t smem_cb = SAMPLE_WARPS * sizeof(float) * 4 * ((size_t)S2 + 2);
-    auto k_cbwd = d_grad_ed != nullptr ? (det ? k_composite_bwd<true, true> : k_composite_bwd<false, true>)
-                                       : (det ? k_composite_bwd<true> : k_composite_bwd<false>);
+    auto k_cbwd = d_grad_dist != nullptr
+                      ? (d_grad_ed != nullptr ? (det ? k_composite_bwd<true, true, true> : k_composite_bwd<false, true, true>)
+                                              : (det ? k_composite_bwd<true, false, true> : k_composite_bwd<false, false, true>))
+                      : (d_grad_ed != nullptr ? (det ? k_composite_bwd<true, true> : k_composite_bwd<false, true>)
+                                              : (det ? k_composite_bwd<true> : k_composite_bwd<false>));
     TN_CUDA(cudaFuncSetAttribute(k_cbwd, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_cb));
     const uint32_t gridR = (R + SAMPLE_WARPS - 1) / SAMPLE_WARPS;
     if (r->profile) cudaEventRecord(r->evb[0], s);
@@ -1225,7 +1299,7 @@ extern "C" int tn_render_train_backward(tn_tracer *h, const float *d_grad_rgb, c
     RenderState *r = h->render;
     if (!r || !r->train_valid) return fail(TN_ERR_STATE, "tn_render_train_backward: no training forward to continue from");
     DeviceGuard g(h->device);
-    return train_backward_impl(h, own_bufs(r), r->t_R, r->t_S2, r->t_det, r->t_bg, d_grad_rgb, d_grad_acc, nullptr, use_gradient_scaling,
+    return train_backward_impl(h, own_bufs(r), r->t_R, r->t_S2, r->t_det, r->t_bg, d_grad_rgb, d_grad_acc, nullptr, nullptr, use_gradient_scaling,
                                d_grad_field, d_grad_params12, nullptr, nullptr, nullptr, (cudaStream_t)stream);
 }
 
@@ -1275,25 +1349,33 @@ extern "C" int tn_render_train_forward_saved(tn_tracer *h, const tn_render_confi
     return TN_OK;
 }
 
-// optional input: the gradient of the expected depth d_grad_expected_depth f32[R] (DESIGN.md §4.10); optional outputs: the gradients at
-// the ray origins / directions of the forward, f32[R,3] each (0 on empty rays; §4.8), and at the mesh vertex positions, f32[V,3] (§4.9)
-extern "C" int tn_render_train_backward_saved(tn_tracer *h, const void *d_saved, const float *d_grad_rgb, const float *d_grad_acc,
-                                              const float *d_grad_expected_depth, int use_gradient_scaling, float *d_grad_field,
-                                              float *const *d_grad_params12, float *d_grad_origins, float *d_grad_directions, float *d_grad_xyz,
-                                              void *stream) {
-    if (!h || !d_saved || !d_grad_rgb || !d_grad_field || !d_grad_params12) return fail(TN_ERR_ARG, "null argument");
+// the header of a saved state, read back to the host (waits until the stream has reached the caller), if it belongs to the current
+// field and weights of this tracer; `what` names the caller in the errors
+static int read_saved_header(tn_tracer *h, const void *d_saved, cudaStream_t s, const char *what, SavedHeader *hd) {
     RenderState *r = h->render;
-    if (!r || !r->n_active.p) return fail(TN_ERR_STATE, "tn_render_train_backward_saved: no training forward on this tracer");
+    if (!r || !r->n_active.p) return fail(TN_ERR_STATE, std::string(what) + ": no training forward on this tracer");
+    TN_CUDA(cudaMemcpyAsync(hd, d_saved, sizeof(*hd), cudaMemcpyDeviceToHost, s));
+    TN_CUDA(cudaStreamSynchronize(s));
+    if (hd->magic != SAVED_MAGIC) return fail(TN_ERR_STATE, std::string(what) + ": d_saved holds no training forward");
+    if (hd->gen != r->gen)
+        return fail(TN_ERR_STATE, std::string(what) + ": the field or the weights changed (tn_render_set_field / "
+                                  "tn_render_set_weights) since the forward, or the forward ran on another tracer");
+    return TN_OK;
+}
+
+// optional inputs: the gradients of the expected depth d_grad_expected_depth f32[R] (DESIGN.md §4.10) and of the distortion
+// d_grad_distortion f32[R] (§4.11); optional outputs: the gradients at the ray origins / directions of the forward, f32[R,3] each (0 on
+// empty rays; §4.8), and at the mesh vertex positions, f32[V,3] (§4.9)
+extern "C" int tn_render_train_backward_saved2(tn_tracer *h, const void *d_saved, const float *d_grad_rgb, const float *d_grad_acc,
+                                               const float *d_grad_expected_depth, const float *d_grad_distortion, int use_gradient_scaling,
+                                               float *d_grad_field, float *const *d_grad_params12, float *d_grad_origins,
+                                               float *d_grad_directions, float *d_grad_xyz, void *stream) {
+    if (!h || !d_saved || !d_grad_rgb || !d_grad_field || !d_grad_params12) return fail(TN_ERR_ARG, "null argument");
     DeviceGuard g(h->device);
     cudaStream_t s = (cudaStream_t)stream;
     // the launch shapes depend on the call's R and S2: read the header back (waits until the stream has reached this backward)
     SavedHeader hd{};
-    TN_CUDA(cudaMemcpyAsync(&hd, d_saved, sizeof(hd), cudaMemcpyDeviceToHost, s));
-    TN_CUDA(cudaStreamSynchronize(s));
-    if (hd.magic != SAVED_MAGIC) return fail(TN_ERR_STATE, "tn_render_train_backward_saved: d_saved holds no training forward");
-    if (hd.gen != r->gen)
-        return fail(TN_ERR_STATE, "tn_render_train_backward_saved: the field or the weights changed (tn_render_set_field / "
-                                  "tn_render_set_weights) since the forward, or the forward ran on another tracer");
+    TN_TRY(read_saved_header(h, d_saved, s, "tn_render_train_backward_saved", &hd));
     const bool rays = d_grad_origins != nullptr || d_grad_directions != nullptr || d_grad_xyz != nullptr;
     if (rays && hd.mesh_gen != h->mesh_gen)
         return fail(TN_ERR_STATE, "tn_render_train_backward_saved: tn_load_tetrahedra or tn_update_vertices ran since the forward "
@@ -1303,8 +1385,36 @@ extern "C" int tn_render_train_backward_saved(tn_tracer *h, const void *d_saved,
                                   "tn_render_train_forward_saved)");
     TrainBufs b{};
     saved_layout(hd.R, hd.S2, (uint8_t *)d_saved, &b);
-    return train_backward_impl(h, b, hd.R, hd.S2, hd.det != 0, hd.bg, d_grad_rgb, d_grad_acc, d_grad_expected_depth, use_gradient_scaling,
-                               d_grad_field, d_grad_params12, d_grad_origins, d_grad_directions, d_grad_xyz, s);
+    return train_backward_impl(h, b, hd.R, hd.S2, hd.det != 0, hd.bg, d_grad_rgb, d_grad_acc, d_grad_expected_depth, d_grad_distortion,
+                               use_gradient_scaling, d_grad_field, d_grad_params12, d_grad_origins, d_grad_directions, d_grad_xyz, s);
+}
+
+extern "C" int tn_render_train_backward_saved(tn_tracer *h, const void *d_saved, const float *d_grad_rgb, const float *d_grad_acc,
+                                              const float *d_grad_expected_depth, int use_gradient_scaling, float *d_grad_field,
+                                              float *const *d_grad_params12, float *d_grad_origins, float *d_grad_directions, float *d_grad_xyz,
+                                              void *stream) {
+    return tn_render_train_backward_saved2(h, d_saved, d_grad_rgb, d_grad_acc, d_grad_expected_depth, nullptr, use_gradient_scaling, d_grad_field,
+                                           d_grad_params12, d_grad_origins, d_grad_directions, d_grad_xyz, stream);
+}
+
+// the distortion loss of every ray of a saved training forward (DESIGN.md §4.11): d_distortion f32[R], 0 on empty rays
+extern "C" int tn_render_train_distortion(tn_tracer *h, const void *d_saved, float *d_distortion, void *stream) {
+    if (!h || !d_saved || !d_distortion) return fail(TN_ERR_ARG, "null argument");
+    DeviceGuard g(h->device);
+    cudaStream_t s = (cudaStream_t)stream;
+    SavedHeader hd{};
+    TN_TRY(read_saved_header(h, d_saved, s, "tn_render_train_distortion", &hd));
+    TrainBufs b{};
+    saved_layout(hd.R, hd.S2, (uint8_t *)d_saved, &b);
+    DistortionParams p{hd.S2, b.n_active, b.ray_list, b.ebins_f, b.sbins_f, b.out_f, d_distortion};
+    // the same staging as k_composite, below k_composite_bwd's, which the forward has checked against the device's limit
+    const size_t smem = SAMPLE_WARPS * sizeof(float) * 2 * ((size_t)hd.S2 + 2);
+    TN_CUDA(cudaFuncSetAttribute(k_distortion, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    TN_CUDA(cudaMemsetAsync(d_distortion, 0, sizeof(float) * (size_t)hd.R, s));
+    k_distortion<<<(hd.R + SAMPLE_WARPS - 1) / SAMPLE_WARPS, SAMPLE_WARPS * 32, smem, s>>>(p);
+    h->launches += 1;
+    TN_CUDA(cudaGetLastError());
+    return TN_OK;
 }
 
 // deterministic mode of the fused training step (see the header): applies from the next tn_render_train_forward on

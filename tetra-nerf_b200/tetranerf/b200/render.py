@@ -191,7 +191,8 @@ class FusedRenderer:
 
     def train_backward_saved(self, state: "TrainState", grad_rgb: torch.Tensor, grad_acc: Optional[torch.Tensor], num_vertices: int,
                              use_gradient_scaling: bool = False, grad_origins: bool = False, grad_directions: bool = False,
-                             grad_vertices: bool = False, grad_expected_depth: Optional[torch.Tensor] = None):
+                             grad_vertices: bool = False, grad_expected_depth: Optional[torch.Tensor] = None,
+                             grad_distortion: Optional[torch.Tensor] = None):
         """backward of the train_forward_saved call that returned `state`; outputs as train_backward.  Raises RuntimeError if
         set_field / set_weights ran since that forward.  Waits until the stream has reached it (it reads the call's shape back).
         grad_origins / grad_directions: also the gradients at the forward's ray origins / directions (the sample distances held fixed;
@@ -200,27 +201,38 @@ class FusedRenderer:
         (the matched tetrahedra held fixed as well; DESIGN §4.9) -> (grad_field, grads, grad_origins or None, grad_directions or None,
         grad_vertices f32[V,3]); then it raises RuntimeError if load_tetrahedra or update_vertices ran since that forward.
         grad_expected_depth f32[R] or [R,1]: dL/d expected_depth of a forward with expected_depth=True (RuntimeError otherwise); the
-        outputs keep the form above."""
+        outputs keep the form above.  grad_distortion f32[R] or [R,1]: dL/d distortion (train_distortion; DESIGN §4.11), for any forward;
+        None runs the same kernels as before it existed."""
         if tuple(grad_rgb.shape) != (state.R, 3) or (grad_acc is not None and grad_acc.numel() != state.R):
             raise RuntimeError(f"the forward rendered {state.R} rays: grad_rgb must be [{state.R}, 3] and grad_acc [{state.R}], got "
                                f"{tuple(grad_rgb.shape)} and {None if grad_acc is None else tuple(grad_acc.shape)}")
-        g_ed = grad_expected_depth
-        if g_ed is not None:
-            if g_ed.numel() != state.R or g_ed.device != self.device or g_ed.dtype != torch.float32:
-                raise RuntimeError(f"grad_expected_depth must be a float32 [{state.R}] tensor on the tracer's device, got {tuple(g_ed.shape)}")
-            g_ed = g_ed.reshape(-1).contiguous()
+        g_ed, g_dist = grad_expected_depth, grad_distortion
+        for name, t in (("grad_expected_depth", g_ed), ("grad_distortion", g_dist)):
+            if t is not None and (t.numel() != state.R or t.device != self.device or t.dtype != torch.float32):
+                raise RuntimeError(f"{name} must be a float32 [{state.R}] tensor on the tracer's device, got {tuple(t.shape)}")
+        g_ed = g_ed.reshape(-1).contiguous() if g_ed is not None else None
+        g_dist = g_dist.reshape(-1).contiguous() if g_dist is not None else None
         grad_rgb = grad_rgb.contiguous()
         grad_acc = grad_acc.contiguous() if grad_acc is not None else None
         go = torch.empty((state.R, 3), dtype=torch.float32, device=self.device) if grad_origins else None
         gd = torch.empty((state.R, 3), dtype=torch.float32, device=self.device) if grad_directions else None
         gv = torch.empty((num_vertices, 3), dtype=torch.float32, device=self.device) if grad_vertices else None
         gfield, gp, arr = self._grad_outputs(num_vertices)
-        ext._check(_lib.tn_render_train_backward_saved(self.tracer.handle, state.blob.data_ptr(), grad_rgb.data_ptr(), _ptr(grad_acc),
-                                                       _ptr(g_ed), int(use_gradient_scaling), gfield.data_ptr(), arr, _ptr(go), _ptr(gd),
-                                                       _ptr(gv), self._stream()))
+        ext._check(_lib.tn_render_train_backward_saved2(self.tracer.handle, state.blob.data_ptr(), grad_rgb.data_ptr(), _ptr(grad_acc),
+                                                        _ptr(g_ed), _ptr(g_dist), int(use_gradient_scaling), gfield.data_ptr(), arr, _ptr(go),
+                                                        _ptr(gd), _ptr(gv), self._stream()))
         if grad_vertices:
             return gfield, gp, go, gd, gv
         return (gfield, gp, go, gd) if grad_origins or grad_directions else (gfield, gp)
+
+    def train_distortion(self, state: "TrainState") -> torch.Tensor:
+        """the distortion loss per ray of the train_forward_saved call that returned `state` -> f32[R,1], 0 on empty rays: mip-NeRF 360's
+        sum_i sum_j w_i w_j |u_i - u_j| + 1/3 sum_i w_i^2 delta_i over the fine samples, u / delta the midpoints / widths of the spacing
+        bins, w the weights of rgb (nerfstudio's distortion_loss per ray; DESIGN §4.11).  Raises RuntimeError if set_field / set_weights
+        ran since that forward.  Waits until the stream has reached it (it reads the call's shape back)."""
+        out = torch.empty((state.R, 1), dtype=torch.float32, device=self.device)
+        ext._check(_lib.tn_render_train_distortion(self.tracer.handle, state.blob.data_ptr(), out.data_ptr(), self._stream()))
+        return out
 
     # ---- surface extraction ---------------------------------------------------------------------------------------------------------
     def extract_surface(self, level: float) -> Dict[str, torch.Tensor]:
@@ -335,9 +347,34 @@ class FusedTrainRenderDepth(torch.autograd.Function):
         return _fused_backward(ctx, g_rgb, g_acc, g_ed)
 
 
-def _fused_forward(ctx, name, expected_depth, fr, settings, use_gradient_scaling, origins, directions, jitter_coarse, jitter_fine, field, params):
-    """forward of FusedTrainRender / FusedTrainRenderDepth: checks the optional vertex positions, runs the saved training forward and
-    keeps what the backward needs in ctx -> the forward's outputs"""
+class FusedTrainRenderDistortion(torch.autograd.Function):
+    """FusedTrainRender with the distortion loss per ray (DESIGN §4.11), and the expected depth when asked.  Arguments: those of
+    FusedTrainRender (the optional vertex positions included) with a flag `expected_depth` after use_gradient_scaling.  Outputs
+    (rgb, accumulation, depth, distortion, ray_mask), or (rgb, accumulation, depth, expected_depth, distortion, ray_mask) with
+    expected_depth=True; distortion f32[R,1] is FusedRenderer.train_distortion, 0 on empty rays.  rgb, accumulation, expected_depth and
+    distortion are differentiable: a distortion loss reaches the field, the MLP and, when they require grad, the ray origins / directions
+    and the vertex positions, with the spacing bins held fixed.  The other outputs are the same bits as FusedTrainRender's."""
+
+    @staticmethod
+    def forward(ctx, fr, settings, use_gradient_scaling, expected_depth, origins, directions, jitter_coarse, jitter_fine, field, *params):
+        out = _fused_forward(ctx, "FusedTrainRenderDistortion", expected_depth, fr, settings, use_gradient_scaling, origins, directions,
+                             jitter_coarse, jitter_fine, field, params, first=4)
+        dist = fr.train_distortion(ctx.state)
+        ctx.ed = bool(expected_depth)
+        ed = (out["expected_depth"],) if expected_depth else ()
+        return (out["rgb"], out["accumulation"], out["depth"], *ed, dist, out["ray_mask"])
+
+    @staticmethod
+    def backward(ctx, g_rgb, g_acc, _g_depth, *rest):
+        g_ed, g_dist = (rest[0], rest[1]) if ctx.ed else (None, rest[0])
+        return _fused_backward(ctx, g_rgb, g_acc, g_ed, g_dist)
+
+
+def _fused_forward(ctx, name, expected_depth, fr, settings, use_gradient_scaling, origins, directions, jitter_coarse, jitter_fine, field, params,
+                   first=3):
+    """forward of FusedTrainRender / FusedTrainRenderDepth / FusedTrainRenderDistortion: checks the optional vertex positions, runs the
+    saved training forward and keeps what the backward needs in ctx -> the forward's outputs.  `first`: the index of `origins` among the
+    op's arguments"""
     if len(params) == len(PARAM_ORDER) + 1:
         xyz, borrowed = params[-1], fr.tracer._vertices
         if borrowed is None or xyz.data_ptr() != borrowed.data_ptr() or xyz.shape != borrowed.shape:
@@ -349,26 +386,29 @@ def _fused_forward(ctx, name, expected_depth, fr, settings, use_gradient_scaling
     elif len(params) != len(PARAM_ORDER):
         raise RuntimeError(f"{name} takes the {len(PARAM_ORDER)} MLP parameters and optionally the vertex positions")
     out, state = fr.train_forward_saved(origins, directions, settings, jitter_coarse, jitter_fine, expected_depth=expected_depth)
-    ctx.fr, ctx.state, ctx.gs = fr, state, bool(use_gradient_scaling)
+    ctx.fr, ctx.state, ctx.gs, ctx.first = fr, state, bool(use_gradient_scaling), first
     ctx.ray_shapes = (origins.shape, directions.shape)
     ctx.save_for_backward(field, *params)  # their version counters reject a backward after an in-place change
     ctx.mark_non_differentiable(out["depth"], out["ray_mask"])
     return out
 
 
-def _fused_backward(ctx, g_rgb, g_acc, g_ed):
-    """backward of FusedTrainRender / FusedTrainRenderDepth (g_ed: the expected depth's gradient, or None)"""
+def _fused_backward(ctx, g_rgb, g_acc, g_ed, g_dist=None):
+    """backward of FusedTrainRender / FusedTrainRenderDepth / FusedTrainRenderDistortion (g_ed, g_dist: the expected depth's and the
+    distortion's gradients, or None)"""
     field = ctx.saved_tensors[0]
     if g_rgb is None:
         g_rgb = torch.zeros((ctx.state.R, 3), dtype=torch.float32, device=field.device)
-    want_o, want_d = ctx.needs_input_grad[3], ctx.needs_input_grad[4]
-    has_xyz = len(ctx.needs_input_grad) == 8 + len(PARAM_ORDER) + 1
+    first = ctx.first
+    want_o, want_d = ctx.needs_input_grad[first], ctx.needs_input_grad[first + 1]
+    has_xyz = len(ctx.needs_input_grad) == first + 5 + len(PARAM_ORDER) + 1
     want_v = has_xyz and ctx.needs_input_grad[-1]
     g_acc = g_acc.reshape(-1) if g_acc is not None else None
     g_ed = g_ed.reshape(-1) if g_ed is not None else None
+    g_dist = g_dist.reshape(-1) if g_dist is not None else None
     res = ctx.fr.train_backward_saved(ctx.state, g_rgb, g_acc, field.shape[1], ctx.gs, grad_origins=want_o, grad_directions=want_d,
-                                      grad_vertices=want_v, grad_expected_depth=g_ed)
+                                      grad_vertices=want_v, grad_expected_depth=g_ed, grad_distortion=g_dist)
     gfield, gp, go, gd, gv = res + (None,) * (5 - len(res))
     go = go.reshape(ctx.ray_shapes[0]) if go is not None else None
     gd = gd.reshape(ctx.ray_shapes[1]) if gd is not None else None
-    return (None, None, None, go, gd, None, None, gfield) + tuple(gp[n] for n in PARAM_ORDER) + ((gv,) if has_xyz else ())
+    return (None,) * first + (go, gd, None, None, gfield) + tuple(gp[n] for n in PARAM_ORDER) + ((gv,) if has_xyz else ())

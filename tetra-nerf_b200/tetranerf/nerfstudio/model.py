@@ -87,6 +87,10 @@ class TetrahedraNerfConfig(ModelConfig):
     (expected_depth - target)^2, the target batch["depth_image"] [R,1] in the model's frame"""
     is_euclidean_depth: bool = False
     """the depth target is the distance along the ray; False: z-depth, multiplied by the ray bundle's metadata["directions_norm"]"""
+    distortion_loss_mult: float = 0.0
+    """> 0: training outputs also hold "distortion" f32[R,1], mip-NeRF 360's distortion of each ray's weights over its spacing bins (0 on
+    empty rays; DESIGN §4.11), and the loss dict gains distortion_loss = distortion_loss_mult * its mean over the rays with hits, as
+    nerfacto's distortion_loss_mult.  Training only; 0 changes nothing"""
 
     def __post_init__(self):
         if self.tetrahedra_path is not None and self.num_tetrahedra_vertices is None:
@@ -156,6 +160,22 @@ class GradientScaler(torch.autograd.Function):
         (ray_dist,) = ctx.saved_tensors
         s = torch.square(ray_dist).clamp(0, 1)
         return g_colors * s, g_sigmas * s, g_dist
+
+
+def distortion_per_ray(weights: torch.Tensor, sdist: torch.Tensor) -> torch.Tensor:
+    """mip-NeRF 360's distortion of each ray (nerfstudio's losses.distortion_loss before its mean), in O(S) per ray: weights [R,S,1],
+    sdist [R,S+1] sorted spacing bins -> [R,1].  With u the bin midpoints, delta their widths and W_<j, P_<j the exclusive prefix sums of
+    w and w u, sum_i sum_j w_i w_j |u_i - u_j| = 2 sum_j w_j (u_j W_<j - P_<j), so no [R,S,S] tensor is formed; autograd gives
+    dd/dw_j = 2 sum_i w_i |u_j - u_i| + 2/3 w_j delta_j"""
+    w = weights[..., 0]
+    u = (sdist[..., 1:] + sdist[..., :-1]) / 2
+    delta = sdist[..., 1:] - sdist[..., :-1]
+    zero = torch.zeros_like(w[..., :1])
+    w_excl = torch.cumsum(torch.cat((zero, w[..., :-1]), -1), -1)
+    p_excl = torch.cumsum(torch.cat((zero, (w * u)[..., :-1]), -1), -1)
+    inter = 2 * torch.sum(w * (u * w_excl - p_excl), -1, keepdim=True)
+    intra = torch.sum(w**2 * delta, -1, keepdim=True) / 3
+    return inter + intra
 
 
 class TetrahedraNerf(Model):
@@ -337,6 +357,9 @@ class TetrahedraNerf(Model):
     def _expected_depth_on(self) -> bool:
         return self.config.render_expected_depth or self.config.depth_loss_mult > 0
 
+    def _distortion_on(self) -> bool:
+        return self.config.distortion_loss_mult > 0 and self.training
+
     def get_outputs(self, ray_bundle: RayBundle):
         outputs = self._get_outputs(ray_bundle)
         # the z-depth target's conversion to a distance along the ray, for get_loss_dict only: in training, and in nerfstudio's eval
@@ -374,7 +397,7 @@ class TetrahedraNerf(Model):
     def _get_outputs_fused_train(self, origins, directions):
         """training step on the fused CUDA pipeline: ONE differentiable op (forward + wgmma backward) instead of the reference's op
         sequence; the stratified draws are the same two torch.rand calls the reference makes (model.py:169-174, PDFSampler)."""
-        from ..b200.render import PARAM_ORDER, FusedTrainRender, FusedTrainRenderDepth, RenderSettings
+        from ..b200.render import PARAM_ORDER, FusedTrainRender, FusedTrainRenderDepth, FusedTrainRenderDistortion, RenderSettings
 
         c = self.config
         bg = (1.0, 1.0, 1.0) if c.background_color == "white" else (0.0, 0.0, 0.0)
@@ -386,6 +409,10 @@ class TetrahedraNerf(Model):
         named = dict(self.named_parameters())
         xyz = (self.tetrahedra_vertices,) if c.optimize_vertices else ()  # the tensor the tracer borrowed (get_tetrahedra_tracer)
         args = (fr, st, c.use_gradient_scaling, origins, directions, jc, jf, self.tetrahedra_field, *[named[n] for n in PARAM_ORDER], *xyz)
+        if self._distortion_on():
+            res = FusedTrainRenderDistortion.apply(*args[:3], self._expected_depth_on(), *args[3:])
+            keys = ["rgb", "accumulation", "depth"] + (["expected_depth"] if self._expected_depth_on() else []) + ["distortion", "ray_mask"]
+            return dict(zip(keys, res))
         if self._expected_depth_on():
             rgb, acc, depth, ed, mask = FusedTrainRenderDepth.apply(*args)
             return {"rgb": rgb, "accumulation": acc, "depth": depth, "expected_depth": ed, "ray_mask": mask}
@@ -413,6 +440,8 @@ class TetrahedraNerf(Model):
         outputs = {"rgb": rgb, "accumulation": accumulation, "depth": depth, "ray_mask": ray_mask}
         if self._expected_depth_on():
             outputs["expected_depth"] = depth.clone()
+        if self._distortion_on():
+            outputs["distortion"] = torch.zeros((R, 1), dtype=torch.float32, device=device)
         if bool(ray_mask.any()):
             bundle = dataclasses.replace(ray_bundle[ray_mask], nears=nears[ray_mask], fars=fars[ray_mask])
             if isinstance(self.sampler_uniform, TetrahedraSampler):
@@ -442,6 +471,9 @@ class TetrahedraNerf(Model):
             depth[ray_mask] = self.renderer_depth(weights, samples)
             if self._expected_depth_on():
                 outputs["expected_depth"][ray_mask] = self.renderer_expected_depth(weights, samples)
+            if self._distortion_on():  # over the spacing bins of the samples that give rgb (nerfstudio's ray_samples_to_sdist)
+                sdist = torch.cat((samples.spacing_starts[..., 0], samples.spacing_ends[..., -1:, 0]), -1)
+                outputs["distortion"][ray_mask] = distortion_per_ray(weights, sdist)
         return outputs
 
     # ---- geometry export -----------------------------------------------------------------------------------------------------------------
@@ -461,6 +493,9 @@ class TetrahedraNerf(Model):
         losses = {"rgb_loss": self.rgb_loss(image, outputs["rgb"])}
         if self.config.depth_loss_mult > 0:
             losses["depth_loss"] = self.config.depth_loss_mult * self._depth_loss(outputs, batch)
+        if self._distortion_on():  # mean over the rays with hits (empty rays hold 0)
+            n = outputs["ray_mask"].sum().clamp_min(1)
+            losses["distortion_loss"] = self.config.distortion_loss_mult * outputs["distortion"].sum() / n
         return scale_dict(losses, self.config.loss_coefficients)
 
     def _depth_loss(self, outputs, batch) -> torch.Tensor:
