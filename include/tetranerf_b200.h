@@ -223,6 +223,24 @@ int tn_render_train_distortion(tn_tracer *h, const void *d_saved, float *d_disto
  * bit; gradients differ from it by rounding (another summation order).  Costs extra device memory: ~0.9 GB at 8192 rays x 257 fine
  * samples (the [samples,64] feature gradient, the sort, partition partials).  The eval render (tn_render) is unaffected. */
 int tn_render_set_deterministic(tn_tracer *h, int enable);
+/* ---- occupancy culling of the fused paths (DESIGN.md §4.12; the reference config's use_occupancy_field) -------------------------
+ * tn_occupancy_update writes d_occ f32[T] (T = the loaded mesh's tetrahedra): occ[t] <- max(decay * occ[t], m_t), m_t the largest
+ * density sigma (softplus of the density head, no GradientScaler, bf16x3 as tn_surface_extract) over 11 probes of tetrahedron t: its 4
+ * vertices, 6 edge midpoints and centroid, as barycentric points.  decay = 0 recomputes from scratch (the old values are not read).
+ * One thread writes each entry, without atomics: bitwise reproducible.  11 probe rows per tetrahedron run through the density MLP in
+ * chunks of 2^19 tetrahedra (a 176 MB workspace the tracer keeps).  TN_ERR_STATE without mesh, field or weights; TN_ERR_ARG if decay is
+ * not finite and >= 0.
+ * tn_render_set_occupancy borrows d_occ f32[T] (NULL: culling off, every kernel runs as without it) and a threshold (TN_ERR_ARG unless
+ * finite and >= 0).  While it is set, a sample of tn_render (both precisions, expected depth and normals included) or of a training
+ * forward that is matched to a tetrahedron t with occ[t] < threshold is culled: its density is the constant 0 (weight 0, no gradient),
+ * its MLP is not evaluated; the PDF sampler sees the resulting coarse weights.  Unmatched samples are evaluated as without culling.  The
+ * MLP passes and the training backward's MLP run over the live rows only, compacted in row order.  A saved forward records its culled
+ * samples in its own state, so its backward never reads d_occ again (an update in between leaves its gradients as they were); the state
+ * is no larger than without culling.  With every occ[t] >= threshold, outputs and gradients are the bits of no occupancy (the default
+ * mode's float reductions aside).  tn_render and the training forwards return TN_ERR_STATE if a mesh with another number of
+ * tetrahedra was loaded since.  Surface extraction and the fused pixel gather are unaffected. */
+int tn_occupancy_update(tn_tracer *h, float *d_occ, float decay, void *stream);
+int tn_render_set_occupancy(tn_tracer *h, const float *d_occ, float threshold);
 /* ---- surface extraction: the density iso-surface sigma = level of the field as a triangle mesh, by marching tetrahedra on the loaded
  * mesh (DESIGN.md §4.6).  sigma is the density the renderer uses (density head of mlp_base, no GradientScaler), always evaluated in
  * bf16x3.  A vertex is inside when sigma(F[:, v]) >= level; every mesh edge (a, b), a < b, with one end inside and one outside gives one

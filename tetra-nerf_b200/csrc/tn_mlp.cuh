@@ -60,6 +60,10 @@ struct MlpParams {
     const float *dirbias;      // FINE: [n_active,128]  = b4 + W4[:, :27] . enc(dir)
     float *out;                // COARSE: density [rows] ; FINE: (sigma,r,g,b) [rows,4]
     uint32_t *tile_ctr;        // device counter (zeroed before the launch): dynamic tile scheduler
+    // MAP (occupancy culling, DESIGN §4.12): the tiles cover the compact rows 0 .. *n_rows - 1, and compact row c is sample row
+    // rowmap[c] of vi / bary / out / the per-ray bias (ascending, so a ray's rows stay contiguous and in slot order)
+    const uint32_t *rowmap;
+    const uint32_t *n_rows;
 };
 
 constexpr uint32_t MLP_NO_TILE = 0xFFFFFFFFu;  // sentinel: the scheduler has run dry
@@ -112,6 +116,23 @@ __device__ __forceinline__ GatherRows load_gather_rows(const uint4 *__restrict__
         if (row < total_rows) {
             r.v[rr] = __ldg(vi + row);
             r.b[rr][0] = __ldg(bary + 3 * row); r.b[rr][1] = __ldg(bary + 3 * row + 1); r.b[rr][2] = __ldg(bary + 3 * row + 2);
+        }
+    }
+    return r;
+}
+// the same through a compact-row map: compact rows at or past total_rows read as unmatched
+__device__ __forceinline__ GatherRows load_gather_rows_mapped(const uint4 *__restrict__ vi, const float *__restrict__ bary, const uint32_t *__restrict__ rowmap,
+                                                          uint64_t row0, uint64_t total_rows) {
+    GatherRows r;
+#pragma unroll
+    for (int rr = 0; rr < 2; ++rr) {
+        const uint64_t row = row0 + 8u * rr;
+        r.v[rr] = make_uint4(TN_EMPTY, TN_EMPTY, TN_EMPTY, TN_EMPTY);
+        r.b[rr][0] = r.b[rr][1] = r.b[rr][2] = 0.f;
+        if (row < total_rows) {
+            const size_t s = __ldg(rowmap + row);
+            r.v[rr] = __ldg(vi + s);
+            r.b[rr][0] = __ldg(bary + 3 * s); r.b[rr][1] = __ldg(bary + 3 * s + 1); r.b[rr][2] = __ldg(bary + 3 * s + 2);
         }
     }
     return r;
@@ -197,7 +218,8 @@ __device__ __forceinline__ void layer_mma(float (&d)[64], const uint32_t (&ah)[4
     reg_fence(d);
 }
 
-template <bool FINE, int PREC>
+// MAP: the tiles run over the compact rows of p.rowmap (occupancy culling); otherwise over every row
+template <bool FINE, int PREC, bool MAP = false>
 __global__ void __launch_bounds__(MLP_THREADS, 1) k_mlp(const MlpParams p) {
     using namespace tc;
     extern __shared__ __align__(1024) uint8_t tn_mlp_smem[];
@@ -211,9 +233,10 @@ __global__ void __launch_bounds__(MLP_THREADS, 1) k_mlp(const MlpParams p) {
     const uint32_t wg = threadIdx.x >> 7, tid = threadIdx.x & 127u;
     const uint32_t warp = tid >> 5, lane = threadIdx.x & 31u, g = lane >> 2, t = lane & 3u;
     const uint32_t n_active = *p.n_active;
-    const uint64_t total_rows = (uint64_t)n_active * p.S;
+    const uint64_t total_rows = MAP ? (uint64_t)*p.n_rows : (uint64_t)n_active * p.S;
     const uint32_t ntiles = (uint32_t)((total_rows + MLP_TILE - 1) / MLP_TILE);
     if (blockIdx.x * MLP_WGS >= ntiles) return;  // (uniform over the CTA)
+    auto sample_row = [&](uint64_t row) -> uint64_t { return MAP ? (uint64_t)__ldg(p.rowmap + row) : row; };
 
     if (threadIdx.x == 0) {
         mbar_init(w_bar, 1);
@@ -255,14 +278,17 @@ __global__ void __launch_bounds__(MLP_THREADS, 1) k_mlp(const MlpParams p) {
         uint32_t ah[32], al[32];
         {
             uint32_t xh[16], xl[16];
-            gather_rows<PREC, true>(load_gather_rows(p.vi, p.bary, row0, total_rows), p.fshadow, t, xh, xl);
+            if constexpr (MAP) gather_rows<PREC, true>(load_gather_rows_mapped(p.vi, p.bary, p.rowmap, row0, total_rows), p.fshadow, t, xh, xl);
+            else gather_rows<PREC, true>(load_gather_rows(p.vi, p.bary, row0, total_rows), p.fshadow, t, xh, xl);
             // Into L1 while this tile's MMAs run: the next tile's indices, so its gather starts with the field loads, and (FINE) this
             // tile's bias rows of layer 4, read right after that layer's MMA wait.  Prefetches hold no registers: keeping the 14
             // index words of the next tile in registers instead spills k_mlp<true, 3> at its 168-register limit.
-            if (next != MLP_NO_TILE) prefetch_gather_rows(p.vi, p.bary, (uint64_t)next * MLP_TILE + lrow, total_rows);
+            // (MAP: the next tile's map entries, whose loads are the first step of its gather)
+            if constexpr (MAP) { if (next != MLP_NO_TILE && lrow == warp * 16u) prefetch_l1(p.rowmap + (uint64_t)next * MLP_TILE + lrow); }
+            else if (next != MLP_NO_TILE) prefetch_gather_rows(p.vi, p.bary, (uint64_t)next * MLP_TILE + lrow, total_rows);
             if (FINE) {
-                db0 = p.dirbias + (size_t)((uint32_t)min(row0, total_rows - 1) / p.S) * 128;
-                db1 = p.dirbias + (size_t)((uint32_t)min(row1, total_rows - 1) / p.S) * 128;
+                db0 = p.dirbias + (size_t)((uint32_t)sample_row(min(row0, total_rows - 1)) / p.S) * 128;
+                db1 = p.dirbias + (size_t)((uint32_t)sample_row(min(row1, total_rows - 1)) / p.S) * 128;
                 prefetch_l1(db0 + 32 * t);  // the four threads of a row cover its four 128-byte lines
                 prefetch_l1(db1 + 32 * t);
             }
@@ -338,13 +364,14 @@ __global__ void __launch_bounds__(MLP_THREADS, 1) k_mlp(const MlpParams p) {
             const uint64_t row = t == 0 ? row0 : row1;
             const float dn = t == 0 ? dens0 : dens1;
             if (row < total_rows) {
+                const uint64_t orow = sample_row(row);
                 const float sigma = softplus_f(dn + head_s[512]);
                 if (FINE) {
                     const float c0 = t == 0 ? col0[0] : col1[0], c1 = t == 0 ? col0[1] : col1[1], c2 = t == 0 ? col0[2] : col1[2];
-                    reinterpret_cast<float4 *>(p.out)[row] =
+                    reinterpret_cast<float4 *>(p.out)[orow] =
                         make_float4(sigma, sigmoid_f(c0 + head_s[513]), sigmoid_f(c1 + head_s[514]), sigmoid_f(c2 + head_s[515]));
                 } else {
-                    p.out[row] = sigma;
+                    p.out[orow] = sigma;
                 }
             }
         }
@@ -354,9 +381,9 @@ __global__ void __launch_bounds__(MLP_THREADS, 1) k_mlp(const MlpParams p) {
 }
 
 // launches one k_mlp pass with the shared memory of that pass
-template <bool FINE, int PREC>
+template <bool FINE, int PREC, bool MAP = false>
 inline int launch_mlp(const MlpParams &p, uint32_t grid, cudaStream_t s) {
-    auto k = k_mlp<FINE, PREC>;
+    auto k = k_mlp<FINE, PREC, MAP>;
     TN_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)mlp_smem_bytes(FINE)));
     k<<<grid, MLP_THREADS, mlp_smem_bytes(FINE), s>>>(p);
     return TN_OK;

@@ -66,6 +66,8 @@ struct MlpBwdParams {
     float *gw;                  // packed MLP gradient accumulators (zeroed by the caller), see GW_* offsets
     float *g_dirbias;           // [n_active,128] gradient at the per-ray direction bias (zeroed by the caller)
     uint32_t *tile_ctr;
+    const uint32_t *rowmap;     // MAP: compact row -> sample row of the forward's live samples (occupancy culling, DESIGN §4.12)
+    const uint32_t *n_rows;     // MAP: device count of compact rows
 };
 // deterministic mode (k_mlp_bwd<true>): gw, g_dirbias, gshadow and tile_ctr are not used
 struct MlpBwdDetParams : MlpBwdParams {
@@ -204,8 +206,11 @@ __device__ __forceinline__ void frag_pair(float x0, float x1, float y0, float y1
     tc::split_pack2(y0, y1, ah[i + 1], al[i + 1]);
 }
 
-// DX: store the dX rows to p.dx (always so in the deterministic mode)
-template <bool DET, bool DX = DET>
+// DX: store the dX rows to p.dx (always so in the deterministic mode).  MAP: the tiles run over the compact rows of p.rowmap, every
+// per-sample array (dout, vi, bary, dx) and the per-ray bias are addressed by the mapped sample row.  Rays stay contiguous and in slot
+// order in compact row space, so a (tile, slot) pair still names one direction-bias partial row in the deterministic mode: tile t
+// spans slots [a_t, b_t] with a_{t+1} >= b_t, hence t + slot is strictly increasing over the pairs and below ntiles + n_active.
+template <bool DET, bool DX = DET, bool MAP = false>
 __global__ void __launch_bounds__(BWD_THREADS, 1) k_mlp_bwd(const MlpBwdParamsT<DET, DX> p) {
     using namespace tc;
     extern __shared__ __align__(1024) uint8_t tn_bwd_smem[];
@@ -218,8 +223,9 @@ __global__ void __launch_bounds__(BWD_THREADS, 1) k_mlp_bwd(const MlpBwdParamsT<
 
     const uint32_t tid = threadIdx.x, warp = tid >> 5, lane = tid & 31u, g = lane >> 2, t = lane & 3u;
     const uint32_t n_active = *p.n_active;
-    const uint64_t total_rows = (uint64_t)n_active * p.S;
+    const uint64_t total_rows = MAP ? (uint64_t)*p.n_rows : (uint64_t)n_active * p.S;
     const uint32_t ntiles = (uint32_t)((total_rows + BWD_TILE - 1) / BWD_TILE);
+    auto sample_row = [&](uint64_t row) -> uint64_t { return MAP ? (uint64_t)__ldg(p.rowmap + row) : row; };
     uint32_t first_tile = blockIdx.x;
     if constexpr (DET) {
         if (ntiles == 0) return;
@@ -294,7 +300,7 @@ __global__ void __launch_bounds__(BWD_THREADS, 1) k_mlp_bwd(const MlpBwdParamsT<
         const uint64_t row0 = (uint64_t)tile * BWD_TILE + R0, row1 = row0 + 8u;
         const bool valid0 = row0 < total_rows, valid1 = row1 < total_rows;
         const float4 z4 = make_float4(0.f, 0.f, 0.f, 0.f);
-        const float4 g0 = valid0 ? __ldg(p.dout + row0) : z4, g1 = valid1 ? __ldg(p.dout + row1) : z4;
+        const float4 g0 = valid0 ? __ldg(p.dout + sample_row(row0)) : z4, g1 = valid1 ? __ldg(p.dout + sample_row(row1)) : z4;
 
         uint32_t ah[32], al[32];
         unsigned long long mask[3];
@@ -303,7 +309,8 @@ __global__ void __launch_bounds__(BWD_THREADS, 1) k_mlp_bwd(const MlpBwdParamsT<
         // ---------- forward layer 1; X also goes to shared memory for dW1 ----------
         {
             uint32_t xh[16], xl[16];
-            gather_rows<3>(load_gather_rows(p.vi, p.bary, row0, total_rows), p.fshadow, t, xh, xl);
+            if constexpr (MAP) gather_rows<3>(load_gather_rows_mapped(p.vi, p.bary, p.rowmap, row0, total_rows), p.fshadow, t, xh, xl);
+            else gather_rows<3>(load_gather_rows(p.vi, p.bary, row0, total_rows), p.fshadow, t, xh, xl);
 #pragma unroll
             for (int c = 0; c < 8; ++c) {
                 const int i = 4 * (c >> 1) + 2 * (c & 1);
@@ -397,7 +404,7 @@ __global__ void __launch_bounds__(BWD_THREADS, 1) k_mlp_bwd(const MlpBwdParamsT<
             wgmma_commit();
             wgmma_wait0();
             reg_fence(d);
-            const uint32_t ray0 = (uint32_t)(min(row0, total_rows - 1) / p.S), ray1 = (uint32_t)(min(row1, total_rows - 1) / p.S);
+            const uint32_t ray0 = (uint32_t)(sample_row(min(row0, total_rows - 1)) / p.S), ray1 = (uint32_t)(sample_row(min(row1, total_rows - 1)) / p.S);
             const float *db0 = p.dirbias + (size_t)ray0 * 128, *db1 = p.dirbias + (size_t)ray1 * 128;
 #pragma unroll
             for (int j = 0; j < 16; ++j) {
@@ -515,14 +522,15 @@ __global__ void __launch_bounds__(BWD_THREADS, 1) k_mlp_bwd(const MlpBwdParamsT<
             float4 q[8];  // this thread's row (row0 for even t, row1 for odd t), columns 8j + 4 (t >> 1) .. +3
 #pragma unroll
             for (int j = 0; j < 8; ++j) q[j] = quad_of_row(make_float2(dx[4 * j], dx[4 * j + 1]), make_float2(dx[4 * j + 2], dx[4 * j + 3]), t);
-            const uint64_t row = (t & 1u) ? row1 : row0;
+            const uint64_t crow = (t & 1u) ? row1 : row0;
+            const uint64_t row = crow < total_rows ? sample_row(crow) : crow;
             if constexpr (DET) {  // dX rows to HBM; the field gradient is summed per vertex in a fixed order afterwards
-                if (row < total_rows) {
+                if (crow < total_rows) {
                     float4 *dst = reinterpret_cast<float4 *>(p.dx + row * 64 + 4u * (t >> 1));
 #pragma unroll
                     for (int j = 0; j < 8; ++j) dst[2 * j] = q[j];
                 }
-            } else if (row < total_rows) {
+            } else if (crow < total_rows) {
                 if constexpr (DX) {
                     float4 *dst = reinterpret_cast<float4 *>(p.dx + row * 64 + 4u * (t >> 1));
 #pragma unroll

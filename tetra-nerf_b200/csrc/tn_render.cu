@@ -14,6 +14,7 @@
 #include <cmath>
 #include <vector>
 
+#include <cstddef>
 #include <cstdlib>
 #include <cub/cub.cuh>
 #include "tn_common.cuh"
@@ -84,6 +85,18 @@ struct RenderState {
     // dL/dx per sample of the last such backward
     DevArray<float> ray_dx;
     DevArray<float4> ray_gx;
+    // occupancy culling (tn_render_set_occupancy; DESIGN §4.12): the borrowed per-tetrahedron field and its threshold (occ == nullptr:
+    // off), the live-row flags and compact-row maps of the passes (coarse, fine, the backward's rebuilt one) and the backward's row count
+    const float *occ = nullptr;
+    float occ_thr = 0.f;
+    uint32_t occ_T = 0;                // the mesh's tetrahedron count when the occupancy was set
+    bool t_cull = false;               // the last tracer-held training forward culled
+    DevArray<uint8_t> live_flag;
+    DevArray<uint32_t> rowmap_c, rowmap_f, rowmap_b, rows_b;
+    // tn_occupancy_update: probe rows of one chunk of tetrahedra, their densities, the chunk's row count and tile counter
+    DevArray<uint4> occ_vi;
+    DevArray<float> occ_bary, occ_sig;
+    DevArray<uint32_t> occ_small;
 };
 
 void free_render(tn_tracer *h) {
@@ -185,7 +198,23 @@ struct SampleParams {
     // of the call (DESIGN §4.10)
     float *edepth;
     uint32_t *dbounds;
+    // occupancy culling: the trace's visited cells [R,M] and the per-tetrahedron occupancy (nullptr: off) with its threshold
+    const uint32_t *cells;
+    const float *occ;
+    float occ_thr;
 };
+
+// a culled sample (matched to a tetrahedron whose occupancy is below the threshold): vi = (E, E, E, TN_CULLED), weights 0.  Every
+// consumer that tests vi.x treats it as unmatched (no field gradient, no ray or vertex gradient, no normal); k_live_rows tells it from a
+// truly unmatched sample, whose density MLP(0) is still evaluated, and gives it sigma = 0 without evaluating the MLP.
+#define TN_CULLED 0xFFFFFFFEu
+__device__ __forceinline__ void cull_sample(const SampleParams &p, size_t row, uint32_t seg, uint4 &vi, float &b0, float &b1, float &b2) {
+    if (vi.x == TN_EMPTY) return;
+    if (__ldg(p.occ + __ldg(p.cells + row + seg)) < p.occ_thr) {
+        vi = make_uint4(TN_EMPTY, TN_EMPTY, TN_EMPTY, TN_CULLED);
+        b0 = b1 = b2 = 0.f;
+    }
+}
 
 // lane 0 writes the local outputs; lanes < gather_world each post the pixel to one rank's gathered buffer (three 8-byte stores)
 __device__ __forceinline__ void store_pixel(const SampleParams &p, uint32_t ray, int lane, float r, float g, float b, float a, float depth, uint8_t mask) {
@@ -225,9 +254,10 @@ __device__ __forceinline__ float linspace_f(float start, float end, uint32_t ste
 
 // find_visited_cells for one sample distance d: binary search over the staged prefix-max of t_out, then the segment's own
 // (t_in, t_out) from the trace output (L1: the warp has just read the row)
-__device__ __forceinline__ void match_sample(float d, uint32_t n, const float2 *__restrict__ dist, const float *pm, size_t row,
-                                             const uint4 *__restrict__ verts, const float *__restrict__ bary, uint4 &vi, float &b0,
-                                             float &b1, float &b2) {
+// returns the matched segment (meaningful when vi.x != E)
+__device__ __forceinline__ uint32_t match_sample(float d, uint32_t n, const float2 *__restrict__ dist, const float *pm, size_t row,
+                                                 const uint4 *__restrict__ verts, const float *__restrict__ bary, uint4 &vi, float &b0,
+                                                 float &b1, float &b2) {
     vi = make_uint4(TN_EMPTY, TN_EMPTY, TN_EMPTY, TN_EMPTY);
     b0 = b1 = b2 = 0.f;
     uint32_t lo = 0, hi = n;  // first p with pm[p] >= d  (== the reference's monotone pointer walk for sorted samples)
@@ -235,7 +265,7 @@ __device__ __forceinline__ void match_sample(float d, uint32_t n, const float2 *
         const uint32_t mid = (lo + hi) >> 1;
         if (pm[mid] < d) lo = mid + 1; else hi = mid;
     }
-    if (lo >= n) return;
+    if (lo >= n) return lo;
     const float2 h = __ldg(dist + row + lo);
     if (h.x <= d) {
         vi = __ldg(verts + row + lo);
@@ -246,6 +276,7 @@ __device__ __forceinline__ void match_sample(float d, uint32_t n, const float2 *
         b1 = __fadd_rn(__fmul_rn(omm, __ldg(c + 1)), __fmul_rn(mult, __ldg(c + 4)));
         b2 = __fadd_rn(__fmul_rn(omm, __ldg(c + 2)), __fmul_rn(mult, __ldg(c + 5)));
     }
+    return lo;
 }
 
 // shared memory per warp.  Only the prefix-max of t_out (binary-searched by every sample) is staged per segment; t_in / t_out are
@@ -328,7 +359,8 @@ __global__ void __launch_bounds__(SAMPLE_WARPS * 32) k_sample_coarse(const Sampl
     for (uint32_t j = lane; j < S; j += 32) {
         const float dmid = (e[j + 1] + e[j]) / 2.f;  // model.py:557
         uint4 vi; float b0, b1, b2;
-        match_sample(dmid, n, p.dist, pm, row, p.verts, p.bary, vi, b0, b1, b2);
+        const uint32_t seg = match_sample(dmid, n, p.dist, pm, row, p.verts, p.bary, vi, b0, b1, b2);
+        if (p.occ != nullptr) cull_sample(p, row, seg, vi, b0, b1, b2);
         const size_t g = (size_t)slot * S + j;
         p.vi_c[g] = vi;
         p.bary_c[3 * g] = b0; p.bary_c[3 * g + 1] = b1; p.bary_c[3 * g + 2] = b2;
@@ -427,7 +459,8 @@ __global__ void __launch_bounds__(SAMPLE_WARPS * 32) k_sample_fine(const SampleP
     for (uint32_t j = lane; j < S2; j += 32) {
         const float dmid = (y[j + 1] + y[j]) / 2.f;  // model.py:585
         uint4 vi; float b0, b1, b2;
-        match_sample(dmid, n, p.dist, pm, row, p.verts, p.bary, vi, b0, b1, b2);
+        const uint32_t seg = match_sample(dmid, n, p.dist, pm, row, p.verts, p.bary, vi, b0, b1, b2);
+        if (p.occ != nullptr) cull_sample(p, row, seg, vi, b0, b1, b2);
         const size_t g = (size_t)slot * S2 + j;
         p.vi_f[g] = vi;
         p.bary_f[3 * g] = b0; p.bary_f[3 * g + 1] = b1; p.bary_f[3 * g + 2] = b2;
@@ -715,10 +748,13 @@ __global__ void k_ray_flags(uint32_t R, const uint32_t *__restrict__ num, uint32
     if (i < R) flag[i] = num[i] > 0 ? 1u : 0u;
 }
 // dW and the seven column sums: the non-empty partitions in index order
-__global__ void k_det_reduce_parts(const uint32_t *__restrict__ n_active, uint32_t S, const float *__restrict__ part, float *__restrict__ gw) {
+// (n_rows != nullptr: the tiles of the compact rows of occupancy culling)
+__global__ void k_det_reduce_parts(const uint32_t *__restrict__ n_active, uint32_t S, const uint32_t *__restrict__ n_rows, const float *__restrict__ part,
+                                   float *__restrict__ gw) {
     const uint32_t e = blockIdx.x * blockDim.x + threadIdx.x;
     if (e >= BWD_PART_STRIDE) return;
-    const uint32_t ntiles = (uint32_t)(((uint64_t)*n_active * S + BWD_TILE - 1) / BWD_TILE);
+    const uint64_t rows = n_rows != nullptr ? (uint64_t)*n_rows : (uint64_t)*n_active * S;
+    const uint32_t ntiles = (uint32_t)((rows + BWD_TILE - 1) / BWD_TILE);
     float acc = 0.f;
     for (uint32_t q = 0; q < BWD_PARTS; ++q)
         if (bwd_part_lo(q, ntiles) < bwd_part_lo(q + 1, ntiles)) acc += part[(size_t)q * BWD_PART_STRIDE + e];
@@ -738,15 +774,27 @@ __global__ void __launch_bounds__(256) k_det_sum_slots(const uint32_t *__restric
     }
     if (t == 0) { out[0] = s[0].x; out[1] = s[0].y; out[2] = s[0].z; out[3] = s[0].w; }
 }
+__device__ __forceinline__ uint32_t lower_bound_u32(const uint32_t *__restrict__ a, uint32_t n, uint32_t x) {
+    uint32_t lo = 0, hi = n;
+    while (lo < hi) { const uint32_t mid = (lo + hi) >> 1; if (__ldg(a + mid) < x) lo = mid + 1; else hi = mid; }
+    return lo;
+}
 // per-ray direction-bias gradient: the partial rows of the 16-row warp blocks b that hold the ray's samples, in block order
-// (k_mlp_bwd<true> wrote block b = 4 tile + warp's partial for ray `slot` to row 4 (tile + slot) + warp)
-__global__ void __launch_bounds__(128) k_det_dirbias(const uint32_t *__restrict__ n_active, uint32_t S, const float *__restrict__ gdb_part,
-                                                     float *__restrict__ g_dirbias) {
+// (k_mlp_bwd<true> wrote block b = 4 tile + warp's partial for ray `slot` to row 4 (tile + slot) + warp).  rowmap != nullptr: the
+// ray's rows are its compact rows, found by binary search of the ascending map (none: a zero gradient)
+__global__ void __launch_bounds__(128) k_det_dirbias(const uint32_t *__restrict__ n_active, uint32_t S, const uint32_t *__restrict__ rowmap,
+                                                     const uint32_t *__restrict__ n_rows, const float *__restrict__ gdb_part, float *__restrict__ g_dirbias) {
     const uint32_t slot = blockIdx.x, k = threadIdx.x;
     if (slot >= *n_active) return;
-    const uint64_t r0 = (uint64_t)slot * S, r1 = r0 + S - 1;
+    uint64_t r0 = (uint64_t)slot * S, r1 = r0 + S;  // [r0, r1)
+    if (rowmap != nullptr) {
+        const uint32_t n = *n_rows;
+        r0 = lower_bound_u32(rowmap, n, slot * S);
+        r1 = lower_bound_u32(rowmap, n, (slot + 1) * S);
+    }
     float acc = 0.f;
-    for (uint64_t b = r0 / 16; b <= r1 / 16; ++b) acc += __ldg(gdb_part + (4 * (b / 4 + slot) + (b & 3)) * 128 + k);
+    if (r1 > r0)
+        for (uint64_t b = r0 / 16; b <= (r1 - 1) / 16; ++b) acc += __ldg(gdb_part + (4 * (b / 4 + slot) + (b & 3)) * 128 + k);
     g_dirbias[(size_t)slot * 128 + k] = acc;
 }
 // W4dir / b4: the per-block partials of k_dirbias_grads<true> in block order
@@ -773,11 +821,6 @@ __global__ void k_det_field_keys(const uint32_t *__restrict__ n_active, uint32_t
     }
     keys[e] = key;
     vals[e] = e;
-}
-__device__ __forceinline__ uint32_t lower_bound_u32(const uint32_t *__restrict__ a, uint32_t n, uint32_t x) {
-    uint32_t lo = 0, hi = n;
-    while (lo < hi) { const uint32_t mid = (lo + hi) >> 1; if (__ldg(a + mid) < x) lo = mid + 1; else hi = mid; }
-    return lo;
 }
 // step 2 (after the stable sort by vertex): one warp per vertex sums w_k dX[row] over its entries in sorted (= row) order -> [V,64]
 __global__ void __launch_bounds__(256) k_det_field_grad(uint32_t V, uint32_t n, const uint32_t *__restrict__ keys, const uint32_t *__restrict__ vals,
@@ -844,6 +887,69 @@ __global__ void __launch_bounds__(SAMPLE_WARPS * 32) k_dirbias_only(const Sample
     const uint32_t slot = blockIdx.x * SAMPLE_WARPS + warp;
     if (slot >= *p.n_active) return;
     dir_bias(p, p.ray_list[slot], slot, lane);
+}
+
+// ---- occupancy culling (DESIGN §4.12) ---------------------------------------------------------------------------------------------
+// live rows of one pass: flag[g] = 1 for every sample row g < n_active * S that is not culled (matched to an occupied tetrahedron, or
+// unmatched), 0 for culled rows and rows past the active ones.  outw 1 / 4: a culled row's output (density, or sigma and colour) is
+// set to 0 here, since k_mlp skips it; outw 0: flags only (the backward's rebuild of its forward's map).
+__global__ void k_live_rows(const uint32_t *__restrict__ n_active, uint32_t S, uint64_t n, const uint4 *__restrict__ vi, uint32_t outw,
+                            uint8_t *__restrict__ flag, float *__restrict__ out) {
+    const uint64_t g = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (g >= n) return;
+    uint8_t live = 0;
+    if (g < (uint64_t)*n_active * S) {
+        const uint4 v = __ldg(vi + g);
+        live = (v.x == TN_EMPTY && v.w == TN_CULLED) ? 0 : 1;
+        if (!live && outw == 1) out[g] = 0.f;
+        if (!live && outw == 4) reinterpret_cast<float4 *>(out)[g] = make_float4(0.f, 0.f, 0.f, 0.f);
+    }
+    flag[g] = live;
+}
+
+// compact-row map of one pass: map[c] = the c-th live sample row in row order (so each ray's live rows stay contiguous, in slot order),
+// *n_rows = their number; all on the device
+static int compact_rows(tn_tracer *h, RenderState *r, const uint32_t *n_active, uint32_t S, size_t R, const uint4 *vi, float *out, uint32_t outw,
+                        DevArray<uint32_t> &map, uint32_t *n_rows, cudaStream_t s) {
+    const size_t n = R * S;
+    TN_TRY(r->live_flag.grow(n)); TN_TRY(map.grow(n));
+    size_t bytes = 0;
+    cub::CountingInputIterator<uint32_t> it(0u);
+    TN_CUDA(cub::DeviceSelect::Flagged(nullptr, bytes, it, r->live_flag.p, map.p, n_rows, (int64_t)n, s));
+    TN_TRY(r->cub_tmp.grow(bytes));
+    k_live_rows<<<(uint32_t)((n + 255) / 256), 256, 0, s>>>(n_active, S, n, vi, outw, r->live_flag.p, out);
+    TN_CUDA(cub::DeviceSelect::Flagged(r->cub_tmp.p, bytes, it, r->live_flag.p, map.p, n_rows, (int64_t)n, s));
+    h->launches += 2;
+    return TN_OK;
+}
+
+// ---- tn_occupancy_update: 11 probes per tetrahedron (4 vertices, 6 edge midpoints, centroid), as barycentric weights of the cell's
+// vertices 1..3 (vertex 0 gets 1 - b0 - b1 - b2, as the interpolation forms it); every weight is exact in float
+__constant__ float c_probe[11][3] = {{0.f, 0.f, 0.f},    {1.f, 0.f, 0.f},    {0.f, 1.f, 0.f},     {0.f, 0.f, 1.f},
+                                     {0.5f, 0.f, 0.f},   {0.f, 0.5f, 0.f},   {0.f, 0.f, 0.5f},    {0.5f, 0.5f, 0.f},
+                                     {0.5f, 0.f, 0.5f},  {0.f, 0.5f, 0.5f},  {0.25f, 0.25f, 0.25f}};
+constexpr uint32_t OCC_PROBES = 11;
+constexpr uint32_t OCC_CHUNK = 1u << 19;  // tetrahedra per k_mlp launch (5.8 M probe rows, 176 MB of rows and densities)
+
+// probe rows of tetrahedra t0 .. t0 + nt - 1 (vi = the cell, one row per probe); count[0] = nt (k_mlp's "rays" of S = 11), count[1] = 0
+// (its tile counter)
+__global__ void k_occ_rows(uint32_t t0, uint32_t nt, const uint32_t *__restrict__ cells, uint4 *__restrict__ vi, float *__restrict__ bary,
+                           uint32_t *__restrict__ count) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i == 0) { count[0] = nt; count[1] = 0; }
+    if (i >= nt * OCC_PROBES) return;
+    const uint32_t t = t0 + i / OCC_PROBES, k = i % OCC_PROBES;
+    vi[i] = __ldg(reinterpret_cast<const uint4 *>(cells) + t);
+    bary[3 * (size_t)i] = c_probe[k][0]; bary[3 * (size_t)i + 1] = c_probe[k][1]; bary[3 * (size_t)i + 2] = c_probe[k][2];
+}
+// one thread per tetrahedron, no atomics: occ = max(decay occ, max of the probe densities); decay 0 replaces it
+__global__ void k_occ_reduce(uint32_t t0, uint32_t nt, const float *__restrict__ sig, float decay, float *__restrict__ occ) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= nt) return;
+    float m = sig[(size_t)i * OCC_PROBES];
+#pragma unroll
+    for (uint32_t k = 1; k < OCC_PROBES; ++k) m = fmaxf(m, sig[(size_t)i * OCC_PROBES + k]);
+    occ[t0 + i] = decay == 0.f ? m : fmaxf(decay * occ[t0 + i], m);
 }
 
 static int ensure_ws(RenderState *r, size_t R, size_t M, size_t Sc, size_t S2) {
@@ -950,7 +1056,8 @@ extern "C" int tn_render_set_weights(tn_tracer *h, const float *const *P, void *
 // caller's saved-state blob (tn_render_train_forward_saved)
 struct TrainBufs {
     uint32_t *n_active;        // 16-byte block: active rays | tile counter of the coarse pass | of the fine pass | (unused); then words
-                               // 4, 5: the clip bounds of the expected depth (in the slot the saved state reserves for the block)
+                               // 4, 5: the clip bounds of the expected depth, 6, 7: the live rows of the coarse / fine pass when the
+                               // forward culled (in the slot the saved state reserves for the block)
     uint32_t *ray_list;        // [R] slot -> ray
     float *ebins_f, *sbins_f;  // [R,S2+1] euclidean / spacing bins of the fine pass
     uint4 *vi_f;               // [R*S2] matched vertices
@@ -971,6 +1078,9 @@ struct SavedHeader {
     uint32_t pad2;
     uint64_t gen;              // RenderState::gen at the forward
     uint64_t mesh_gen;         // tn_tracer::mesh_gen at the forward (the ray gradients read the mesh positions)
+    uint32_t cull;             // 1: the forward culled samples by occupancy (its culled rows are marked in vi_f, DESIGN §4.12)
+    uint32_t live_c, live_f;   // culling: the live rows of its coarse / fine pass (copied on the device from the n_active slot)
+    uint32_t pad3;
 };
 constexpr size_t SAVED_ALIGN = 256;
 static_assert(sizeof(SavedHeader) <= SAVED_ALIGN, "saved-state header exceeds its slot");
@@ -979,7 +1089,7 @@ static size_t saved_layout(size_t R, size_t S2, uint8_t *base, TrainBufs *b) {
     size_t off = SAVED_ALIGN;  // header
     auto take = [&](size_t bytes) { uint8_t *p = base ? base + off : nullptr; off += (bytes + SAVED_ALIGN - 1) / SAVED_ALIGN * SAVED_ALIGN; return p; };
     TrainBufs t{};
-    t.n_active = (uint32_t *)take(24);  // (one 256-byte slot either way)
+    t.n_active = (uint32_t *)take(32);  // (one 256-byte slot either way)
     t.ray_list = (uint32_t *)take(4 * R);
     t.ebins_f = (float *)take(4 * R * (S2 + 1));
     t.sbins_f = (float *)take(4 * R * (S2 + 1));
@@ -1019,6 +1129,9 @@ static int render_impl(tn_tracer *h, const tn_render_config *cfg, const float *d
     if (R == 0) return TN_OK;
     if ((uint64_t)R * (uint64_t)(Sc + Sf + 1) >= (1ull << 32)) return fail(TN_ERR_ARG, "tn_render: rays x samples must stay below 2^32 per call (split the batch)");
     const bool single = Sf == 0;                       // one pass only: the colours come from the coarse samples
+    const bool cull = r->occ != nullptr;               // occupancy culling (DESIGN §4.12)
+    if (cull && r->occ_T != h->mesh.T)
+        return fail(TN_ERR_STATE, "tn_render: the occupancy was set for a mesh with another number of tetrahedra (tn_render_set_occupancy)");
     const uint32_t S2 = single ? Sc : Sc + Sf + 1;     // PDFSampler include_original (model.py:463)
     DeviceGuard g(h->device);
     cudaStream_t s = (cudaStream_t)stream;
@@ -1072,6 +1185,7 @@ static int render_impl(tn_tracer *h, const tn_render_config *cfg, const float *d
     p.far_plane = cfg->far_plane; p.bg0 = cfg->background[0]; p.bg1 = cfg->background[1]; p.bg2 = cfg->background[2];
     if (tf != nullptr) { p.train = 1; p.jit_c = tf->jit_c; p.jit_f = tf->jit_f; p.sbins_f = b.sbins_f; p.enc = b.enc; }
     p.edepth = d_edepth; p.dbounds = b.n_active + 4;
+    if (cull) { p.cells = r->cells.p; p.occ = r->occ; p.occ_thr = r->occ_thr; }
     if (r->gather_world) {
         if (R > r->gather_stride) return fail(TN_ERR_ARG, "tn_render: more rays than the gathered-pixel buffers were sized for (tn_render_set_gather)");
         for (int k = 0; k < 8; ++k) p.peer[k] = r->peer[k];
@@ -1083,8 +1197,8 @@ static int render_impl(tn_tracer *h, const tn_render_config *cfg, const float *d
     if (!single) TN_CUDA(cudaFuncSetAttribute(k_sample_fine, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_sf));
     auto k_comp = d_edepth != nullptr ? k_composite<true> : k_composite<false>;
     TN_CUDA(cudaFuncSetAttribute(k_comp, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_c));
-    auto launch_coarse = prec == 2 ? launch_mlp<false, 2> : launch_mlp<false, 3>;
-    auto launch_fine = prec == 2 ? launch_mlp<true, 2> : launch_mlp<true, 3>;
+    auto launch_coarse = cull ? (prec == 2 ? launch_mlp<false, 2, true> : launch_mlp<false, 3, true>) : (prec == 2 ? launch_mlp<false, 2> : launch_mlp<false, 3>);
+    auto launch_fine = cull ? (prec == 2 ? launch_mlp<true, 2, true> : launch_mlp<true, 3, true>) : (prec == 2 ? launch_mlp<true, 2> : launch_mlp<true, 3>);
     const uint32_t gridR = (R + SAMPLE_WARPS - 1) / SAMPLE_WARPS;
 
     if (det) {
@@ -1106,6 +1220,10 @@ static int render_impl(tn_tracer *h, const tn_render_config *cfg, const float *d
     const uint32_t grid_c = (uint32_t)std::min<uint64_t>((tiles_c + MLP_WGS - 1) / MLP_WGS, (uint64_t)sms);
     const uint32_t grid_f = (uint32_t)std::min<uint64_t>((tiles_f + MLP_WGS - 1) / MLP_WGS, (uint64_t)sms);
     if (!single) {
+        if (cull) {  // the coarse pass's MLP runs on its live rows only; culled rows get density 0
+            TN_TRY(compact_rows(h, r, b.n_active, Sc, R, r->vi_c.p, r->dens_c.p, 1, r->rowmap_c, b.n_active + 6, s));
+            mc.rowmap = r->rowmap_c.p; mc.n_rows = b.n_active + 6;
+        }
         rc = launch_coarse(mc, grid_c, s);
         if (rc) return rc;
     }
@@ -1118,6 +1236,10 @@ static int render_impl(tn_tracer *h, const tn_render_config *cfg, const float *d
     if (!single) { mf.vi = b.vi_f; mf.bary = b.bary_f; }
     else p.ebins_f = r->ebins_c.p;  // k_composite integrates over the coarse bins
     mf.tile_ctr = b.n_active + 2;
+    if (cull) {  // the same for the pass that gives the colours: culled rows get (sigma, r, g, b) = 0
+        TN_TRY(compact_rows(h, r, b.n_active, S2, R, mf.vi, b.out_f, 4, r->rowmap_f, b.n_active + 7, s));
+        mf.rowmap = r->rowmap_f.p; mf.n_rows = b.n_active + 7;
+    }
     rc = launch_fine(mf, grid_f, s);
     if (rc) return rc;
     TN_EV(5);
@@ -1144,6 +1266,7 @@ static int render_impl(tn_tracer *h, const tn_render_config *cfg, const float *d
     if (tf != nullptr && tf->saved == nullptr) {
         r->train_valid = true;
         r->t_det = det;
+        r->t_cull = cull;
         r->t_R = R; r->t_M = M; r->t_Sc = Sc; r->t_Sf = Sf; r->t_S2 = S2;
         r->t_bg[0] = cfg->background[0]; r->t_bg[1] = cfg->background[1]; r->t_bg[2] = cfg->background[2];
     }
@@ -1176,7 +1299,9 @@ extern "C" int tn_render_train_forward(tn_tracer *h, const tn_render_config *cfg
 // d_grad_dist != nullptr: dL/d distortion f32[R] (k_distortion).
 // Any of d_grad_o / d_grad_d / d_grad_xyz != nullptr: also the gradients at the ray origins / directions (tn_ray_grads.cu) and at the
 // mesh vertex positions (tn_vertex_grads.cu), into the non-null ones.
-static int train_backward_impl(tn_tracer *h, const TrainBufs &b, uint32_t R, uint32_t S2, bool det, const float *bg, const float *d_grad_rgb,
+// cull: the forward culled by occupancy; its map of live fine rows is rebuilt from the culled marks in b.vi_f (never from the occupancy,
+// which may have changed since)
+static int train_backward_impl(tn_tracer *h, const TrainBufs &b, uint32_t R, uint32_t S2, bool det, bool cull, const float *bg, const float *d_grad_rgb,
                                const float *d_grad_acc, const float *d_grad_ed, const float *d_grad_dist, int use_gradient_scaling, float *d_grad_field,
                                float *const *d_grad_params12, float *d_grad_o, float *d_grad_d, float *d_grad_xyz, cudaStream_t s) {
     RenderState *r = h->render;
@@ -1217,18 +1342,25 @@ static int train_backward_impl(tn_tracer *h, const TrainBufs &b, uint32_t R, uin
     bp.n_active = b.n_active; bp.S = S2; bp.vi = b.vi_f; bp.bary = b.bary_f; bp.fshadow = r->fshadow.p; bp.wimg = r->wimg_bwd.p;
     bp.bias = r->bias.p; bp.head = r->head.p; bp.dirbias = b.dirbias; bp.dout = r->dout.p; bp.gshadow = r->gshadow.p;
     bp.gw = r->gw.p; bp.g_dirbias = r->g_dirbias.p; bp.tile_ctr = r->n_active.p + 3;
+    if (cull) {
+        TN_TRY(r->rows_b.grow(1));
+        TN_TRY(compact_rows(h, r, b.n_active, S2, R, b.vi_f, nullptr, 0, r->rowmap_b, r->rows_b.p, s));
+        bp.rowmap = r->rowmap_b.p; bp.n_rows = r->rows_b.p;
+    }
     const uint64_t tiles = ((uint64_t)R * S2 + BWD_TILE - 1) / BWD_TILE;
     if (!det) {
         const uint32_t grid = r->bwd_grid ? r->bwd_grid : (uint32_t)std::min<uint64_t>(tiles, (uint64_t)sms);
         if (!rays) {
-            TN_CUDA(cudaFuncSetAttribute(k_mlp_bwd<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)BWD_SMEM_BYTES));
-            k_mlp_bwd<false><<<grid, BWD_THREADS, BWD_SMEM_BYTES, s>>>(bp);
+            auto k = cull ? k_mlp_bwd<false, false, true> : k_mlp_bwd<false>;
+            TN_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)BWD_SMEM_BYTES));
+            k<<<grid, BWD_THREADS, BWD_SMEM_BYTES, s>>>(bp);
         } else {  // the same backward, storing the dX rows for k_ray_grads as well
             MlpBwdDxParams xp{};
             static_cast<MlpBwdParams &>(xp) = bp;
             xp.dx = r->ray_dx.p;
-            TN_CUDA(cudaFuncSetAttribute(k_mlp_bwd<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)BWD_SMEM_BYTES));
-            k_mlp_bwd<false, true><<<grid, BWD_THREADS, BWD_SMEM_BYTES, s>>>(xp);
+            auto k = cull ? k_mlp_bwd<false, true, true> : k_mlp_bwd<false, true>;
+            TN_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)BWD_SMEM_BYTES));
+            k<<<grid, BWD_THREADS, BWD_SMEM_BYTES, s>>>(xp);
         }
         if (r->profile) cudaEventRecord(r->evb[2], s);
         k_dirbias_grads<false><<<(R + DBG_SLOTS - 1) / DBG_SLOTS, 256, 0, s>>>(b.n_active, r->g_dirbias.p, b.enc, r->gw.p, nullptr);
@@ -1238,13 +1370,14 @@ static int train_backward_impl(tn_tracer *h, const TrainBufs &b, uint32_t R, uin
         MlpBwdDetParams dp{};
         static_cast<MlpBwdParams &>(dp) = bp;
         dp.part = r->det_part.p; dp.gdb_part = r->det_gdb.p; dp.dx = r->det_dx.p;
-        TN_CUDA(cudaFuncSetAttribute(k_mlp_bwd<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)BWD_DET_SMEM_BYTES));
+        auto kd = cull ? k_mlp_bwd<true, true, true> : k_mlp_bwd<true>;
+        TN_CUDA(cudaFuncSetAttribute(kd, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)BWD_DET_SMEM_BYTES));
         const uint32_t grid = r->bwd_grid ? r->bwd_grid : std::min<uint32_t>(BWD_PARTS, (uint32_t)sms);
-        k_mlp_bwd<true><<<grid, BWD_THREADS, BWD_DET_SMEM_BYTES, s>>>(dp);
+        kd<<<grid, BWD_THREADS, BWD_DET_SMEM_BYTES, s>>>(dp);
         if (r->profile) cudaEventRecord(r->evb[2], s);
-        k_det_reduce_parts<<<(BWD_PART_STRIDE + 255) / 256, 256, 0, s>>>(b.n_active, S2, r->det_part.p, r->gw.p);
+        k_det_reduce_parts<<<(BWD_PART_STRIDE + 255) / 256, 256, 0, s>>>(b.n_active, S2, bp.n_rows, r->det_part.p, r->gw.p);
         k_det_sum_slots<<<1, 256, 0, s>>>(b.n_active, r->det_sums.p, r->gw.p + GW_SUMS);
-        k_det_dirbias<<<R, 128, 0, s>>>(b.n_active, S2, r->det_gdb.p, r->g_dirbias.p);
+        k_det_dirbias<<<R, 128, 0, s>>>(b.n_active, S2, bp.rowmap, bp.n_rows, r->det_gdb.p, r->g_dirbias.p);
         k_dirbias_grads<true><<<(R + DBG_SLOTS - 1) / DBG_SLOTS, 256, 0, s>>>(b.n_active, r->g_dirbias.p, b.enc, r->gw.p, r->det_dbg.p);
         k_det_reduce_dbg<<<(DBG_PART + 255) / 256, 256, 0, s>>>(b.n_active, r->det_dbg.p, r->gw.p);
         // field gradient: stable sort of (vertex, row * 4 + k) by vertex, then per-vertex sums in row order
@@ -1299,7 +1432,7 @@ extern "C" int tn_render_train_backward(tn_tracer *h, const float *d_grad_rgb, c
     RenderState *r = h->render;
     if (!r || !r->train_valid) return fail(TN_ERR_STATE, "tn_render_train_backward: no training forward to continue from");
     DeviceGuard g(h->device);
-    return train_backward_impl(h, own_bufs(r), r->t_R, r->t_S2, r->t_det, r->t_bg, d_grad_rgb, d_grad_acc, nullptr, nullptr, use_gradient_scaling,
+    return train_backward_impl(h, own_bufs(r), r->t_R, r->t_S2, r->t_det, r->t_cull, r->t_bg, d_grad_rgb, d_grad_acc, nullptr, nullptr, use_gradient_scaling,
                                d_grad_field, d_grad_params12, nullptr, nullptr, nullptr, (cudaStream_t)stream);
 }
 
@@ -1340,12 +1473,15 @@ extern "C" int tn_render_train_forward_saved(tn_tracer *h, const tn_render_confi
     rc = render_impl(h, cfg, d_origins, d_directions, R, d_rgb, d_acc, d_depth, d_mask, &tf, nullptr, d_expected_depth, stream);
     if (rc) return rc;
     RenderState *r = h->render;
+    const bool cull = r->occ != nullptr;
     const SavedHeader hd{SAVED_MAGIC, R, cfg->max_ray_triangles, cfg->num_samples, cfg->num_fine_samples, S2, r->det ? 1u : 0u,
                          d_expected_depth != nullptr ? 1u : 0u, {cfg->background[0], cfg->background[1], cfg->background[2]}, 0, r->gen,
-                         h->mesh_gen};
+                         h->mesh_gen, cull ? 1u : 0u, 0, 0, 0};
     DeviceGuard g(h->device);
     // pageable source: staged before the call returns, so `hd` may go out of scope
     TN_CUDA(cudaMemcpyAsync(d_saved, &hd, sizeof(hd), cudaMemcpyHostToDevice, (cudaStream_t)stream));
+    if (cull)  // the live-row counts, from words 6, 7 of the forward's n_active slot
+        TN_CUDA(cudaMemcpyAsync((uint8_t *)d_saved + offsetof(SavedHeader, live_c), b.n_active + 6, 8, cudaMemcpyDeviceToDevice, (cudaStream_t)stream));
     return TN_OK;
 }
 
@@ -1385,7 +1521,7 @@ extern "C" int tn_render_train_backward_saved2(tn_tracer *h, const void *d_saved
                                   "tn_render_train_forward_saved)");
     TrainBufs b{};
     saved_layout(hd.R, hd.S2, (uint8_t *)d_saved, &b);
-    return train_backward_impl(h, b, hd.R, hd.S2, hd.det != 0, hd.bg, d_grad_rgb, d_grad_acc, d_grad_expected_depth, d_grad_distortion,
+    return train_backward_impl(h, b, hd.R, hd.S2, hd.det != 0, hd.cull != 0, hd.bg, d_grad_rgb, d_grad_acc, d_grad_expected_depth, d_grad_distortion,
                                use_gradient_scaling, d_grad_field, d_grad_params12, d_grad_origins, d_grad_directions, d_grad_xyz, s);
 }
 
@@ -1422,6 +1558,55 @@ extern "C" int tn_render_set_deterministic(tn_tracer *h, int enable) {
     if (!h) return fail(TN_ERR_ARG, "null tracer");
     DeviceGuard g(h->device);
     state(h)->det = enable != 0;
+    return TN_OK;
+}
+
+// occupancy culling (see the header; DESIGN §4.12): borrowed f32[T]; NULL switches it off
+extern "C" int tn_render_set_occupancy(tn_tracer *h, const float *d_occ, float threshold) {
+    if (!h) return fail(TN_ERR_ARG, "null tracer");
+    if (!std::isfinite(threshold) || threshold < 0.f)
+        return fail(TN_ERR_ARG, "tn_render_set_occupancy: the threshold must be finite and >= 0");
+    DeviceGuard g(h->device);
+    RenderState *r = state(h);
+    r->occ = d_occ;
+    r->occ_thr = threshold;
+    r->occ_T = h->mesh.T;
+    return TN_OK;
+}
+
+// d_occ f32[T] <- max(decay * d_occ, the largest probe density of each tetrahedron): probe rows in chunks of OCC_CHUNK tetrahedra
+// through k_mlp<false, 3> (the density the renderer uses, bf16x3), then one thread per tetrahedron
+extern "C" int tn_occupancy_update(tn_tracer *h, float *d_occ, float decay, void *stream) {
+    if (!h || !d_occ) return fail(TN_ERR_ARG, "null argument");
+    if (!std::isfinite(decay) || decay < 0.f) return fail(TN_ERR_ARG, "tn_occupancy_update: the decay must be finite and >= 0");
+    if (!h->mesh.nodes.p) return fail(TN_ERR_STATE, "tn_occupancy_update: no tetrahedra loaded");
+    RenderInputs in{};
+    if (render_inputs(h, &in) != TN_OK) return fail(TN_ERR_STATE, "tn_occupancy_update: call tn_render_set_field and tn_render_set_weights first");
+    if (in.V != h->mesh.V) return fail(TN_ERR_ARG, "tn_occupancy_update: field has a different vertex count than the mesh");
+    DeviceGuard g(h->device);
+    cudaStream_t s = (cudaStream_t)stream;
+    RenderState *r = h->render;
+    const uint32_t T = h->mesh.T;
+    const uint32_t chunk = std::min(T, OCC_CHUNK);
+    if (chunk == 0) return TN_OK;
+    const size_t rows = (size_t)chunk * OCC_PROBES;
+    TN_TRY(r->occ_vi.grow(rows)); TN_TRY(r->occ_bary.grow(3 * rows)); TN_TRY(r->occ_sig.grow(rows)); TN_TRY(r->occ_small.grow(2));
+    int sms = 132;
+    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, h->device);
+    for (uint32_t t0 = 0; t0 < T; t0 += chunk) {
+        const uint32_t nt = std::min(chunk, T - t0);
+        const uint64_t n = (uint64_t)nt * OCC_PROBES;
+        k_occ_rows<<<(uint32_t)((n + 255) / 256), 256, 0, s>>>(t0, nt, h->mesh.cells, r->occ_vi.p, r->occ_bary.p, r->occ_small.p);
+        MlpParams mp{};
+        mp.n_active = r->occ_small.p; mp.S = OCC_PROBES; mp.vi = r->occ_vi.p; mp.bary = r->occ_bary.p; mp.fshadow = in.fshadow;
+        mp.wimg = in.wimg; mp.bias = in.bias; mp.head = in.head; mp.out = r->occ_sig.p; mp.tile_ctr = r->occ_small.p + 1;
+        const uint64_t tiles = (n + MLP_TILE - 1) / MLP_TILE;
+        const uint32_t grid = (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>((tiles + MLP_WGS - 1) / MLP_WGS, (uint64_t)sms));
+        TN_TRY(launch_mlp<false, 3>(mp, grid, s));
+        k_occ_reduce<<<(nt + 255) / 256, 256, 0, s>>>(t0, nt, r->occ_sig.p, decay, d_occ);
+        h->launches += 3;
+    }
+    TN_CUDA(cudaGetLastError());
     return TN_OK;
 }
 

@@ -234,6 +234,28 @@ class FusedRenderer:
         ext._check(_lib.tn_render_train_distortion(self.tracer.handle, state.blob.data_ptr(), out.data_ptr(), self._stream()))
         return out
 
+    # ---- occupancy culling (DESIGN §4.12) -------------------------------------------------------------------------------------------
+    def _check_occupancy(self, occ: torch.Tensor) -> None:
+        T = self.tracer._cells.numel() // 4 if self.tracer._cells is not None else 0
+        if occ.device != self.device or occ.dtype != torch.float32 or not occ.is_contiguous() or tuple(occ.shape) != (T,):
+            raise RuntimeError(f"the occupancy must be a contiguous float32 [{T}] tensor (one entry per tetrahedron) on the tracer's device")
+
+    def set_occupancy(self, occ: Optional[torch.Tensor], threshold: float = 0.0) -> None:
+        """cull, in every later render and training forward, the samples matched to a tetrahedron t with occ[t] < threshold: their
+        density is the constant 0 and their MLP is not evaluated (unmatched samples are evaluated as before).  occ f32[T] is borrowed
+        (kept alive here); None switches culling off.  A saved training forward's backward does not read occ again."""
+        if occ is not None:
+            self._check_occupancy(occ)
+        ext._check(_lib.tn_render_set_occupancy(self.tracer.handle, _ptr(occ), C.c_float(float(threshold))))
+        self._occ = occ
+
+    def update_occupancy(self, occ: torch.Tensor, decay: float = 0.0) -> torch.Tensor:
+        """occ f32[T] <- max(decay * occ, the largest density over the 4 vertices, 6 edge midpoints and centroid of each tetrahedron),
+        in place, with the current field and weights (decay 0: recomputed; bitwise reproducible) -> occ"""
+        self._check_occupancy(occ)
+        ext._check(_lib.tn_occupancy_update(self.tracer.handle, occ.data_ptr(), C.c_float(float(decay)), self._stream()))
+        return occ
+
     # ---- surface extraction ---------------------------------------------------------------------------------------------------------
     def extract_surface(self, level: float) -> Dict[str, torch.Tensor]:
         """the density iso-surface sigma = level (finite, > 0) of the current field and weights, by marching tetrahedra on the tracer's

@@ -14,8 +14,9 @@ the work happens:
 
 Evaluation images / metrics (`get_image_metrics_and_images`, reference :676-713) are provided with PSNR and SSIM computed in torch
 (torchmetrics / LPIPS are used when nerfstudio and its dependencies are installed); appearance embeddings (reference :440-446,
-608-620) run on the unfused path.  Out of scope and absent: the unused occupancy field (:98,256-265).  nerfstudio itself is imported when it is
-installed; otherwise the minimal look-alikes of `_ns_compat` are used.
+608-620) run on the unfused path.  The occupancy field the reference declares but never reads (:98,256-265) culls empty tetrahedra on the
+fused paths here (DESIGN §4.12).  nerfstudio itself is imported when it is installed; otherwise the minimal look-alikes of `_ns_compat`
+are used.
 """
 from __future__ import annotations
 
@@ -73,6 +74,18 @@ class TetrahedraNerfConfig(ModelConfig):
     background_color: Literal["random", "last_sample", "black", "white"] = "white"
     appearance_embed_dim: int = 0
     use_occupancy_field: bool = False
+    """register the reference's `tetrahedra_occupancy` f32[T] buffer and cull, on the fused render and training paths, the samples that
+    fall in a tetrahedron whose occupancy (the largest density over its vertices, edge midpoints and centroid) is below
+    occupancy_threshold: their density is 0 and their MLP is skipped (DESIGN §4.12).  Needs the fused pipeline (RuntimeError otherwise)"""
+    occupancy_threshold: float = 0.01
+    """density below which a tetrahedron is culled: a culled cell removes at most 1 - exp(-0.01 l) of opacity over a chord of length l"""
+    occupancy_update_interval: int = 16
+    """training steps between two occupancy updates (the first one at occupancy_warmup_steps)"""
+    occupancy_decay: float = 0.95
+    """an update sets occupancy = max(occupancy_decay * occupancy, the new probe maximum), so a cell that empties out is culled after a
+    few updates rather than at once"""
+    occupancy_warmup_steps: int = 256
+    """training steps without culling at the start, so the randomly initialised field is not culled away"""
     render_normals: bool = False
     """eval renders also return "normals" f32[R,3], the composited normal of the density field (fused path only; training ignores it)"""
     optimize_vertices: bool = False
@@ -201,6 +214,7 @@ class TetrahedraNerf(Model):
             self._register_vertices(torch.empty((V, 3), dtype=torch.float32))
             self.register_buffer("tetrahedra_cells", torch.empty((T, 4), dtype=torch.int32))
             self.register_parameter("tetrahedra_field", nn.Parameter(torch.empty((self.config.field_dim, V), dtype=torch.float32)))
+            self._register_occupancy(T)
             self._tetrahedra_initialized = False
 
     # ---- initialisation (reference :268-392) --------------------------------------------------------
@@ -208,8 +222,17 @@ class TetrahedraNerf(Model):
     def _init_tetrahedra_field(tetrahedra_field):
         tetrahedra_field.uniform_(-1e-4, 1e-4)
 
+    def _register_occupancy(self, T: int):
+        """`tetrahedra_occupancy` f32[T] of zeros (the reference's key, shape and dtype, model.py:256-265), with use_occupancy_field.  All
+        zeros means "never computed": it is recomputed before its first use"""
+        self._occ_ready = False
+        self._occ_step = 0
+        if self.config.use_occupancy_field:
+            self.register_buffer("tetrahedra_occupancy", torch.zeros((T,), dtype=torch.float32))
+
     def _load_from_state_dict(self, state_dict, prefix, *args, **kwargs):
         complete = all(f"{prefix}{k}" in state_dict for k in ("tetrahedra_vertices", "tetrahedra_cells", "tetrahedra_field"))
+        self._occ_ready = False  # a loaded buffer is checked for zeros again
         super()._load_from_state_dict(state_dict, prefix, *args, **kwargs)
         if complete:
             self._tetrahedra_initialized = True
@@ -228,10 +251,14 @@ class TetrahedraNerf(Model):
             with torch.no_grad():
                 self.tetrahedra_vertices.copy_(vertices.to(self.tetrahedra_vertices.device))
             self.tetrahedra_cells.copy_(cells.to(torch.int32).to(self.tetrahedra_cells.device))
+            if self.config.use_occupancy_field:
+                self.tetrahedra_occupancy.zero_()
+                self._occ_ready = False
         else:
             self._register_vertices(vertices.float())
             self.register_buffer("tetrahedra_cells", cells.to(torch.int32))
             self.register_parameter("tetrahedra_field", nn.Parameter(torch.empty((self.config.field_dim, V), dtype=torch.float32)))
+            self._register_occupancy(len(cells))
         self._init_tetrahedra_field(self.tetrahedra_field.data)
         if self.config.initialize_colors:
             assert colors is not None and colors.dtype == torch.uint8
@@ -353,6 +380,31 @@ class TetrahedraNerf(Model):
             self._fused_versions = versions
         return self._fused
 
+    def _apply_occupancy(self, fr, training: bool) -> None:
+        """sets (or clears) the culling of the fused renderer `fr` for the next call.  Training: no culling before
+        occupancy_warmup_steps, then an update every occupancy_update_interval steps, at the start of the step (so after the previous
+        optimizer step, as the vertex refit).  A buffer that was never computed (all zeros) is recomputed with decay 0 first."""
+        c = self.config
+        if not c.use_occupancy_field:
+            fr.set_occupancy(None)
+            return
+        occ = self.tetrahedra_occupancy
+        step = self._occ_step
+        if training:
+            self._occ_step += 1
+            if step < c.occupancy_warmup_steps:
+                fr.set_occupancy(None)
+                return
+        fresh = False
+        if not self._occ_ready:
+            if not bool(occ.any()):
+                fr.update_occupancy(occ, 0.0)
+                fresh = True
+            self._occ_ready = True
+        if training and not fresh and (step - c.occupancy_warmup_steps) % max(1, c.occupancy_update_interval) == 0:
+            fr.update_occupancy(occ, c.occupancy_decay)
+        fr.set_occupancy(occ, c.occupancy_threshold)
+
     # ---- forward (reference :520-662) ---------------------------------------------------------------------
     def _expected_depth_on(self) -> bool:
         return self.config.render_expected_depth or self.config.depth_loss_mult > 0
@@ -374,6 +426,8 @@ class TetrahedraNerf(Model):
         assert self.collider is not None
         origins, directions = ray_bundle.origins.contiguous(), ray_bundle.directions.contiguous()
         normals = self.config.render_normals and not self.training
+        if self.config.use_occupancy_field and self._fused_unsupported():
+            raise RuntimeError(f"use_occupancy_field culls on the fused CUDA pipeline, which does not support {', '.join(self._fused_unsupported())}")
         if normals and self._fused_unsupported():
             raise RuntimeError(f"render_normals runs on the fused CUDA pipeline, which does not support {', '.join(self._fused_unsupported())}")
         if normals or (not self.training and not torch.is_grad_enabled() and self._fused_supported()):
@@ -383,7 +437,9 @@ class TetrahedraNerf(Model):
             st = RenderSettings(self.config.max_intersected_triangles, self.config.num_samples, self.config.num_fine_samples,
                                 self.config.use_biased_sampler, float(self.collider.far_plane), bg)
             with torch.no_grad():
-                return self._fused_renderer().render(origins, directions, st, normals=normals, expected_depth=self._expected_depth_on())
+                fr = self._fused_renderer()
+                self._apply_occupancy(fr, training=False)
+                return fr.render(origins, directions, st, normals=normals, expected_depth=self._expected_depth_on())
         unfused_train = os.environ.get("TETRANERF_B200_UNFUSED_TRAIN", "0") == "1"
         if self.training and torch.is_grad_enabled() and self.config.optimize_vertices:
             causes = self._fused_unsupported() + (["num_fine_samples=0"] if self.config.num_fine_samples == 0 else []) \
@@ -403,6 +459,8 @@ class TetrahedraNerf(Model):
         bg = (1.0, 1.0, 1.0) if c.background_color == "white" else (0.0, 0.0, 0.0)
         st = RenderSettings(c.max_intersected_triangles, c.num_samples, c.num_fine_samples, c.use_biased_sampler, float(self.collider.far_plane), bg)
         fr = self._fused_renderer()
+        with torch.no_grad():
+            self._apply_occupancy(fr, training=True)
         R, dev = origins.shape[0], origins.device
         jc = torch.rand((R, c.num_samples + 1), dtype=torch.float32, device=dev) if getattr(self.sampler_uniform, "train_stratified", True) else None
         jf = torch.rand((R, c.num_fine_samples + 1), dtype=torch.float32, device=dev) if getattr(self.sampler_pdf, "train_stratified", True) else None

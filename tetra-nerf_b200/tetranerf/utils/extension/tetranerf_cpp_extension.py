@@ -76,6 +76,8 @@ _lib.tn_render_set_deterministic.argtypes = [_vp, _i]
 _lib.tn_render_set_backward_grid.argtypes = [_vp, _u32]
 _lib.tn_surface_extract.argtypes = [_vp, C.c_float, C.POINTER(_u32), C.POINTER(_u32), _vp]
 _lib.tn_surface_copy.argtypes = [_vp, _vp, _vp, _vp, _vp, _vp, _vp]
+_lib.tn_occupancy_update.argtypes = [_vp, _vp, C.c_float, _vp]
+_lib.tn_render_set_occupancy.argtypes = [_vp, _vp, C.c_float]
 
 LIBRARY_PATH = str(_LIB_PATH)
 
