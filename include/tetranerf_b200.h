@@ -241,6 +241,14 @@ int tn_render_set_deterministic(tn_tracer *h, int enable);
  * tetrahedra was loaded since.  Surface extraction and the fused pixel gather are unaffected. */
 int tn_occupancy_update(tn_tracer *h, float *d_occ, float decay, void *stream);
 int tn_render_set_occupancy(tn_tracer *h, const float *d_occ, float threshold);
+/* ---- occupancy sampling (DESIGN.md §4.13): tn_render_set_occupancy2 is tn_render_set_occupancy (which calls it with 0) plus
+ * place_samples.  With place_samples != 0, tn_render and the training forwards also place each ray's coarse bins in its kept records
+ * only -- a record is skipped when its cell is a tetrahedron t with occ[t] < threshold, kept otherwise (gap records between hull faces
+ * included): the biased sampler gives every kept record an equal share, the uniform one samples the kept length uniformly.  near / far,
+ * the spacing bins' definition, the fine pass, the composite and every backward are unchanged; a ray with no skipped record, or no kept
+ * one, gets the bins of place_samples = 0.  The saved training state has the same size and layout.  Every accepted setting runs with
+ * it (the coarse sampler stages 2 (M + 2) more floats per ray).  TN_ERR_ARG if place_samples is set without d_occ. */
+int tn_render_set_occupancy2(tn_tracer *h, const float *d_occ, float threshold, int place_samples);
 /* ---- surface extraction: the density iso-surface sigma = level of the field as a triangle mesh, by marching tetrahedra on the loaded
  * mesh (DESIGN.md §4.6).  sigma is the density the renderer uses (density head of mlp_base, no GradientScaler), always evaluated in
  * bf16x3.  A vertex is inside when sigma(F[:, v]) >= level; every mesh edge (a, b), a < b, with one end inside and one outside gives one

@@ -89,6 +89,7 @@ struct RenderState {
     // off), the live-row flags and compact-row maps of the passes (coarse, fine, the backward's rebuilt one) and the backward's row count
     const float *occ = nullptr;
     float occ_thr = 0.f;
+    bool occ_place = false;            // occupancy sampling (DESIGN §4.13): coarse bins in the kept records only
     uint32_t occ_T = 0;                // the mesh's tetrahedron count when the occupancy was set
     bool t_cull = false;               // the last tracer-held training forward culled
     DevArray<uint8_t> live_flag;
@@ -206,11 +207,13 @@ struct SampleParams {
 
 // a culled sample (matched to a tetrahedron whose occupancy is below the threshold): vi = (E, E, E, TN_CULLED), weights 0.  Every
 // consumer that tests vi.x treats it as unmatched (no field gradient, no ray or vertex gradient, no normal); k_live_rows tells it from a
-// truly unmatched sample, whose density MLP(0) is still evaluated, and gives it sigma = 0 without evaluating the MLP.
+// truly unmatched sample, whose density MLP(0) is still evaluated, and gives it sigma = 0 without evaluating the MLP.  A sample matched
+// to a gap record (cell E, between two hull faces of a non-convex mesh) has no tetrahedron and is never culled.
 #define TN_CULLED 0xFFFFFFFEu
+__device__ __forceinline__ bool cell_culled(const SampleParams &p, uint32_t cell) { return cell != TN_EMPTY && __ldg(p.occ + cell) < p.occ_thr; }
 __device__ __forceinline__ void cull_sample(const SampleParams &p, size_t row, uint32_t seg, uint4 &vi, float &b0, float &b1, float &b2) {
     if (vi.x == TN_EMPTY) return;
-    if (__ldg(p.occ + __ldg(p.cells + row + seg)) < p.occ_thr) {
+    if (cell_culled(p, __ldg(p.cells + row + seg))) {
         vi = make_uint4(TN_EMPTY, TN_EMPTY, TN_EMPTY, TN_CULLED);
         b0 = b1 = b2 = 0.f;
     }
@@ -287,10 +290,17 @@ __device__ __forceinline__ uint32_t match_sample(float d, uint32_t n, const floa
 __host__ __device__ __forceinline__ size_t seg_arr(uint32_t M) { return (size_t)M + 2; }
 __host__ __device__ __forceinline__ size_t coarse_floats(uint32_t M, uint32_t Sc, uint32_t biased) { return seg_arr(M) * (biased ? 2 : 1) + (size_t)Sc + 2; }
 __host__ __device__ __forceinline__ size_t fine_floats(uint32_t M, uint32_t Smax) { return seg_arr(M) + 4 * ((size_t)Smax + 2); }
+// occupancy sampling (PLACE): pm, cum, the kept records' indices kix, e -- either sampler; at most 160 KB per block (M = 2048,
+// Sc = 4096), so every accepted setting fits
+__host__ __device__ __forceinline__ size_t place_floats(uint32_t M, uint32_t Sc) { return 3 * seg_arr(M) + (size_t)Sc + 2; }
 
 // ORDERED (deterministic mode): the slot of a ray is its rank among the rays with hits (p.ray_slot), so slot order = ray order;
-// otherwise slots are claimed with an atomic counter
-template <bool ORDERED>
+// otherwise slots are claimed with an atomic counter.
+// PLACE (occupancy sampling, DESIGN §4.13; needs p.occ): a ray with both skipped records (a tetrahedron below the threshold) and kept
+// ones places its bins in the kept records only: the biased sampler gives each kept record an equal share of [0, 1], the uniform one
+// spreads them uniformly over the kept length.  near / far and the spacing bins' definition stay as they are.  A ray with no skipped or
+// no kept record takes the code path of !PLACE, so its bins are the same bits.
+template <bool ORDERED, bool PLACE = false>
 __global__ void __launch_bounds__(SAMPLE_WARPS * 32) k_sample_coarse(const SampleParams p) {
     extern __shared__ float sm[];
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -298,8 +308,8 @@ __global__ void __launch_bounds__(SAMPLE_WARPS * 32) k_sample_coarse(const Sampl
     if (ray >= p.R) return;
     const uint32_t M = p.M, S = p.Sc;
     const size_t A = seg_arr(M);
-    float *pm = sm + (size_t)warp * coarse_floats(M, S, p.biased);
-    float *cum = pm + A, *e = cum + (p.biased ? A : 0);
+    float *pm = sm + (size_t)warp * (PLACE ? place_floats(M, S) : coarse_floats(M, S, p.biased));
+    float *cum = pm + A, *e = PLACE ? cum + 2 * A : cum + (p.biased ? A : 0);
     const uint32_t n = p.num[ray];
     if constexpr (ORDERED) {
         if (ray == p.R - 1 && lane == 0) *p.n_active = p.ray_slot[ray] + (n > 0 ? 1u : 0u);
@@ -318,42 +328,101 @@ __global__ void __launch_bounds__(SAMPLE_WARPS * 32) k_sample_coarse(const Sampl
     }
     const size_t row = (size_t)ray * M;
     const float near = __ldg(&p.dist[row]).x, far = __ldg(&p.dist[row + n - 1]).y;
+    bool placed = false;
+    uint32_t nk = 0;  // PLACE: the kept records, their indices in kix[0..nk) in ray order
+    uint32_t *kix = reinterpret_cast<uint32_t *>(cum + A);
+    if constexpr (PLACE) {
+        for (uint32_t base = 0; base < n; base += 32) {
+            const uint32_t k = base + lane;
+            const bool kept = k < n && !cell_culled(p, __ldg(p.cells + row + k));
+            const uint32_t bal = __ballot_sync(0xffffffffu, kept);
+            if (kept) kix[nk + __popc(bal & ((1u << lane) - 1u))] = k;
+            nk += __popc(bal);
+        }
+        placed = nk > 0 && nk < n;  // (warp-uniform)
+    }
     for (uint32_t k = lane; k < n; k += 32) {
         const float2 h = __ldg(&p.dist[row + k]);
         pm[k] = h.y;
-        if (p.biased) cum[k + 1] = fmaxf(h.y - h.x, 0.f);  // map_from_real_distances_to_biased_with_bounds, model.py:111-122
+        if (p.biased && !placed) cum[k + 1] = fmaxf(h.y - h.x, 0.f);  // map_from_real_distances_to_biased_with_bounds, model.py:111-122
     }
-    if (p.biased && lane == 0) cum[0] = near;
+    if (p.biased && !placed && lane == 0) cum[0] = near;
+    if (placed && !p.biased) {  // cum[i] = the kept length before the i-th kept record, cum[nk] = all of it
+        __syncwarp();
+        for (uint32_t i = lane; i < nk; i += 32) {
+            const float2 h = __ldg(&p.dist[row + kix[i]]);
+            cum[i + 1] = fmaxf(h.y - h.x, 0.f);
+        }
+        if (lane == 0) cum[0] = 0.f;
+    }
     __syncwarp();
     smem_scan_max(pm, pm, n, lane);  // in place
-    if (p.biased) {
+    if (p.biased && !placed) {
         // cum[k] = start + sum_{i<k} len_i : scan over [start, len_0, len_1, ...]
         smem_scan_add(cum, n + 1, lane);
     }
-    for (uint32_t j = lane; j <= S; j += 32) {
-        float b = linspace_f(0.f, 1.f, S + 1, j);
-        if (p.jit_c != nullptr) {  // stratified training bins (model.py:169-174; nerfstudio SpacedSampler): jitter between the neighbouring bin centres
-            const float lower = j == 0 ? b : (b + linspace_f(0.f, 1.f, S + 1, j - 1)) / 2.0f;
-            const float upper = j == S ? b : (linspace_f(0.f, 1.f, S + 1, j + 1) + b) / 2.0f;
-            b = lower + (upper - lower) * __ldg(p.jit_c + (size_t)ray * (S + 1) + j);
+    if (placed) {
+        if (!p.biased) smem_scan_add(cum, nk + 1, lane);
+        for (uint32_t j = lane; j <= S; j += 32) {
+            float b = linspace_f(0.f, 1.f, S + 1, j);
+            if (p.jit_c != nullptr) {  // the same stratified jitter as below
+                const float lower = j == 0 ? b : (b + linspace_f(0.f, 1.f, S + 1, j - 1)) / 2.0f;
+                const float upper = j == S ? b : (linspace_f(0.f, 1.f, S + 1, j + 1) + b) / 2.0f;
+                b = lower + (upper - lower) * __ldg(p.jit_c + (size_t)ray * (S + 1) + j);
+            }
+            uint32_t i;
+            float off;
+            if (p.biased) {  // map_from_real_distances_to_biased_with_bounds over the kept records
+                const float uni = (b * far + (1.f - b) * near - near) / (far - near);
+                float rest = uni * (float)nk;
+                float iv = fminf(floorf(rest), (float)(nk - 1));
+                iv = fmaxf(iv, 0.f);
+                rest = rest - iv;
+                i = (uint32_t)iv;
+                const float2 hk = __ldg(&p.dist[row + kix[i]]);
+                off = fmaxf(hk.y - hk.x, 0.f) * rest;
+            } else {  // x = b L: the last kept record whose cumulative start is <= x
+                const float x = b * cum[nk];
+                uint32_t lo = 1, hi = nk;
+                while (lo < hi) { const uint32_t mid = (lo + hi) >> 1; if (cum[mid] <= x) lo = mid + 1; else hi = mid; }
+                i = lo - 1;
+                off = x - cum[i];
+            }
+            const float2 h = __ldg(&p.dist[row + kix[i]]);
+            e[j] = fminf(h.x + off, fmaxf(h.x, h.y));  // (rounding never leaves the record)
         }
-        float eu = b * far + (1.f - b) * near;  // spacing_to_euclidean_fn (model.py:177)
-        float sb = b;
-        if (p.biased) {
-            const float uni = (eu - near) / (far - near);
-            float rest = uni * (float)n;
-            float iv = fminf(floorf(rest), (float)(n - 1));
-            iv = fmaxf(iv, 0.f);
-            rest = rest - iv;
-            const uint32_t k = (uint32_t)iv;
-            const float2 hk = __ldg(&p.dist[row + k]);
-            const float len = fmaxf(hk.y - hk.x, 0.f);
-            eu = cum[k] + len * rest;
-            sb = (eu - near) / (far - near);  // model.py:182
+        __syncwarp();
+        smem_scan_max(e, e, S + 1, lane);  // sorted bins even where two records overlap by a rounding
+        for (uint32_t j = lane; j <= S; j += 32) {
+            p.ebins_c[(size_t)slot * (S + 1) + j] = e[j];
+            p.sbins_c[(size_t)slot * (S + 1) + j] = (e[j] - near) / (far - near);  // model.py:182
         }
-        e[j] = eu;
-        p.ebins_c[(size_t)slot * (S + 1) + j] = eu;
-        p.sbins_c[(size_t)slot * (S + 1) + j] = sb;
+    } else {
+        for (uint32_t j = lane; j <= S; j += 32) {
+            float b = linspace_f(0.f, 1.f, S + 1, j);
+            if (p.jit_c != nullptr) {  // stratified training bins (model.py:169-174; nerfstudio SpacedSampler): jitter between the neighbouring bin centres
+                const float lower = j == 0 ? b : (b + linspace_f(0.f, 1.f, S + 1, j - 1)) / 2.0f;
+                const float upper = j == S ? b : (linspace_f(0.f, 1.f, S + 1, j + 1) + b) / 2.0f;
+                b = lower + (upper - lower) * __ldg(p.jit_c + (size_t)ray * (S + 1) + j);
+            }
+            float eu = b * far + (1.f - b) * near;  // spacing_to_euclidean_fn (model.py:177)
+            float sb = b;
+            if (p.biased) {
+                const float uni = (eu - near) / (far - near);
+                float rest = uni * (float)n;
+                float iv = fminf(floorf(rest), (float)(n - 1));
+                iv = fmaxf(iv, 0.f);
+                rest = rest - iv;
+                const uint32_t k = (uint32_t)iv;
+                const float2 hk = __ldg(&p.dist[row + k]);
+                const float len = fmaxf(hk.y - hk.x, 0.f);
+                eu = cum[k] + len * rest;
+                sb = (eu - near) / (far - near);  // model.py:182
+            }
+            e[j] = eu;
+            p.ebins_c[(size_t)slot * (S + 1) + j] = eu;
+            p.sbins_c[(size_t)slot * (S + 1) + j] = sb;
+        }
     }
     __syncwarp();
     for (uint32_t j = lane; j < S; j += 32) {
@@ -1137,7 +1206,8 @@ static int render_impl(tn_tracer *h, const tn_render_config *cfg, const float *d
     cudaStream_t s = (cudaStream_t)stream;
     // dynamic shared memory of the per-ray kernels (4 warps per block, one ray per warp): checked before anything is allocated or
     // launched, so a setting that cannot run fails as an argument error and leaves no CUDA error behind
-    const size_t smem_sc = SAMPLE_WARPS * sizeof(float) * coarse_floats(M, Sc, cfg->use_biased_sampler);
+    const bool place = cull && r->occ_place;           // occupancy sampling (DESIGN §4.13)
+    const size_t smem_sc = SAMPLE_WARPS * sizeof(float) * (place ? place_floats(M, Sc) : coarse_floats(M, Sc, cfg->use_biased_sampler));
     const size_t smem_sf = SAMPLE_WARPS * sizeof(float) * fine_floats(M, std::max(Sc, S2));
     const size_t smem_c = SAMPLE_WARPS * sizeof(float) * 2 * ((size_t)S2 + 2);
     const size_t smem_cb = SAMPLE_WARPS * sizeof(float) * 4 * ((size_t)S2 + 2);  // k_composite_bwd, which the backward launches
@@ -1191,7 +1261,7 @@ static int render_impl(tn_tracer *h, const tn_render_config *cfg, const float *d
         for (int k = 0; k < 8; ++k) p.peer[k] = r->peer[k];
         p.gather_world = r->gather_world; p.gather_rank = r->gather_rank; p.gather_stride = r->gather_stride;
     }
-    auto k_coarse_sample = det ? k_sample_coarse<true> : k_sample_coarse<false>;
+    auto k_coarse_sample = place ? (det ? k_sample_coarse<true, true> : k_sample_coarse<false, true>) : (det ? k_sample_coarse<true> : k_sample_coarse<false>);
     TN_CUDA(cudaFuncSetAttribute(k_coarse_sample, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_sc));
     // (single pass: k_sample_fine is not launched, and its staging at S2 = Sc can exceed the limit where the call itself fits)
     if (!single) TN_CUDA(cudaFuncSetAttribute(k_sample_fine, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_sf));
@@ -1561,17 +1631,25 @@ extern "C" int tn_render_set_deterministic(tn_tracer *h, int enable) {
     return TN_OK;
 }
 
-// occupancy culling (see the header; DESIGN §4.12): borrowed f32[T]; NULL switches it off
-extern "C" int tn_render_set_occupancy(tn_tracer *h, const float *d_occ, float threshold) {
+// occupancy culling (see the header; DESIGN §4.12): borrowed f32[T]; NULL switches it off.  place_samples: occupancy sampling
+// (DESIGN §4.13), which needs an occupancy
+extern "C" int tn_render_set_occupancy2(tn_tracer *h, const float *d_occ, float threshold, int place_samples) {
     if (!h) return fail(TN_ERR_ARG, "null tracer");
     if (!std::isfinite(threshold) || threshold < 0.f)
         return fail(TN_ERR_ARG, "tn_render_set_occupancy: the threshold must be finite and >= 0");
+    if (place_samples && d_occ == nullptr)
+        return fail(TN_ERR_ARG, "tn_render_set_occupancy2: placing the samples by occupancy needs an occupancy (d_occ is NULL)");
     DeviceGuard g(h->device);
     RenderState *r = state(h);
     r->occ = d_occ;
     r->occ_thr = threshold;
+    r->occ_place = place_samples != 0;
     r->occ_T = h->mesh.T;
     return TN_OK;
+}
+
+extern "C" int tn_render_set_occupancy(tn_tracer *h, const float *d_occ, float threshold) {
+    return tn_render_set_occupancy2(h, d_occ, threshold, 0);
 }
 
 // d_occ f32[T] <- max(decay * d_occ, the largest probe density of each tetrahedron): probe rows in chunks of OCC_CHUNK tetrahedra

@@ -31,7 +31,8 @@ class RenderSettings:
     num_samples in [1, 4096], num_fine_samples in [0, 4096] (0 = single pass).  Two-pass settings must also fit the per-ray kernels'
     shared memory: 16 (M + 4 S2 + 10) bytes per block with S2 = num_samples + num_fine_samples + 1, at most the device's opt-in limit
     (232,448 B on an H100: num_samples + num_fine_samples <= 3500 at M = 512, <= 3116 at M = 2048); beyond it render and the
-    training forwards raise RuntimeError before anything runs."""
+    training forwards raise RuntimeError before anything runs.  Occupancy sampling (set_occupancy(..., place_samples=True)) adds
+    32 (M + 2) bytes per block to the coarse sampler only, at most 164 KB in all: every setting above still runs with it."""
 
     max_intersected_triangles: int = 512
     num_samples: int = 256
@@ -240,13 +241,15 @@ class FusedRenderer:
         if occ.device != self.device or occ.dtype != torch.float32 or not occ.is_contiguous() or tuple(occ.shape) != (T,):
             raise RuntimeError(f"the occupancy must be a contiguous float32 [{T}] tensor (one entry per tetrahedron) on the tracer's device")
 
-    def set_occupancy(self, occ: Optional[torch.Tensor], threshold: float = 0.0) -> None:
+    def set_occupancy(self, occ: Optional[torch.Tensor], threshold: float = 0.0, place_samples: bool = False) -> None:
         """cull, in every later render and training forward, the samples matched to a tetrahedron t with occ[t] < threshold: their
         density is the constant 0 and their MLP is not evaluated (unmatched samples are evaluated as before).  occ f32[T] is borrowed
-        (kept alive here); None switches culling off.  A saved training forward's backward does not read occ again."""
+        (kept alive here); None switches culling off.  A saved training forward's backward does not read occ again.
+        place_samples (needs occ): also place each ray's coarse bins in its records outside those tetrahedra only, so the sample budget
+        lands where the density can be non-zero (DESIGN §4.13)."""
         if occ is not None:
             self._check_occupancy(occ)
-        ext._check(_lib.tn_render_set_occupancy(self.tracer.handle, _ptr(occ), C.c_float(float(threshold))))
+        ext._check(_lib.tn_render_set_occupancy2(self.tracer.handle, _ptr(occ), C.c_float(float(threshold)), 1 if place_samples else 0))
         self._occ = occ
 
     def update_occupancy(self, occ: torch.Tensor, decay: float = 0.0) -> torch.Tensor:

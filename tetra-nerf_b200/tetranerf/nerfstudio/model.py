@@ -86,6 +86,10 @@ class TetrahedraNerfConfig(ModelConfig):
     few updates rather than at once"""
     occupancy_warmup_steps: int = 256
     """training steps without culling at the start, so the randomly initialised field is not culled away"""
+    occupancy_sampling: bool = False
+    """also place each ray's coarse samples in its tetrahedra at or above occupancy_threshold only, so the num_samples /
+    num_fine_samples budget is not spent on culled empty space (DESIGN §4.13); applies exactly when culling does.  Needs
+    use_occupancy_field (RuntimeError otherwise)"""
     render_normals: bool = False
     """eval renders also return "normals" f32[R,3], the composited normal of the density field (fused path only; training ignores it)"""
     optimize_vertices: bool = False
@@ -403,7 +407,10 @@ class TetrahedraNerf(Model):
             self._occ_ready = True
         if training and not fresh and (step - c.occupancy_warmup_steps) % max(1, c.occupancy_update_interval) == 0:
             fr.update_occupancy(occ, c.occupancy_decay)
-        fr.set_occupancy(occ, c.occupancy_threshold)
+        if c.occupancy_sampling:
+            fr.set_occupancy(occ, c.occupancy_threshold, place_samples=True)
+        else:
+            fr.set_occupancy(occ, c.occupancy_threshold)
 
     # ---- forward (reference :520-662) ---------------------------------------------------------------------
     def _expected_depth_on(self) -> bool:
@@ -426,6 +433,8 @@ class TetrahedraNerf(Model):
         assert self.collider is not None
         origins, directions = ray_bundle.origins.contiguous(), ray_bundle.directions.contiguous()
         normals = self.config.render_normals and not self.training
+        if self.config.occupancy_sampling and not self.config.use_occupancy_field:
+            raise RuntimeError("occupancy_sampling places the samples by the occupancy field: it needs use_occupancy_field=True")
         if self.config.use_occupancy_field and self._fused_unsupported():
             raise RuntimeError(f"use_occupancy_field culls on the fused CUDA pipeline, which does not support {', '.join(self._fused_unsupported())}")
         if normals and self._fused_unsupported():

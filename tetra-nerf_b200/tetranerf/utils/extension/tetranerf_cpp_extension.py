@@ -78,6 +78,7 @@ _lib.tn_surface_extract.argtypes = [_vp, C.c_float, C.POINTER(_u32), C.POINTER(_
 _lib.tn_surface_copy.argtypes = [_vp, _vp, _vp, _vp, _vp, _vp, _vp]
 _lib.tn_occupancy_update.argtypes = [_vp, _vp, C.c_float, _vp]
 _lib.tn_render_set_occupancy.argtypes = [_vp, _vp, C.c_float]
+_lib.tn_render_set_occupancy2.argtypes = [_vp, _vp, C.c_float, _i]
 
 LIBRARY_PATH = str(_LIB_PATH)
 
