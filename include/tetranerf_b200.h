@@ -125,7 +125,8 @@ typedef struct tn_render_config {
     float background[3];        /* renderer background colour (white = 1,1,1; model.py:93) */
 } tn_render_config;
 
-/* field: f32[64,V] feature-major.  Keeps a [V,64] row-major shadow inside the tracer. */
+/* field: f32[64,V] feature-major.  Keeps a [V,64] shadow inside the tracer, one row per vertex with its features in the order of
+ * the MLP's A fragments (csrc/tn_common.cuh, field_pos). */
 int tn_render_set_field(tn_tracer *h, const float *d_field, uint32_t C, uint32_t V, void *stream);
 /* operand precision of the inference MLP (tn_render; the training forward always uses 3):
  *   3 = "bf16x3": a*w = a_hi*w_hi + a_lo*w_hi + a_hi*w_lo in bf16 halves, 3 MMAs per K step, ~5e-7 absolute on unit-scale outputs;

@@ -207,9 +207,15 @@ void free_render(tn_tracer *h);
 void free_surface(tn_tracer *h);
 // a value no earlier call returned (tn_render.cu): the generation of a field, weights or mesh
 uint64_t next_generation();
+// The field shadow `fshadow` [V,64] (tn_render_set_field) keeps one 256-byte row per vertex with its features in fragment order: in
+// each 16-feature block b (one k-step of the MLP's layer 0), feature 16b + 8h + 2t + e (h, e in {0, 1}, t in 0..3) is stored at
+// 16b + 4t + 2h + e.  The four features thread t of a wgmma A fragment row needs in k-step b, the column pairs 2t and 8 + 2t, are then
+// one 16-byte load at 16b + 4t, and column pairs stay adjacent.  This is the only statement of the layout: the writer and every
+// reader of the shadow go through it.  (The gradient shadow `gshadow` keeps the canonical order.)
+__host__ __device__ constexpr uint32_t field_pos(uint32_t f) { return (f & ~15u) | ((f & 6u) << 1) | ((f >> 2) & 2u) | (f & 1u); }
 // the field and weights of the fused render as the surface extraction reads them; TN_ERR_STATE unless both were set
 struct RenderInputs {
-    const float *fshadow;   // [V,64]
+    const float *fshadow;   // [V,64] in fragment order (field_pos)
     uint32_t V;
     const uint8_t *wimg;    // bf16 hi/lo weight image of k_mlp<*, 3>
     const float *bias, *head, *w4dir;
@@ -225,7 +231,7 @@ struct NormalsLaunch {
     const float *bary;                    // [n_active*S,3]
     const float *ebins;                   // [n_active,S+1] its euclidean bin edges
     const float *out_f;                   // [n_active*S] (sigma, r, g, b)
-    const float *fshadow;                 // [V,64]
+    const float *fshadow;                 // [V,64] in fragment order (field_pos)
     const uint8_t *wimg;                  // weight image of k_mlp<*, prec>
     const float *bias, *head;
     const float *xyz;                     // [V,3] mesh vertex positions
@@ -240,7 +246,7 @@ struct RayGradsLaunch {
     const float *ebins;                   // [n_active,S+1] euclidean bin edges of the fine pass
     const uint4 *vi;                      // [n_active*S] matched vertex ids
     const float *dx;                      // [n_active*S,64] gradient at the interpolated features
-    const float *fshadow;                 // [V,64]
+    const float *fshadow;                 // [V,64] in fragment order (field_pos)
     const float *xyz;                     // [V,3] mesh vertex positions
     const float *enc;                     // [n_active,27] encoded directions (entries 24..26: the direction itself)
     const float *g_dirbias;               // [n_active,128] gradient at the per-ray direction bias

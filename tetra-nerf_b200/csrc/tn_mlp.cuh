@@ -9,7 +9,8 @@
 // One persistent CTA per SM with MLP_WGS warpgroups.  The whole weight image (224 KB: four layers, bf16 or fp16 hi/lo halves)
 // is staged into shared memory once per CTA by TMA bulk copies and stays resident.  Each warpgroup then works through 64-sample
 // tiles on its own, entirely in registers:
-//   gather    the four vertex rows of each of its two samples per thread are read from the [V,64] field shadow, interpolated with
+//   gather    the four vertex rows of each of its two samples per thread are read from the [V,64] field shadow (stored in fragment
+//             order, so a thread reads its 16 features of a row as four 16-byte loads), interpolated with
 //             the reference's FMA order and converted straight into the layer-0 A fragments (see tn_tc.cuh for the layout);
 //   layers    every Linear is a chain of wgmma m64n128k16 with A from registers and B = the resident weight block; the epilogue
 //             (bias + ReLU) turns the fp32 accumulator into the next layer's A fragments in place -- activations never touch
@@ -53,7 +54,7 @@ struct MlpParams {
     uint32_t S;                // samples per ray in this pass
     const uint4 *vi;           // [n_active*S] matched vertex ids (E = unmatched)
     const float *bary;         // [n_active*S,3]
-    const float *fshadow;      // [V,64] row-major field
+    const float *fshadow;      // [V,64] field, one row per vertex in fragment order (field_pos)
     const uint8_t *wimg;       // weight image: L1 | L2 | L3 | L4(base part), see tn_mlp_pack.cuh
     const float *bias;         // b1,b2,b3 [3][128]
     const float *head;         // wd[128], wc[3][128], bd, bc[3]
@@ -71,23 +72,33 @@ constexpr uint32_t MLP_NO_TILE = 0xFFFFFFFFu;  // sentinel: the scheduler has ru
 __device__ __forceinline__ float softplus_f(float x) { return x > 20.0f ? x : log1pf(expf(x)); }  // torch Softplus(beta=1, threshold=20)
 __device__ __forceinline__ float sigmoid_f(float x) { return 1.0f / (1.0f + expf(-x)); }
 
-// 8-byte read-only load that does not allocate in L1 (the gathered field rows stream through; L1 is left to the biases)
-__device__ __forceinline__ float2 ldg_stream2(const float *p) {
-    float2 v;
-    asm volatile("ld.global.nc.L1::no_allocate.v2.f32 {%0, %1}, [%2];" : "=f"(v.x), "=f"(v.y) : "l"(p));
-    return v;
-}
-// 8-byte read-only load that allocates in L1
-__device__ __forceinline__ float2 ldg_l1_2(const float *p) {
-    float2 v;
-    asm volatile("ld.global.nc.v2.f32 {%0, %1}, [%2];" : "=f"(v.x), "=f"(v.y) : "l"(p));
-    return v;
-}
-// 16-byte variant
+// 16-byte read-only load that does not allocate in L1 (the gathered field rows stream through; L1 is left to the biases)
 __device__ __forceinline__ float4 ldg_stream(const float4 *p) {
     float4 v;
     asm volatile("ld.global.nc.L1::no_allocate.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "l"(p));
     return v;
+}
+// 16-byte read-only load that allocates in L1
+__device__ __forceinline__ float4 ldg_l1(const float4 *p) {
+    float4 v;
+    asm volatile("ld.global.nc.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "l"(p));
+    return v;
+}
+
+// the 16 features of one field-shadow row that thread t of a fragment row needs, as four 16-byte loads: q[kk] holds column pairs
+// 2kk (features 16kk + 2t, +1) and 2kk + 1 (16kk + 8 + 2t, +1) -- one load per k-step, since the shadow is in fragment order (field_pos)
+template <bool ALLOC_L1>
+__device__ __forceinline__ void load_field_quads(const float *__restrict__ row, uint32_t t, float4 (&q)[4]) {
+#pragma unroll
+    for (int kk = 0; kk < 4; ++kk) {
+        const float4 *p = reinterpret_cast<const float4 *>(row + field_pos(16u * kk + 2u * t));
+        q[kk] = ALLOC_L1 ? ldg_l1(p) : ldg_stream(p);
+    }
+}
+// column pair c (features 8c + 2t, +1) of the quads load_field_quads returned
+__device__ __forceinline__ float2 field_pair(const float4 (&q)[4], int c) {
+    const float4 v = q[c >> 1];
+    return (c & 1) ? make_float2(v.z, v.w) : make_float2(v.x, v.y);
 }
 
 // named barrier of one warpgroup (ids 1.. ; 0 is __syncthreads)
@@ -153,25 +164,22 @@ __device__ __forceinline__ void prefetch_gather_rows(const uint4 *vi, const floa
 
 // the interpolated features of the thread's two rows, as the layer-0 A fragments (K = 64: 4 k-steps x 4 registers).
 // tetrahedra_tracer.cu:203-220: v1*b0, + v2*b1, + v3*b2, + v0*w0 (fused multiply-adds), per feature.
-// All 64 field loads of the two rows are issued before the first one is consumed, so a thread has its whole gather in flight at
-// once instead of one L2 round trip per column pair.  The loads are unconditional: an unmatched row reads vertex 0's features and
-// its result is replaced by 0 (a branch around the loads would keep the compiler from hoisting them over the FMAs).
+// All 32 field loads of the two rows (16 bytes each: one per row, vertex and k-step, see field_pos) are issued before the first one
+// is consumed, so a thread has its whole gather in flight at once instead of one L2 round trip per k-step.  The loads are
+// unconditional: an unmatched row reads vertex 0's features and its result is replaced by 0 (a branch around the loads would keep
+// the compiler from hoisting them over the FMAs).
 // ALLOC_L1: the loads allocate in L1 (k_mlp).  Samples next to each other along a ray lie in the same or adjacent tetrahedra, so
 // most of a row's four vertices are among its neighbours' and the repeats of a field row, within a warp and across the warpgroups
 // of an SM, are served from L1 instead of L2.  Otherwise they stream past L1 (k_mlp_bwd, k_mlp_normals).
 template <int PREC, bool ALLOC_L1 = false>
 __device__ __forceinline__ void gather_rows(const GatherRows &r, const float *__restrict__ fshadow, uint32_t t, uint32_t (&xh)[16], uint32_t (&xl)[16]) {
-    float2 a[2][4][8];  // [row][vertex][column pair]
+    float4 a[2][4][4];  // [row][vertex][k-step]
 #pragma unroll
     for (int rr = 0; rr < 2; ++rr) {
         const uint4 v = r.v[rr].x != TN_EMPTY ? r.v[rr] : make_uint4(0u, 0u, 0u, 0u);
         const uint32_t vs[4] = {v.x, v.y, v.z, v.w};
 #pragma unroll
-        for (int k = 0; k < 4; ++k) {
-            const float *f = fshadow + (size_t)vs[k] * 64 + 2 * t;
-#pragma unroll
-            for (int c = 0; c < 8; ++c) a[rr][k][c] = ALLOC_L1 ? ldg_l1_2(f + 8 * c) : ldg_stream2(f + 8 * c);
-        }
+        for (int k = 0; k < 4; ++k) load_field_quads<ALLOC_L1>(fshadow + (size_t)vs[k] * 64, t, a[rr][k]);
     }
 #pragma unroll
     for (int rr = 0; rr < 2; ++rr) {
@@ -180,7 +188,7 @@ __device__ __forceinline__ void gather_rows(const GatherRows &r, const float *__
         const float w0 = __fsub_rn(1.0f, __fadd_rn(__fadd_rn(b0, b1), b2));
 #pragma unroll
         for (int c = 0; c < 8; ++c) {  // column pair 8c + 2t, +1  ->  k-step c / 2, register 2 (c & 1) + rr
-            const float2 a0 = a[rr][0][c], a1 = a[rr][1][c], a2 = a[rr][2][c], a3 = a[rr][3][c];
+            const float2 a0 = field_pair(a[rr][0], c), a1 = field_pair(a[rr][1], c), a2 = field_pair(a[rr][2], c), a3 = field_pair(a[rr][3], c);
             float2 o;
             o.x = __fmaf_rn(b0, a1.x, 0.f); o.y = __fmaf_rn(b0, a1.y, 0.f);
             o.x = __fmaf_rn(b1, a2.x, o.x); o.y = __fmaf_rn(b1, a2.y, o.y);

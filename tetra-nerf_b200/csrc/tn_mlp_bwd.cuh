@@ -56,7 +56,7 @@ struct MlpBwdParams {
     uint32_t S;                 // samples per ray of the fine pass (S2)
     const uint4 *vi;            // [rows] matched vertex ids
     const float *bary;          // [rows,3]
-    const float *fshadow;       // [V,64]
+    const float *fshadow;       // [V,64] in fragment order (field_pos)
     const uint8_t *wimg;        // backward weight image (7 stages of 32 KB, see tn_render_set_weights)
     const float *bias;          // b1 b2 b3 [3][128]
     const float *head;          // wd[128] wc[3][128] ...

@@ -146,7 +146,9 @@ __global__ void __launch_bounds__(NRM_THREADS, 1) k_mlp_normals(const NormalsPar
     for (uint32_t i = threadIdx.x; i < 128; i += NRM_THREADS) wd_s[i] = p.head[i];
     auto draw = [&]() {  // k_mlp's scheduler
         const uint32_t nx = gridDim.x * NRM_WGS + atomicAdd(p.tile_ctr, 1u);
-        return nx < ntiles ? nx : MLP_NO_TILE;
+        // the tile count read again rather than kept live through the tile loop: at 255 registers k_mlp_normals<2> would spill it
+        const uint32_t nt = (uint32_t)(((uint64_t)*p.n_active * p.S + MLP_TILE - 1) / MLP_TILE);
+        return nx < nt ? nx : MLP_NO_TILE;
     };
     if (tid == 0) {
         const uint32_t first = blockIdx.x * NRM_WGS + wg;
@@ -247,21 +249,18 @@ __global__ void __launch_bounds__(NRM_THREADS, 1) k_mlp_normals(const NormalsPar
             uint4 v = row < total_rows ? __ldg(p.vi + row) : make_uint4(TN_EMPTY, TN_EMPTY, TN_EMPTY, TN_EMPTY);
             if (v.x == TN_EMPTY) v = make_uint4(0u, 0u, 0u, 0u);  // (the result of an unmatched row is discarded)
             const uint32_t vs[4] = {v.x, v.y, v.z, v.w};
-            float2 a[4][8];
+            float4 a[4][4];
 #pragma unroll
-            for (int k = 0; k < 4; ++k) {
-                const float *f = p.fshadow + (size_t)vs[k] * 64 + 2 * t;
-#pragma unroll
-                for (int c = 0; c < 8; ++c) a[k][c] = ldg_stream2(f + 8 * c);
-            }
+            for (int k = 0; k < 4; ++k) load_field_quads<false>(p.fshadow + (size_t)vs[k] * 64, t, a[k]);
             float s3[3];
 #pragma unroll
             for (int k = 1; k < 4; ++k) {
                 float acc = 0.f;
 #pragma unroll
                 for (int c = 0; c < 8; ++c) {
-                    acc = fmaf(gg[2 * c], a[k][c].x - a[0][c].x, acc);
-                    acc = fmaf(gg[2 * c + 1], a[k][c].y - a[0][c].y, acc);
+                    const float2 fk = field_pair(a[k], c), f0 = field_pair(a[0], c);
+                    acc = fmaf(gg[2 * c], fk.x - f0.x, acc);
+                    acc = fmaf(gg[2 * c + 1], fk.y - f0.y, acc);
                 }
                 s3[k - 1] = acc;
             }
@@ -284,7 +283,10 @@ __global__ void __launch_bounds__(NRM_THREADS, 1) k_mlp_normals(const NormalsPar
                     tet_cofactors(p.xyz, vs, cf, det);
                     if (det != 0.0) {
                         const float q0 = t == 0 ? q[0][0] : q[1][0], q1 = t == 0 ? q[0][1] : q[1][1], q2 = t == 0 ? q[0][2] : q[1][2];
-                        const double sc = ldexp(1.0, wexp) / det;  // undo the seed's power of two
+                        // undo the seed's power of two.  2^wexp is built from its bits (wexp lies in [-156, 120], well inside the
+                        // normal range): the same value as ldexp(1.0, wexp), without the constants of ldexp's range checks, which the
+                        // compiler would keep live through the tile loop (and spill, in k_mlp_normals<2>)
+                        const double sc = __longlong_as_double((long long)(1023 + wexp) << 52) / det;
                         o.x = (float)((q0 * cf[0][0] + q1 * cf[1][0] + q2 * cf[2][0]) * sc);
                         o.y = (float)((q0 * cf[0][1] + q1 * cf[1][1] + q2 * cf[2][1]) * sc);
                         o.z = (float)((q0 * cf[0][2] + q1 * cf[1][2] + q2 * cf[2][2]) * sc);

@@ -35,6 +35,7 @@ __global__ void __launch_bounds__(RG_WARPS * 32) k_ray_grads(const RayGradsLaunc
     const uint32_t S = p.S, ray = p.ray_list[slot];
     const float *eb = p.ebins + (size_t)slot * (S + 1);
     double go[3] = {0.0, 0.0, 0.0}, gd[3] = {0.0, 0.0, 0.0};  // this lane's samples: sum dL/dx, sum t dL/dx
+    const uint32_t fp = field_pos(2u * (uint32_t)lane);  // where the lane's feature pair (2 lane, +1) sits in a field-shadow row
     for (uint32_t base = 0; base < S; base += 32) {
         const uint32_t j = base + (uint32_t)lane;
         const size_t row = (size_t)slot * S + j;
@@ -46,10 +47,10 @@ __global__ void __launch_bounds__(RG_WARPS * 32) k_ray_grads(const RayGradsLaunc
             if (v0 == TN_EMPTY) continue;  // (warp-uniform)
             const uint32_t v1 = __shfl_sync(0xffffffffu, v.y, k), v2 = __shfl_sync(0xffffffffu, v.z, k), v3 = __shfl_sync(0xffffffffu, v.w, k);
             const float2 g = __ldg(reinterpret_cast<const float2 *>(p.dx + ((size_t)slot * S + base + k) * 64) + lane);
-            const float2 f0 = __ldg(reinterpret_cast<const float2 *>(p.fshadow + (size_t)v0 * 64) + lane);
-            const float2 f1 = __ldg(reinterpret_cast<const float2 *>(p.fshadow + (size_t)v1 * 64) + lane);
-            const float2 f2 = __ldg(reinterpret_cast<const float2 *>(p.fshadow + (size_t)v2 * 64) + lane);
-            const float2 f3 = __ldg(reinterpret_cast<const float2 *>(p.fshadow + (size_t)v3 * 64) + lane);
+            const float2 f0 = __ldg(reinterpret_cast<const float2 *>(p.fshadow + (size_t)v0 * 64 + fp));
+            const float2 f1 = __ldg(reinterpret_cast<const float2 *>(p.fshadow + (size_t)v1 * 64 + fp));
+            const float2 f2 = __ldg(reinterpret_cast<const float2 *>(p.fshadow + (size_t)v2 * 64 + fp));
+            const float2 f3 = __ldg(reinterpret_cast<const float2 *>(p.fshadow + (size_t)v3 * 64 + fp));
             float a = fmaf(g.y, f1.y - f0.y, g.x * (f1.x - f0.x));
             float b = fmaf(g.y, f2.y - f0.y, g.x * (f2.x - f0.x));
             float c = fmaf(g.y, f3.y - f0.y, g.x * (f3.x - f0.x));

@@ -31,7 +31,7 @@ int launch_trace_internal(tn_tracer *h, const float *o, const float *d, uint32_t
 
 struct RenderState {
     // field
-    DevArray<float> fshadow;   // [V,64]
+    DevArray<float> fshadow;   // [V,64] in fragment order (field_pos)
     uint32_t V = 0;
     // weights
     DevArray<uint8_t> wimg;    // L1 32K | L2 64K | L3 64K | L4(base part) 64K  (bf16 hi/lo)
@@ -134,7 +134,8 @@ static RenderState *state(tn_tracer *h) {
 }
 
 // ---------------------------------------------------------------------------------------------------
-__global__ void k_transpose64(const float *__restrict__ in, float *__restrict__ out, uint32_t V) {  // [64,V] -> [V,64]
+// [64,V] -> [V,64], each row in fragment order (field_pos)
+__global__ void k_transpose64(const float *__restrict__ in, float *__restrict__ out, uint32_t V) {
     __shared__ float tile[64][33];
     const uint32_t v0 = blockIdx.x * 32;
     for (uint32_t c = threadIdx.y; c < 64; c += blockDim.y) {
@@ -145,8 +146,8 @@ __global__ void k_transpose64(const float *__restrict__ in, float *__restrict__ 
     for (uint32_t r = threadIdx.y; r < 32; r += blockDim.y) {
         const uint32_t v = v0 + r;
         if (v < V) {
-            out[(size_t)v * 64 + threadIdx.x] = tile[threadIdx.x][r];
-            out[(size_t)v * 64 + 32 + threadIdx.x] = tile[32 + threadIdx.x][r];
+            out[(size_t)v * 64 + field_pos(threadIdx.x)] = tile[threadIdx.x][r];
+            out[(size_t)v * 64 + field_pos(32 + threadIdx.x)] = tile[32 + threadIdx.x][r];
         }
     }
 }

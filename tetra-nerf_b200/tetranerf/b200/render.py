@@ -320,6 +320,10 @@ class FusedRenderer:
         return ptr.value
 
     def debug_buffers(self):
+        """test hook: device pointers of the intermediate buffers of the last render, by name.  "fshadow" is the field as the fused
+        MLP reads it, f32[V,64] with each vertex's row in fragment order: within each 16-feature block b, feature
+        16b + 8h + 2t + e (h, e in {0, 1}, t in 0..3) sits at position 16b + 4t + 2h + e, so one 16-byte load gives a thread of
+        a wgmma A fragment row the four features it needs in one k-step (csrc/tn_common.cuh, field_pos)."""
         arr = (_vp * 16)()
         ext._check(_lib.tn_render_debug_buffers(self.tracer.handle, arr))
         names = ["num", "dist", "n_active", "ray_list", "ebins_c", "sbins_c", "vi_c", "bary_c", "dens_c", "ebins_f", "vi_f", "bary_f",
