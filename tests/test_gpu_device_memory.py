@@ -5,6 +5,7 @@ of the process holds.  Each test reads only the change around its own calls, so 
   gradients, a surface extraction) gives back every byte when the tracer is destroyed;
 * repeating an identical training step or render allocates nothing;
 * alternating shapes reach a fixed point once each shape has run (every buffer grows to the larger of its two needs);
+* a saved training step leaves the tracer's own fine-pass state unallocated;
 * calls that fail with an argument, mesh or state error allocate nothing."""
 import contextlib
 import gc
@@ -140,6 +141,19 @@ def test_alternating_shapes_reach_a_fixed_point(small_mesh):
         assert _bytes() == fixed
         _train_step(fr, len(V), b, rb, det=True)
         assert _bytes() == fixed
+
+
+def test_saved_step_leaves_the_tracer_state_unallocated(small_mesh):
+    """the fine pass of a saved training step writes into its blob only, so the first tracer-held forward after it allocates the
+    tracer's own saved-state blob"""
+    V, C = small_mesh
+    tr, fr, _ = _setup(V, C)
+    st = _settings()
+    o, d, jc, jf = rays = _rays(500, st)
+    _saved_step(fr, len(V), st, rays, det=False)
+    b = _bytes()
+    fr.train_forward(o, d, st, jc, jf)
+    assert _bytes() - b >= fr.train_saved_bytes(500, st) - 256
 
 
 def test_failed_calls_allocate_nothing(small_mesh, cube_mesh):

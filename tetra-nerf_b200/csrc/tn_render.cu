@@ -29,6 +29,34 @@ namespace tn {
 int launch_trace_internal(tn_tracer *h, const float *o, const float *d, uint32_t R, uint32_t M, uint32_t *num, uint32_t *cells, float *bary,
                           float *dist, uint32_t *verts, int dense, cudaStream_t s);
 
+// the buffers a render or training forward leaves behind (and a training forward's backward continues from), laid out by saved_layout
+// in a saved-state blob: the caller's (tn_render_train_forward_saved) or the tracer's own (RenderState::own)
+struct TrainBufs {
+    uint32_t *n_active;        // 16-byte block: active rays | tile counter of the coarse pass | of the fine pass | of the normals pass;
+                               // then words 4, 5: the clip bounds of the expected depth, 6, 7: the live rows of the coarse / fine pass
+                               // when the forward culled (in the slot the saved state reserves for the block)
+    uint32_t *ray_list;        // [R] slot -> ray
+    float *ebins_f, *sbins_f;  // [R,S2+1] euclidean / spacing bins of the fine pass
+    uint4 *vi_f;               // [R*S2] matched vertices
+    float *bary_f;             // [R*S2,3] their weights
+    float *out_f;              // [R*S2] (sigma, r, g, b) head pre-activations
+    float *dirbias, *enc;      // [R,128] direction bias, [R,27] encoded direction
+};
+
+// header of a saved-state blob: what a training forward ran with, which its backward continues in
+constexpr uint32_t SAVED_MAGIC = 0x53564e54u;  // "TNVS"
+struct SavedHeader {
+    uint32_t magic, R, M, Sc, Sf, S2, det;
+    uint32_t edepth;           // 1: the forward produced the expected depth (its clip bounds are in words 4, 5 of the n_active slot)
+    float bg[3];
+    uint32_t pad2;
+    uint64_t gen;              // RenderState::gen at the forward
+    uint64_t mesh_gen;         // tn_tracer::mesh_gen at the forward (the ray gradients read the mesh positions)
+    uint32_t cull;             // 1: the forward culled samples by occupancy (its culled rows are marked in vi_f, DESIGN §4.12)
+    uint32_t live_c, live_f;   // culling: the live rows of its coarse / fine pass (copied on the device from the n_active slot)
+    uint32_t pad3;
+};
+
 struct RenderState {
     // field
     DevArray<float> fshadow;   // [V,64] in fragment order (field_pos)
@@ -45,20 +73,17 @@ struct RenderState {
     // workspace
     DevArray<uint32_t> num, cells, verts;  // trace output: [R], [R,M], [R,M,4]
     DevArray<float> bary, dist;            // [R,M,6], [R,M,2]
-    DevArray<uint32_t> n_active, ray_list; // 8 words (see TrainBufs), [R] slot -> ray
     DevArray<float> ebins_c, sbins_c, bary_c, dens_c;  // [R,Sc+1], [R,Sc+1], [R*Sc,3], [R*Sc]
     DevArray<uint4> vi_c;                  // [R*Sc]
-    DevArray<float> ebins_f, bary_f, out_f, dirbias;   // [R,S2+1], [R*S2,3], [R*S2,4], [R,128]
-    DevArray<uint4> vi_f;                  // [R*S2]
+    // the tracer's own fine-pass state (tn_render, tn_render_train_forward): a saved-state blob, its arrays as the last call that wrote
+    // it laid them out, and the host-side header of the last tn_render_train_forward (magic 0: no forward to continue from)
+    DevArray<uint8_t> own;
+    TrainBufs own_b{};
+    SavedHeader last{};
     // training: backward weight image, per-sample head gradients, accumulators (scratch of every backward, saved state or not)
     DevArray<uint8_t> wimg_bwd;        // 7 stages of 32 KB (tn_mlp_bwd.cuh)
-    DevArray<float> sbins_f, enc;      // tn_render_train_forward: [R,S2+1] spacing bins of the fine pass, [R,27] encoded directions (per slot)
     DevArray<float4> dout;             // [R*S2] gradients at the head pre-activations
-    DevArray<float> gshadow, gw, g_dirbias;  // [V,64], [GW_TOTAL], [R,128]
-    // what the last training forward ran with (the backward continues from its buffers)
-    bool train_valid = false;
-    uint32_t t_R = 0, t_M = 0, t_Sc = 0, t_Sf = 0, t_S2 = 0;
-    float t_bg[3] = {1.f, 1.f, 1.f};
+    DevArray<float> gshadow, gw, g_dirbias;  // [V,64], [GW_TOTAL] + the backward kernel's tile counter, [R,128]
     // fused pixel gather (tn_render_set_gather): peer[k] = rank k's [world * rays_per_rank, 6] gathered-pixel buffer
     float *peer[8] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
     uint32_t gather_world = 0, gather_rank = 0, gather_stride = 0;
@@ -68,7 +93,6 @@ struct RenderState {
     cudaEvent_t evb[4] = {nullptr, nullptr, nullptr, nullptr};  // backward: start | composite_bwd | mlp_bwd | finalize
     // deterministic mode (tn_render_set_deterministic): ordered slots in the training forward, fixed-order reductions in its backward
     bool det = false;                  // mode of the next training forward (initial value: TETRANERF_B200_DETERMINISTIC)
-    bool t_det = false;                // mode the last training forward ran in: its backward continues in it
     uint32_t bwd_grid = 0;             // CTAs of the backward MLP kernel (test hook; 0 = default)
     int smem_optin = 0;                // the device's opt-in dynamic shared memory per block (read on the first render call)
     DevArray<uint32_t> ray_flag, ray_slot;  // [R] ray has hits, its slot (exclusive scan)
@@ -91,7 +115,6 @@ struct RenderState {
     float occ_thr = 0.f;
     bool occ_place = false;            // occupancy sampling (DESIGN §4.13): coarse bins in the kept records only
     uint32_t occ_T = 0;                // the mesh's tetrahedron count when the occupancy was set
-    bool t_cull = false;               // the last tracer-held training forward culled
     DevArray<uint8_t> live_flag;
     DevArray<uint32_t> rowmap_c, rowmap_f, rowmap_b, rows_b;
     // tn_occupancy_update: probe rows of one chunk of tetrahedra, their densities, the chunk's row count and tile counter
@@ -1022,21 +1045,19 @@ __global__ void k_occ_reduce(uint32_t t0, uint32_t nt, const float *__restrict__
     occ[t0 + i] = decay == 0.f ? m : fmaxf(decay * occ[t0 + i], m);
 }
 
-static int ensure_ws(RenderState *r, size_t R, size_t M, size_t Sc, size_t S2) {
+// trace and coarse pass (the fine pass writes into a saved-state layout)
+static int ensure_ws(RenderState *r, size_t R, size_t M, size_t Sc) {
     TN_TRY(r->num.grow(R)); TN_TRY(r->cells.grow(R * M)); TN_TRY(r->verts.grow(4 * R * M)); TN_TRY(r->bary.grow(6 * R * M));
     TN_TRY(r->dist.grow(2 * R * M));
-    TN_TRY(r->n_active.grow(8)); TN_TRY(r->ray_list.grow(R));  // n_active words 4, 5: clip bounds of the expected depth
     TN_TRY(r->ebins_c.grow(R * (Sc + 1))); TN_TRY(r->sbins_c.grow(R * (Sc + 1))); TN_TRY(r->bary_c.grow(3 * R * Sc));
     TN_TRY(r->dens_c.grow(R * Sc)); TN_TRY(r->vi_c.grow(R * Sc));
-    TN_TRY(r->ebins_f.grow(R * (S2 + 1))); TN_TRY(r->bary_f.grow(3 * R * S2)); TN_TRY(r->out_f.grow(4 * R * S2));
-    TN_TRY(r->dirbias.grow(128 * R)); TN_TRY(r->vi_f.grow(R * S2));
     return TN_OK;
 }
 
-// training forward: the tracer-held pair's fine bins and encodings, and the gradient scratch of every backward
+// training forward: the gradient scratch of every backward
 static int ensure_train_ws(RenderState *r, size_t R, size_t S2, uint32_t V) {
-    TN_TRY(r->sbins_f.grow(R * (S2 + 1))); TN_TRY(r->enc.grow(27 * R)); TN_TRY(r->dout.grow(R * S2)); TN_TRY(r->g_dirbias.grow(128 * R));
-    TN_TRY(r->gw.grow(GW_TOTAL));
+    TN_TRY(r->dout.grow(R * S2)); TN_TRY(r->g_dirbias.grow(128 * R));
+    TN_TRY(r->gw.grow(GW_TOTAL + 1));
     TN_TRY(r->gshadow.grow(64 * (size_t)V));
     return TN_OK;
 }
@@ -1122,60 +1143,32 @@ extern "C" int tn_render_set_weights(tn_tracer *h, const float *const *P, void *
     return TN_OK;
 }
 
-// the buffers a training forward leaves for its backward: the tracer's own (tn_render_train_forward, the "last call") or those of a
-// caller's saved-state blob (tn_render_train_forward_saved)
-struct TrainBufs {
-    uint32_t *n_active;        // 16-byte block: active rays | tile counter of the coarse pass | of the fine pass | (unused); then words
-                               // 4, 5: the clip bounds of the expected depth, 6, 7: the live rows of the coarse / fine pass when the
-                               // forward culled (in the slot the saved state reserves for the block)
-    uint32_t *ray_list;        // [R] slot -> ray
-    float *ebins_f, *sbins_f;  // [R,S2+1] euclidean / spacing bins of the fine pass
-    uint4 *vi_f;               // [R*S2] matched vertices
-    float *bary_f;             // [R*S2,3] their weights
-    float *out_f;              // [R*S2] (sigma, r, g, b) head pre-activations
-    float *dirbias, *enc;      // [R,128] direction bias, [R,27] encoded direction
-};
-static TrainBufs own_bufs(RenderState *r) {
-    return TrainBufs{r->n_active.p, r->ray_list.p, r->ebins_f.p, r->sbins_f.p, r->vi_f.p, r->bary_f.p, r->out_f.p, r->dirbias.p, r->enc.p};
-}
-
-// saved-state blob of tn_render_train_forward_saved: this header, then the TrainBufs arrays, each 256-byte aligned
-constexpr uint32_t SAVED_MAGIC = 0x53564e54u;  // "TNVS"
-struct SavedHeader {
-    uint32_t magic, R, M, Sc, Sf, S2, det;
-    uint32_t edepth;           // 1: the forward produced the expected depth (its clip bounds are in words 4, 5 of the n_active slot)
-    float bg[3];
-    uint32_t pad2;
-    uint64_t gen;              // RenderState::gen at the forward
-    uint64_t mesh_gen;         // tn_tracer::mesh_gen at the forward (the ray gradients read the mesh positions)
-    uint32_t cull;             // 1: the forward culled samples by occupancy (its culled rows are marked in vi_f, DESIGN §4.12)
-    uint32_t live_c, live_f;   // culling: the live rows of its coarse / fine pass (copied on the device from the n_active slot)
-    uint32_t pad3;
-};
+// saved-state blob: the SavedHeader, then the TrainBufs arrays, each 256-byte aligned
 constexpr size_t SAVED_ALIGN = 256;
 static_assert(sizeof(SavedHeader) <= SAVED_ALIGN, "saved-state header exceeds its slot");
-// bytes of the blob for R rays of S2 fine samples; with base != nullptr also the array pointers inside it
-static size_t saved_layout(size_t R, size_t S2, uint8_t *base, TrainBufs *b) {
+// bytes of the blob for R rays of S2 fine samples; with base != nullptr also the array pointers inside it.  eval: no spacing bins or
+// encodings (nullptr, 0 bytes), which only the backward reads -- the layout of the eval render in the tracer's own blob
+static size_t saved_layout(size_t R, size_t S2, uint8_t *base, TrainBufs *b, bool eval = false) {
     size_t off = SAVED_ALIGN;  // header
     auto take = [&](size_t bytes) { uint8_t *p = base ? base + off : nullptr; off += (bytes + SAVED_ALIGN - 1) / SAVED_ALIGN * SAVED_ALIGN; return p; };
     TrainBufs t{};
     t.n_active = (uint32_t *)take(32);  // (one 256-byte slot either way)
     t.ray_list = (uint32_t *)take(4 * R);
     t.ebins_f = (float *)take(4 * R * (S2 + 1));
-    t.sbins_f = (float *)take(4 * R * (S2 + 1));
+    if (!eval) t.sbins_f = (float *)take(4 * R * (S2 + 1));
     t.vi_f = (uint4 *)take(16 * R * S2);
     t.bary_f = (float *)take(12 * R * S2);
     t.out_f = (float *)take(16 * R * S2);
     t.dirbias = (float *)take(512 * R);
-    t.enc = (float *)take(4 * 27 * R);
+    if (!eval) t.enc = (float *)take(4 * 27 * R);
     if (b) *b = t;
     return off;
 }
 
-// training-mode inputs of the forward (nullptr = eval); saved == nullptr: the tracer's own buffers
+// training-mode inputs of the forward (nullptr = eval); saved == nullptr: the tracer's own blob
 struct TrainFwd {
     const float *jit_c, *jit_f;
-    const TrainBufs *saved;
+    void *saved;
 };
 
 static int render_impl(tn_tracer *h, const tn_render_config *cfg, const float *d_origins, const float *d_directions, uint32_t R,
@@ -1224,11 +1217,15 @@ static int render_impl(tn_tracer *h, const tn_render_config *cfg, const float *d
                                         ", above the device's shared-memory limit of " + std::to_string(r->smem_optin) +
                                         " bytes (fewer samples or a smaller max_ray_triangles)");
     }
-    TN_TRY(ensure_ws(r, R, M, Sc, S2));
+    TN_TRY(ensure_ws(r, R, M, Sc));
+    const bool own = tf == nullptr || tf->saved == nullptr;  // the fine pass writes into the tracer's own blob
+    if (own) TN_TRY(r->own.grow(saved_layout(R, S2, nullptr, nullptr, tf == nullptr)));
     if (d_normals != nullptr) TN_TRY(r->grad_n.grow((size_t)R * S2));
     if (tf != nullptr) TN_TRY(ensure_train_ws(r, R, S2, r->V));
-    r->train_valid = false;
-    const TrainBufs b = tf != nullptr && tf->saved != nullptr ? *tf->saved : own_bufs(r);
+    r->last = SavedHeader{};
+    TrainBufs b{};
+    saved_layout(R, S2, own ? r->own.p : (uint8_t *)tf->saved, &b, tf == nullptr);
+    if (own) r->own_b = b;
     const int prec = tf != nullptr ? 3 : r->mlp_prec;  // the training forward keeps bf16x3 (its backward recomputes in bf16x3)
     TN_CUDA(cudaMemsetAsync(b.n_active, 0, 16, s));
     if (d_edepth != nullptr) {  // clip bounds: min starts at the largest key, max at the smallest
@@ -1334,12 +1331,17 @@ static int render_impl(tn_tracer *h, const tn_render_config *cfg, const float *d
         if (rc) return rc;
         h->launches += 2;
     }
-    if (tf != nullptr && tf->saved == nullptr) {
-        r->train_valid = true;
-        r->t_det = det;
-        r->t_cull = cull;
-        r->t_R = R; r->t_M = M; r->t_Sc = Sc; r->t_Sf = Sf; r->t_S2 = S2;
-        r->t_bg[0] = cfg->background[0]; r->t_bg[1] = cfg->background[1]; r->t_bg[2] = cfg->background[2];
+    if (tf != nullptr) {  // what the backward continues with: kept on the host for the tracer's own blob, in the caller's blob otherwise
+        const SavedHeader hd{SAVED_MAGIC, R, M, Sc, Sf, S2, det ? 1u : 0u, d_edepth != nullptr ? 1u : 0u,
+                             {cfg->background[0], cfg->background[1], cfg->background[2]}, 0, r->gen, h->mesh_gen, cull ? 1u : 0u, 0, 0, 0};
+        if (own) {
+            r->last = hd;
+        } else {
+            // pageable source: staged before the call returns, so `hd` may go out of scope
+            TN_CUDA(cudaMemcpyAsync(tf->saved, &hd, sizeof(hd), cudaMemcpyHostToDevice, s));
+            if (cull)  // the live-row counts, from words 6, 7 of the forward's n_active slot
+                TN_CUDA(cudaMemcpyAsync((uint8_t *)tf->saved + offsetof(SavedHeader, live_c), b.n_active + 6, 8, cudaMemcpyDeviceToDevice, s));
+        }
     }
     return TN_OK;
 }
@@ -1361,21 +1363,23 @@ extern "C" int tn_render_train_forward(tn_tracer *h, const tn_render_config *cfg
     return render_impl(h, cfg, d_origins, d_directions, R, d_rgb, d_acc, d_depth, d_mask, &tf, nullptr, nullptr, stream);
 }
 
-// backward of a training forward of R rays x S2 fine samples whose buffers are `b`, in the mode (det) and with the background it ran
-// with: d_grad_rgb f32[R,3] (dL/d rgb), d_grad_acc f32[R] or NULL (dL/d accumulation) -> d_grad_field f32[64,V] and the twelve MLP
-// parameter gradients (same order / layouts as tn_render_set_weights); every output element is written.  Reads `b` and the field /
-// weights; writes only the tracer's gradient scratch.  The coarse pass carries no gradient (PDFSampler detaches its bins).  No
-// [samples,128] tensor touches HBM.
+// backward of the training forward whose buffers are `b` and whose header is `hd` (R rays x S2 fine samples, continued in the forward's
+// mode and with its background): d_grad_rgb f32[R,3] (dL/d rgb), d_grad_acc f32[R] or NULL (dL/d accumulation) -> d_grad_field
+// f32[64,V] and the twelve MLP parameter gradients (same order / layouts as tn_render_set_weights); every output element is written.
+// Reads `b` and the field / weights; writes only the tracer's gradient scratch.  The coarse pass carries no gradient (PDFSampler
+// detaches its bins).  No [samples,128] tensor touches HBM.
 // d_grad_ed != nullptr: dL/d expected depth f32[R] of a forward that produced it (its clip bounds in b.n_active[4, 5]).
 // d_grad_dist != nullptr: dL/d distortion f32[R] (k_distortion).
 // Any of d_grad_o / d_grad_d / d_grad_xyz != nullptr: also the gradients at the ray origins / directions (tn_ray_grads.cu) and at the
 // mesh vertex positions (tn_vertex_grads.cu), into the non-null ones.
-// cull: the forward culled by occupancy; its map of live fine rows is rebuilt from the culled marks in b.vi_f (never from the occupancy,
-// which may have changed since)
-static int train_backward_impl(tn_tracer *h, const TrainBufs &b, uint32_t R, uint32_t S2, bool det, bool cull, const float *bg, const float *d_grad_rgb,
-                               const float *d_grad_acc, const float *d_grad_ed, const float *d_grad_dist, int use_gradient_scaling, float *d_grad_field,
+// hd.cull: the forward culled by occupancy; its map of live fine rows is rebuilt from the culled marks in b.vi_f (never from the
+// occupancy, which may have changed since)
+static int train_backward_impl(tn_tracer *h, const TrainBufs &b, const SavedHeader &hd, const float *d_grad_rgb, const float *d_grad_acc,
+                               const float *d_grad_ed, const float *d_grad_dist, int use_gradient_scaling, float *d_grad_field,
                                float *const *d_grad_params12, float *d_grad_o, float *d_grad_d, float *d_grad_xyz, cudaStream_t s) {
     RenderState *r = h->render;
+    const uint32_t R = hd.R, S2 = hd.S2;
+    const bool det = hd.det != 0, cull = hd.cull != 0;
     int sms = 132;
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, h->device);
     const uint32_t V = r->V;
@@ -1386,17 +1390,15 @@ static int train_backward_impl(tn_tracer *h, const TrainBufs &b, uint32_t R, uin
         if (!det) TN_TRY(r->ray_dx.grow(64 * rows));
         TN_TRY(r->ray_gx.grow(rows));
     }
-    TN_CUDA(cudaMemsetAsync(r->gw.p, 0, sizeof(float) * GW_TOTAL, s));
+    TN_CUDA(cudaMemsetAsync(r->gw.p, 0, sizeof(float) * (GW_TOTAL + 1), s));  // the accumulators and the tile counter after them
     if (!det) {  // (deterministic mode writes every element of these)
         TN_CUDA(cudaMemsetAsync(r->gshadow.p, 0, sizeof(float) * 64 * (size_t)V, s));
         TN_CUDA(cudaMemsetAsync(r->g_dirbias.p, 0, 512 * (size_t)R, s));
-        // tile counter of the backward kernel: word 3 of the tracer's own 16-byte block (scratch even when `b` is a saved state)
-        TN_CUDA(cudaMemsetAsync(r->n_active.p + 3, 0, 4, s));
     }
     CompositeBwdParams cb{};
     cb.S2 = S2; cb.use_gradient_scaling = use_gradient_scaling ? 1u : 0u; cb.n_active = b.n_active; cb.ray_list = b.ray_list;
     cb.ebins_f = b.ebins_f; cb.sbins_f = b.sbins_f; cb.out_f = b.out_f; cb.grad_rgb = d_grad_rgb; cb.grad_acc = d_grad_acc;
-    cb.bg0 = bg[0]; cb.bg1 = bg[1]; cb.bg2 = bg[2]; cb.dout = r->dout.p; cb.sums = det ? (float *)r->det_sums.p : r->gw.p + GW_SUMS;
+    cb.bg0 = hd.bg[0]; cb.bg1 = hd.bg[1]; cb.bg2 = hd.bg[2]; cb.dout = r->dout.p; cb.sums = det ? (float *)r->det_sums.p : r->gw.p + GW_SUMS;
     cb.grad_ed = d_grad_ed; cb.dbounds = b.n_active + 4; cb.grad_dist = d_grad_dist;
     const size_t smem_cb = SAMPLE_WARPS * sizeof(float) * 4 * ((size_t)S2 + 2);
     auto k_cbwd = d_grad_dist != nullptr
@@ -1412,7 +1414,8 @@ static int train_backward_impl(tn_tracer *h, const TrainBufs &b, uint32_t R, uin
     MlpBwdParams bp{};
     bp.n_active = b.n_active; bp.S = S2; bp.vi = b.vi_f; bp.bary = b.bary_f; bp.fshadow = r->fshadow.p; bp.wimg = r->wimg_bwd.p;
     bp.bias = r->bias.p; bp.head = r->head.p; bp.dirbias = b.dirbias; bp.dout = r->dout.p; bp.gshadow = r->gshadow.p;
-    bp.gw = r->gw.p; bp.g_dirbias = r->g_dirbias.p; bp.tile_ctr = r->n_active.p + 3;
+    bp.gw = r->gw.p; bp.g_dirbias = r->g_dirbias.p;
+    bp.tile_ctr = reinterpret_cast<uint32_t *>(r->gw.p + GW_TOTAL);  // (default mode only: the deterministic kernel has no tile counter)
     if (cull) {
         TN_TRY(r->rows_b.grow(1));
         TN_TRY(compact_rows(h, r, b.n_active, S2, R, b.vi_f, nullptr, 0, r->rowmap_b, r->rows_b.p, s));
@@ -1501,10 +1504,10 @@ extern "C" int tn_render_train_backward(tn_tracer *h, const float *d_grad_rgb, c
                                         float *d_grad_field, float *const *d_grad_params12, void *stream) {
     if (!h || !d_grad_rgb || !d_grad_field || !d_grad_params12) return fail(TN_ERR_ARG, "null argument");
     RenderState *r = h->render;
-    if (!r || !r->train_valid) return fail(TN_ERR_STATE, "tn_render_train_backward: no training forward to continue from");
+    if (!r || r->last.magic != SAVED_MAGIC) return fail(TN_ERR_STATE, "tn_render_train_backward: no training forward to continue from");
     DeviceGuard g(h->device);
-    return train_backward_impl(h, own_bufs(r), r->t_R, r->t_S2, r->t_det, r->t_cull, r->t_bg, d_grad_rgb, d_grad_acc, nullptr, nullptr, use_gradient_scaling,
-                               d_grad_field, d_grad_params12, nullptr, nullptr, nullptr, (cudaStream_t)stream);
+    return train_backward_impl(h, r->own_b, r->last, d_grad_rgb, d_grad_acc, nullptr, nullptr, use_gradient_scaling, d_grad_field, d_grad_params12,
+                               nullptr, nullptr, nullptr, (cudaStream_t)stream);
 }
 
 // ---- the training pair with per-call saved state: everything the backward reads that a later call could overwrite goes to the
@@ -1537,30 +1540,17 @@ extern "C" int tn_render_train_forward_saved(tn_tracer *h, const tn_render_confi
     int rc = saved_shape(cfg, R, &S2);
     if (rc) return rc;
     if ((uintptr_t)d_saved % SAVED_ALIGN) return fail(TN_ERR_ARG, "tn_render_train_forward_saved: d_saved must be 256-byte aligned");
-    TrainBufs b{};
-    if (saved_bytes < saved_layout(R, S2, (uint8_t *)d_saved, &b))
+    if (saved_bytes < saved_layout(R, S2, nullptr, nullptr))
         return fail(TN_ERR_ARG, "tn_render_train_forward_saved: saved_bytes is smaller than tn_render_train_saved_bytes");
-    TrainFwd tf{d_jitter_coarse, d_jitter_fine, &b};
-    rc = render_impl(h, cfg, d_origins, d_directions, R, d_rgb, d_acc, d_depth, d_mask, &tf, nullptr, d_expected_depth, stream);
-    if (rc) return rc;
-    RenderState *r = h->render;
-    const bool cull = r->occ != nullptr;
-    const SavedHeader hd{SAVED_MAGIC, R, cfg->max_ray_triangles, cfg->num_samples, cfg->num_fine_samples, S2, r->det ? 1u : 0u,
-                         d_expected_depth != nullptr ? 1u : 0u, {cfg->background[0], cfg->background[1], cfg->background[2]}, 0, r->gen,
-                         h->mesh_gen, cull ? 1u : 0u, 0, 0, 0};
-    DeviceGuard g(h->device);
-    // pageable source: staged before the call returns, so `hd` may go out of scope
-    TN_CUDA(cudaMemcpyAsync(d_saved, &hd, sizeof(hd), cudaMemcpyHostToDevice, (cudaStream_t)stream));
-    if (cull)  // the live-row counts, from words 6, 7 of the forward's n_active slot
-        TN_CUDA(cudaMemcpyAsync((uint8_t *)d_saved + offsetof(SavedHeader, live_c), b.n_active + 6, 8, cudaMemcpyDeviceToDevice, (cudaStream_t)stream));
-    return TN_OK;
+    TrainFwd tf{d_jitter_coarse, d_jitter_fine, d_saved};
+    return render_impl(h, cfg, d_origins, d_directions, R, d_rgb, d_acc, d_depth, d_mask, &tf, nullptr, d_expected_depth, stream);
 }
 
 // the header of a saved state, read back to the host (waits until the stream has reached the caller), if it belongs to the current
 // field and weights of this tracer; `what` names the caller in the errors
 static int read_saved_header(tn_tracer *h, const void *d_saved, cudaStream_t s, const char *what, SavedHeader *hd) {
     RenderState *r = h->render;
-    if (!r || !r->n_active.p) return fail(TN_ERR_STATE, std::string(what) + ": no training forward on this tracer");
+    if (!r || !r->gw.p) return fail(TN_ERR_STATE, std::string(what) + ": no training forward on this tracer");
     TN_CUDA(cudaMemcpyAsync(hd, d_saved, sizeof(*hd), cudaMemcpyDeviceToHost, s));
     TN_CUDA(cudaStreamSynchronize(s));
     if (hd->magic != SAVED_MAGIC) return fail(TN_ERR_STATE, std::string(what) + ": d_saved holds no training forward");
@@ -1592,8 +1582,8 @@ extern "C" int tn_render_train_backward_saved2(tn_tracer *h, const void *d_saved
                                   "tn_render_train_forward_saved)");
     TrainBufs b{};
     saved_layout(hd.R, hd.S2, (uint8_t *)d_saved, &b);
-    return train_backward_impl(h, b, hd.R, hd.S2, hd.det != 0, hd.cull != 0, hd.bg, d_grad_rgb, d_grad_acc, d_grad_expected_depth, d_grad_distortion,
-                               use_gradient_scaling, d_grad_field, d_grad_params12, d_grad_origins, d_grad_directions, d_grad_xyz, s);
+    return train_backward_impl(h, b, hd, d_grad_rgb, d_grad_acc, d_grad_expected_depth, d_grad_distortion, use_gradient_scaling, d_grad_field,
+                               d_grad_params12, d_grad_origins, d_grad_directions, d_grad_xyz, s);
 }
 
 extern "C" int tn_render_train_backward_saved(tn_tracer *h, const void *d_saved, const float *d_grad_rgb, const float *d_grad_acc,
@@ -1739,12 +1729,14 @@ extern "C" int tn_render_get_backward_timings(tn_tracer *h, float *ms3) {
     return TN_OK;
 }
 
-// test / debug hook: device pointers of the intermediate buffers of the last tn_render call
+// test / debug hook: device pointers of the intermediate buffers of the last tn_render call (the fine pass's: of the last call that wrote
+// the tracer's own blob)
 extern "C" int tn_render_debug_buffers(tn_tracer *h, void **ptrs16) {
     if (!h || !h->render) return fail(TN_ERR_STATE, "no render state");
     RenderState *r = h->render;
-    void *v[16] = {r->num.p, r->dist.p, r->n_active.p, r->ray_list.p, r->ebins_c.p, r->sbins_c.p, r->vi_c.p, r->bary_c.p,
-                   r->dens_c.p, r->ebins_f.p, r->vi_f.p, r->bary_f.p, r->out_f.p, r->dirbias.p, r->fshadow.p, r->wimg.p};
+    const TrainBufs &b = r->own_b;
+    void *v[16] = {r->num.p, r->dist.p, b.n_active, b.ray_list, r->ebins_c.p, r->sbins_c.p, r->vi_c.p, r->bary_c.p,
+                   r->dens_c.p, b.ebins_f, b.vi_f, b.bary_f, b.out_f, b.dirbias, r->fshadow.p, r->wimg.p};
     for (int i = 0; i < 16; ++i) ptrs16[i] = v[i];
     return TN_OK;
 }
