@@ -109,6 +109,28 @@ int tn_interpolate_values_backward_deterministic(int device, uint32_t D, uint32_
                                                  const float *d_w, const float *d_grad_in, float *d_grad_field, void *d_workspace,
                                                  size_t *workspace_bytes, void *stream);
 
+/* ---- mesh refinement: one pass of longest-edge bisection (DESIGN.md §4.14).  A pure function of device arrays (no tracer): d_xyz
+ * f32[V,3], d_cells u32[T,4], d_candidates u8[T] (non-zero = candidate).  Edge {a, b} has key (min << 32) | max and squared length
+ * ((xa-xb)^2 + (ya-yb)^2) + (za-zb)^2 in float64 from the fp32 coordinates, every operation rounded on its own; priority is the larger
+ * squared length, ties to the smaller key, and a tetrahedron's longest edge is the highest-priority one of its six.
+ *   propose: each candidate whose longest edge has squared length >= (double)min_length^2 proposes it; P = the sorted distinct proposals;
+ *   vote:    each tetrahedron with an edge in P votes for its highest-priority such edge;
+ *   accept:  an edge of P is accepted iff every tetrahedron around it voted for it (so accepted edges share no tetrahedron, and the
+ *            highest-priority proposal is always accepted); beyond max_new_vertices the highest-priority accepted edges are kept;
+ *   split:   kept edges in ascending key order become vertices V, V+1, ...; each tetrahedron around kept edge (a, b) keeps its slot
+ *            with b replaced by the new vertex m and appends a child at T + rank (rank = its position among the split tetrahedra, in
+ *            index order) with a replaced by m: each half has half the parent's signed volume and its orientation.
+ * Outputs (capacities the caller provides: d_cells_out u32[2T,4], d_parent_cell u32[2T], d_parent_edge u32[min(T, max_new_vertices),2]):
+ * d_cells_out[:T + n_split], d_parent_edge[:n_new] = (a, b), a < b, of vertex V + i, d_parent_cell[:T + n_split] (identity on the first
+ * T, the split parent after).  counts3 (host) = n_proposed (|P|), n_new (kept edges = new vertices), n_split.  New positions and field
+ * values are not computed here: (x_a + x_b) * 0.5 per vertex tensor (tetranerf/b200/refine.py).  The output depends on the inputs only,
+ * bitwise.  TN_ERR_ARG for a vertex index >= V, V + max_new_vertices > 2^32 - 1 or min_length < 0.  Workspace as
+ * tn_interpolate_values_backward_deterministic: d_workspace == NULL writes the size to *workspace_bytes and does nothing else (60 bytes
+ * per tetrahedron plus CUB's temporary storage: 129.7 MB at 2.02 M tetrahedra on an H100).  Synchronous (three small read-backs). */
+int tn_refine_edges(int device, const float *d_xyz, uint32_t V, const uint32_t *d_cells, uint32_t T, const uint8_t *d_candidates,
+                    float min_length, uint32_t max_new_vertices, uint32_t *d_cells_out, uint32_t *d_parent_edge, uint32_t *d_parent_cell,
+                    uint32_t *counts3, void *d_workspace, size_t *workspace_bytes, void *stream);
+
 /* ---- fused forward render (new; replaces model.py:531-662 between trace_rays and the pixel) -------
  * Weights are passed once (tn_render_set_weights) in nerfstudio state-dict layout and repacked on
  * the device.  See DESIGN.md §"fused render". */

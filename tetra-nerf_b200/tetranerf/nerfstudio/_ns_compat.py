@@ -3,15 +3,15 @@
 nerfstudio is an un-vendored dependency of the reference (setup.py:133) and is not installed in this
 environment; `model.py` imports the real package when it is available and falls back to these look-alikes
 otherwise, so that the drop-in `TetrahedraNerf` / `TetrahedraSampler` API can be exercised (tests, bench).
-Only what model.py:10-28 imports is provided, with the arithmetic of nerfstudio 0.3.x restated (same
+Only what model.py imports is provided (plus `Optimizers`, what the training callbacks receive), with the arithmetic of nerfstudio 0.3.x restated (same
 restatement as oracle/oracle.py, which is the parity reference for these pieces).
 """
 from __future__ import annotations
 
 import dataclasses
 from dataclasses import dataclass, field
-from enum import Enum
-from typing import Any, Callable, Dict, Optional, Type
+from enum import Enum, auto
+from typing import Any, Callable, Dict, List, Optional, Tuple, Type
 
 import torch
 from torch import nn
@@ -319,3 +319,61 @@ class Model(nn.Module):
 
 def scale_dict(d: Dict[str, torch.Tensor], coefficients: Dict[str, float]) -> Dict[str, torch.Tensor]:
     return {k: (v * coefficients[k] if k in coefficients else v) for k, v in d.items()}
+
+
+# ---- engine/callbacks.py, engine/optimizers.py --------------------------------------------------------
+class TrainingCallbackLocation(Enum):
+    BEFORE_TRAIN_ITERATION = auto()
+    AFTER_TRAIN_ITERATION = auto()
+
+
+@dataclass
+class TrainingCallbackAttributes:
+    optimizers: Optional["Optimizers"] = None
+    grad_scaler: Optional[Any] = None
+    pipeline: Optional[Any] = None
+
+
+class TrainingCallback:
+    """func(*args, **kwargs, step=step) at the locations in where_to_run, every update_every_num_iters steps or at the listed iters"""
+
+    def __init__(self, where_to_run: List[TrainingCallbackLocation], func: Callable, update_every_num_iters: Optional[int] = None,
+                 iters: Optional[Tuple[int, ...]] = None, args: Optional[List] = None, kwargs: Optional[Dict] = None):
+        assert update_every_num_iters is None or iters is None, "only one of update_every_num_iters and iters"
+        self.where_to_run, self.func, self.update_every_num_iters, self.iters = where_to_run, func, update_every_num_iters, iters
+        self.args, self.kwargs = args or [], kwargs or {}
+
+    def run_callback(self, step: int) -> None:
+        if self.update_every_num_iters is not None:
+            if step % self.update_every_num_iters == 0:
+                self.func(*self.args, **self.kwargs, step=step)
+        elif self.iters is not None:
+            if step in self.iters:
+                self.func(*self.args, **self.kwargs, step=step)
+        else:
+            self.func(*self.args, **self.kwargs, step=step)
+
+    def run_callback_at_location(self, step: int, location: TrainingCallbackLocation) -> None:
+        if location in self.where_to_run:
+            self.run_callback(step=step)
+
+
+class Optimizers:
+    """one torch optimizer per param group: `config` maps a group name to {"optimizer": factory(params) -> torch.optim.Optimizer}"""
+
+    def __init__(self, config: Dict[str, Dict[str, Callable]], param_groups: Dict[str, List[nn.Parameter]]):
+        self.config = config
+        self.optimizers = {name: config[name]["optimizer"](params) for name, params in param_groups.items()}
+        self.parameters = {name: params for name, params in param_groups.items()}
+
+    def zero_grad_all(self) -> None:
+        for opt in self.optimizers.values():
+            opt.zero_grad()
+
+    def optimizer_step_all(self) -> None:
+        for opt in self.optimizers.values():
+            opt.step()
+
+    def load_optimizers(self, loaded_state: Dict[str, Any]) -> None:
+        for k, v in loaded_state.items():
+            self.optimizers[k].load_state_dict(v)

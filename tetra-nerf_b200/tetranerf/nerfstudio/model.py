@@ -33,6 +33,7 @@ from torch.nn import Parameter
 
 try:  # the real thing when available (reference model.py:10-28)
     from nerfstudio.cameras.rays import RayBundle, RaySamples
+    from nerfstudio.engine.callbacks import TrainingCallback, TrainingCallbackAttributes, TrainingCallbackLocation
     from nerfstudio.field_components.encodings import NeRFEncoding
     from nerfstudio.field_components.field_heads import DensityFieldHead, FieldHeadNames, RGBFieldHead
     from nerfstudio.field_components.mlp import MLP
@@ -45,7 +46,8 @@ try:  # the real thing when available (reference model.py:10-28)
     HAVE_NERFSTUDIO = True
 except ImportError:
     from ._ns_compat import (AccumulationRenderer, DensityFieldHead, DepthRenderer, FieldHeadNames, MLP, MSELoss, Model, ModelConfig,
-                             NeRFEncoding, PDFSampler, RayBundle, RaySamples, RGBFieldHead, RGBRenderer, Sampler, UniformSampler, scale_dict)
+                             NeRFEncoding, PDFSampler, RayBundle, RaySamples, RGBFieldHead, RGBRenderer, Sampler, TrainingCallback,
+                             TrainingCallbackAttributes, TrainingCallbackLocation, UniformSampler, scale_dict)
 
     HAVE_NERFSTUDIO = False
 
@@ -108,6 +110,26 @@ class TetrahedraNerfConfig(ModelConfig):
     """> 0: training outputs also hold "distortion" f32[R,1], mip-NeRF 360's distortion of each ray's weights over its spacing bins (0 on
     empty rays; DESIGN §4.11), and the loss dict gains distortion_loss = distortion_loss_mult * its mean over the rays with hits, as
     nerfacto's distortion_loss_mult.  Training only; 0 changes nothing"""
+    refine_every: int = 0
+    """> 0: refine the mesh during training every refine_every steps in [refine_start, refine_stop) (TetrahedraNerf.refine, DESIGN §4.14):
+    the tetrahedra whose field gradient stays large have their longest edges bisected, the new vertices taking the mean of their edge's
+    endpoints, so the field is unchanged and the optimizer gains degrees of freedom where the images need them.  0 = off, nothing
+    changes.  With use_biased_sampler a refined ray shares its samples over more records, so renders are not preserved at the moment of
+    refinement (by design; the uniform sampler preserves them).  Refinement raises the number of tetrahedra per ray: watch that
+    max_intersected_triangles still covers the rays.  The refined mesh is no longer Delaunay, which nothing downstream requires"""
+    refine_start: int = 500
+    """first training step at which the mesh may be refined"""
+    refine_stop: int = 15000
+    """no refinement from this training step on"""
+    refine_fraction: float = 0.05
+    """share of the tetrahedra that are candidates in one refinement: the highest-scoring ones with a score > 0, a tetrahedron scoring the
+    mean over its vertices of the mean per-step gradient norm of their field column since the last refinement"""
+    refine_passes: int = 3
+    """bisection passes per refinement; a tetrahedron split in one pass, and its children, are not candidates again in the same one"""
+    refine_min_edge_length: float = 0.0
+    """a candidate proposes its longest edge only when that is at least this long"""
+    refine_max_vertices: Optional[int] = None
+    """refinement stops adding vertices at this many mesh vertices (None: no limit)"""
 
     def __post_init__(self):
         if self.tetrahedra_path is not None and self.num_tetrahedra_vertices is None:
@@ -209,6 +231,7 @@ class TetrahedraNerf(Model):
         self._tetrahedra_tracer = None
         self._fused = None
         self._fused_versions = None
+        self._grad_acc = self._grad_cnt = None  # refinement statistics (refine_every > 0): not part of the state dict
         if self.config.tetrahedra_path is None and metadata is not None and "points3D_xyz" in metadata:
             self._load_points_from_metadata(**metadata)
         else:
@@ -237,6 +260,18 @@ class TetrahedraNerf(Model):
     def _load_from_state_dict(self, state_dict, prefix, *args, **kwargs):
         complete = all(f"{prefix}{k}" in state_dict for k in ("tetrahedra_vertices", "tetrahedra_cells", "tetrahedra_field"))
         self._occ_ready = False  # a loaded buffer is checked for zeros again
+        # a refined checkpoint holds more vertices and tetrahedra than the config the model was built from: take its sizes in place,
+        # through .data, so the Parameter objects an optimizer built before the load holds stay the model's (DESIGN §4.14)
+        resized = False
+        for name in ("tetrahedra_vertices", "tetrahedra_cells", "tetrahedra_field", "tetrahedra_occupancy"):
+            cur, new = getattr(self, name, None), state_dict.get(prefix + name)
+            if isinstance(cur, torch.Tensor) and isinstance(new, torch.Tensor) and new.shape != cur.shape:
+                _set_data(cur, torch.empty(new.shape, dtype=cur.dtype, device=cur.device))
+                resized = True
+        if resized:
+            self.config.num_tetrahedra_vertices, self.config.num_tetrahedra_cells = len(self.tetrahedra_vertices), len(self.tetrahedra_cells)
+            self._tetrahedra_tracer = self._fused = self._fused_versions = None
+            self._grad_acc = self._grad_cnt = None
         super()._load_from_state_dict(state_dict, prefix, *args, **kwargs)
         if complete:
             self._tetrahedra_initialized = True
@@ -543,6 +578,120 @@ class TetrahedraNerf(Model):
                 outputs["distortion"][ray_mask] = distortion_per_ray(weights, sdist)
         return outputs
 
+    # ---- mesh refinement (DESIGN §4.14) ------------------------------------------------------------------------------------------------
+    def get_training_callbacks(self, training_callback_attributes: TrainingCallbackAttributes) -> List[TrainingCallback]:
+        """with refine_every > 0: after every training iteration, the field-gradient statistics; every refine_every steps in
+        [refine_start, refine_stop), `refine` with the trainer's optimizers.  None otherwise"""
+        c = self.config
+        if c.refine_every <= 0:
+            return []
+        optimizers = training_callback_attributes.optimizers
+
+        def refine(step: int):
+            if c.refine_start <= step < c.refine_stop and step % c.refine_every == 0:
+                self.refine(optimizers)
+
+        after = [TrainingCallbackLocation.AFTER_TRAIN_ITERATION]
+        return [TrainingCallback(after, lambda step: self.accumulate_refine_statistics()), TrainingCallback(after, refine)]
+
+    def accumulate_refine_statistics(self) -> None:
+        """acc_v += ||dL/dF[:, v]||_2 and cnt_v += 1 where that column is non-zero, from the field gradient of the step that just ran
+        (before it is zeroed; under DDP the all-reduced one, so every rank decides alike).  No gradient: nothing happens"""
+        g = self.tetrahedra_field.grad
+        if g is None:
+            return
+        with torch.no_grad():
+            norm = torch.linalg.vector_norm(g, dim=0)
+            if self._grad_acc is None or self._grad_acc.shape != norm.shape or self._grad_acc.device != norm.device:
+                self._grad_acc = torch.zeros_like(norm)
+                self._grad_cnt = torch.zeros(norm.shape, dtype=torch.int32, device=norm.device)
+            self._grad_acc += norm
+            self._grad_cnt += (norm > 0).to(torch.int32)
+
+    def refine(self, optimizers=None) -> Dict[str, Any]:
+        """bisects the longest edges of the tetrahedra whose field gradient stayed large since the last call: up to refine_passes
+        passes of `tetranerf.b200.refine.refine_edges` over the refine_fraction highest-scoring tetrahedra (score: the mean over its
+        vertices of acc_v / max(cnt_v, 1)), stopping at refine_max_vertices.  The field, the positions, the occupancy and, in
+        `optimizers` (nerfstudio's Optimizers, a dict of torch optimizers or one optimizer), every per-vertex state tensor of the field
+        and vertex parameters (RAdam's exp_avg / exp_avg_sq; `step` is kept) are carried over: new vertices take their edge's
+        endpoint average, new tetrahedra their parent's occupancy.  The Parameter objects stay the same; their .grad is cleared.  The
+        tracer is reloaded and the statistics reset.  -> counts before / after, per-pass proposals and acceptances, seconds taken"""
+        import time
+
+        from ..b200 import refine as rf
+
+        c = self.config
+        t0 = time.perf_counter()
+        V0, T0 = len(self.tetrahedra_vertices), len(self.tetrahedra_cells)
+        res: Dict[str, Any] = {"vertices_before": V0, "tetrahedra_before": T0, "passes": []}
+        field = self.tetrahedra_field
+        dev = field.device
+        if self._grad_acc is not None and len(self._grad_acc) == V0:
+            score = self._grad_acc / self._grad_cnt.clamp_min(1).to(self._grad_acc.dtype)
+        else:
+            score = torch.zeros((V0,), dtype=torch.float32, device=dev)
+        with torch.no_grad():
+            xyz, cells = self.tetrahedra_vertices.detach(), self.tetrahedra_cells
+            cand = rf.select_candidates(score.to(dev), cells, c.refine_fraction)
+            parent_edges, parent_cells = [], []
+            for _ in range(max(0, c.refine_passes)):
+                room = None if c.refine_max_vertices is None else c.refine_max_vertices - len(xyz)
+                if (room is not None and room <= 0) or not bool(cand.any()):
+                    break
+                out = rf.refine_edges(xyz, cells, cand, c.refine_min_edge_length, room)
+                res["passes"].append({"proposed": out["n_proposed"], "accepted": out["n_accepted"], "split": out["n_split"]})
+                if out["n_accepted"] == 0:
+                    break
+                T = len(cells)
+                split = torch.zeros((T,), dtype=torch.bool, device=dev)
+                split[out["parent_cell"][T:].long()] = True
+                cand = torch.cat((cand & ~split, torch.zeros((out["n_split"],), dtype=torch.bool, device=dev)))
+                xyz, cells = rf.migrate_vertices(xyz, out["parent_edge"], 0), out["cells"]
+                parent_edges.append(out["parent_edge"])
+                parent_cells.append(out["parent_cell"])
+            if parent_edges:
+                self._apply_refinement(parent_edges, parent_cells, xyz, cells, optimizers)
+        res["vertices_after"], res["tetrahedra_after"] = len(self.tetrahedra_vertices), len(self.tetrahedra_cells)
+        self._grad_acc = self._grad_cnt = None
+        if dev.type == "cuda":
+            torch.cuda.synchronize(dev)
+        res["seconds"] = time.perf_counter() - t0
+        return res
+
+    def _apply_refinement(self, parent_edges, parent_cells, xyz, cells, optimizers) -> None:
+        """installs the refined mesh (xyz, cells) after the passes given by their parent_edge / parent_cell tables"""
+        from ..b200 import refine as rf
+
+        def per_vertex(t, dim):
+            for pe in parent_edges:
+                t = rf.migrate_vertices(t, pe, dim)
+            return t
+
+        params = [(self.tetrahedra_field, 1)] + ([(self.tetrahedra_vertices, 0)] if self.config.optimize_vertices else [])
+        opts = getattr(optimizers, "optimizers", optimizers)
+        opts = list(opts.values()) if isinstance(opts, dict) else ([] if opts is None else [opts])
+        for p, dim in params:
+            old_shape = p.shape
+            for opt in opts:
+                st = opt.state.get(p)
+                for k, v in (st or {}).items():
+                    if isinstance(v, torch.Tensor) and v.shape == old_shape:  # exp_avg, exp_avg_sq (not the scalar step)
+                        st[k] = per_vertex(v, dim)
+        _set_data(self.tetrahedra_field, per_vertex(self.tetrahedra_field.data, 1))
+        self.tetrahedra_field.grad = None
+        _set_data(self.tetrahedra_vertices, xyz)
+        self.tetrahedra_vertices.grad = None
+        if self.config.use_occupancy_field:
+            occ = self.tetrahedra_occupancy.data
+            for pc in parent_cells:
+                occ = rf.migrate_cells(occ, pc)
+            self.tetrahedra_occupancy.data = occ
+        self.tetrahedra_cells.data = cells.contiguous()
+        self.config.num_tetrahedra_vertices, self.config.num_tetrahedra_cells = len(xyz), len(cells)
+        if self._tetrahedra_tracer is not None:
+            self._tetrahedra_tracer.load_tetrahedra(self.tetrahedra_vertices.detach(), self.tetrahedra_cells)
+            self._tracer_vertices = (self.tetrahedra_vertices.data_ptr(), len(xyz), self.tetrahedra_vertices._version)
+
     # ---- geometry export -----------------------------------------------------------------------------------------------------------------
     def extract_surface(self, level: float) -> Dict[str, torch.Tensor]:
         """the density iso-surface sigma = level of the trained field as a triangle mesh, by marching tetrahedra on the model's own
@@ -597,6 +746,14 @@ class TetrahedraNerf(Model):
         if lp is not None:
             metrics["lpips"] = float(lp)
         return metrics, images
+
+
+def _set_data(t: torch.Tensor, new: torch.Tensor) -> None:
+    """t.data = new for a `new` of another shape.  Autograd caches a leaf's gradient accumulator, with the leaf's shape, for as long as
+    a graph that reaches it is alive (the previous step's loss usually is), and `.data =` drops that cache only on a dtype or device
+    change: so the data passes through an empty tensor of another dtype first, and the next graph gets an accumulator of the new shape"""
+    t.data = torch.empty(0, dtype=torch.float64 if new.dtype != torch.float64 else torch.float32, device=new.device)
+    t.data = new
 
 
 def _psnr(a: torch.Tensor, b: torch.Tensor, data_range: float = 1.0) -> torch.Tensor:
