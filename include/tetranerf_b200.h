@@ -39,14 +39,15 @@ int tn_synchronize(tn_tracer *h, void *stream);
  * src/tetrahedra_tracer.cpp:244-340 (unique-face build :45-71 + acceleration structure).
  * Borrows d_xyz / d_cells (caller keeps them alive, as the reference, tetrahedra_tracer.h:300-303).
  * Returns TN_ERR_MESH "A triangle is shared by more than two tetrahedra!" like :64-66.
+ * The adjacency walk is on iff the hull is a closed convex surface and no interior face is folded (the fold test of
+ * tn_update_vertices); otherwise every trace takes the all-hits gather.  Either way a trace gives the bits of the all-hits gather.
  * Synchronous (the face table is sized on the host). */
 int tn_load_tetrahedra(tn_tracer *h, const float *d_xyz, uint32_t V, const uint32_t *d_cells, uint32_t T, void *stream);
 /* Moves the loaded mesh's vertices to d_xyz f32[V,3] (same V, same cells; borrowed like load_tetrahedra's) and refits the tracer in
  * place: the positions in the leaf and walk records, the boxes of both BVHs (the load's Morton order is kept) and the coordinate bound.
  * Every trace afterwards gives the same bits as the all-hits gather of a fresh tn_load_tetrahedra at d_xyz (the reference's algorithm
- * on any triangle soup), and while the walk stays on, the same bits as its walk.  (A fresh load has no fold test: on a folded mesh it may
- * still take the walk, whose results there are not covered by this guarantee.)  The adjacency walk stays on iff the mesh was
- * walkable at load, its hull is still convex and no interior face is folded: *folded_faces (may be NULL) receives the number of interior
+ * on any triangle soup), and while the walk stays on, the same bits as its walk.  The adjacency walk is on iff the hull was a closed
+ * convex surface at load and still is, and no interior face is folded: *folded_faces (may be NULL) receives the number of interior
  * faces whose two opposite vertices are not certified (float64 orient3d on the fp32 positions, with a forward error bound) to lie strictly
  * on opposite sides; *walkable (may be NULL) whether the walk is on.  Otherwise every trace takes the all-hits gather.  TN_ERR_ARG if V
  * differs from the load's or a coordinate is not finite (the tracer is then unchanged).  Like tn_load_tetrahedra, it starts a new mesh

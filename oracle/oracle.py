@@ -54,6 +54,8 @@ def lib() -> C.CDLL:
         _LIB.orc_mesh_num_faces.argtypes = [C.c_void_p]
         _LIB.orc_mesh_faces.argtypes = [C.c_void_p, u32p, u32p]
         _LIB.orc_ray_tri.argtypes = [f32p] * 6
+        _LIB.orc_ray_tri_pairs.argtypes = [f32p, f32p, f32p, C.c_uint32, u32p, u32p, u8p, f32p, C.c_int]
+        _LIB.orc_ray_tri_pairs.restype = None
         _LIB.orc_trace.argtypes = [C.c_void_p, f32p, f32p, C.c_uint32, C.c_uint32, u32p, u32p, f32p, f32p, u32p, C.c_int, C.c_int]
         _LIB.orc_trace_triangles.argtypes = [C.c_void_p, f32p, f32p, C.c_uint32, C.c_uint32, u32p, u32p, f32p, f32p, u32p, C.c_int, C.c_int]
         _LIB.orc_post_process_one.argtypes = [C.c_void_p, C.c_uint32, C.c_uint32, u32p, f32p, f32p, u32p, u32p, f32p, f32p, u32p]
@@ -237,6 +239,20 @@ def ray_tri(o, d, p0, p1, p2):
     tuv = np.zeros(3, np.float32)
     hit = lib().orc_ray_tri(*[_f(x) for x in a], _f(tuv))
     return bool(hit), tuv
+
+
+def ray_tri_pairs(xyz, origins, directions, ray, tri, nthreads: int = 0):
+    """ray_tri on n (ray, triangle) pairs: ray i32[n] indexes origins / directions [R,3], tri [n,3] vertex ids of xyz in the winding to
+    test -> (hit bool[n], tuv f32[n,3])"""
+    x, o, d = (_c(a, np.float32).reshape(-1, 3) for a in (xyz, origins, directions))
+    r = _c(ray, np.uint32).reshape(-1)
+    t = _c(tri, np.uint32).reshape(-1, 3)
+    n = len(r)
+    hit = np.zeros((n,), np.uint8)
+    tuv = np.zeros((n, 3), np.float32)
+    if n:
+        lib().orc_ray_tri_pairs(_f(x), _f(o), _f(d), n, _u(r), _u(t), hit.ctypes.data_as(u8p), _f(tuv), nthreads)
+    return hit.astype(bool), tuv
 
 
 # =====================================================================================

@@ -451,6 +451,18 @@ int orc_ray_tri(const float *o, const float *d, const float *p0, const float *p1
     if (!rs.valid) return 0;
     return ray_tri(rs, p0, p1, p2, tuv[0], tuv[1], tuv[2]) ? 1 : 0;
 }
+// orc_ray_tri over n (ray, triangle) pairs: pair i tests ray ray[i] of o / d against the triangle with vertex ids tri[3i..3i+2] of xyz,
+// in that winding; hit[i] = 0 / 1, tuv[3i..3i+2] = (t, u, v) on a hit.  The step loop of oracle/walk.py.
+void orc_ray_tri_pairs(const float *xyz, const float *o, const float *d, uint32_t n, const uint32_t *ray, const uint32_t *tri, uint8_t *hit,
+                       float *tuv, int nthreads) {
+    parallel_for(n, nthreads, [&](uint32_t i) {
+        const RaySetup rs = ray_setup(o + 3 * (size_t)ray[i], d + 3 * (size_t)ray[i]);
+        float t = 0.f, u = 0.f, v = 0.f;
+        hit[i] = rs.valid && ray_tri(rs, xyz + 3 * (size_t)tri[3 * (size_t)i], xyz + 3 * (size_t)tri[3 * (size_t)i + 1],
+                                     xyz + 3 * (size_t)tri[3 * (size_t)i + 2], t, u, v) ? 1 : 0;
+        tuv[3 * (size_t)i] = t; tuv[3 * (size_t)i + 1] = u; tuv[3 * (size_t)i + 2] = v;
+    });
+}
 
 // raw sorted face hits (reference: trace_rays_triangles, optix_trace_rays_triangles.cu:49-114)
 // outputs: num[R], faces[R,M], bary[R,M,2], dist[R,M], verts[R,M,3]; tails zero (py_binding.cpp:90-94)

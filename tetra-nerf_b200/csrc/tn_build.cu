@@ -334,7 +334,8 @@ int build_mesh(tn_tracer *h, const float *d_xyz, uint32_t V, const uint32_t *d_c
     TN_CUDA(cudaMemcpyAsync(hbounds, bounds.p, sizeof(hbounds), cudaMemcpyDeviceToHost, s));
     TN_CUDA(cudaStreamSynchronize(s));
     m.xyz = d_xyz; m.cells = d_cells; m.V = V; m.T = T; m.F = F; m.lv = lv; m.absmax = absmax_of(hbounds);
-    m.walkable = walkable; m.H = walkable ? H : 0; m.hull_lv = hlv;
+    // the walk records are built for every convex hull, so that a refit which unfolds the mesh turns the walk on again
+    m.walkable = walkable && ft.folded == 0; m.H = walkable ? H : 0; m.hull_lv = hlv;
     h->mesh = std::move(m);
     return TN_OK;
 }

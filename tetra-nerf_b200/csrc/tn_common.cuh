@@ -193,6 +193,7 @@ struct FaceTables {
     DevArray<uint32_t> hull_list;  // [H] tetrahedra owning a hull face, ascending
     uint32_t F = 0, H = 0;
     bool walkable = false;       // the hull is a closed convex surface
+    uint32_t folded = 0;         // walkable: interior faces the fold test (k_fold_faces) does not certify unfolded
     DevArray<unsigned long long> hull_ekey;  // walkable: the sorted hull edges (Mesh::hull_ekey / hull_eface)
     DevArray<uint32_t> hull_eface;
     uint32_t hull_ne = 0;

@@ -236,7 +236,7 @@ int build_faces_device(const float *d_xyz, uint32_t V, const uint32_t *d_cells, 
     TN_TRY(val.grow(n)); TN_TRY(val2.grow(n));
     TN_TRY(kab.grow(n)); TN_TRY(kab2.grow(n));
     TN_TRY(flag.grow(n)); TN_TRY(fid.grow(n));
-    TN_TRY(d_small.grow(4));  // [0] err, [1] selected count
+    TN_TRY(d_small.grow(4));  // [0] err, [1] selected count, [2] hull faces, [3] folded faces
     TN_CUDA(cudaMemsetAsync(d_small.p, 0, 16, s));
     // temporary storage: the largest request of the CUB calls below
     size_t tb = 0, t1 = 0;
@@ -252,7 +252,7 @@ int build_faces_device(const float *d_xyz, uint32_t V, const uint32_t *d_cells, 
     TN_CUDA(cub::DeviceRadixSort::SortPairs(tmp.p, tb, kab.p, kab2.p, val2.p, val.p, (int)n, 0, 64, s));  // val: slots grouped by face, slot order inside
     k_face_heads<<<nb, 256, 0, s>>>(d_cells, val.p, n, flag.p, d_small.p);
     TN_CUDA(cub::DeviceScan::ExclusiveSum(tmp.p, tb, flag.p, fid.p, (int)n, s));
-    uint32_t h_small[2] = {0, 0}, last[2] = {0, 0};
+    uint32_t h_small[4] = {0, 0, 0, 0}, last[2] = {0, 0};
     TN_CUDA(cudaMemcpyAsync(h_small, d_small.p, 4, cudaMemcpyDeviceToHost, s));
     TN_CUDA(cudaMemcpyAsync(&last[0], flag.p + (n - 1), 4, cudaMemcpyDeviceToHost, s));
     TN_CUDA(cudaMemcpyAsync(&last[1], fid.p + (n - 1), 4, cudaMemcpyDeviceToHost, s));
@@ -290,10 +290,14 @@ int build_faces_device(const float *d_xyz, uint32_t V, const uint32_t *d_cells, 
         k_hull_edges<<<(ne + 255) / 256, 256, 0, s>>>(out.tri.p, hull_faces.p, Hf, kab.p, eface.p);
         TN_CUDA(cub::DeviceRadixSort::SortPairs(tmp.p, tb, kab.p, kab2.p, eface.p, eface2.p, (int)ne, 0, 64, s));
         k_hull_check<<<(ne + 255) / 256, 256, 0, s>>>(d_xyz, (const uint4 *)d_cells, out.tri.p, out.tt.p, kab2.p, eface2.p, ne, d_small.p);
-        TN_CUDA(cudaMemcpyAsync(h_small, d_small.p, 4, cudaMemcpyDeviceToHost, s));
+        // the refit's fold test on the load's tables: the walk sees only the chain of tetrahedra from the hull entry, and on a folded mesh
+        // a line also crosses faces off that chain (DESIGN §4.9), so a mesh with an uncertified face loads with the walk off
+        k_fold_faces<<<(F + 255) / 256, 256, 0, s>>>(d_xyz, (const uint4 *)d_cells, out.tri.p, out.tt.p, F, d_small.p + 3);
+        TN_CUDA(cudaMemcpyAsync(h_small, d_small.p, 16, cudaMemcpyDeviceToHost, s));
         TN_CUDA(cudaStreamSynchronize(s));
         walkable = (h_small[0] & 4u) == 0;
-        if (launches) *launches += 2;
+        out.folded = h_small[3];
+        if (launches) *launches += 3;
         if (walkable) {  // kept for the convexity test of a refit (tn_update_vertices)
             TN_TRY(out.hull_ekey.grow(ne)); TN_TRY(out.hull_eface.grow(ne));
             TN_CUDA(cudaMemcpyAsync(out.hull_ekey.p, kab2.p, 8 * (size_t)ne, cudaMemcpyDeviceToDevice, s));
