@@ -132,6 +132,19 @@ int tn_refine_edges(int device, const float *d_xyz, uint32_t V, const uint32_t *
                     float min_length, uint32_t max_new_vertices, uint32_t *d_cells_out, uint32_t *d_parent_edge, uint32_t *d_parent_cell,
                     uint32_t *counts3, void *d_workspace, size_t *workspace_bytes, void *stream);
 
+/* ---- field smoothness along the mesh edges (DESIGN.md §4.15).  Over the unique undirected edges of the loaded mesh (E of them; an edge
+ * {i, j} joins two distinct vertices of one cell), with f the field of tn_render_set_field:
+ *   S = sum_{i,j} sum_c (f[c,i] - f[c,j])^2,   loss = mult S / (E 64),   d loss / df[c,i] = mult 2 / (E 64) sum_{j in N(i)} (f[c,i] - f[c,j]).
+ * d_sum (device, one double) receives S; d_grad_field f32[64,V] (NULL: not computed; every element of a non-NULL one is written) the
+ * gradient of loss, 0 for a vertex no cell uses; *n_edges (host, may be NULL) E.  One pass over a vertex adjacency (CSR: row offsets
+ * u32[V+1], neighbours u32[2E], each row ascending) that the tracer builds from the loaded cells on the first call after
+ * tn_load_tetrahedra and keeps until the next one (tn_update_vertices keeps it: same cells); that call synchronises once to size it,
+ * later calls are asynchronous.  Nothing is allocated before the first call.  Neighbours are summed in CSR order in fp32 and S in double
+ * in a fixed order, without atomics: every call, in either mode of tn_render_set_deterministic, gives the same bits.  TN_ERR_STATE
+ * without a mesh or a field, or if the field's vertex count differs from the mesh's; TN_ERR_ARG if mult is not finite or a cell holds a
+ * vertex index >= V. */
+int tn_field_smoothness(tn_tracer *h, float mult, double *d_sum, float *d_grad_field, uint32_t *n_edges, void *stream);
+
 /* ---- fused forward render (new; replaces model.py:531-662 between trace_rays and the pixel) -------
  * Weights are passed once (tn_render_set_weights) in nerfstudio state-dict layout and repacked on
  * the device.  See DESIGN.md §"fused render". */

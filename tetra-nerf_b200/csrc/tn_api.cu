@@ -77,6 +77,7 @@ int tn_load_tetrahedra(tn_tracer *h, const float *d_xyz, uint32_t V, const uint3
     if (!d_xyz || !d_cells) return tn::fail(TN_ERR_ARG, "load_tetrahedra: null pointer");
     tn::DeviceGuard g(h->device);
     h->mesh_gen = tn::next_generation();  // any earlier surface extraction is stale from here on, even if the build fails
+    h->adj_valid = false;                 // the vertex adjacency of the old cells, likewise
     return tn::build_mesh(h, d_xyz, V, d_cells, T, (cudaStream_t)stream);
 }
 

@@ -179,6 +179,13 @@ struct tn_tracer {
     tn::DevArray<uint32_t> d_refit;  // 16 words of tn_update_vertices scratch: flags, counts and bounds, read back once per refit
     tn::RenderState *render = nullptr;
     tn::SurfaceState *surface = nullptr;
+    // vertex adjacency of the loaded mesh (tn_field_smoothness, tn_smoothness.cu): built on the first call after a tn_load_tetrahedra,
+    // kept by tn_update_vertices (same cells); nothing is allocated before that first call
+    bool adj_valid = false;
+    uint32_t adj_E = 0;                    // unique undirected edges
+    tn::DevArray<uint32_t> adj_off;        // [V+1] CSR row offsets
+    tn::DevArray<uint32_t> adj_nbr;        // [2E] neighbours, each row ascending
+    tn::DevArray<double> adj_part;         // one partial sum per block of the smoothness kernel
 };
 
 namespace tn {
@@ -223,6 +230,8 @@ struct RenderInputs {
     uint64_t gen;           // generation of field + weights
 };
 int render_inputs(tn_tracer *h, RenderInputs *out);
+// the fused render's field shadow [V,64] (fragment order, field_pos) and its V; TN_ERR_STATE if tn_render_set_field never ran
+int field_shadow(const tn_tracer *h, const float **fshadow, uint32_t *V);
 // the normal map of a fused render (tn_normals.cu), launched after its composite on the render's own buffers
 struct NormalsLaunch {
     const uint32_t *n_active, *ray_list;  // active rays, slot -> ray

@@ -8,6 +8,7 @@
 #include <cub/cub.cuh>
 
 #include "tn_common.cuh"
+#include "tn_edges.cuh"
 
 namespace tn {
 
@@ -20,9 +21,6 @@ __device__ __forceinline__ double edge_len2(const float *__restrict__ xyz, uint3
     const double dz = __dsub_rn((double)xyz[3 * (size_t)a + 2], (double)xyz[3 * (size_t)b + 2]);
     return __dadd_rn(__dadd_rn(__dmul_rn(dx, dx), __dmul_rn(dy, dy)), __dmul_rn(dz, dz));
 }
-__device__ __forceinline__ unsigned long long edge_key(uint32_t a, uint32_t b) {
-    return a < b ? ((unsigned long long)a << 32) | b : ((unsigned long long)b << 32) | a;
-}
 // priority: the larger squared length, ties to the smaller key
 __device__ __forceinline__ bool higher(double l, unsigned long long k, double lo, unsigned long long ko) {
     return l > lo || (l == lo && k < ko);
@@ -33,15 +31,12 @@ __device__ __forceinline__ uint32_t find_key(const unsigned long long *__restric
     return lo < n && P[lo] == k ? lo : TN_EMPTY;
 }
 
-// the six edges of a tetrahedron as local vertex pairs
-#define TN_REF_EDGES const int EA[6] = {0, 0, 0, 1, 1, 2}, EB[6] = {1, 2, 3, 2, 3, 3}
-
 // every candidate proposes its longest edge when that is at least min_length long; flags[0] |= 1 on a vertex index >= V
 __global__ void k_ref_propose(uint32_t T, uint32_t V, const float *__restrict__ xyz, const uint4 *__restrict__ cells,
                               const uint8_t *__restrict__ cand, double min_len2, unsigned long long *__restrict__ prop, uint32_t *__restrict__ flags) {
     const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
     if (t >= T) return;
-    TN_REF_EDGES;
+    TN_TET_EDGES;
     const uint4 c = cells[t];
     const uint32_t v[4] = {c.x, c.y, c.z, c.w};
     if (v[0] >= V || v[1] >= V || v[2] >= V || v[3] >= V) {
@@ -69,7 +64,7 @@ __global__ void k_ref_vote(uint32_t T, const float *__restrict__ xyz, const uint
                            const uint32_t *__restrict__ nP, uint32_t *__restrict__ incident, uint32_t *__restrict__ votes, uint32_t *__restrict__ voted) {
     const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
     if (t >= T) return;
-    TN_REF_EDGES;
+    TN_TET_EDGES;
     const uint32_t n = *nP;
     const uint4 c = cells[t];
     const uint32_t v[4] = {c.x, c.y, c.z, c.w};

@@ -145,6 +145,14 @@ int render_inputs(tn_tracer *h, RenderInputs *out) {
     return TN_OK;
 }
 
+int field_shadow(const tn_tracer *h, const float **fshadow, uint32_t *V) {
+    const RenderState *r = h->render;
+    if (!r || !r->fshadow.p) return TN_ERR_STATE;
+    *fshadow = r->fshadow.p;
+    *V = r->V;
+    return TN_OK;
+}
+
 static RenderState *state(tn_tracer *h) {
     if (!h->render) {
         h->render = new RenderState();

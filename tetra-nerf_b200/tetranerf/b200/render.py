@@ -259,6 +259,19 @@ class FusedRenderer:
         ext._check(_lib.tn_occupancy_update(self.tracer.handle, occ.data_ptr(), C.c_float(float(decay)), self._stream()))
         return occ
 
+    # ---- field smoothness (DESIGN §4.15) ------------------------------------------------------------------------------------------
+    def field_smoothness(self, mult: float = 1.0, grad: bool = False):
+        """the field's smoothness along the mesh edges, for the field of the last set_field on the tracer's mesh -> (S f64[] on the
+        device, E, grad_field f32[64,V] or None): S = sum over the E unique undirected edges {i, j} of sum_c (F[c,i] - F[c,j])^2, and
+        with grad=True the gradient of mult * S / (E * 64), 0 for a vertex no cell uses.  The first call after load_tetrahedra builds
+        the vertex adjacency and waits for the stream once; later calls do not wait.  Bitwise reproducible in every mode."""
+        S = torch.empty((), dtype=torch.float64, device=self.device)
+        V = self.tracer._vertices.shape[0] if self.tracer._vertices is not None else 0
+        g = torch.empty((64, V), dtype=torch.float32, device=self.device) if grad else None
+        E = C.c_uint32(0)
+        ext._check(_lib.tn_field_smoothness(self.tracer.handle, C.c_float(float(mult)), S.data_ptr(), _ptr(g), C.byref(E), self._stream()))
+        return S, int(E.value), g
+
     # ---- surface extraction ---------------------------------------------------------------------------------------------------------
     def extract_surface(self, level: float) -> Dict[str, torch.Tensor]:
         """the density iso-surface sigma = level (finite, > 0) of the current field and weights, by marching tetrahedra on the tracer's
@@ -397,6 +410,28 @@ class FusedTrainRenderDistortion(torch.autograd.Function):
     def backward(ctx, g_rgb, g_acc, _g_depth, *rest):
         g_ed, g_dist = (rest[0], rest[1]) if ctx.ed else (None, rest[0])
         return _fused_backward(ctx, g_rgb, g_acc, g_ed, g_dist)
+
+
+class FieldSmoothness(torch.autograd.Function):
+    """mult * S / (E * 64) as one differentiable op (FusedRenderer.field_smoothness; DESIGN §4.15), a float32 scalar: S the sum over the
+    mesh's unique undirected edges of the squared feature differences, E their number.  Arguments (fr, mult, field): the renderer must
+    already hold `field` as its current field (set_field), which is what the kernel reads; `field` is passed so that autograd routes the
+    gradient to it.  The forward computes the gradient in the same pass; the backward scales it by the incoming scalar.  An in-place
+    change of `field` before the backward raises RuntimeError."""
+
+    @staticmethod
+    def forward(ctx, fr, mult, field):
+        if tuple(field.shape) != (64, fr.tracer._vertices.shape[0] if fr.tracer._vertices is not None else -1):
+            raise RuntimeError(f"FieldSmoothness: the field must be [64, V] for the tracer's V vertices, got {tuple(field.shape)}")
+        S, E, g = fr.field_smoothness(mult, grad=ctx.needs_input_grad[2])
+        ctx.g = g
+        ctx.save_for_backward(field)  # its version counter rejects a backward after an in-place change
+        return (S * (float(mult) / (E * 64) if E > 0 else 0.0)).to(torch.float32)
+
+    @staticmethod
+    def backward(ctx, g_loss):
+        _ = ctx.saved_tensors  # raises if the field changed in place since the forward
+        return None, None, ctx.g * g_loss
 
 
 def _fused_forward(ctx, name, expected_depth, fr, settings, use_gradient_scaling, origins, directions, jitter_coarse, jitter_fine, field, params,

@@ -110,6 +110,12 @@ class TetrahedraNerfConfig(ModelConfig):
     """> 0: training outputs also hold "distortion" f32[R,1], mip-NeRF 360's distortion of each ray's weights over its spacing bins (0 on
     empty rays; DESIGN §4.11), and the loss dict gains distortion_loss = distortion_loss_mult * its mean over the rays with hits, as
     nerfacto's distortion_loss_mult.  Training only; 0 changes nothing"""
+    field_smoothness_mult: float = 0.0
+    """> 0: the loss dict gains field_smoothness_loss = field_smoothness_mult * S / (E * field_dim), S the sum over the mesh's E unique
+    undirected edges {i, j} of sum_c (F[c,i] - F[c,j])^2: a uniform-weight neighbour-difference regulariser on tetrahedra_field, as
+    explicit-feature radiance fields use, that keeps the vertices few rays see from drifting (DESIGN §4.15).  It does not depend on the
+    vertex positions.  After refine() the next loss is taken on the refined mesh, and the refinement score then sees the sum of both field
+    gradients (rendering and smoothness).  Needs the fused pipeline (RuntimeError otherwise).  Training only; 0 changes nothing"""
     refine_every: int = 0
     """> 0: refine the mesh during training every refine_every steps in [refine_start, refine_stop) (TetrahedraNerf.refine, DESIGN §4.14):
     the tetrahedra whose field gradient stays large have their longest edges bisected, the new vertices taking the mean of their edge's
@@ -712,7 +718,19 @@ class TetrahedraNerf(Model):
         if self._distortion_on():  # mean over the rays with hits (empty rays hold 0)
             n = outputs["ray_mask"].sum().clamp_min(1)
             losses["distortion_loss"] = self.config.distortion_loss_mult * outputs["distortion"].sum() / n
+        if self.config.field_smoothness_mult > 0 and self.training:
+            losses["field_smoothness_loss"] = self._field_smoothness_loss()
         return scale_dict(losses, self.config.loss_coefficients)
+
+    def _field_smoothness_loss(self) -> torch.Tensor:
+        """field_smoothness_mult * S / (E * 64) on the current field and mesh (FieldSmoothness), differentiable to tetrahedra_field"""
+        bad = self._fused_unsupported()
+        if bad:
+            raise RuntimeError(f"field_smoothness_mult runs on the fused CUDA pipeline, which does not support {', '.join(bad)}")
+        from ..b200.render import FieldSmoothness
+
+        fr = self._fused_renderer()  # refreshes the field shadow the kernel reads, whichever path rendered the step
+        return FieldSmoothness.apply(fr, self.config.field_smoothness_mult, self.tetrahedra_field)
 
     def _depth_loss(self, outputs, batch) -> torch.Tensor:
         """mean over rays with hits and a finite target > 0 of (expected_depth - target)^2; the target batch["depth_image"] [R,1] is a
