@@ -250,6 +250,25 @@ int tn_render_train_backward_saved2(tn_tracer *h, const void *d_saved, const flo
                                     float *d_grad_field, float *const *d_grad_params12, float *d_grad_origins, float *d_grad_directions,
                                     float *d_grad_xyz, void *stream);
 int tn_render_train_distortion(tn_tracer *h, const void *d_saved, float *d_distortion, void *stream);
+/* ---- learned background (DESIGN.md §4.16).  tn_render_set_background borrows d_map f32[H,W,3], W = 2H (TN_ERR_ARG otherwise, or
+ * unless 1 <= H <= 16384), an environment map in the mesh's frame, z up; NULL switches back to cfg->background.  For a ray direction d,
+ * n = d / |d|: u = W (atan2(n_y, n_x) / 2 pi + 1/2) - 1/2 (columns modulo W), v = H (1 - n_z) / 2 - 1/2 clamped to [0, H - 1], and
+ * bg(d) is the bilinear lerp of the four texels around (u, v), so a constant map returns its constant exactly.  While it is set,
+ * tn_render and the training forwards composite rgb = sum_j w_j c_j + (1 - accumulation) bg(d) on active rays and rgb = bg(d) on empty
+ * ones (eval mode still clamps every pixel to [0, 1]), inside the kernels that write the pixels, so the fused pixel gather carries them;
+ * every other output is the same bits.  A training forward over a map records that in its saved state with the map's generation, which
+ * every set bumps, and keeps its ray directions (12 more bytes per ray in tn_render_train_saved_bytes, which then depends on whether a
+ * map is set); a backward after another set returns TN_ERR_STATE.  Its backward takes dL/dw_j = grad_rgb . (c_j - bg(d)) + grad_acc.
+ * tn_render_train_backward_saved3 is tn_render_train_backward_saved2 with one more optional output, d_grad_background f32[H,W,3]:
+ * s = grad_rgb (1 - accumulation) per ray (grad_rgb on empty rays) scattered to the four texels with the bilinear weights (float
+ * atomics; the deterministic mode sorts by texel and sums in ray order, bitwise reproducible).  TN_ERR_STATE if the forward had no map.
+ * d_grad_directions then also gains (d bg / d d)^T s on every ray, empty ones included (the u-derivative is 0 where
+ * n_x^2 + n_y^2 < 1e-8, at the poles).  Origins are untouched.  With no map set every kernel runs as without this feature. */
+int tn_render_set_background(tn_tracer *h, const float *d_map, uint32_t H, uint32_t W);
+int tn_render_train_backward_saved3(tn_tracer *h, const void *d_saved, const float *d_grad_rgb, const float *d_grad_acc,
+                                    const float *d_grad_expected_depth, const float *d_grad_distortion, int use_gradient_scaling,
+                                    float *d_grad_field, float *const *d_grad_params12, float *d_grad_origins, float *d_grad_directions,
+                                    float *d_grad_xyz, float *d_grad_background, void *stream);
 /* Deterministic mode of the fused training step (enable != 0; initial value: 1 if the environment variable TETRANERF_B200_DETERMINISTIC
  * is 1, else 0).  Read by tn_render_train_forward; tn_render_train_backward continues in the mode of the forward it belongs to.  With
  * identical inputs, on the same build and GPU model, forward outputs and every gradient are then bitwise identical from run to run and

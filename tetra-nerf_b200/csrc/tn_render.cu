@@ -17,6 +17,7 @@
 #include <cstddef>
 #include <cstdlib>
 #include <cub/cub.cuh>
+#include "tn_background.cuh"
 #include "tn_common.cuh"
 #include "tn_composite.cuh"
 #include "tn_direnc.cuh"
@@ -41,6 +42,7 @@ struct TrainBufs {
     float *bary_f;             // [R*S2,3] their weights
     float *out_f;              // [R*S2] (sigma, r, g, b) head pre-activations
     float *dirbias, *enc;      // [R,128] direction bias, [R,27] encoded direction
+    float *dirs;               // [R,3] the ray directions of a training forward with a background map (nullptr: none kept)
 };
 
 // header of a saved-state blob: what a training forward ran with, which its backward continues in
@@ -55,6 +57,9 @@ struct SavedHeader {
     uint32_t cull;             // 1: the forward culled samples by occupancy (its culled rows are marked in vi_f, DESIGN §4.12)
     uint32_t live_c, live_f;   // culling: the live rows of its coarse / fine pass (copied on the device from the n_active slot)
     uint32_t pad3;
+    uint32_t bgmap;            // 1: the forward composited over the background map (tn_render_set_background; its directions are kept)
+    uint32_t bg_H, bg_W, pad4;
+    uint64_t bg_gen;           // RenderState::bg_gen at the forward
 };
 
 struct RenderState {
@@ -121,6 +126,13 @@ struct RenderState {
     DevArray<uint4> occ_vi;
     DevArray<float> occ_bary, occ_sig;
     DevArray<uint32_t> occ_small;
+    // background map (tn_render_set_background; DESIGN §4.16): borrowed f32[H,W,3] (nullptr: the constant cfg->background), its
+    // generation (bumped by every set), and the backward's per-ray grad_rgb (1 - accumulation) and deterministic sort buffers
+    const float *bgmap = nullptr;
+    uint32_t bg_H = 0, bg_W = 0;
+    uint64_t bg_gen = 0;
+    DevArray<float> bg_s;
+    DevArray<uint32_t> bg_keys, bg_vals;
 };
 
 void free_render(tn_tracer *h) {
@@ -235,6 +247,9 @@ struct SampleParams {
     const uint32_t *cells;
     const float *occ;
     float occ_thr;
+    // background map (nullptr: the constant bg0..bg2)
+    const float *bgmap;
+    uint32_t bg_H, bg_W;
 };
 
 // a culled sample (matched to a tetrahedron whose occupancy is below the threshold): vi = (E, E, E, TN_CULLED), weights 0.  Every
@@ -347,7 +362,12 @@ __global__ void __launch_bounds__(SAMPLE_WARPS * 32) k_sample_coarse(const Sampl
         if (ray == p.R - 1 && lane == 0) *p.n_active = p.ray_slot[ray] + (n > 0 ? 1u : 0u);
     }
     if (n == 0) {  // model.py:640-650 : background colour, accumulation 0, depth = collider far plane
-        store_pixel(p, ray, lane, p.bg0, p.bg1, p.bg2, 0.f, p.far_plane, 0);
+        float b0 = p.bg0, b1 = p.bg1, b2 = p.bg2;
+        if (p.bgmap != nullptr) {  // bg(d), clamped to [0,1] in eval mode as every other pixel
+            bg_lookup(p.bgmap, p.bg_H, p.bg_W, p.d[3 * (size_t)ray], p.d[3 * (size_t)ray + 1], p.d[3 * (size_t)ray + 2], b0, b1, b2);
+            if (!p.train) { b0 = fminf(fmaxf(b0, 0.f), 1.f); b1 = fminf(fmaxf(b1, 0.f), 1.f); b2 = fminf(fmaxf(b2, 0.f), 1.f); }
+        }
+        store_pixel(p, ray, lane, b0, b1, b2, 0.f, p.far_plane, 0);
         return;
     }
     uint32_t slot = 0;
@@ -629,8 +649,10 @@ __global__ void __launch_bounds__(SAMPLE_WARPS * 32) k_composite(const SamplePar
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) first = min(first, __shfl_xor_sync(0xffffffffu, first, o));
     const uint32_t mi = min(first, S2 - 1);
-    // RGBRenderer: comp + background * (1 - acc); clamped to [0,1] in eval mode only
-    float pr = r + p.bg0 * (1.f - a), pg = g + p.bg1 * (1.f - a), pb = b + p.bg2 * (1.f - a);
+    // RGBRenderer: comp + background * (1 - acc); clamped to [0,1] in eval mode only.  The background is bg(d) with a map
+    float b0 = p.bg0, b1 = p.bg1, b2 = p.bg2;
+    if (p.bgmap != nullptr) bg_lookup(p.bgmap, p.bg_H, p.bg_W, p.d[3 * (size_t)ray], p.d[3 * (size_t)ray + 1], p.d[3 * (size_t)ray + 2], b0, b1, b2);
+    float pr = r + b0 * (1.f - a), pg = g + b1 * (1.f - a), pb = b + b2 * (1.f - a);
     if (!p.train) { pr = fminf(fmaxf(pr, 0.f), 1.f); pg = fminf(fmaxf(pg, 0.f), 1.f); pb = fminf(fmaxf(pb, 0.f), 1.f); }
     store_pixel(p, ray, lane, pr, pg, pb, a, (eb[mi] + eb[mi + 1]) / 2.f, 1);
 }
@@ -662,6 +684,10 @@ struct CompositeBwdParams {
     const float *grad_ed;              // DEPTH: [R] dL/d expected depth
     const uint32_t *dbounds;           // DEPTH: the forward's clip bounds (ordered keys, k_composite<true>)
     const float *grad_dist;            // DIST: [R] dL/d distortion
+    const float *bgmap;                // background map [H,W,3] (nullptr: the constant bg0..bg2); then bg(d) of the saved directions, and
+    uint32_t bg_H, bg_W;               //   bg_s[ray] = grad_rgb (1 - accumulation), the map's and the directions' per-ray weight
+    const float *dirs;
+    float *bg_s;
 };
 
 // ---- distortion loss (DESIGN §4.11; mip-NeRF 360, nerfstudio losses.distortion_loss) over the fine pass of one ray: spacing bins s_0..s_S2,
@@ -721,6 +747,8 @@ __global__ void __launch_bounds__(SAMPLE_WARPS * 32) k_composite_bwd(const Compo
     const float4 *of = reinterpret_cast<const float4 *>(p.out_f) + (size_t)slot * S2;
     const float gr = p.grad_rgb[3 * (size_t)ray], gg = p.grad_rgb[3 * (size_t)ray + 1], gb = p.grad_rgb[3 * (size_t)ray + 2];
     const float ga = p.grad_acc != nullptr ? p.grad_acc[ray] : 0.f;
+    float bg0 = p.bg0, bg1 = p.bg1, bg2 = p.bg2;
+    if (p.bgmap != nullptr) bg_lookup(p.bgmap, p.bg_H, p.bg_W, p.dirs[3 * (size_t)ray], p.dirs[3 * (size_t)ray + 1], p.dirs[3 * (size_t)ray + 2], bg0, bg1, bg2);
     for (uint32_t j = lane; j < S2; j += 32) tr[j] = (eb[j + 1] - eb[j]) * of[j].x;  // x_j
     __syncwarp();
     smem_scan_add(tr, S2, lane);  // inclusive cumsum of x
@@ -765,6 +793,7 @@ __global__ void __launch_bounds__(SAMPLE_WARPS * 32) k_composite_bwd(const Compo
             cw += __shfl_sync(0xffffffffu, iw, 31); cp += __shfl_sync(0xffffffffu, ip, 31);
         }
     }
+    float acc = 0.f;  // (background map only)
     for (uint32_t j = lane; j < S2; j += 32) {
         const float excl = j == 0 ? 0.f : tr[j - 1];
         const float x = (eb[j + 1] - eb[j]) * of[j].x;
@@ -774,12 +803,17 @@ __global__ void __launch_bounds__(SAMPLE_WARPS * 32) k_composite_bwd(const Compo
         wj = fin ? wj : nan_to_num_f(wj);
         const float4 c = of[j];
         float g;
-        if constexpr (DEPTH) g = fin ? (gr * (c.y - p.bg0) + gg * (c.z - p.bg1) + gb * (c.w - p.bg2) + ga + gd * (((eb[j] + eb[j + 1]) / 2.f - draw) / den)) : 0.f;
-        else g = fin ? (gr * (c.y - p.bg0) + gg * (c.z - p.bg1) + gb * (c.w - p.bg2) + ga) : 0.f;
+        if constexpr (DEPTH) g = fin ? (gr * (c.y - bg0) + gg * (c.z - bg1) + gb * (c.w - bg2) + ga + gd * (((eb[j] + eb[j + 1]) / 2.f - draw) / den)) : 0.f;
+        else g = fin ? (gr * (c.y - bg0) + gg * (c.z - bg1) + gb * (c.w - bg2) + ga) : 0.f;
         if constexpr (DIST) g = fin ? g + fx[j] : 0.f;  // (read before this lane overwrites fx[j] below)
         w[j] = wj;
         gw[j] = g * wj;
         fx[j] = fin ? g * (T - wj) : 0.f;  // first term of dL/dx_j
+        acc += wj;
+    }
+    if (p.bgmap != nullptr) {  // the forward's accumulation: the same weights, summed in k_composite's order
+        const float oma = 1.f - warp_sum_f(acc);
+        if (lane == 0) { p.bg_s[3 * (size_t)ray] = gr * oma; p.bg_s[3 * (size_t)ray + 1] = gg * oma; p.bg_s[3 * (size_t)ray + 2] = gb * oma; }
     }
     __syncwarp();
     const float total = smem_scan_add(gw, S2, lane);  // inclusive cumsum of g_k w_k -> suffix_j = total - gw[j]
@@ -1155,8 +1189,9 @@ extern "C" int tn_render_set_weights(tn_tracer *h, const float *const *P, void *
 constexpr size_t SAVED_ALIGN = 256;
 static_assert(sizeof(SavedHeader) <= SAVED_ALIGN, "saved-state header exceeds its slot");
 // bytes of the blob for R rays of S2 fine samples; with base != nullptr also the array pointers inside it.  eval: no spacing bins or
-// encodings (nullptr, 0 bytes), which only the backward reads -- the layout of the eval render in the tracer's own blob
-static size_t saved_layout(size_t R, size_t S2, uint8_t *base, TrainBufs *b, bool eval = false) {
+// encodings (nullptr, 0 bytes), which only the backward reads -- the layout of the eval render in the tracer's own blob.  dirs: a
+// training forward over a background map also keeps its ray directions, last (12 bytes per ray; the other arrays stay where they are)
+static size_t saved_layout(size_t R, size_t S2, uint8_t *base, TrainBufs *b, bool eval = false, bool dirs = false) {
     size_t off = SAVED_ALIGN;  // header
     auto take = [&](size_t bytes) { uint8_t *p = base ? base + off : nullptr; off += (bytes + SAVED_ALIGN - 1) / SAVED_ALIGN * SAVED_ALIGN; return p; };
     TrainBufs t{};
@@ -1169,6 +1204,7 @@ static size_t saved_layout(size_t R, size_t S2, uint8_t *base, TrainBufs *b, boo
     t.out_f = (float *)take(16 * R * S2);
     t.dirbias = (float *)take(512 * R);
     if (!eval) t.enc = (float *)take(4 * 27 * R);
+    if (dirs) t.dirs = (float *)take(12 * R);
     if (b) *b = t;
     return off;
 }
@@ -1227,12 +1263,13 @@ static int render_impl(tn_tracer *h, const tn_render_config *cfg, const float *d
     }
     TN_TRY(ensure_ws(r, R, M, Sc));
     const bool own = tf == nullptr || tf->saved == nullptr;  // the fine pass writes into the tracer's own blob
-    if (own) TN_TRY(r->own.grow(saved_layout(R, S2, nullptr, nullptr, tf == nullptr)));
+    const bool keep_dirs = tf != nullptr && r->bgmap != nullptr;  // the backward looks the background up again
+    if (own) TN_TRY(r->own.grow(saved_layout(R, S2, nullptr, nullptr, tf == nullptr, keep_dirs)));
     if (d_normals != nullptr) TN_TRY(r->grad_n.grow((size_t)R * S2));
     if (tf != nullptr) TN_TRY(ensure_train_ws(r, R, S2, r->V));
     r->last = SavedHeader{};
     TrainBufs b{};
-    saved_layout(R, S2, own ? r->own.p : (uint8_t *)tf->saved, &b, tf == nullptr);
+    saved_layout(R, S2, own ? r->own.p : (uint8_t *)tf->saved, &b, tf == nullptr, keep_dirs);
     if (own) r->own_b = b;
     const int prec = tf != nullptr ? 3 : r->mlp_prec;  // the training forward keeps bf16x3 (its backward recomputes in bf16x3)
     TN_CUDA(cudaMemsetAsync(b.n_active, 0, 16, s));
@@ -1262,6 +1299,8 @@ static int render_impl(tn_tracer *h, const tn_render_config *cfg, const float *d
     if (tf != nullptr) { p.train = 1; p.jit_c = tf->jit_c; p.jit_f = tf->jit_f; p.sbins_f = b.sbins_f; p.enc = b.enc; }
     p.edepth = d_edepth; p.dbounds = b.n_active + 4;
     if (cull) { p.cells = r->cells.p; p.occ = r->occ; p.occ_thr = r->occ_thr; }
+    if (r->bgmap != nullptr) { p.bgmap = r->bgmap; p.bg_H = r->bg_H; p.bg_W = r->bg_W; }
+    if (keep_dirs) TN_CUDA(cudaMemcpyAsync(b.dirs, d_directions, 12 * (size_t)R, cudaMemcpyDeviceToDevice, s));
     if (r->gather_world) {
         if (R > r->gather_stride) return fail(TN_ERR_ARG, "tn_render: more rays than the gathered-pixel buffers were sized for (tn_render_set_gather)");
         for (int k = 0; k < 8; ++k) p.peer[k] = r->peer[k];
@@ -1340,8 +1379,9 @@ static int render_impl(tn_tracer *h, const tn_render_config *cfg, const float *d
         h->launches += 2;
     }
     if (tf != nullptr) {  // what the backward continues with: kept on the host for the tracer's own blob, in the caller's blob otherwise
-        const SavedHeader hd{SAVED_MAGIC, R, M, Sc, Sf, S2, det ? 1u : 0u, d_edepth != nullptr ? 1u : 0u,
-                             {cfg->background[0], cfg->background[1], cfg->background[2]}, 0, r->gen, h->mesh_gen, cull ? 1u : 0u, 0, 0, 0};
+        SavedHeader hd{SAVED_MAGIC, R, M, Sc, Sf, S2, det ? 1u : 0u, d_edepth != nullptr ? 1u : 0u,
+                       {cfg->background[0], cfg->background[1], cfg->background[2]}, 0, r->gen, h->mesh_gen, cull ? 1u : 0u, 0, 0, 0};
+        if (keep_dirs) { hd.bgmap = 1; hd.bg_H = r->bg_H; hd.bg_W = r->bg_W; hd.bg_gen = r->bg_gen; }
         if (own) {
             r->last = hd;
         } else {
@@ -1382,10 +1422,17 @@ extern "C" int tn_render_train_forward(tn_tracer *h, const tn_render_config *cfg
 // mesh vertex positions (tn_vertex_grads.cu), into the non-null ones.
 // hd.cull: the forward culled by occupancy; its map of live fine rows is rebuilt from the culled marks in b.vi_f (never from the
 // occupancy, which may have changed since)
+// hd.bgmap: the forward composited over the background map, which has the same generation (the caller checked): g_j takes bg(d) of
+// the saved directions, and the map gradient (d_grad_bg f32[H,W,3], or NULL) and the directions' background term follow (DESIGN §4.16)
 static int train_backward_impl(tn_tracer *h, const TrainBufs &b, const SavedHeader &hd, const float *d_grad_rgb, const float *d_grad_acc,
                                const float *d_grad_ed, const float *d_grad_dist, int use_gradient_scaling, float *d_grad_field,
-                               float *const *d_grad_params12, float *d_grad_o, float *d_grad_d, float *d_grad_xyz, cudaStream_t s) {
+                               float *const *d_grad_params12, float *d_grad_o, float *d_grad_d, float *d_grad_xyz, float *d_grad_bg,
+                               cudaStream_t s) {
     RenderState *r = h->render;
+    if (hd.bgmap && r->bg_gen != hd.bg_gen)
+        return fail(TN_ERR_STATE, "tn_render_train_backward: the background map changed (tn_render_set_background) since the forward");
+    if (d_grad_bg != nullptr && !hd.bgmap)
+        return fail(TN_ERR_STATE, "tn_render_train_backward_saved3: the forward composited over no background map (tn_render_set_background)");
     const uint32_t R = hd.R, S2 = hd.S2;
     const bool det = hd.det != 0, cull = hd.cull != 0;
     int sms = 132;
@@ -1408,6 +1455,13 @@ static int train_backward_impl(tn_tracer *h, const TrainBufs &b, const SavedHead
     cb.ebins_f = b.ebins_f; cb.sbins_f = b.sbins_f; cb.out_f = b.out_f; cb.grad_rgb = d_grad_rgb; cb.grad_acc = d_grad_acc;
     cb.bg0 = hd.bg[0]; cb.bg1 = hd.bg[1]; cb.bg2 = hd.bg[2]; cb.dout = r->dout.p; cb.sums = det ? (float *)r->det_sums.p : r->gw.p + GW_SUMS;
     cb.grad_ed = d_grad_ed; cb.dbounds = b.n_active + 4; cb.grad_dist = d_grad_dist;
+    const bool bg_grads = hd.bgmap && (d_grad_bg != nullptr || d_grad_d != nullptr);
+    if (hd.bgmap) {
+        TN_TRY(r->bg_s.grow(3 * (size_t)R));
+        cb.bgmap = r->bgmap; cb.bg_H = hd.bg_H; cb.bg_W = hd.bg_W; cb.dirs = b.dirs; cb.bg_s = r->bg_s.p;
+        // s = grad_rgb on the empty rays; k_composite_bwd writes grad_rgb (1 - accumulation) over the active ones
+        if (bg_grads) TN_CUDA(cudaMemcpyAsync(r->bg_s.p, d_grad_rgb, 12 * (size_t)R, cudaMemcpyDeviceToDevice, s));
+    }
     const size_t smem_cb = SAMPLE_WARPS * sizeof(float) * 4 * ((size_t)S2 + 2);
     auto k_cbwd = d_grad_dist != nullptr
                       ? (d_grad_ed != nullptr ? (det ? k_composite_bwd<true, true, true> : k_composite_bwd<false, true, true>)
@@ -1499,6 +1553,19 @@ static int train_backward_impl(tn_tracer *h, const TrainBufs &b, const SavedHead
             h->launches += 1;
         }
     }
+    if (bg_grads) {  // after k_ray_grads: its direction gradients gain the background's term
+        BackgroundGradsLaunch bl{};
+        bl.R = R; bl.H = hd.bg_H; bl.W = hd.bg_W; bl.map = r->bgmap; bl.dirs = b.dirs; bl.s = r->bg_s.p; bl.det = det;
+        bl.grad_map = d_grad_bg; bl.grad_d = d_grad_d;
+        if (det && d_grad_bg != nullptr) {
+            TN_TRY(r->bg_keys.grow(8 * (size_t)R)); TN_TRY(r->bg_vals.grow(8 * (size_t)R));
+            TN_TRY(background_sort_bytes(R, hd.bg_H, hd.bg_W, &bl.cub_bytes));
+            TN_TRY(r->cub_tmp.grow(bl.cub_bytes));
+            bl.keys = r->bg_keys.p; bl.vals = r->bg_vals.p; bl.cub_tmp = r->cub_tmp.p;
+        }
+        TN_TRY(launch_background_grads(bl, s));
+        h->launches += det && d_grad_bg != nullptr ? 3 : 1;
+    }
     k_scatter_grads<<<(128 * 155 + 255) / 256, 256, 0, s>>>(r->gw.p, go);
     k_transpose_v64<<<(V + 31) / 32, dim3(32, 8), 0, s>>>(r->gshadow.p, d_grad_field, V);
     if (r->profile) cudaEventRecord(r->evb[3], s);
@@ -1515,7 +1582,7 @@ extern "C" int tn_render_train_backward(tn_tracer *h, const float *d_grad_rgb, c
     if (!r || r->last.magic != SAVED_MAGIC) return fail(TN_ERR_STATE, "tn_render_train_backward: no training forward to continue from");
     DeviceGuard g(h->device);
     return train_backward_impl(h, r->own_b, r->last, d_grad_rgb, d_grad_acc, nullptr, nullptr, use_gradient_scaling, d_grad_field, d_grad_params12,
-                               nullptr, nullptr, nullptr, (cudaStream_t)stream);
+                               nullptr, nullptr, nullptr, nullptr, (cudaStream_t)stream);
 }
 
 // ---- the training pair with per-call saved state: everything the backward reads that a later call could overwrite goes to the
@@ -1534,7 +1601,7 @@ extern "C" int tn_render_train_saved_bytes(tn_tracer *h, const tn_render_config 
     uint32_t S2 = 0;
     const int rc = saved_shape(cfg, R, &S2);
     if (rc) return rc;
-    *bytes = saved_layout(R, S2, nullptr, nullptr);
+    *bytes = saved_layout(R, S2, nullptr, nullptr, false, h->render != nullptr && h->render->bgmap != nullptr);
     return TN_OK;
 }
 
@@ -1548,7 +1615,7 @@ extern "C" int tn_render_train_forward_saved(tn_tracer *h, const tn_render_confi
     int rc = saved_shape(cfg, R, &S2);
     if (rc) return rc;
     if ((uintptr_t)d_saved % SAVED_ALIGN) return fail(TN_ERR_ARG, "tn_render_train_forward_saved: d_saved must be 256-byte aligned");
-    if (saved_bytes < saved_layout(R, S2, nullptr, nullptr))
+    if (saved_bytes < saved_layout(R, S2, nullptr, nullptr, false, h->render != nullptr && h->render->bgmap != nullptr))
         return fail(TN_ERR_ARG, "tn_render_train_forward_saved: saved_bytes is smaller than tn_render_train_saved_bytes");
     TrainFwd tf{d_jitter_coarse, d_jitter_fine, d_saved};
     return render_impl(h, cfg, d_origins, d_directions, R, d_rgb, d_acc, d_depth, d_mask, &tf, nullptr, d_expected_depth, stream);
@@ -1571,10 +1638,11 @@ static int read_saved_header(tn_tracer *h, const void *d_saved, cudaStream_t s, 
 // optional inputs: the gradients of the expected depth d_grad_expected_depth f32[R] (DESIGN.md §4.10) and of the distortion
 // d_grad_distortion f32[R] (§4.11); optional outputs: the gradients at the ray origins / directions of the forward, f32[R,3] each (0 on
 // empty rays; §4.8), and at the mesh vertex positions, f32[V,3] (§4.9)
-extern "C" int tn_render_train_backward_saved2(tn_tracer *h, const void *d_saved, const float *d_grad_rgb, const float *d_grad_acc,
+// optional output of saved3: the gradient at the background map of a forward that composited over one, f32[H,W,3] (DESIGN.md §4.16)
+extern "C" int tn_render_train_backward_saved3(tn_tracer *h, const void *d_saved, const float *d_grad_rgb, const float *d_grad_acc,
                                                const float *d_grad_expected_depth, const float *d_grad_distortion, int use_gradient_scaling,
                                                float *d_grad_field, float *const *d_grad_params12, float *d_grad_origins,
-                                               float *d_grad_directions, float *d_grad_xyz, void *stream) {
+                                               float *d_grad_directions, float *d_grad_xyz, float *d_grad_background, void *stream) {
     if (!h || !d_saved || !d_grad_rgb || !d_grad_field || !d_grad_params12) return fail(TN_ERR_ARG, "null argument");
     DeviceGuard g(h->device);
     cudaStream_t s = (cudaStream_t)stream;
@@ -1589,9 +1657,17 @@ extern "C" int tn_render_train_backward_saved2(tn_tracer *h, const void *d_saved
         return fail(TN_ERR_STATE, "tn_render_train_backward_saved: the forward produced no expected depth (pass d_expected_depth to "
                                   "tn_render_train_forward_saved)");
     TrainBufs b{};
-    saved_layout(hd.R, hd.S2, (uint8_t *)d_saved, &b);
+    saved_layout(hd.R, hd.S2, (uint8_t *)d_saved, &b, false, hd.bgmap != 0);
     return train_backward_impl(h, b, hd, d_grad_rgb, d_grad_acc, d_grad_expected_depth, d_grad_distortion, use_gradient_scaling, d_grad_field,
-                               d_grad_params12, d_grad_origins, d_grad_directions, d_grad_xyz, s);
+                               d_grad_params12, d_grad_origins, d_grad_directions, d_grad_xyz, d_grad_background, s);
+}
+
+extern "C" int tn_render_train_backward_saved2(tn_tracer *h, const void *d_saved, const float *d_grad_rgb, const float *d_grad_acc,
+                                               const float *d_grad_expected_depth, const float *d_grad_distortion, int use_gradient_scaling,
+                                               float *d_grad_field, float *const *d_grad_params12, float *d_grad_origins,
+                                               float *d_grad_directions, float *d_grad_xyz, void *stream) {
+    return tn_render_train_backward_saved3(h, d_saved, d_grad_rgb, d_grad_acc, d_grad_expected_depth, d_grad_distortion, use_gradient_scaling,
+                                           d_grad_field, d_grad_params12, d_grad_origins, d_grad_directions, d_grad_xyz, nullptr, stream);
 }
 
 extern "C" int tn_render_train_backward_saved(tn_tracer *h, const void *d_saved, const float *d_grad_rgb, const float *d_grad_acc,
@@ -1610,7 +1686,7 @@ extern "C" int tn_render_train_distortion(tn_tracer *h, const void *d_saved, flo
     SavedHeader hd{};
     TN_TRY(read_saved_header(h, d_saved, s, "tn_render_train_distortion", &hd));
     TrainBufs b{};
-    saved_layout(hd.R, hd.S2, (uint8_t *)d_saved, &b);
+    saved_layout(hd.R, hd.S2, (uint8_t *)d_saved, &b, false, hd.bgmap != 0);
     DistortionParams p{hd.S2, b.n_active, b.ray_list, b.ebins_f, b.sbins_f, b.out_f, d_distortion};
     // the same staging as k_composite, below k_composite_bwd's, which the forward has checked against the device's limit
     const size_t smem = SAMPLE_WARPS * sizeof(float) * 2 * ((size_t)hd.S2 + 2);
@@ -1649,6 +1725,21 @@ extern "C" int tn_render_set_occupancy2(tn_tracer *h, const float *d_occ, float 
 
 extern "C" int tn_render_set_occupancy(tn_tracer *h, const float *d_occ, float threshold) {
     return tn_render_set_occupancy2(h, d_occ, threshold, 0);
+}
+
+// background map (see the header; DESIGN §4.16): borrowed f32[H,W,3], W = 2H; NULL switches back to cfg->background.  Every call starts a
+// new generation, so the backward of a forward before it returns TN_ERR_STATE
+extern "C" int tn_render_set_background(tn_tracer *h, const float *d_map, uint32_t H, uint32_t W) {
+    if (!h) return fail(TN_ERR_ARG, "null tracer");
+    if (d_map != nullptr && (H == 0 || H > 16384 || W != 2 * H))
+        return fail(TN_ERR_ARG, "tn_render_set_background: the map must be [H, 2H, 3] with 1 <= H <= 16384");
+    DeviceGuard g(h->device);
+    RenderState *r = state(h);
+    r->bgmap = d_map;
+    r->bg_H = d_map != nullptr ? H : 0;
+    r->bg_W = d_map != nullptr ? W : 0;
+    r->bg_gen = next_generation();
+    return TN_OK;
 }
 
 // d_occ f32[T] <- max(decay * d_occ, the largest probe density of each tetrahedron): probe rows in chunks of OCC_CHUNK tetrahedra

@@ -5,6 +5,7 @@ it needs the CUDA library -- there is no PyTorch fallback."""
 from __future__ import annotations
 
 import ctypes as C
+import math
 from dataclasses import dataclass
 from typing import Dict, Optional
 
@@ -55,6 +56,37 @@ def _ptr(t: Optional[torch.Tensor]):
     return t.data_ptr() if t is not None else None
 
 
+BACKGROUND_POLE_EPS = 1e-8  # BG_POLE_EPS of csrc/tn_background.cuh
+
+
+def background_lookup(bg_map: torch.Tensor, directions: torch.Tensor) -> torch.Tensor:
+    """bg(d) of the background map f32[H,2H,3] for directions [..., 3] -> [..., 3], in torch (differentiable to both), the lookup the
+    fused kernels make (csrc/tn_background.cuh; DESIGN §4.16): n = d / |d|, u = W (atan2(n_y, n_x) / 2 pi + 1/2) - 1/2 with columns
+    modulo W, v = H (1 - n_z) / 2 - 1/2 clamped to [0, H - 1], bilinear in the lerp form, so a constant map returns its constant
+    exactly.  No grid_sample: its CUDA backward is not deterministic.  As the fused backward, the u-derivative is 0 where
+    n_x^2 + n_y^2 < BACKGROUND_POLE_EPS (near the poles, where atan2's derivative is unbounded, and 0/0 at the poles themselves)."""
+    H, W = int(bg_map.shape[0]), int(bg_map.shape[1])
+    n = directions / torch.linalg.vector_norm(directions, dim=-1, keepdim=True)
+    pole = (n[..., 0] * n[..., 0] + n[..., 1] * n[..., 1] < BACKGROUND_POLE_EPS)[..., None]
+    nxy = torch.where(pole, n[..., :2].detach(), n[..., :2])  # (where's backward drops the detached branch's NaN at the pole)
+    u = W * (torch.atan2(nxy[..., 1], nxy[..., 0]) / (2 * math.pi) + 0.5) - 0.5
+    v = (H * (1 - n[..., 2]) / 2 - 0.5).clamp(0, H - 1)
+    fi, fj = torch.floor(u), torch.floor(v)
+    fu, fv = (u - fi)[..., None], (v - fj)[..., None]
+    i0 = torch.remainder(fi.long(), W)
+    i1 = torch.remainder(i0 + 1, W)
+    j0 = fj.long().clamp(0, H - 1)
+    j1 = (j0 + 1).clamp(max=H - 1)
+    flat = bg_map.reshape(-1, 3)
+
+    def lerp(a, b, t):
+        return a + t * (b - a)
+
+    top = lerp(flat[j0 * W + i0], flat[j0 * W + i1], fu)
+    bot = lerp(flat[j1 * W + i0], flat[j1 * W + i1], fu)
+    return lerp(top, bot, fv)
+
+
 def _config(settings: RenderSettings) -> "ext._Cfg":
     return ext._Cfg(settings.max_intersected_triangles, settings.num_samples, settings.num_fine_samples, int(settings.use_biased_sampler),
                     float(settings.far_plane), (C.c_float * 3)(*settings.background))
@@ -74,6 +106,7 @@ class FusedRenderer:
         self.tracer = tracer
         self.device = tracer.device
         self._keep = None
+        self._bg = None
 
     def _stream(self):
         return torch.cuda.current_stream(self.device).cuda_stream
@@ -125,6 +158,22 @@ class FusedRenderer:
                                   self._stream()))
         return out
 
+    def set_background(self, bg_map: Optional[torch.Tensor]) -> None:
+        """composite, in every later render and training forward, over the background map bg_map f32[H,2H,3] (borrowed, kept alive
+        here; None: back to the settings' constant background): rgb = sum_j w_j c_j + (1 - accumulation) bg(d) on rays with hits,
+        rgb = bg(d) on empty ones (background_lookup; DESIGN §4.16).  Every call starts a new generation: the backward of a training
+        forward before it raises RuntimeError.  A training forward over a map keeps its directions, 12 more bytes per ray."""
+        if bg_map is not None:
+            if (bg_map.device != self.device or bg_map.dtype != torch.float32 or not bg_map.is_contiguous() or bg_map.dim() != 3
+                    or bg_map.shape[2] != 3 or bg_map.shape[1] != 2 * bg_map.shape[0]):
+                raise RuntimeError("the background map must be a contiguous float32 [H, 2H, 3] tensor on the tracer's device, got "
+                                   f"{tuple(bg_map.shape)}")
+            H, W = bg_map.shape[0], bg_map.shape[1]
+        else:
+            H = W = 0
+        ext._check(_lib.tn_render_set_background(self.tracer.handle, _ptr(bg_map), H, W))
+        self._bg = bg_map
+
     # ---- fused training step ------------------------------------------------------------------------------------------------------
     def _train_args(self, origins, directions, settings, jitter_coarse, jitter_fine):
         """checks the inputs of a training forward, allocates its outputs and sets the mode of the call -> (R, outputs, C arguments)"""
@@ -172,7 +221,9 @@ class FusedRenderer:
         return gfield, gp
 
     def train_saved_bytes(self, R: int, settings: RenderSettings) -> int:
-        """device bytes of the saved state of one training forward of R rays"""
+        """device bytes of the saved state of one training forward of R rays, for the renderer's state now: with a background map set
+        (set_background) the forward also keeps its ray directions, 12 bytes per ray more.  A blob sized before a set_background that
+        adds a map is too small for the forwards after it (they raise RuntimeError); train_forward_saved sizes its blob on every call"""
         n = C.c_size_t()
         ext._check(_lib.tn_render_train_saved_bytes(self.tracer.handle, C.byref(_config(settings)), int(R), C.byref(n)))
         return n.value
@@ -193,7 +244,7 @@ class FusedRenderer:
     def train_backward_saved(self, state: "TrainState", grad_rgb: torch.Tensor, grad_acc: Optional[torch.Tensor], num_vertices: int,
                              use_gradient_scaling: bool = False, grad_origins: bool = False, grad_directions: bool = False,
                              grad_vertices: bool = False, grad_expected_depth: Optional[torch.Tensor] = None,
-                             grad_distortion: Optional[torch.Tensor] = None):
+                             grad_distortion: Optional[torch.Tensor] = None, grad_background: bool = False):
         """backward of the train_forward_saved call that returned `state`; outputs as train_backward.  Raises RuntimeError if
         set_field / set_weights ran since that forward.  Waits until the stream has reached it (it reads the call's shape back).
         grad_origins / grad_directions: also the gradients at the forward's ray origins / directions (the sample distances held fixed;
@@ -203,7 +254,10 @@ class FusedRenderer:
         grad_vertices f32[V,3]); then it raises RuntimeError if load_tetrahedra or update_vertices ran since that forward.
         grad_expected_depth f32[R] or [R,1]: dL/d expected_depth of a forward with expected_depth=True (RuntimeError otherwise); the
         outputs keep the form above.  grad_distortion f32[R] or [R,1]: dL/d distortion (train_distortion; DESIGN §4.11), for any forward;
-        None runs the same kernels as before it existed."""
+        None runs the same kernels as before it existed.  grad_background: also the gradient at the background map of a forward over
+        one (set_background; DESIGN §4.16; RuntimeError otherwise, or after another set_background) -> always the 6-tuple (grad_field,
+        grads, grad_origins or None, grad_directions or None, grad_vertices or None, grad_background f32[H,2H,3]).  With a map the
+        direction gradients also hold the background's term, on every ray."""
         if tuple(grad_rgb.shape) != (state.R, 3) or (grad_acc is not None and grad_acc.numel() != state.R):
             raise RuntimeError(f"the forward rendered {state.R} rays: grad_rgb must be [{state.R}, 3] and grad_acc [{state.R}], got "
                                f"{tuple(grad_rgb.shape)} and {None if grad_acc is None else tuple(grad_acc.shape)}")
@@ -218,10 +272,17 @@ class FusedRenderer:
         go = torch.empty((state.R, 3), dtype=torch.float32, device=self.device) if grad_origins else None
         gd = torch.empty((state.R, 3), dtype=torch.float32, device=self.device) if grad_directions else None
         gv = torch.empty((num_vertices, 3), dtype=torch.float32, device=self.device) if grad_vertices else None
+        gbg = None
+        if grad_background:
+            if self._bg is None:
+                raise RuntimeError("grad_background: no background map is set (set_background)")
+            gbg = torch.empty_like(self._bg)
         gfield, gp, arr = self._grad_outputs(num_vertices)
-        ext._check(_lib.tn_render_train_backward_saved2(self.tracer.handle, state.blob.data_ptr(), grad_rgb.data_ptr(), _ptr(grad_acc),
+        ext._check(_lib.tn_render_train_backward_saved3(self.tracer.handle, state.blob.data_ptr(), grad_rgb.data_ptr(), _ptr(grad_acc),
                                                         _ptr(g_ed), _ptr(g_dist), int(use_gradient_scaling), gfield.data_ptr(), arr, _ptr(go),
-                                                        _ptr(gd), _ptr(gv), self._stream()))
+                                                        _ptr(gd), _ptr(gv), _ptr(gbg), self._stream()))
+        if grad_background:
+            return gfield, gp, go, gd, gv, gbg
         if grad_vertices:
             return gfield, gp, go, gd, gv
         return (gfield, gp, go, gd) if grad_origins or grad_directions else (gfield, gp)
@@ -357,7 +418,11 @@ class FusedTrainRender(torch.autograd.Function):
     An optional 13th tensor after the twelve parameters is the mesh's vertex positions f32[V,3], the very tensor the tracer borrowed
     (load_tetrahedra / update_vertices); when it requires grad the backward returns its gradient too (DESIGN §4.9: the sample distances
     and the matched tetrahedra held fixed), so an optimizer can move the points.  It raises if the tensor changed in place since the
-    tracer was loaded or refit (the trace would be stale), and an in-place change of it before the backward raises, as for the field."""
+    tracer was loaded or refit (the trace would be stale), and an in-place change of it before the backward raises, as for the field.
+
+    An optional last tensor, after the vertex positions when they are given, is the background map f32[H,2H,3] the renderer holds
+    (set_background; DESIGN §4.16); when it requires grad the backward returns its gradient too, and an in-place change of it before the
+    backward raises.  The same trailing tensors, and the same rules, apply to FusedTrainRenderDepth and FusedTrainRenderDistortion."""
 
     @staticmethod
     def forward(ctx, fr, settings, use_gradient_scaling, origins, directions, jitter_coarse, jitter_fine, field, *params):
@@ -439,6 +504,11 @@ def _fused_forward(ctx, name, expected_depth, fr, settings, use_gradient_scaling
     """forward of FusedTrainRender / FusedTrainRenderDepth / FusedTrainRenderDistortion: checks the optional vertex positions, runs the
     saved training forward and keeps what the backward needs in ctx -> the forward's outputs.  `first`: the index of `origins` among the
     op's arguments"""
+    bg = None
+    if len(params) > len(PARAM_ORDER) and params[-1].dim() == 3:  # the background map
+        bg, params = params[-1], params[:-1]
+        if fr._bg is None or bg.data_ptr() != fr._bg.data_ptr() or bg.shape != fr._bg.shape:
+            raise RuntimeError(f"{name}: the background map must be the tensor the renderer holds (set_background)")
     if len(params) == len(PARAM_ORDER) + 1:
         xyz, borrowed = params[-1], fr.tracer._vertices
         if borrowed is None or xyz.data_ptr() != borrowed.data_ptr() or xyz.shape != borrowed.shape:
@@ -448,11 +518,12 @@ def _fused_forward(ctx, name, expected_depth, fr, settings, use_gradient_scaling
             raise RuntimeError(f"{name}: the vertex positions changed in place since the tracer was loaded or refit; call "
                                "update_vertices first")
     elif len(params) != len(PARAM_ORDER):
-        raise RuntimeError(f"{name} takes the {len(PARAM_ORDER)} MLP parameters and optionally the vertex positions")
+        raise RuntimeError(f"{name} takes the {len(PARAM_ORDER)} MLP parameters and optionally the vertex positions and the background map")
     out, state = fr.train_forward_saved(origins, directions, settings, jitter_coarse, jitter_fine, expected_depth=expected_depth)
     ctx.fr, ctx.state, ctx.gs, ctx.first = fr, state, bool(use_gradient_scaling), first
     ctx.ray_shapes = (origins.shape, directions.shape)
-    ctx.save_for_backward(field, *params)  # their version counters reject a backward after an in-place change
+    ctx.has_xyz, ctx.has_bg = len(params) == len(PARAM_ORDER) + 1, bg is not None
+    ctx.save_for_backward(field, *params, *((bg,) if bg is not None else ()))  # their version counters reject a backward after an in-place change
     ctx.mark_non_differentiable(out["depth"], out["ray_mask"])
     return out
 
@@ -465,14 +536,16 @@ def _fused_backward(ctx, g_rgb, g_acc, g_ed, g_dist=None):
         g_rgb = torch.zeros((ctx.state.R, 3), dtype=torch.float32, device=field.device)
     first = ctx.first
     want_o, want_d = ctx.needs_input_grad[first], ctx.needs_input_grad[first + 1]
-    has_xyz = len(ctx.needs_input_grad) == first + 5 + len(PARAM_ORDER) + 1
-    want_v = has_xyz and ctx.needs_input_grad[-1]
+    has_xyz, has_bg = ctx.has_xyz, ctx.has_bg
+    want_v = has_xyz and ctx.needs_input_grad[first + 5 + len(PARAM_ORDER)]
+    want_bg = has_bg and ctx.needs_input_grad[-1]
     g_acc = g_acc.reshape(-1) if g_acc is not None else None
     g_ed = g_ed.reshape(-1) if g_ed is not None else None
     g_dist = g_dist.reshape(-1) if g_dist is not None else None
     res = ctx.fr.train_backward_saved(ctx.state, g_rgb, g_acc, field.shape[1], ctx.gs, grad_origins=want_o, grad_directions=want_d,
-                                      grad_vertices=want_v, grad_expected_depth=g_ed, grad_distortion=g_dist)
-    gfield, gp, go, gd, gv = res + (None,) * (5 - len(res))
+                                      grad_vertices=want_v, grad_expected_depth=g_ed, grad_distortion=g_dist, grad_background=want_bg)
+    gfield, gp, go, gd, gv, gbg = res + (None,) * (6 - len(res))
     go = go.reshape(ctx.ray_shapes[0]) if go is not None else None
     gd = gd.reshape(ctx.ray_shapes[1]) if gd is not None else None
-    return (None,) * first + (go, gd, None, None, gfield) + tuple(gp[n] for n in PARAM_ORDER) + ((gv,) if has_xyz else ())
+    return (None,) * first + (go, gd, None, None, gfield) + tuple(gp[n] for n in PARAM_ORDER) + ((gv,) if has_xyz else ()) \
+        + ((gbg,) if has_bg else ())

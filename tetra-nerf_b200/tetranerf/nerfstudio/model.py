@@ -136,6 +136,12 @@ class TetrahedraNerfConfig(ModelConfig):
     """a candidate proposes its longest edge only when that is at least this long"""
     refine_max_vertices: Optional[int] = None
     """refinement stops adding vertices at this many mesh vertices (None: no limit)"""
+    background_envmap_height: int = 0
+    """> 0: learn the light that leaves the mesh as an environment map: the parameter `background_envmap` f32[H, 2H, 3] (H this value;
+    "fields" group, in the state dict only when enabled) in the model's frame, z up, equal-area in latitude, initialised to
+    background_color (white or black; RuntimeError otherwise), so the first render is the constant-background render bit for bit.
+    Every path composites rgb = sum_j w_j c_j + (1 - accumulation) bg(d), and rgb = bg(d) on rays that miss the mesh (DESIGN §4.16).
+    0 = off, nothing changes"""
 
     def __post_init__(self):
         if self.tetrahedra_path is not None and self.num_tetrahedra_vertices is None:
@@ -389,6 +395,13 @@ class TetrahedraNerf(Model):
         self.renderer_depth = DepthRenderer()
         self.renderer_expected_depth = DepthRenderer(method="expected")
         self.rgb_loss = MSELoss()
+        H = self.config.background_envmap_height
+        if H > 0:
+            if self.config.background_color not in ("white", "black"):
+                raise RuntimeError(f"background_envmap_height > 0 starts the map at background_color, which must be 'white' or 'black', "
+                                   f"got {self.config.background_color!r}")
+            init = 1.0 if self.config.background_color == "white" else 0.0
+            self.register_parameter("background_envmap", nn.Parameter(torch.full((H, 2 * H, 3), init, dtype=torch.float32)))
 
     def get_param_groups(self) -> Dict[str, List[Parameter]]:
         if not self.config.optimize_vertices:
@@ -453,6 +466,17 @@ class TetrahedraNerf(Model):
         else:
             fr.set_occupancy(occ, c.occupancy_threshold)
 
+    def _apply_background(self, fr) -> None:
+        """points the fused renderer `fr` at background_envmap, or at the constant background when it is off.  The renderer is set again
+        only when the map's storage changed, so a training forward's backward stays valid across other renders"""
+        m = self.background_envmap.detach() if self.config.background_envmap_height > 0 else None
+        cur = fr._bg
+        if m is None:
+            if cur is not None:
+                fr.set_background(None)
+        elif cur is None or cur.data_ptr() != m.data_ptr() or cur.shape != m.shape:
+            fr.set_background(m)
+
     # ---- forward (reference :520-662) ---------------------------------------------------------------------
     def _expected_depth_on(self) -> bool:
         return self.config.render_expected_depth or self.config.depth_loss_mult > 0
@@ -489,6 +513,7 @@ class TetrahedraNerf(Model):
             with torch.no_grad():
                 fr = self._fused_renderer()
                 self._apply_occupancy(fr, training=False)
+                self._apply_background(fr)
                 return fr.render(origins, directions, st, normals=normals, expected_depth=self._expected_depth_on())
         unfused_train = os.environ.get("TETRANERF_B200_UNFUSED_TRAIN", "0") == "1"
         if self.training and torch.is_grad_enabled() and self.config.optimize_vertices:
@@ -511,12 +536,14 @@ class TetrahedraNerf(Model):
         fr = self._fused_renderer()
         with torch.no_grad():
             self._apply_occupancy(fr, training=True)
+        self._apply_background(fr)
         R, dev = origins.shape[0], origins.device
         jc = torch.rand((R, c.num_samples + 1), dtype=torch.float32, device=dev) if getattr(self.sampler_uniform, "train_stratified", True) else None
         jf = torch.rand((R, c.num_fine_samples + 1), dtype=torch.float32, device=dev) if getattr(self.sampler_pdf, "train_stratified", True) else None
         named = dict(self.named_parameters())
         xyz = (self.tetrahedra_vertices,) if c.optimize_vertices else ()  # the tensor the tracer borrowed (get_tetrahedra_tracer)
-        args = (fr, st, c.use_gradient_scaling, origins, directions, jc, jf, self.tetrahedra_field, *[named[n] for n in PARAM_ORDER], *xyz)
+        bg = (self.background_envmap,) if c.background_envmap_height > 0 else ()  # the tensor the renderer holds (_apply_background)
+        args = (fr, st, c.use_gradient_scaling, origins, directions, jc, jf, self.tetrahedra_field, *[named[n] for n in PARAM_ORDER], *xyz, *bg)
         if self._distortion_on():
             res = FusedTrainRenderDistortion.apply(*args[:3], self._expected_depth_on(), *args[3:])
             keys = ["rgb", "accumulation", "depth"] + (["expected_depth"] if self._expected_depth_on() else []) + ["distortion", "ray_mask"]
@@ -542,7 +569,14 @@ class TetrahedraNerf(Model):
         ray_mask = count > 0
         device = ray_mask.device
         R = ray_mask.shape[0]
-        rgb = self.get_background_color((R, 3), device=device)
+        envmap = self.config.background_envmap_height > 0
+        if envmap:  # bg(d) on every ray (the torch restatement of the fused lookup), clamped in eval mode as every pixel
+            from ..b200.render import background_lookup
+
+            bg = background_lookup(self.background_envmap, directions)
+            rgb = bg if self.training else bg.clamp(0.0, 1.0)
+        else:
+            rgb = self.get_background_color((R, 3), device=device)
         accumulation = torch.zeros((R, 1), dtype=torch.float32, device=device)
         depth = torch.full((R, 1), self.collider.far_plane, dtype=torch.float32, device=device)
         outputs = {"rgb": rgb, "accumulation": accumulation, "depth": depth, "ray_mask": ray_mask}
@@ -574,7 +608,15 @@ class TetrahedraNerf(Model):
             if self.config.use_gradient_scaling:
                 colors, sigmas, _ = GradientScaler.apply(colors, sigmas, samples.spacing_ends + samples.spacing_starts)
             weights = samples.get_weights(sigmas)
-            rgb[ray_mask] = self.renderer_rgb(rgb=colors, weights=weights)
+            if envmap:  # RGBRenderer over the per-ray background
+                if not self.training:
+                    colors = torch.nan_to_num(colors)
+                comp = torch.sum(weights * colors, dim=-2) + bg[ray_mask] * (1.0 - torch.sum(weights, dim=-2))
+                rgb = rgb.clone()
+                rgb[ray_mask] = comp if self.training else comp.clamp(0.0, 1.0)
+                outputs["rgb"] = rgb
+            else:
+                rgb[ray_mask] = self.renderer_rgb(rgb=colors, weights=weights)
             accumulation[ray_mask] = self.renderer_accumulation(weights)
             depth[ray_mask] = self.renderer_depth(weights, samples)
             if self._expected_depth_on():

@@ -67,6 +67,8 @@ _lib.tn_render_train_forward_saved.argtypes = [_vp, C.POINTER(_Cfg), _vp, _vp, _
 _lib.tn_render_train_backward_saved.argtypes = [_vp, _vp, _vp, _vp, _vp, _i, _vp, C.POINTER(_vp), _vp, _vp, _vp, _vp]
 _lib.tn_render_train_backward_saved2.argtypes = [_vp, _vp, _vp, _vp, _vp, _vp, _i, _vp, C.POINTER(_vp), _vp, _vp, _vp, _vp]
 _lib.tn_render_train_distortion.argtypes = [_vp, _vp, _vp, _vp]
+_lib.tn_render_train_backward_saved3.argtypes = [_vp, _vp, _vp, _vp, _vp, _vp, _i, _vp, C.POINTER(_vp), _vp, _vp, _vp, _vp, _vp]
+_lib.tn_render_set_background.argtypes = [_vp, _vp, _u32, _u32]
 _lib.tn_render_debug_buffers.argtypes = [_vp, C.POINTER(_vp)]
 _lib.tn_render_set_profiling.argtypes = [_vp, _i]
 _lib.tn_render_set_mlp_precision.argtypes = [_vp, _i]

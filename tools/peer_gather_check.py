@@ -1,5 +1,7 @@
-"""torchrun --nproc-per-node N tools/peer_gather_check.py : the fused peer-store pixel gather (tn_render_set_gather) against the 1-GPU
-render of the whole batch, bit for bit, on every rank; also the NCCL all_gather path (tetranerf.b200.distributed.sharded_render)."""
+"""torchrun --nproc-per-node N tools/peer_gather_check.py [--background] : the fused peer-store pixel gather (tn_render_set_gather) against
+the 1-GPU render of the whole batch, bit for bit, on every rank; also the NCCL all_gather path (tetranerf.b200.distributed.sharded_render).
+--background: every render composites over the same N(0,1) background map (FusedRenderer.set_background, DESIGN §4.16), so the gathered
+pixels of the active rays and of the rays that miss the mesh come from the map lookup inside the pixel-writing kernels."""
 import os
 import sys
 from pathlib import Path
@@ -30,11 +32,16 @@ def main():
     R = Rper * world
     o, d = syn.camera_rays(R, seed=77)
     o[5] = [5, 5, 5]; d[5] = [1, 0, 0]
+    if "--background" in sys.argv:  # a miss in every rank's shard, looking elsewhere on the map
+        for r in range(world):
+            o[r * Rper + 7] = [-4, 0.5, 0.5]; d[r * Rper + 7] = [-0.8, 0.2, 0.56]
     tr = cpp.TetrahedraTracer(dev)
     tr.load_tetrahedra(torch.from_numpy(V).to(dev), torch.from_numpy(C).to(dev))
     fr = FusedRenderer(tr)
     fr.set_field(torch.from_numpy(field).to(dev))
     fr.set_weights(params)
+    if "--background" in sys.argv:  # the same map on every rank (seeded on the CPU)
+        fr.set_background(torch.randn((8, 16, 3), generator=torch.Generator().manual_seed(5)).to(dev))
     st = RenderSettings.tetra_nerf()
     do, dd = torch.from_numpy(o).to(dev), torch.from_numpy(d).to(dev)
     whole = {k: v.clone() for k, v in fr.render(do, dd, st).items()}  # every rank renders the whole batch itself: the reference result
@@ -55,7 +62,8 @@ def main():
     assert torch.equal(gathered[:, 5] > 0.5, whole["ray_mask"])
     dist.barrier()
     if rank == 0:
-        print(f"peer_gather_check ok: world {world}, {R} rays, fused peer-store gather == NCCL gather == 1-GPU render (bitwise)")
+        bg = ", over a background map" if "--background" in sys.argv else ""
+        print(f"peer_gather_check ok: world {world}, {R} rays{bg}, fused peer-store gather == NCCL gather == 1-GPU render (bitwise)")
     dist.destroy_process_group()
 
 
