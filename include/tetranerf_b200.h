@@ -54,6 +54,19 @@ int tn_load_tetrahedra(tn_tracer *h, const float *d_xyz, uint32_t V, const uint3
  * generation: a pending ray / vertex gradient backward returns TN_ERR_STATE and tn_surface_copy refuses an earlier extraction.
  * Synchronous (one small read-back).  DESIGN.md §4.9. */
 int tn_update_vertices(tn_tracer *h, const float *d_xyz, uint32_t V, uint32_t *folded_faces, int *walkable, void *stream);
+/* Fold guard of a vertex step (DESIGN.md §4.17): scales back, per vertex, a proposed move of the loaded mesh's vertices from d_xyz_old
+ * (P0, f32[V,3]) to d_xyz_new (P1, f32[V,3], overwritten with the result) so that tn_update_vertices at the result certifies every interior
+ * face it certifies at P0, and, if the mesh is walkable at P0 (the load kept its hull edges, all of them pass the convexity test at P0 and
+ * no interior face is uncertified), keeps every hull edge convex, so the walk stays on.  Faces already uncertified at P0 are not guarded.
+ * A vertex whose P1 row differs bitwise from its P0 row ends at P1 (bitwise), at P0 + 2^-k (P1 - P0) for the smallest round k in
+ * 1..max_halvings its guarded faces and hull edges needed (each op rounded to fp32 in that order, no FMA), or frozen at P0 (bitwise).
+ * If nothing would fold, d_xyz_new is unchanged.  The result depends on (P0, P1, cells) alone: bitwise reproducible.  counts3 (may be
+ * NULL) receives the vertices limited (1 <= k <= max_halvings), the vertices frozen and the rounds run (1 when nothing fails; one small
+ * read-back each).  Uses the loaded mesh's face table and hull edges; neither position array is borrowed.  TN_ERR_STATE without a mesh;
+ * TN_ERR_ARG if V differs from the load's, max_halvings > 23 or a coordinate of either array is not finite (d_xyz_new is then unchanged).
+ * Synchronous, like tn_update_vertices. */
+int tn_guard_vertex_step(tn_tracer *h, const float *d_xyz_old, float *d_xyz_new, uint32_t V, uint32_t max_halvings, uint32_t *counts3,
+                         void *stream);
 int tn_num_faces(tn_tracer *h, uint32_t *F);
 /* copies out the unique-face tables in reference numbering: d_tri u32[F,3], d_tt u32[F,2]
  * (triangle_indices / triangle_tetrahedra of src/optix_types.h:4-5) */

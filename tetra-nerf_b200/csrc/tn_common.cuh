@@ -186,6 +186,12 @@ struct tn_tracer {
     tn::DevArray<uint32_t> adj_off;        // [V+1] CSR row offsets
     tn::DevArray<uint32_t> adj_nbr;        // [2E] neighbours, each row ascending
     tn::DevArray<double> adj_part;         // one partial sum per block of the smoothness kernel
+    // scratch of tn_guard_vertex_step (tn_fold_guard.cu), grown on its first call and kept
+    tn::DevArray<uint4> guard_face;        // [F] per interior face certified at P0: (a, b, c, p); a = TN_EMPTY otherwise
+    tn::DevArray<uint32_t> guard_faceq;    // [F] its other opposite vertex q
+    tn::DevArray<float> guard_p1;          // [3V] the proposed positions
+    tn::DevArray<uint8_t> guard_vtx;       // [3V] per vertex: exponent state, failure mark, changed in the last round
+    tn::DevArray<uint32_t> guard_counts;   // [8] flags and counters, read back once per round
 };
 
 namespace tn {

@@ -14,6 +14,7 @@
 #include <cub/device/device_select.cuh>
 
 #include "tn_common.cuh"
+#include "tn_predicates.cuh"
 
 namespace tn {
 
@@ -134,30 +135,6 @@ __global__ void k_hull_edges(const uint4 *__restrict__ tri, const uint32_t *__re
     ekey[e] = ((unsigned long long)a << 32) | b;
     eface[e] = f;
 }
-__device__ bool hull_pair_ok(const float *__restrict__ xyz, const uint4 *__restrict__ cells, const uint4 *__restrict__ tri, const uint2 *__restrict__ tt,
-                             uint32_t f, uint32_t g) {
-    // outward normal of hull face f: away from its tetrahedron's 4th vertex
-    const uint4 c4 = cells[tt[f].x];
-    const uint32_t cv[4] = {c4.x, c4.y, c4.z, c4.w};
-    const uint4 ft = tri[f], gt = tri[g];
-    const uint32_t fv[3] = {ft.x, ft.y, ft.z}, gv[3] = {gt.x, gt.y, gt.z};
-    uint32_t inner = 0;
-    for (int q = 0; q < 4; ++q)
-        if (cv[q] != fv[0] && cv[q] != fv[1] && cv[q] != fv[2]) inner = cv[q];
-    auto P = [&](uint32_t v, int a) { return (double)xyz[3 * (size_t)v + a]; };
-    double e1[3], e2[3], n[3];
-    for (int a = 0; a < 3; ++a) { e1[a] = P(fv[1], a) - P(fv[0], a); e2[a] = P(fv[2], a) - P(fv[0], a); }
-    n[0] = e1[1] * e2[2] - e1[2] * e2[1]; n[1] = e1[2] * e2[0] - e1[0] * e2[2]; n[2] = e1[0] * e2[1] - e1[1] * e2[0];
-    double si = 0, nn = 0;
-    for (int a = 0; a < 3; ++a) { si += n[a] * (P(inner, a) - P(fv[0], a)); nn += n[a] * n[a]; }
-    if (si > 0) for (int a = 0; a < 3; ++a) n[a] = -n[a];
-    for (int k = 0; k < 3; ++k) {
-        double sd = 0, dd = 0;
-        for (int a = 0; a < 3; ++a) { const double d = P(gv[k], a) - P(fv[0], a); sd += n[a] * d; dd += d * d; }
-        if (sd > 1e-9 * sqrt(nn * dd) + 1e-30) return false;  // a vertex of the neighbouring hull face lies outside
-    }
-    return true;
-}
 __global__ void k_hull_check(const float *__restrict__ xyz, const uint4 *__restrict__ cells, const uint4 *__restrict__ tri, const uint2 *__restrict__ tt,
                              const unsigned long long *__restrict__ ekey, const uint32_t *__restrict__ eface, uint32_t n, uint32_t *__restrict__ err) {
     const uint32_t p = blockIdx.x * blockDim.x + threadIdx.x;
@@ -173,34 +150,7 @@ __global__ void k_iota(uint32_t *__restrict__ v, uint32_t n) {
 }
 
 // ---- fold test of a refit: for every interior face (a, b, c), the opposite vertices p, q of its two tetrahedra must lie strictly on
-// opposite sides of its plane.  orient3d(a, b, c, x) = det[a - x; b - x; c - x] in float64 on the fp32 positions, with every operation
-// rounded individually (no FMA contraction, the op order of oracle/vertex_grads.py's restatement) and Shewchuk's forward error bound
-// (7 + 56 eps) eps * permanent, eps = 2^-53: a sign the bound cannot certify counts as folded, so rounding can only turn the walk off.
-__device__ __forceinline__ bool orient3d_sign(const float *__restrict__ xyz, uint32_t ia, uint32_t ib, uint32_t ic, uint32_t ix, int &sign) {
-    auto P = [&](uint32_t v, int a) { return (double)__ldg(xyz + 3 * (size_t)v + a); };
-    const double adx = __dsub_rn(P(ia, 0), P(ix, 0)), ady = __dsub_rn(P(ia, 1), P(ix, 1)), adz = __dsub_rn(P(ia, 2), P(ix, 2));
-    const double bdx = __dsub_rn(P(ib, 0), P(ix, 0)), bdy = __dsub_rn(P(ib, 1), P(ix, 1)), bdz = __dsub_rn(P(ib, 2), P(ix, 2));
-    const double cdx = __dsub_rn(P(ic, 0), P(ix, 0)), cdy = __dsub_rn(P(ic, 1), P(ix, 1)), cdz = __dsub_rn(P(ic, 2), P(ix, 2));
-    const double bdxcdy = __dmul_rn(bdx, cdy), cdxbdy = __dmul_rn(cdx, bdy);
-    const double cdxady = __dmul_rn(cdx, ady), adxcdy = __dmul_rn(adx, cdy);
-    const double adxbdy = __dmul_rn(adx, bdy), bdxady = __dmul_rn(bdx, ady);
-    const double det = __dadd_rn(__dadd_rn(__dmul_rn(adz, __dsub_rn(bdxcdy, cdxbdy)), __dmul_rn(bdz, __dsub_rn(cdxady, adxcdy))),
-                                 __dmul_rn(cdz, __dsub_rn(adxbdy, bdxady)));
-    const double perm = __dadd_rn(__dadd_rn(__dmul_rn(__dadd_rn(fabs(bdxcdy), fabs(cdxbdy)), fabs(adz)),
-                                            __dmul_rn(__dadd_rn(fabs(cdxady), fabs(adxcdy)), fabs(bdz))),
-                                  __dmul_rn(__dadd_rn(fabs(adxbdy), fabs(bdxady)), fabs(cdz)));
-    const double eps = 1.1102230246251565e-16;  // 2^-53
-    const double bound = __dmul_rn(__dmul_rn(__dadd_rn(7.0, __dmul_rn(56.0, eps)), eps), perm);
-    sign = det > bound ? 1 : (-det > bound ? -1 : 0);
-    return sign != 0;
-}
-__device__ __forceinline__ uint32_t opposite_vertex(const uint4 c, const uint4 f) {
-    const uint32_t cv[4] = {c.x, c.y, c.z, c.w};
-    uint32_t o = cv[0];
-    for (int q = 0; q < 4; ++q)
-        if (cv[q] != f.x && cv[q] != f.y && cv[q] != f.z) o = cv[q];
-    return o;
-}
+// opposite sides of its plane (face_unfolded, tn_predicates.cuh) ----
 __global__ void k_fold_faces(const float *__restrict__ xyz, const uint4 *__restrict__ cells, const uint4 *__restrict__ tri, const uint2 *__restrict__ tt,
                              uint32_t F, uint32_t *__restrict__ folded) {
     const uint32_t f = blockIdx.x * blockDim.x + threadIdx.x;
@@ -208,10 +158,7 @@ __global__ void k_fold_faces(const float *__restrict__ xyz, const uint4 *__restr
     const uint2 o = tt[f];
     if (o.y == TN_EMPTY) return;
     const uint4 t = tri[f];
-    int sp = 0, sq = 0;
-    const bool cp = orient3d_sign(xyz, t.x, t.y, t.z, opposite_vertex(cells[o.x], t), sp);
-    const bool cq = orient3d_sign(xyz, t.x, t.y, t.z, opposite_vertex(cells[o.y], t), sq);
-    if (!(cp && cq && sp == -sq)) atomicAdd(folded, 1u);
+    if (!face_unfolded(xyz, t.x, t.y, t.z, opposite_vertex(cells[o.x], t), opposite_vertex(cells[o.y], t))) atomicAdd(folded, 1u);
 }
 
 int launch_refit_checks(const tn_tracer *h, const float *d_xyz, uint32_t *d_counts, cudaStream_t s) {

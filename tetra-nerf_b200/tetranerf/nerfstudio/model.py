@@ -54,6 +54,10 @@ except ImportError:
 from ..utils.extension import TetrahedraTracer, interpolate_values, triangulate
 
 
+VERTEX_FOLD_GUARD_MAX_HALVINGS = 8
+"""vertex_fold_guard: the most times a vertex's step is halved before the vertex is held at its old position instead (2^-8 of the step)"""
+
+
 @dataclass
 class TetrahedraNerfConfig(ModelConfig):
     """Field-for-field the reference config (model.py:70-107)."""
@@ -97,6 +101,13 @@ class TetrahedraNerfConfig(ModelConfig):
     optimize_vertices: bool = False
     """train the mesh vertex positions too: `tetrahedra_vertices` becomes a parameter in its own param group "vertices" (same state-dict
     key and shape), the tracer is refit after every optimizer step (topology fixed), training runs on the fused path only (DESIGN §4.9)"""
+    vertex_fold_guard: bool = False
+    """with optimize_vertices: before each refit, scale back per vertex the part of the optimizer's step that would fold the mesh
+    (TetrahedraTracer.guard_vertex_step, DESIGN §4.17): every interior face certified unfolded at the last load or refit stays so, and
+    a mesh the adjacency walk ran on keeps it.  A vertex of a face the step would fold moves 2^-k of its step, k the round in
+    1..VERTEX_FOLD_GUARD_MAX_HALVINGS after which none of its faces fails, or stays where it was.  The optimizer state is not touched.  A different
+    policy from the default (where a folding step is taken, warned about once, and the walk turns off), hence an option.  Needs
+    optimize_vertices (RuntimeError otherwise).  False changes nothing"""
     render_expected_depth: bool = False
     """every path (fused eval, fused training, unfused) also returns "expected_depth" f32[R,1], nerfstudio's
     DepthRenderer(method="expected") clipped to the batch's smallest / largest sample midpoint, far plane on empty rays (DESIGN §4.10);
@@ -244,6 +255,7 @@ class TetrahedraNerf(Model):
         self._fused = None
         self._fused_versions = None
         self._grad_acc = self._grad_cnt = None  # refinement statistics (refine_every > 0): not part of the state dict
+        self._guard_start = None  # vertex_fold_guard: device copy of the positions the tracer was last loaded or refit at
         if self.config.tetrahedra_path is None and metadata is not None and "points3D_xyz" in metadata:
             self._load_points_from_metadata(**metadata)
         else:
@@ -284,6 +296,7 @@ class TetrahedraNerf(Model):
             self.config.num_tetrahedra_vertices, self.config.num_tetrahedra_cells = len(self.tetrahedra_vertices), len(self.tetrahedra_cells)
             self._tetrahedra_tracer = self._fused = self._fused_versions = None
             self._grad_acc = self._grad_cnt = None
+        self._guard_start = None  # the loaded positions are not a step: the next refit takes them as they are
         super()._load_from_state_dict(state_dict, prefix, *args, **kwargs)
         if complete:
             self._tetrahedra_initialized = True
@@ -349,11 +362,15 @@ class TetrahedraNerf(Model):
             ptr, V, version = self._tracer_vertices
             if (xyz.data_ptr(), len(xyz)) != (ptr, V):  # another tensor: a fresh load
                 self._tetrahedra_tracer.load_tetrahedra(xyz, self.tetrahedra_cells)
+                self._keep_guard_start(xyz)
             elif self.tetrahedra_vertices._version != version:  # moved in place (an optimizer step): refit, same topology
+                if self._guard_start is not None:  # vertex_fold_guard: scale the step back where it would fold the mesh
+                    self._tetrahedra_tracer.guard_vertex_step(self._guard_start, xyz, VERTEX_FOLD_GUARD_MAX_HALVINGS)
                 folded, _ = self._tetrahedra_tracer.update_vertices(xyz)
                 if folded and not self._fold_warned:
                     warnings.warn(f"optimize_vertices: {folded} mesh faces are folded; tracing continues on the all-hits gather (exact, slower)")
                     self._fold_warned = True
+                self._keep_guard_start(xyz)
             self._tracer_vertices = (xyz.data_ptr(), len(xyz), self.tetrahedra_vertices._version)
         if self._tetrahedra_tracer is None:
             if not self._tetrahedra_initialized:
@@ -362,8 +379,18 @@ class TetrahedraNerf(Model):
             self._tetrahedra_tracer = TetrahedraTracer(device)
             self._tetrahedra_tracer.load_tetrahedra(xyz, self.tetrahedra_cells)
             self._tracer_vertices = (xyz.data_ptr(), len(xyz), self.tetrahedra_vertices._version)
+            self._keep_guard_start(xyz)
             self._fold_warned = False
         return self._tetrahedra_tracer
+
+    def _keep_guard_start(self, xyz: torch.Tensor) -> None:
+        """vertex_fold_guard: the positions the tracer now holds are where the next step starts from"""
+        if not (self.config.optimize_vertices and self.config.vertex_fold_guard):
+            return
+        if self._guard_start is not None and self._guard_start.shape == xyz.shape and self._guard_start.device == xyz.device:
+            self._guard_start.copy_(xyz)
+        else:
+            self._guard_start = xyz.clone()
 
     # ---- modules (reference :409-477) ----------------------------------------------------------------
     def populate_modules(self):
@@ -395,6 +422,8 @@ class TetrahedraNerf(Model):
         self.renderer_depth = DepthRenderer()
         self.renderer_expected_depth = DepthRenderer(method="expected")
         self.rgb_loss = MSELoss()
+        if self.config.vertex_fold_guard and not self.config.optimize_vertices:
+            raise RuntimeError("vertex_fold_guard guards the steps of the vertex positions: it needs optimize_vertices=True")
         H = self.config.background_envmap_height
         if H > 0:
             if self.config.background_color not in ("white", "black"):
@@ -739,6 +768,7 @@ class TetrahedraNerf(Model):
         if self._tetrahedra_tracer is not None:
             self._tetrahedra_tracer.load_tetrahedra(self.tetrahedra_vertices.detach(), self.tetrahedra_cells)
             self._tracer_vertices = (self.tetrahedra_vertices.data_ptr(), len(xyz), self.tetrahedra_vertices._version)
+            self._keep_guard_start(self.tetrahedra_vertices.detach())
 
     # ---- geometry export -----------------------------------------------------------------------------------------------------------------
     def extract_surface(self, level: float) -> Dict[str, torch.Tensor]:

@@ -30,6 +30,7 @@ _lib.tn_destroy.argtypes = [_vp]
 _lib.tn_synchronize.argtypes = [_vp, _vp]
 _lib.tn_load_tetrahedra.argtypes = [_vp, _vp, _u32, _vp, _u32, _vp]
 _lib.tn_update_vertices.argtypes = [_vp, _vp, _u32, C.POINTER(_u32), C.POINTER(_i), _vp]
+_lib.tn_guard_vertex_step.argtypes = [_vp, _vp, _vp, _u32, _u32, C.POINTER(_u32 * 3), _vp]
 _lib.tn_num_faces.argtypes = [_vp, C.POINTER(_u32)]
 _lib.tn_get_faces.argtypes = [_vp, _vp, _vp, _vp]
 _lib.tn_trace_rays.argtypes = [_vp, _vp, _vp, _u32, _u32, _vp, _vp, _vp, _vp, _vp, _i, _vp]
@@ -183,6 +184,28 @@ class TetrahedraTracer:
             _check(_lib.tn_update_vertices(self._h, xyz.data_ptr(), xyz.numel() // 3, C.byref(folded), C.byref(walkable), _stream(self._device)))
         self._vertices, self._vertices_version = xyz, xyz._version
         return int(folded.value), bool(walkable.value)
+
+    def guard_vertex_step(self, old: torch.Tensor, new: torch.Tensor, max_halvings: int = 8):
+        """the fold guard of a vertex step (DESIGN §4.17): scales back, in place in `new` f32[V,3], each vertex's move from `old` f32[V,3]
+        (the positions the tracer was last loaded or refit at, typically) that would fold an interior face certified unfolded at `old`, or,
+        on a mesh walkable at `old`, break the hull's convexity.  A moving vertex ends at `new` (bitwise), at old + (new - old) * 2^-k for
+        some 1 <= k <= max_halvings, or back at `old` (bitwise); if nothing would fold, `new` is unchanged.  update_vertices(new) then
+        reports only the faces already uncertified at `old`, and the walk stays on if it was on at `old`.  Uses the loaded mesh's topology;
+        nothing is borrowed.  -> (limited, frozen, rounds): vertices scaled back, vertices moved back to `old`, rounds run.  Raises
+        RuntimeError without a loaded mesh, on another V, a non-finite coordinate (`new` is then unchanged) or max_halvings > 23.  Waits
+        until the stream has reached it; bumps `new`'s version counter when it changed it."""
+        self._check_float_dim3(old, "old")
+        self._check_float_dim3(new, "new")
+        _require(self._cells is not None, "load_tetrahedra must be called first")
+        _require(old.numel() == new.numel(), "old and new must have the same shape")
+        counts = (_u32 * 3)()
+        with torch.cuda.device(self._device):
+            _check(_lib.tn_guard_vertex_step(self._h, old.data_ptr(), new.data_ptr(), new.numel() // 3, int(max_halvings), C.byref(counts),
+                                             _stream(self._device)))
+        limited, frozen, rounds = (int(x) for x in counts)
+        if limited or frozen:
+            torch.autograd.graph.increment_version(new)
+        return limited, frozen, rounds
 
     def num_faces(self) -> int:
         n = _u32(0)
