@@ -10,6 +10,7 @@
 
 #include "tn_background.cuh"
 #include "tn_common.cuh"
+#include "tn_sort.cuh"
 
 namespace tn {
 
@@ -45,18 +46,12 @@ __global__ void __launch_bounds__(256) k_bg_rays(const BackgroundGradsLaunch p) 
     }
 }
 
-__device__ __forceinline__ uint32_t lower_bound_keys(const uint32_t *__restrict__ a, uint32_t n, uint32_t x) {
-    uint32_t lo = 0, hi = n;
-    while (lo < hi) { const uint32_t mid = (lo + hi) >> 1; if (__ldg(a + mid) < x) lo = mid + 1; else hi = mid; }
-    return lo;
-}
-
 // deterministic mode, after the sort: texel x sums w_k s over its entries in sorted order
 __global__ void __launch_bounds__(256) k_bg_texels(const BackgroundGradsLaunch p, const uint32_t *__restrict__ keys,
                                                    const uint32_t *__restrict__ vals) {
     const uint32_t x = blockIdx.x * blockDim.x + threadIdx.x;
     if (x >= p.H * p.W) return;
-    const uint32_t n = 4 * p.R, lo = lower_bound_keys(keys, n, x), hi = lower_bound_keys(keys, n, x + 1);
+    const uint32_t n = 4 * p.R, lo = lower_bound_u32(keys, n, x), hi = lower_bound_u32(keys, n, x + 1);
     float acc[3] = {0.f, 0.f, 0.f};
     for (uint32_t e = lo; e < hi; ++e) {
         const uint32_t v = __ldg(vals + e), ray = v >> 2;
@@ -69,16 +64,7 @@ __global__ void __launch_bounds__(256) k_bg_texels(const BackgroundGradsLaunch p
     for (int c = 0; c < 3; ++c) p.grad_map[3 * (size_t)x + c] = acc[c];
 }
 
-static int key_bits(uint32_t H, uint32_t W) { return 32 - __builtin_clz((H * W) | 1u); }
-
-int background_sort_bytes(uint32_t R, uint32_t H, uint32_t W, size_t *bytes) {
-    *bytes = 0;
-    TN_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, *bytes, (uint32_t *)nullptr, (uint32_t *)nullptr, (uint32_t *)nullptr,
-                                            (uint32_t *)nullptr, (int)(4 * R), 0, key_bits(H, W)));
-    return TN_OK;
-}
-
-int launch_background_grads(const BackgroundGradsLaunch &a, cudaStream_t s) {
+int launch_background_grads(const BackgroundGradsLaunch &a, DevArray<uint8_t> &tmp, cudaStream_t s) {
     const uint32_t blocks = (a.R + 255) / 256;
     if (!a.det || a.grad_map == nullptr) {  // (without a map gradient only the per-ray direction term is left)
         if (a.grad_map != nullptr) TN_CUDA(cudaMemsetAsync(a.grad_map, 0, sizeof(float) * 3 * (size_t)a.H * a.W, s));
@@ -86,8 +72,10 @@ int launch_background_grads(const BackgroundGradsLaunch &a, cudaStream_t s) {
     } else {
         k_bg_rays<true><<<blocks, 256, 0, s>>>(a);
         const uint32_t n = 4 * a.R;
-        size_t bytes = a.cub_bytes;
-        TN_CUDA(cub::DeviceRadixSort::SortPairs(a.cub_tmp, bytes, a.keys, a.keys + n, a.vals, a.vals + n, (int)n, 0, key_bits(a.H, a.W), s));
+        const int end_bit = radix_end_bit(a.H * a.W);
+        TN_TRY(cub_run(tmp, [&](void *t, size_t &bytes) {
+            return cub::DeviceRadixSort::SortPairs(t, bytes, a.keys, a.keys + n, a.vals, a.vals + n, (int)n, 0, end_bit, s);
+        }));
         k_bg_texels<<<(a.H * a.W + 255) / 256, 256, 0, s>>>(a, a.keys + n, a.vals + n);
     }
     TN_CUDA(cudaGetLastError());

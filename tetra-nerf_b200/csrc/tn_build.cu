@@ -12,6 +12,7 @@
 #include <vector>
 
 #include "tn_common.cuh"
+#include "tn_sort.cuh"
 
 namespace tn {
 
@@ -289,10 +290,9 @@ int build_mesh(tn_tracer *h, const float *d_xyz, uint32_t V, const uint32_t *d_c
     TN_CUDA(cudaMemcpyAsync(bounds.p, hb_enc, sizeof(hb_enc), cudaMemcpyHostToDevice, s));
     k_bounds<<<std::min<uint32_t>((V + 255) / 256, 1184u), 256, 0, s>>>(d_xyz, V, bounds.p);
     k_morton<<<(T + 255) / 256, 256, 0, s>>>(d_xyz, (const uint4 *)d_cells, T, bounds.p, keys.p, vals.p);
-    size_t tmp_bytes = 0;
-    TN_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, keys.p, keys2.p, vals.p, m.leaf_tet.p, (int)T, 0, 30, s));
-    TN_TRY(tmp.grow(tmp_bytes));
-    TN_CUDA(cub::DeviceRadixSort::SortPairs(tmp.p, tmp_bytes, keys.p, keys2.p, vals.p, m.leaf_tet.p, (int)T, 0, 30, s));
+    TN_TRY(cub_run(tmp, [&](void *t, size_t &bytes) {
+        return cub::DeviceRadixSort::SortPairs(t, bytes, keys.p, keys2.p, vals.p, m.leaf_tet.p, (int)T, 0, 30, s);
+    }));
     k_leaves<<<(T + 255) / 256, 256, 0, s>>>(d_xyz, (const uint4 *)d_cells, d_tet_faces, m.leaf_tet.p, T, m.leaves.p, m.nodes.p);
     for (int l = 1; l < L; ++l) {
         const uint32_t np = lv.count[l], nc = lv.count[l - 1];
@@ -321,7 +321,9 @@ int build_mesh(tn_tracer *h, const float *d_xyz, uint32_t V, const uint32_t *d_c
         TN_TRY(m.hull_leaves.grow(H));
         TN_TRY(m.hull_tet.grow(H));
         k_morton_subset<<<(H + 255) / 256, 256, 0, s>>>(d_xyz, (const uint4 *)d_cells, d_hull_list, H, bounds.p, keys.p, vals.p);
-        TN_CUDA(cub::DeviceRadixSort::SortPairs(tmp.p, tmp_bytes, keys.p, keys2.p, vals.p, m.hull_tet.p, (int)H, 0, 30, s));
+        TN_TRY(cub_run(tmp, [&](void *t, size_t &bytes) {
+            return cub::DeviceRadixSort::SortPairs(t, bytes, keys.p, keys2.p, vals.p, m.hull_tet.p, (int)H, 0, 30, s);
+        }));
         k_leaves<<<(H + 255) / 256, 256, 0, s>>>(d_xyz, (const uint4 *)d_cells, d_tet_faces, m.hull_tet.p, H, m.hull_leaves.p, m.hull_nodes.p);
         for (int l = 1; l < HL; ++l) {
             const uint32_t np = hlv.count[l], nc = hlv.count[l - 1];

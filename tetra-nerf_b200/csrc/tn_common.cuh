@@ -292,14 +292,11 @@ struct BackgroundGradsLaunch {
     const float *s;                       // [R,3] grad_rgb (1 - accumulation) per ray (grad_rgb on empty rays)
     bool det;                             // deterministic mode: a stable sort by texel and per-texel sums in ray order
     uint32_t *keys, *vals;                // deterministic mode: [2][4R] sort buffers
-    uint8_t *cub_tmp;                     // deterministic mode: sort temporary storage, cub_bytes of it
-    size_t cub_bytes;
     float *grad_map;                      // out: [H,W,3], or nullptr
     float *grad_d;                        // in / out: [R,3] += (d bg / d d)^T s, or nullptr
 };
-int launch_background_grads(const BackgroundGradsLaunch &a, cudaStream_t s);
-// CUB temporary bytes of the deterministic sort of launch_background_grads
-int background_sort_bytes(uint32_t R, uint32_t H, uint32_t W, size_t *bytes);
+// tmp: the temporary storage of the deterministic mode's sort, grown as it needs
+int launch_background_grads(const BackgroundGradsLaunch &a, DevArray<uint8_t> &tmp, cudaStream_t s);
 int launch_walk(tn_tracer *h, const float *o, const float *d, uint32_t R, uint32_t M, uint32_t *num, uint32_t *cells, float *bary,
                 float *dist, uint32_t *verts, unsigned long long *keys, uint32_t *list, uint32_t *list_count, int kind, cudaStream_t s);
 int launch_tail_fill(tn_tracer *h, uint32_t R, uint32_t M, const uint32_t *num, uint32_t *cells, float *bary, float *dist, uint32_t *verts,

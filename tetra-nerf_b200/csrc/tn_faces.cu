@@ -15,6 +15,7 @@
 
 #include "tn_common.cuh"
 #include "tn_predicates.cuh"
+#include "tn_sort.cuh"
 
 namespace tn {
 
@@ -185,20 +186,22 @@ int build_faces_device(const float *d_xyz, uint32_t V, const uint32_t *d_cells, 
     TN_TRY(flag.grow(n)); TN_TRY(fid.grow(n));
     TN_TRY(d_small.grow(4));  // [0] err, [1] selected count, [2] hull faces, [3] folded faces
     TN_CUDA(cudaMemsetAsync(d_small.p, 0, 16, s));
-    // temporary storage: the largest request of the CUB calls below
-    size_t tb = 0, t1 = 0;
-    TN_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, t1, key_c.p, key_c2.p, val.p, val2.p, (int)n, 0, 32, s)); tb = std::max(tb, t1);
-    TN_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, t1, kab.p, kab2.p, val2.p, val.p, (int)n, 0, 64, s)); tb = std::max(tb, t1);
-    TN_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, t1, flag.p, fid.p, (int)n, s)); tb = std::max(tb, t1);
-    TN_CUDA(cub::DeviceSelect::Flagged(nullptr, t1, key_c.p, (uint8_t *)nullptr, key_c2.p, d_small.p + 1, (int)n, s)); tb = std::max(tb, t1);
-    TN_TRY(tmp.grow(tb));
-
+    // val: slots grouped by face, slot order inside.  The largest CUB request of the build: the scratch is sized for it up front, so the
+    // calls below run without freeing and reallocating it in between
+    auto sort_faces = [&](void *t, size_t &bytes) {
+        return cub::DeviceRadixSort::SortPairs(t, bytes, kab.p, kab2.p, val2.p, val.p, (int)n, 0, 64, s);
+    };
+    size_t largest = 0;
+    TN_CUDA(sort_faces(nullptr, largest));
+    TN_TRY(tmp.grow(largest));
     k_face_slots<<<nb, 256, 0, s>>>(d_cells, n, V, key_c.p, val.p, d_small.p);
-    TN_CUDA(cub::DeviceRadixSort::SortPairs(tmp.p, tb, key_c.p, key_c2.p, val.p, val2.p, (int)n, 0, 32, s));
+    TN_TRY(cub_run(tmp, [&](void *t, size_t &bytes) {
+        return cub::DeviceRadixSort::SortPairs(t, bytes, key_c.p, key_c2.p, val.p, val2.p, (int)n, 0, 32, s);
+    }));
     k_face_keys2<<<nb, 256, 0, s>>>(d_cells, val2.p, n, kab.p);
-    TN_CUDA(cub::DeviceRadixSort::SortPairs(tmp.p, tb, kab.p, kab2.p, val2.p, val.p, (int)n, 0, 64, s));  // val: slots grouped by face, slot order inside
+    TN_TRY(cub_run(tmp, sort_faces));
     k_face_heads<<<nb, 256, 0, s>>>(d_cells, val.p, n, flag.p, d_small.p);
-    TN_CUDA(cub::DeviceScan::ExclusiveSum(tmp.p, tb, flag.p, fid.p, (int)n, s));
+    TN_TRY(cub_run(tmp, [&](void *t, size_t &bytes) { return cub::DeviceScan::ExclusiveSum(t, bytes, flag.p, fid.p, (int)n, s); }));
     uint32_t h_small[4] = {0, 0, 0, 0}, last[2] = {0, 0};
     TN_CUDA(cudaMemcpyAsync(h_small, d_small.p, 4, cudaMemcpyDeviceToHost, s));
     TN_CUDA(cudaMemcpyAsync(&last[0], flag.p + (n - 1), 4, cudaMemcpyDeviceToHost, s));
@@ -220,13 +223,17 @@ int build_faces_device(const float *d_xyz, uint32_t V, const uint32_t *d_cells, 
     k_iota<<<(std::max(T, F) + 255) / 256, 256, 0, s>>>(iota.p, std::max(T, F));
     // tetrahedra owning a hull face, in tetrahedron order
     TN_TRY(out.hull_list.grow(T));
-    TN_CUDA(cub::DeviceSelect::Flagged(tmp.p, tb, iota.p, bflag.p, out.hull_list.p, d_small.p + 1, (int)T, s));
+    TN_TRY(cub_run(tmp, [&](void *t, size_t &bytes) {
+        return cub::DeviceSelect::Flagged(t, bytes, iota.p, bflag.p, out.hull_list.p, d_small.p + 1, (int)T, s);
+    }));
     uint32_t H = 0, Hf = 0;
     TN_CUDA(cudaMemcpyAsync(&H, d_small.p + 1, 4, cudaMemcpyDeviceToHost, s));
     // hull faces -> edges -> sorted -> pair checks
     k_hull_face_flags<<<(F + 255) / 256, 256, 0, s>>>(out.tt.p, F, bflag.p);
     TN_TRY(hull_faces.grow(F));
-    TN_CUDA(cub::DeviceSelect::Flagged(tmp.p, tb, iota.p, bflag.p, hull_faces.p, d_small.p + 2, (int)F, s));
+    TN_TRY(cub_run(tmp, [&](void *t, size_t &bytes) {
+        return cub::DeviceSelect::Flagged(t, bytes, iota.p, bflag.p, hull_faces.p, d_small.p + 2, (int)F, s);
+    }));
     TN_CUDA(cudaMemcpyAsync(&Hf, d_small.p + 2, 4, cudaMemcpyDeviceToHost, s));
     TN_CUDA(cudaStreamSynchronize(s));
     out.H = H;
@@ -235,7 +242,9 @@ int build_faces_device(const float *d_xyz, uint32_t V, const uint32_t *d_cells, 
         const uint32_t ne = 3 * Hf;
         TN_TRY(eface.grow(ne)); TN_TRY(eface2.grow(ne));
         k_hull_edges<<<(ne + 255) / 256, 256, 0, s>>>(out.tri.p, hull_faces.p, Hf, kab.p, eface.p);
-        TN_CUDA(cub::DeviceRadixSort::SortPairs(tmp.p, tb, kab.p, kab2.p, eface.p, eface2.p, (int)ne, 0, 64, s));
+        TN_TRY(cub_run(tmp, [&](void *t, size_t &bytes) {
+            return cub::DeviceRadixSort::SortPairs(t, bytes, kab.p, kab2.p, eface.p, eface2.p, (int)ne, 0, 64, s);
+        }));
         k_hull_check<<<(ne + 255) / 256, 256, 0, s>>>(d_xyz, (const uint4 *)d_cells, out.tri.p, out.tt.p, kab2.p, eface2.p, ne, d_small.p);
         // the refit's fold test on the load's tables: the walk sees only the chain of tetrahedra from the hull entry, and on a folded mesh
         // a line also crosses faces off that chain (DESIGN §4.9), so a mesh with an uncertified face loads with the walk off

@@ -10,6 +10,7 @@
 #include <cub/cub.cuh>
 
 #include "tn_common.cuh"
+#include "tn_sort.cuh"
 
 namespace tn {
 
@@ -298,17 +299,12 @@ __global__ void k_ivb_keys(uint32_t n, uint32_t V, const uint32_t *__restrict__ 
     keys[e] = v < V ? v : V;  // empty slots (E) sort behind every vertex
     vals[e] = e;
 }
-__device__ __forceinline__ uint32_t lower_bound_keys(const uint32_t *__restrict__ a, uint32_t n, uint32_t x) {
-    uint32_t lo = 0, hi = n;
-    while (lo < hi) { const uint32_t mid = (lo + hi) >> 1; if (__ldg(a + mid) < x) lo = mid + 1; else hi = mid; }
-    return lo;
-}
 template <int D>
 __global__ void __launch_bounds__(256) k_ivb_det(uint32_t V, uint32_t C, uint32_t n, const uint32_t *__restrict__ keys, const uint32_t *__restrict__ vals,
                                                  const float *__restrict__ w, const float *__restrict__ gin, float *__restrict__ grow) {
     const uint32_t v = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31u;
     if (v >= V) return;
-    const uint32_t lo = lower_bound_keys(keys, n, v), hi = lower_bound_keys(keys, n, v + 1);
+    const uint32_t lo = lower_bound_u32(keys, n, v), hi = lower_bound_u32(keys, n, v + 1);
     for (uint32_t c0 = 0; c0 < C; c0 += 32) {
         const uint32_t c = c0 + lane;
         float acc = 0.f;
@@ -420,11 +416,14 @@ extern "C" int tn_interpolate_values_backward_deterministic(int device, uint32_t
     tn::DeviceGuard g(device);
     cudaStream_t s = (cudaStream_t)stream;
     const uint32_t n = (uint32_t)n64;
-    const int end_bit = 32 - __builtin_clz(V | 1u);  // keys are <= V
+    const int end_bit = tn::radix_end_bit(V);  // keys are <= V
     auto al = [](size_t b) { return (b + 255) & ~(size_t)255; };
+    // the sort, written once: with null buffers for the workspace size, with the workspace's buffers in the run
+    auto sort = [&](void *t, size_t &bytes, const uint32_t *k0, uint32_t *k1, const uint32_t *v0, uint32_t *v1) {
+        return cub::DeviceRadixSort::SortPairs(t, bytes, k0, k1, v0, v1, (int)n, 0, end_bit, s);
+    };
     size_t cub_bytes = 0;
-    TN_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, cub_bytes, (const uint32_t *)nullptr, (uint32_t *)nullptr, (const uint32_t *)nullptr,
-                                            (uint32_t *)nullptr, (int)n, 0, end_bit, s));
+    TN_CUDA(sort(nullptr, cub_bytes, nullptr, nullptr, nullptr, nullptr));
     const size_t kb = al(sizeof(uint32_t) * (size_t)n), sb = al(sizeof(float) * (size_t)V * C);
     const size_t need = 4 * kb + sb + al(cub_bytes);
     if (!d_workspace) { *workspace_bytes = need; return TN_OK; }
@@ -439,7 +438,7 @@ extern "C" int tn_interpolate_values_backward_deterministic(int device, uint32_t
     float *grow = (float *)(ws + 4 * kb);
     void *tmp = ws + 4 * kb + sb;
     tn::k_ivb_keys<<<(n + 255) / 256, 256, 0, s>>>(n, V, d_vi, k0, v0);
-    TN_CUDA(cub::DeviceRadixSort::SortPairs(tmp, cub_bytes, k0, k1, v0, v1, (int)n, 0, end_bit, s));
+    TN_CUDA(sort(tmp, cub_bytes, k0, k1, v0, v1));
     const uint32_t blocks = (uint32_t)(((uint64_t)V * 32 + 255) / 256);
     switch (D) {
         case 2: tn::k_ivb_det<2><<<blocks, 256, 0, s>>>(V, C, n, k1, v1, d_w, d_grad_in, grow); break;

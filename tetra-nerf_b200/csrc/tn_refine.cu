@@ -154,14 +154,23 @@ extern "C" int tn_refine_edges(int device, const float *d_xyz, uint32_t V, const
     cudaStream_t s = (cudaStream_t)stream;
     auto al = [](size_t b) { return (b + 255) & ~(size_t)255; };
     const int n = (int)T;
+    // every CUB algorithm of the pass, written once: with null buffers and all T items for the workspace size, with the workspace's
+    // buffers in the runs
+    using u64 = unsigned long long;
+    auto sort_keys = [&](void *t, size_t &bytes, const u64 *in, u64 *out) { return cub::DeviceRadixSort::SortKeys(t, bytes, in, out, n, 0, 64, s); };
+    auto unique = [&](void *t, size_t &bytes, u64 *in, u64 *out, uint32_t *count) { return cub::DeviceSelect::Unique(t, bytes, in, out, count, n, s); };
+    auto scan = [&](void *t, size_t &bytes, uint32_t *in, uint32_t *out, int m) { return cub::DeviceScan::ExclusiveSum(t, bytes, in, out, m, s); };
+    auto sort_pairs = [&](void *t, size_t &bytes, const u64 *kin, u64 *kout, const uint32_t *vin, uint32_t *vout, int m) {
+        return cub::DeviceRadixSort::SortPairs(t, bytes, kin, kout, vin, vout, m, 0, 64, s);
+    };
+    auto sum = [&](void *t, size_t &bytes, uint32_t *in, uint32_t *out, int m) { return cub::DeviceReduce::Sum(t, bytes, in, out, m, s); };
     size_t c0 = 0, c1 = 0, c2 = 0, c3 = 0, c4 = 0;
-    TN_CUDA(cub::DeviceRadixSort::SortKeys(nullptr, c0, (const unsigned long long *)nullptr, (unsigned long long *)nullptr, n, 0, 64, s));
-    TN_CUDA(cub::DeviceSelect::Unique(nullptr, c1, (const unsigned long long *)nullptr, (unsigned long long *)nullptr, (uint32_t *)nullptr, n, s));
-    TN_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, c2, (const uint32_t *)nullptr, (uint32_t *)nullptr, n, s));
-    TN_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, c3, (const unsigned long long *)nullptr, (unsigned long long *)nullptr,
-                                            (const uint32_t *)nullptr, (uint32_t *)nullptr, n, 0, 64, s));
-    TN_CUDA(cub::DeviceReduce::Sum(nullptr, c4, (const uint32_t *)nullptr, (uint32_t *)nullptr, n, s));
-    const size_t cub_bytes = std::max(std::max(std::max(c0, c1), std::max(c2, c3)), c4);
+    TN_CUDA(sort_keys(nullptr, c0, nullptr, nullptr));
+    TN_CUDA(unique(nullptr, c1, nullptr, nullptr, nullptr));
+    TN_CUDA(scan(nullptr, c2, nullptr, nullptr, n));
+    TN_CUDA(sort_pairs(nullptr, c3, nullptr, nullptr, nullptr, nullptr, n));
+    TN_CUDA(sum(nullptr, c4, nullptr, nullptr, n));
+    size_t cub_bytes = std::max(std::max(std::max(c0, c1), std::max(c2, c3)), c4);
     const size_t kb = al(sizeof(unsigned long long) * (size_t)T), ub = al(sizeof(uint32_t) * (size_t)T), cb = al(16 * sizeof(uint32_t));
     const size_t need = 3 * kb + 7 * ub + cb + al(cub_bytes);
     if (!d_workspace) { *workspace_bytes = need; return TN_OK; }
@@ -177,14 +186,12 @@ extern "C" int tn_refine_edges(int device, const float *d_xyz, uint32_t V, const
              *rank = (uint32_t *)((uint8_t *)u + 6 * ub);
     uint32_t *ctr = (uint32_t *)(ws + 3 * kb + 7 * ub);  // [0] flags, [1] unique count, [2] accepted count, [3] last vid, [4] last rank
     void *tmp = ws + 3 * kb + 7 * ub + cb;
-    size_t tb = cub_bytes;
     const uint32_t blocks = (T + 255) / 256;
     const double ml = (double)min_length;
     TN_CUDA(cudaMemsetAsync(ctr, 0, 16 * sizeof(uint32_t), s));
     tn::k_ref_propose<<<blocks, 256, 0, s>>>(T, V, d_xyz, (const uint4 *)d_cells, d_candidates, ml * ml, prop, ctr);
-    TN_CUDA(cub::DeviceRadixSort::SortKeys(tmp, tb, prop, sorted, n, 0, 64, s));
-    tb = cub_bytes;
-    TN_CUDA(cub::DeviceSelect::Unique(tmp, tb, sorted, P, ctr + 1, n, s));
+    TN_CUDA(sort_keys(tmp, cub_bytes, prop, sorted));
+    TN_CUDA(unique(tmp, cub_bytes, sorted, P, ctr + 1));
     uint32_t h[2];
     TN_CUDA(cudaMemcpyAsync(h, ctr, 2 * sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
     unsigned long long last = 0;
@@ -204,24 +211,20 @@ extern "C" int tn_refine_edges(int device, const float *d_xyz, uint32_t V, const
     tn::k_ref_vote<<<blocks, 256, 0, s>>>(T, d_xyz, (const uint4 *)d_cells, P, ctr + 1, incident, votes, voted);
     const uint32_t pblocks = (nP + 255) / 256;
     tn::k_ref_accept<<<pblocks, 256, 0, s>>>(nP, d_xyz, P, incident, votes, accepted, prop, vid);
-    tb = cub_bytes;
-    TN_CUDA(cub::DeviceReduce::Sum(tmp, tb, accepted, ctr + 2, (int)nP, s));
+    TN_CUDA(sum(tmp, cub_bytes, accepted, ctr + 2, (int)nP));
     uint32_t nacc = 0;
     TN_CUDA(cudaMemcpyAsync(&nacc, ctr + 2, sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
     TN_CUDA(cudaStreamSynchronize(s));
     if (nacc > max_new_vertices) {  // keep the highest-priority ones
-        tb = cub_bytes;
-        TN_CUDA(cub::DeviceRadixSort::SortPairs(tmp, tb, prop, sorted, vid, rank, (int)nP, 0, 64, s));
+        TN_CUDA(sort_pairs(tmp, cub_bytes, prop, sorted, vid, rank, (int)nP));
         tn::k_ref_cap<<<pblocks, 256, 0, s>>>(nP, max_new_vertices, rank, accepted);
         nacc = max_new_vertices;
     }
     counts3[1] = nacc;
-    tb = cub_bytes;
-    TN_CUDA(cub::DeviceScan::ExclusiveSum(tmp, tb, accepted, vid, (int)nP, s));
+    TN_CUDA(scan(tmp, cub_bytes, accepted, vid, (int)nP));
     tn::k_ref_edges<<<pblocks, 256, 0, s>>>(nP, P, accepted, vid, (uint2 *)d_parent_edge);
     tn::k_ref_split_flags<<<blocks, 256, 0, s>>>(T, voted, accepted, split);
-    tb = cub_bytes;
-    TN_CUDA(cub::DeviceScan::ExclusiveSum(tmp, tb, split, rank, n, s));
+    TN_CUDA(scan(tmp, cub_bytes, split, rank, n));
     tn::k_ref_write<<<blocks, 256, 0, s>>>(T, V, (const uint4 *)d_cells, P, voted, split, rank, vid, (uint4 *)d_cells_out, d_parent_cell);
     TN_CUDA(cudaGetLastError());
     uint32_t hs[2];

@@ -24,6 +24,7 @@
 #include "tn_mlp.cuh"
 #include "tn_mlp_bwd.cuh"
 #include "tn_mlp_pack.cuh"
+#include "tn_sort.cuh"
 
 namespace tn {
 
@@ -909,11 +910,6 @@ __global__ void __launch_bounds__(256) k_det_sum_slots(const uint32_t *__restric
     }
     if (t == 0) { out[0] = s[0].x; out[1] = s[0].y; out[2] = s[0].z; out[3] = s[0].w; }
 }
-__device__ __forceinline__ uint32_t lower_bound_u32(const uint32_t *__restrict__ a, uint32_t n, uint32_t x) {
-    uint32_t lo = 0, hi = n;
-    while (lo < hi) { const uint32_t mid = (lo + hi) >> 1; if (__ldg(a + mid) < x) lo = mid + 1; else hi = mid; }
-    return lo;
-}
 // per-ray direction-bias gradient: the partial rows of the 16-row warp blocks b that hold the ray's samples, in block order
 // (k_mlp_bwd<true> wrote block b = 4 tile + warp's partial for ray `slot` to row 4 (tile + slot) + warp).  rowmap != nullptr: the
 // ray's rows are its compact rows, found by binary search of the ascending map (none: a zero gradient)
@@ -1048,12 +1044,11 @@ static int compact_rows(tn_tracer *h, RenderState *r, const uint32_t *n_active, 
                         DevArray<uint32_t> &map, uint32_t *n_rows, cudaStream_t s) {
     const size_t n = R * S;
     TN_TRY(r->live_flag.grow(n)); TN_TRY(map.grow(n));
-    size_t bytes = 0;
-    cub::CountingInputIterator<uint32_t> it(0u);
-    TN_CUDA(cub::DeviceSelect::Flagged(nullptr, bytes, it, r->live_flag.p, map.p, n_rows, (int64_t)n, s));
-    TN_TRY(r->cub_tmp.grow(bytes));
     k_live_rows<<<(uint32_t)((n + 255) / 256), 256, 0, s>>>(n_active, S, n, vi, outw, r->live_flag.p, out);
-    TN_CUDA(cub::DeviceSelect::Flagged(r->cub_tmp.p, bytes, it, r->live_flag.p, map.p, n_rows, (int64_t)n, s));
+    cub::CountingInputIterator<uint32_t> it(0u);
+    TN_TRY(cub_run(r->cub_tmp, [&](void *t, size_t &bytes) {
+        return cub::DeviceSelect::Flagged(t, bytes, it, r->live_flag.p, map.p, n_rows, (int64_t)n, s);
+    }));
     h->launches += 2;
     return TN_OK;
 }
@@ -1107,11 +1102,10 @@ static int ensure_train_ws(RenderState *r, size_t R, size_t S2, uint32_t V) {
 // deterministic mode, forward: slot of every ray = number of rays with hits before it (exclusive scan)
 static int ordered_slots(RenderState *r, uint32_t R, cudaStream_t s) {
     TN_TRY(r->ray_flag.grow(R)); TN_TRY(r->ray_slot.grow(R));
-    size_t bytes = 0;
-    TN_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, bytes, r->ray_flag.p, r->ray_slot.p, (int)R, s));
-    TN_TRY(r->cub_tmp.grow(bytes));
     k_ray_flags<<<(R + 255) / 256, 256, 0, s>>>(R, r->num.p, r->ray_flag.p);
-    TN_CUDA(cub::DeviceScan::ExclusiveSum(r->cub_tmp.p, bytes, r->ray_flag.p, r->ray_slot.p, (int)R, s));
+    TN_TRY(cub_run(r->cub_tmp, [&](void *t, size_t &bytes) {
+        return cub::DeviceScan::ExclusiveSum(t, bytes, r->ray_flag.p, r->ray_slot.p, (int)R, s);
+    }));
     return TN_OK;
 }
 
@@ -1518,13 +1512,12 @@ static int train_backward_impl(tn_tracer *h, const TrainBufs &b, const SavedHead
         k_det_reduce_dbg<<<(DBG_PART + 255) / 256, 256, 0, s>>>(b.n_active, r->det_dbg.p, r->gw.p);
         // field gradient: stable sort of (vertex, row * 4 + k) by vertex, then per-vertex sums in row order
         const uint32_t n = (uint32_t)(4 * (uint64_t)R * S2);
-        const int end_bit = 32 - __builtin_clz(V | 1u);  // keys are <= V
+        const int end_bit = radix_end_bit(V);  // keys are <= V
         uint32_t *k0 = r->det_keys.p, *k1 = r->det_keys.p + n, *v0 = r->det_vals.p, *v1 = r->det_vals.p + n;
-        size_t bytes = 0;
-        TN_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, bytes, k0, k1, v0, v1, (int)n, 0, end_bit, s));
-        TN_TRY(r->cub_tmp.grow(bytes));
         k_det_field_keys<<<(n + 255) / 256, 256, 0, s>>>(b.n_active, S2, n, V, b.vi_f, k0, v0);
-        TN_CUDA(cub::DeviceRadixSort::SortPairs(r->cub_tmp.p, bytes, k0, k1, v0, v1, (int)n, 0, end_bit, s));
+        TN_TRY(cub_run(r->cub_tmp, [&](void *t, size_t &bytes) {
+            return cub::DeviceRadixSort::SortPairs(t, bytes, k0, k1, v0, v1, (int)n, 0, end_bit, s);
+        }));
         k_det_field_grad<<<(uint32_t)(((uint64_t)V * 32 + 255) / 256), 256, 0, s>>>(V, n, k1, v1, b.bary_f, r->det_dx.p, r->gshadow.p);
         h->launches += 9;
     }
@@ -1559,11 +1552,9 @@ static int train_backward_impl(tn_tracer *h, const TrainBufs &b, const SavedHead
         bl.grad_map = d_grad_bg; bl.grad_d = d_grad_d;
         if (det && d_grad_bg != nullptr) {
             TN_TRY(r->bg_keys.grow(8 * (size_t)R)); TN_TRY(r->bg_vals.grow(8 * (size_t)R));
-            TN_TRY(background_sort_bytes(R, hd.bg_H, hd.bg_W, &bl.cub_bytes));
-            TN_TRY(r->cub_tmp.grow(bl.cub_bytes));
-            bl.keys = r->bg_keys.p; bl.vals = r->bg_vals.p; bl.cub_tmp = r->cub_tmp.p;
+            bl.keys = r->bg_keys.p; bl.vals = r->bg_vals.p;
         }
-        TN_TRY(launch_background_grads(bl, s));
+        TN_TRY(launch_background_grads(bl, r->cub_tmp, s));
         h->launches += det && d_grad_bg != nullptr ? 3 : 1;
     }
     k_scatter_grads<<<(128 * 155 + 255) / 256, 256, 0, s>>>(r->gw.p, go);

@@ -10,6 +10,7 @@
 
 #include "tn_common.cuh"
 #include "tn_edges.cuh"
+#include "tn_sort.cuh"
 
 namespace tn {
 
@@ -127,17 +128,14 @@ static int build_adjacency(tn_tracer *h, cudaStream_t s) {
     TN_TRY(b.grow(n));
     TN_TRY(ctr.grow(2));
     cub::DoubleBuffer<unsigned long long> keys(a.p, b.p);
-    size_t c0 = 0, c1 = 0;
-    TN_CUDA(cub::DeviceRadixSort::SortKeys(nullptr, c0, keys, (int)n, 0, 64, s));
-    TN_CUDA(cub::DeviceSelect::Unique(nullptr, c1, (const unsigned long long *)nullptr, (unsigned long long *)nullptr, (uint32_t *)nullptr,
-                                      (int)n, s));
-    TN_TRY(tmp.grow(std::max(c0, c1)));
     TN_CUDA(cudaMemsetAsync(ctr.p, 0, 2 * sizeof(uint32_t), s));
     if (T > 0) {
         k_adj_pairs<<<(T + 255) / 256, 256, 0, s>>>(T, V, (const uint4 *)h->mesh.cells, a.p, ctr.p);
         h->launches += 1;
-        TN_CUDA(cub::DeviceRadixSort::SortKeys(tmp.p, c0, keys, (int)n, 0, 64, s));
-        TN_CUDA(cub::DeviceSelect::Unique(tmp.p, c1, keys.Current(), keys.Alternate(), ctr.p + 1, (int)n, s));
+        TN_TRY(cub_run(tmp, [&](void *t, size_t &bytes) { return cub::DeviceRadixSort::SortKeys(t, bytes, keys, (int)n, 0, 64, s); }));
+        TN_TRY(cub_run(tmp, [&](void *t, size_t &bytes) {
+            return cub::DeviceSelect::Unique(t, bytes, keys.Current(), keys.Alternate(), ctr.p + 1, (int)n, s);
+        }));
     }
     uint32_t hc[2];
     TN_CUDA(cudaMemcpyAsync(hc, ctr.p, sizeof(hc), cudaMemcpyDeviceToHost, s));

@@ -17,6 +17,7 @@
 #include "tn_common.cuh"
 #include "tn_direnc.cuh"
 #include "tn_mlp.cuh"
+#include "tn_sort.cuh"
 
 namespace tn {
 
@@ -230,12 +231,6 @@ __global__ void k_face_normals(uint32_t F, const uint32_t *__restrict__ faces, c
     for (int k = 0; k < 3; ++k) { keys[3 * (size_t)f + k] = faces[3 * (size_t)f + k]; vals[3 * (size_t)f + k] = f; }
 }
 
-__device__ __forceinline__ uint32_t lower_bound_keys(const uint32_t *__restrict__ a, uint32_t n, uint32_t x) {
-    uint32_t lo = 0, hi = n;
-    while (lo < hi) { const uint32_t mid = (lo + hi) >> 1; if (__ldg(a + mid) < x) lo = mid + 1; else hi = mid; }
-    return lo;
-}
-
 // one warp per vertex: lane 0 sums the normals of the vertex's faces in face order (the stable sort kept it), the warp then forms the
 // direction bias of the colour pass, b4 + W4[:, :27] enc(-n), as k_sample_fine does per ray
 __global__ void __launch_bounds__(256) k_vertex_normals(uint32_t N, uint32_t n, const uint32_t *__restrict__ keys, const uint32_t *__restrict__ vals,
@@ -245,7 +240,7 @@ __global__ void __launch_bounds__(256) k_vertex_normals(uint32_t N, uint32_t n, 
     if (v >= N) return;
     float nx = 0.f, ny = 0.f, nz = 0.f;
     if (lane == 0) {
-        const uint32_t lo = lower_bound_keys(keys, n, v), hi = lower_bound_keys(keys, n, v + 1);
+        const uint32_t lo = lower_bound_u32(keys, n, v), hi = lower_bound_u32(keys, n, v + 1);
         for (uint32_t q = lo; q < hi; ++q) {
             const float *fn = fnrm + 3 * (size_t)__ldg(vals + q);
             nx += fn[0]; ny += fn[1]; nz += fn[2];
@@ -296,8 +291,6 @@ int run_mlp(tn_tracer *h, const RenderInputs &in, const uint32_t *d_count, uint6
 }
 
 uint32_t blocks(uint64_t n, uint32_t per) { return (uint32_t)((n + per - 1) / per); }
-
-int bits_for(uint64_t x) { int b = 1; while (b < 64 && (x >> b) != 0) ++b; return b; }
 }  // namespace
 
 extern "C" int tn_surface_extract(tn_tracer *h, float level, uint32_t *n_vertices, uint32_t *n_faces, void *stream) {
@@ -329,10 +322,7 @@ extern "C" int tn_surface_extract(tn_tracer *h, float level, uint32_t *n_vertice
     TN_TRY(S.tcnt.grow((size_t)T + 1)); TN_TRY(S.toff.grow((size_t)T + 1));
     unsigned long long *tcnt = S.tcnt.p, *toff = S.toff.p;
     k_tet_case<<<blocks((uint64_t)T + 1, 256), 256, 0, s>>>(T, h->mesh.cells, vsig, level, tcnt);
-    size_t bytes = 0;
-    TN_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, bytes, tcnt, toff, (int64_t)T + 1, s));
-    TN_TRY(S.cub.grow(bytes));
-    TN_CUDA(cub::DeviceScan::ExclusiveSum(S.cub.p, bytes, tcnt, toff, (int64_t)T + 1, s));
+    TN_TRY(cub_run(S.cub, [&](void *t, size_t &bytes) { return cub::DeviceScan::ExclusiveSum(t, bytes, tcnt, toff, (int64_t)T + 1, s); }));
     h->launches += 2;
     unsigned long long total = 0;
     TN_CUDA(cudaMemcpyAsync(&total, toff + T, sizeof(total), cudaMemcpyDeviceToHost, s));
@@ -347,13 +337,11 @@ extern "C" int tn_surface_extract(tn_tracer *h, float level, uint32_t *n_vertice
     TN_TRY(S.keys.grow(nslots)); TN_TRY(S.skeys.grow(nslots));
     unsigned long long *keys = S.keys.p, *skeys = S.skeys.p;
     k_tet_edges<<<blocks(T, 256), 256, 0, s>>>(T, V, h->mesh.cells, vsig, level, toff, keys);
-    const int end_bit = bits_for((uint64_t)V * V);
-    TN_CUDA(cub::DeviceRadixSort::SortKeys(nullptr, bytes, keys, skeys, (int64_t)nslots, 0, end_bit, s));
-    TN_TRY(S.cub.grow(bytes));
-    TN_CUDA(cub::DeviceRadixSort::SortKeys(S.cub.p, bytes, keys, skeys, (int64_t)nslots, 0, end_bit, s));
-    TN_CUDA(cub::DeviceSelect::Unique(nullptr, bytes, skeys, keys, d_E, (int64_t)nslots, s));
-    TN_TRY(S.cub.grow(bytes));
-    TN_CUDA(cub::DeviceSelect::Unique(S.cub.p, bytes, skeys, keys, d_E, (int64_t)nslots, s));
+    const int end_bit = radix_end_bit((uint64_t)V * V);
+    TN_TRY(cub_run(S.cub, [&](void *t, size_t &bytes) {
+        return cub::DeviceRadixSort::SortKeys(t, bytes, keys, skeys, (int64_t)nslots, 0, end_bit, s);
+    }));
+    TN_TRY(cub_run(S.cub, [&](void *t, size_t &bytes) { return cub::DeviceSelect::Unique(t, bytes, skeys, keys, d_E, (int64_t)nslots, s); }));
     h->launches += 3;
     uint32_t E = 0;
     TN_CUDA(cudaMemcpyAsync(&E, d_E, sizeof(E), cudaMemcpyDeviceToHost, s));
@@ -382,10 +370,10 @@ extern "C" int tn_surface_extract(tn_tracer *h, float level, uint32_t *n_vertice
     TN_TRY(S.nrm.grow(3 * (size_t)E)); TN_TRY(S.dirbias.grow(128 * (size_t)E));
     uint32_t *nk0 = S.nk0.p, *nk1 = S.nk1.p, *nv0 = S.nv0.p, *nv1 = S.nv1.p;
     k_face_normals<<<blocks(F, 256), 256, 0, s>>>((uint32_t)F, S.faces.p, pos, S.fnrm.p, nk0, nv0);
-    const int vbits = bits_for(E);
-    TN_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, bytes, nk0, nk1, nv0, nv1, (int64_t)n3, 0, vbits, s));
-    TN_TRY(S.cub.grow(bytes));
-    TN_CUDA(cub::DeviceRadixSort::SortPairs(S.cub.p, bytes, nk0, nk1, nv0, nv1, (int64_t)n3, 0, vbits, s));
+    const int vbits = radix_end_bit(E);
+    TN_TRY(cub_run(S.cub, [&](void *t, size_t &bytes) {
+        return cub::DeviceRadixSort::SortPairs(t, bytes, nk0, nk1, nv0, nv1, (int64_t)n3, 0, vbits, s);
+    }));
     k_vertex_normals<<<blocks((uint64_t)E * 32, 256), 256, 0, s>>>(E, (uint32_t)n3, nk1, nv1, S.fnrm.p, in.w4dir, S.nrm.p, S.dirbias.p);
     h->launches += 3;
     // ---- colours: the colour head at the vertex's features, seen along -n ----

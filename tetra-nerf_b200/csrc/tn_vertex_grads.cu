@@ -9,6 +9,7 @@
 // k_det_vertex_grads (deterministic mode): one warp per vertex over the (vertex, row * 4 + k) pairs that the field gradient already sorted
 // stably by vertex; lane l sums entries l, l + 32, ... in float64, a fixed butterfly combines the lanes: the result is bitwise reproducible.
 #include "tn_common.cuh"
+#include "tn_sort.cuh"
 
 namespace tn {
 
@@ -36,16 +37,10 @@ __global__ void __launch_bounds__(256) k_vertex_grads(const VertexGradsLaunch p)
     }
 }
 
-__device__ __forceinline__ uint32_t lower_bound_keys(const uint32_t *__restrict__ a, uint32_t n, uint32_t x) {
-    uint32_t lo = 0, hi = n;
-    while (lo < hi) { const uint32_t mid = (lo + hi) >> 1; if (__ldg(a + mid) < x) lo = mid + 1; else hi = mid; }
-    return lo;
-}
-
 __global__ void __launch_bounds__(256) k_det_vertex_grads(const VertexGradsLaunch p) {
     const uint32_t v = (uint32_t)(((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5), lane = threadIdx.x & 31u;
     if (v >= p.V) return;
-    const uint32_t lo = lower_bound_keys(p.keys, p.n, v), hi = lower_bound_keys(p.keys, p.n, v + 1);
+    const uint32_t lo = lower_bound_u32(p.keys, p.n, v), hi = lower_bound_u32(p.keys, p.n, v + 1);
     double a[3] = {0.0, 0.0, 0.0};
     for (uint32_t i = lo + lane; i < hi; i += 32) {
         const uint32_t e = __ldg(p.vals + i);
