@@ -145,6 +145,28 @@ int tn_refine_edges(int device, const float *d_xyz, uint32_t V, const uint32_t *
                     float min_length, uint32_t max_new_vertices, uint32_t *d_cells_out, uint32_t *d_parent_edge, uint32_t *d_parent_cell,
                     uint32_t *counts3, void *d_workspace, size_t *workspace_bytes, void *stream);
 
+/* ---- mesh coarsening: one pass of empty-space vertex removal by edge collapse (DESIGN.md §4.18).  A pure function of device arrays (no
+ * tracer): d_xyz f32[V,3], d_cells u32[T,4], d_empty u8[T] (non-zero = the cell is empty).  The star of a vertex is the cells that hold
+ * it (a CSR built by one radix sort of the 4T (vertex, cell) pairs); a hull face is a face with one owner, matched on its exact vertices.
+ *   propose: a vertex a with a non-empty star of empty cells, none of which has a hull face through a, tries its neighbours b in
+ *            ascending ((xa-xb)^2 + (ya-yb)^2) + (za-zb)^2 (float64 from the fp32 coordinates, every operation rounded on its own, as
+ *            tn_refine_edges), ties to the smaller b; b is valid when every star cell without b, with b in a's slot, has the certified
+ *            orient3d sign (tn_predicates.cuh) the cell has now.  The first valid b is a's target; a star cell whose sign is not
+ *            certified, or no valid b, makes a propose nothing.  Priority: the smaller squared length, ties to the smaller a;
+ *   vote:    each cell votes for the highest-priority proposing vertex among its four;
+ *   accept:  a proposal is accepted iff every cell of its star voted for it (so accepted vertices share no cell, and the
+ *            highest-priority proposal is always accepted); beyond max_removed the highest-priority accepted ones are kept;
+ *   apply:   the star cells of a kept a that hold its target b are removed, the others get b in a's slot; cells and vertices are
+ *            compacted stably (survivors keep their order, vertex ids are renumbered).
+ * Outputs (capacities: d_cells_out u32[T,4], d_parent_cell u32[T], d_kept_vertex u32[V]): d_cells_out[:T'], d_kept_vertex[:V'] (the old
+ * id of each new vertex, ascending), d_parent_cell[:T'] (the old slot of each new cell, ascending).  counts3 (host) = proposals, vertices
+ * removed (V - V'), cells removed (T - T').  The output depends on the inputs only, bitwise.  TN_ERR_ARG for a vertex index >= V,
+ * T >= 2^29 or V >= 2^31.  Workspace as tn_refine_edges: d_workspace == NULL writes the size to *workspace_bytes and does nothing else.
+ * Synchronous (three small read-backs). */
+int tn_coarsen_vertices(int device, const float *d_xyz, uint32_t V, const uint32_t *d_cells, uint32_t T, const uint8_t *d_empty,
+                        uint32_t max_removed, uint32_t *d_cells_out, uint32_t *d_kept_vertex, uint32_t *d_parent_cell, uint32_t *counts3,
+                        void *d_workspace, size_t *workspace_bytes, void *stream);
+
 /* ---- field smoothness along the mesh edges (DESIGN.md §4.15).  Over the unique undirected edges of the loaded mesh (E of them; an edge
  * {i, j} joins two distinct vertices of one cell), with f the field of tn_render_set_field:
  *   S = sum_{i,j} sum_c (f[c,i] - f[c,j])^2,   loss = mult S / (E 64),   d loss / df[c,i] = mult 2 / (E 64) sum_{j in N(i)} (f[c,i] - f[c,j]).

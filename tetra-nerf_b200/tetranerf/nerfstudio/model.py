@@ -147,6 +147,20 @@ class TetrahedraNerfConfig(ModelConfig):
     """a candidate proposes its longest edge only when that is at least this long"""
     refine_max_vertices: Optional[int] = None
     """refinement stops adding vertices at this many mesh vertices (None: no limit)"""
+    coarsen_every: int = 0
+    """> 0: coarsen the mesh in empty space during training every coarsen_every steps in [coarsen_start, coarsen_stop)
+    (TetrahedraNerf.coarsen, DESIGN §4.18): a non-hull vertex whose tetrahedra all have tetrahedra_occupancy < occupancy_threshold is
+    collapsed into its nearest neighbour that keeps every tetrahedron's orientation, so empty space stops costing trace steps, samples,
+    records and memory.  The hull and the occupied tetrahedra are untouched.  0 = off, nothing changes.  Needs use_occupancy_field and
+    the fused pipeline (RuntimeError at construction otherwise).  It never runs before occupancy_warmup_steps training steps or on an
+    occupancy buffer that was never computed.  When a refinement is due on the same step, coarsening runs first"""
+    coarsen_start: int = 1000
+    """first training step at which the mesh may be coarsened"""
+    coarsen_stop: int = 15000
+    """no coarsening from this training step on"""
+    coarsen_passes: int = 3
+    """collapse passes per coarsening; a pass removes vertices that share no tetrahedron, so later passes reach the neighbours of
+    vertices an earlier pass kept"""
     background_envmap_height: int = 0
     """> 0: learn the light that leaves the mesh as an environment map: the parameter `background_envmap` f32[H, 2H, 3] (H this value;
     "fields" group, in the state dict only when enabled) in the model's frame, z up, equal-area in latitude, initialised to
@@ -424,6 +438,12 @@ class TetrahedraNerf(Model):
         self.rgb_loss = MSELoss()
         if self.config.vertex_fold_guard and not self.config.optimize_vertices:
             raise RuntimeError("vertex_fold_guard guards the steps of the vertex positions: it needs optimize_vertices=True")
+        if self.config.coarsen_every > 0:
+            if not self.config.use_occupancy_field:
+                raise RuntimeError("coarsen_every > 0 removes vertices in empty space as the occupancy field sees it: it needs use_occupancy_field=True")
+            if self._fused_unsupported():
+                raise RuntimeError(f"coarsen_every > 0 reads the occupancy field of the fused CUDA pipeline, which does not support "
+                                   f"{', '.join(self._fused_unsupported())}")
         H = self.config.background_envmap_height
         if H > 0:
             if self.config.background_color not in ("white", "black"):
@@ -658,9 +678,11 @@ class TetrahedraNerf(Model):
     # ---- mesh refinement (DESIGN §4.14) ------------------------------------------------------------------------------------------------
     def get_training_callbacks(self, training_callback_attributes: TrainingCallbackAttributes) -> List[TrainingCallback]:
         """with refine_every > 0: after every training iteration, the field-gradient statistics; every refine_every steps in
-        [refine_start, refine_stop), `refine` with the trainer's optimizers.  None otherwise"""
+        [refine_start, refine_stop), `refine` with the trainer's optimizers.  With coarsen_every > 0: every coarsen_every steps in
+        [coarsen_start, coarsen_stop), `coarsen` with them, after the statistics and before a refinement of the same step.  None
+        otherwise"""
         c = self.config
-        if c.refine_every <= 0:
+        if c.refine_every <= 0 and c.coarsen_every <= 0:
             return []
         optimizers = training_callback_attributes.optimizers
 
@@ -668,8 +690,17 @@ class TetrahedraNerf(Model):
             if c.refine_start <= step < c.refine_stop and step % c.refine_every == 0:
                 self.refine(optimizers)
 
+        def coarsen(step: int):
+            if c.coarsen_start <= step < c.coarsen_stop and step % c.coarsen_every == 0:
+                self.coarsen(optimizers)
+
         after = [TrainingCallbackLocation.AFTER_TRAIN_ITERATION]
-        return [TrainingCallback(after, lambda step: self.accumulate_refine_statistics()), TrainingCallback(after, refine)]
+        cbs = [TrainingCallback(after, lambda step: self.accumulate_refine_statistics())] if c.refine_every > 0 else []
+        if c.coarsen_every > 0:
+            cbs.append(TrainingCallback(after, coarsen))
+        if c.refine_every > 0:
+            cbs.append(TrainingCallback(after, refine))
+        return cbs
 
     def accumulate_refine_statistics(self) -> None:
         """acc_v += ||dL/dF[:, v]||_2 and cnt_v += 1 where that column is non-zero, from the field gradient of the step that just ran
@@ -764,6 +795,88 @@ class TetrahedraNerf(Model):
                 occ = rf.migrate_cells(occ, pc)
             self.tetrahedra_occupancy.data = occ
         self.tetrahedra_cells.data = cells.contiguous()
+        self.config.num_tetrahedra_vertices, self.config.num_tetrahedra_cells = len(xyz), len(cells)
+        if self._tetrahedra_tracer is not None:
+            self._tetrahedra_tracer.load_tetrahedra(self.tetrahedra_vertices.detach(), self.tetrahedra_cells)
+            self._tracer_vertices = (self.tetrahedra_vertices.data_ptr(), len(xyz), self.tetrahedra_vertices._version)
+            self._keep_guard_start(self.tetrahedra_vertices.detach())
+
+    # ---- mesh coarsening (DESIGN §4.18) --------------------------------------------------------------------------------------------------
+    def coarsen_ready(self) -> bool:
+        """the occupancy buffer describes the field: training has passed occupancy_warmup_steps and the buffer was computed (an all-zero
+        buffer would mark every tetrahedron empty)"""
+        c = self.config
+        return (c.use_occupancy_field and self._occ_ready and self._occ_step > c.occupancy_warmup_steps
+                and bool(self.tetrahedra_occupancy.any()))
+
+    def coarsen(self, optimizers=None) -> Dict[str, Any]:
+        """removes vertices in empty space: up to coarsen_passes passes of `tetranerf.b200.coarsen.coarsen_vertices`, a tetrahedron
+        being empty when its tetrahedra_occupancy is below occupancy_threshold.  Nothing happens until `coarsen_ready()`.  The field, the
+        positions, the occupancy (each tetrahedron keeps its parent's), the refinement statistics and, in `optimizers` (as `refine`),
+        every per-vertex state tensor of the field and vertex parameters (`step` is kept) keep the entries of the surviving vertices.
+        The Parameter objects stay the same; their .grad is cleared; the tracer is reloaded.  -> counts before / after, per-pass
+        proposals and removals, seconds taken ("ready": False when nothing could run), and over all the passes "kept_vertex" / "parent_cell"
+        (the old index of each new vertex / tetrahedron; None when nothing was removed), to carry other per-vertex or per-tetrahedron
+        tensors over"""
+        import time
+
+        from ..b200 import coarsen as cv
+        from ..b200 import refine as rf
+
+        c = self.config
+        if not c.use_occupancy_field:
+            raise RuntimeError("coarsen removes vertices in empty space as the occupancy field sees it: it needs use_occupancy_field=True")
+        t0 = time.perf_counter()
+        V0, T0 = len(self.tetrahedra_vertices), len(self.tetrahedra_cells)
+        res: Dict[str, Any] = {"vertices_before": V0, "tetrahedra_before": T0, "passes": [], "ready": self.coarsen_ready()}
+        dev = self.tetrahedra_field.device
+        if res["ready"]:
+            with torch.no_grad():
+                xyz, cells, occ = self.tetrahedra_vertices.detach(), self.tetrahedra_cells, self.tetrahedra_occupancy
+                kept = parent = None
+                for _ in range(max(0, c.coarsen_passes)):
+                    out = cv.coarsen_vertices(xyz, cells, occ < c.occupancy_threshold)
+                    res["passes"].append({"proposed": out["n_proposed"], "removed": out["n_removed"], "cells_removed": out["n_cells_removed"]})
+                    if out["n_removed"] == 0:
+                        break
+                    k, p = out["kept_vertex"].long(), out["parent_cell"].long()
+                    kept, parent = (k, p) if kept is None else (kept[k], parent[p])
+                    xyz, cells, occ = cv.compact_vertices(xyz, k, 0), out["cells"], rf.migrate_cells(occ, p)
+                if kept is not None:
+                    self._apply_coarsening(kept, parent, xyz, cells, optimizers)
+                res["kept_vertex"], res["parent_cell"] = kept, parent
+        res["vertices_after"], res["tetrahedra_after"] = len(self.tetrahedra_vertices), len(self.tetrahedra_cells)
+        if dev.type == "cuda":
+            torch.cuda.synchronize(dev)
+        res["seconds"] = time.perf_counter() - t0
+        return res
+
+    def _apply_coarsening(self, kept_vertex, parent_cell, xyz, cells, optimizers) -> None:
+        """installs the coarsened mesh (xyz, cells): kept_vertex / parent_cell give the old vertex of each new one and the old tetrahedron
+        of each new one over all the passes"""
+        from ..b200 import coarsen as cv
+        from ..b200 import refine as rf
+
+        params = [(self.tetrahedra_field, 1)] + ([(self.tetrahedra_vertices, 0)] if self.config.optimize_vertices else [])
+        opts = getattr(optimizers, "optimizers", optimizers)
+        opts = list(opts.values()) if isinstance(opts, dict) else ([] if opts is None else [opts])
+        for p, dim in params:
+            old_shape = p.shape
+            for opt in opts:
+                st = opt.state.get(p)
+                for k, v in (st or {}).items():
+                    if isinstance(v, torch.Tensor) and v.shape == old_shape:  # exp_avg, exp_avg_sq (not the scalar step)
+                        st[k] = cv.compact_vertices(v, kept_vertex, dim)
+        V0 = len(self.tetrahedra_vertices)
+        _set_data(self.tetrahedra_field, cv.compact_vertices(self.tetrahedra_field.data, kept_vertex, 1))
+        self.tetrahedra_field.grad = None
+        _set_data(self.tetrahedra_vertices, xyz)
+        self.tetrahedra_vertices.grad = None
+        self.tetrahedra_occupancy.data = rf.migrate_cells(self.tetrahedra_occupancy.data, parent_cell)
+        self.tetrahedra_cells.data = cells.contiguous()
+        if self._grad_acc is not None and len(self._grad_acc) == V0:
+            self._grad_acc = cv.compact_vertices(self._grad_acc, kept_vertex, 0)
+            self._grad_cnt = cv.compact_vertices(self._grad_cnt, kept_vertex, 0)
         self.config.num_tetrahedra_vertices, self.config.num_tetrahedra_cells = len(xyz), len(cells)
         if self._tetrahedra_tracer is not None:
             self._tetrahedra_tracer.load_tetrahedra(self.tetrahedra_vertices.detach(), self.tetrahedra_cells)
