@@ -167,6 +167,34 @@ int tn_coarsen_vertices(int device, const float *d_xyz, uint32_t V, const uint32
                         uint32_t max_removed, uint32_t *d_cells_out, uint32_t *d_kept_vertex, uint32_t *d_parent_cell, uint32_t *counts3,
                         void *d_workspace, size_t *workspace_bytes, void *stream);
 
+/* ---- Delaunay flips: one pass of 2-3 and 3-2 flips of the faces that are not locally Delaunay (DESIGN.md §4.19).  A pure function of
+ * device arrays (no tracer): d_xyz f32[V,3], d_cells u32[T,4].  Face slot 4t + k is the face of cell t opposite its vertex k, keyed by
+ * its ascending vertex triple (a, b, c); the slots are sorted by (a, b, c, slot) with two radix sorts.  One slot: a hull face, never
+ * touched; three or more: TN_ERR_MESH.  An interior face's priority is the position of its first slot in that order (smaller first); t0
+ * owns that slot, t1 the other, d / e are their vertices off the face.  Signs are tn_predicates.cuh's certified orient3d_sign and
+ * insphere_sign (Shewchuk's determinants in float64 on the fp32 positions, each operation rounded on its own; uncertified = 0).
+ *   illegal: t0 and t1 certified and insphere(t0 in cell order, e) certified with t0's sign (e strictly inside t0's circumsphere);
+ *   propose: an illegal face with d, e certified on opposite sides of abc (sigma = orient3d(a,b,c,e)) and orient3d(a,b,d,e),
+ *            (b,c,d,e), (c,a,d,e) all certified.  None differs from sigma (d-e crosses the open triangle abc): a 2-3 flip to (a,b,d,e),
+ *            (b,c,d,e), (c,a,d,e).  Exactly one, for the edge (x, y) of (a,b), (b,c), (c,a), z the third face vertex: a 3-2 flip when t0's
+ *            face (x,y,d) and t1's face (x,y,e) are interior with the same other owner t2 (certified), and, p < q < r the link {z,d,e},
+ *            orient3d(p,q,r,x) and (p,q,r,y) are certified and opposite and orient3d(x,y,p,q), (x,y,q,r), (x,y,r,p) certified and equal
+ *            (x-y crosses the open triangle pqr); it gives (p,q,r,x), (p,q,r,y).  Neither proposes when one of its new interior faces
+ *            ((a,d,e), (b,d,e), (c,d,e) / (p,q,r)) is already a face of the mesh.  Anything else proposes nothing.  A new cell is written
+ *            in that order, its last two entries swapped when its sign differs from the sign of the flip's lowest-slot cell;
+ *   vote:    each cell votes for the highest-priority proposal touching it (2 cells for a 2-3 flip, 3 for a 3-2 flip);
+ *   accept:  a proposal is accepted iff all its cells voted for it (so accepted flips share no cell, and the top proposal is always
+ *            accepted); beyond max_flips the highest-priority accepted flips are kept;
+ *   apply:   a flip's old slots s0 < s1 (< s2) take its first two new cells; a 2-3 flip's third cell goes to T + its rank among the kept
+ *            2-3 flips by priority; a 3-2 flip's s2 is removed by a stable compaction, so T' = T + n23 - n32.
+ * Outputs (capacity T + T/2 cells): d_cells_out[:T'] u32[T',4]; d_sources[:T'] u32[T',3], the old slots each new cell's region came from,
+ * ascending and padded with 0xFFFFFFFF (an unchanged cell: (t, E, E); a 2-3 child: (s0, s1, E); a 3-2 child: (s0, s1, s2)).  counts4
+ * (host) = interior faces certified illegal, proposals, 2-3 flips applied, 3-2 flips applied.  The vertices are untouched; the output
+ * depends on the inputs only, bitwise.  TN_ERR_ARG for a vertex index >= V or T >= 2^29.  Workspace as tn_coarsen_vertices.
+ * Synchronous (two small read-backs). */
+int tn_flip_delaunay(int device, const float *d_xyz, uint32_t V, const uint32_t *d_cells, uint32_t T, uint32_t max_flips, uint32_t *d_cells_out,
+                     uint32_t *d_sources, uint32_t *counts4, void *d_workspace, size_t *workspace_bytes, void *stream);
+
 /* ---- field smoothness along the mesh edges (DESIGN.md §4.15).  Over the unique undirected edges of the loaded mesh (E of them; an edge
  * {i, j} joins two distinct vertices of one cell), with f the field of tn_render_set_field:
  *   S = sum_{i,j} sum_c (f[c,i] - f[c,j])^2,   loss = mult S / (E 64),   d loss / df[c,i] = mult 2 / (E 64) sum_{j in N(i)} (f[c,i] - f[c,j]).

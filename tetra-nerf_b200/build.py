@@ -8,7 +8,7 @@ from pathlib import Path
 HERE = Path(__file__).resolve().parent
 CSRC = HERE / "csrc"
 LIB = CSRC / "libtetranerf_b200.so"
-SOURCES = ["tn_api.cu", "tn_build.cu", "tn_trace.cu", "tn_ops.cu", "tn_find.cu", "tn_render.cu", "tn_mlp_debug.cu", "tn_walk.cu", "tn_faces.cu", "tn_surface.cu", "tn_normals.cu", "tn_ray_grads.cu", "tn_vertex_grads.cu", "tn_refine.cu", "tn_smoothness.cu", "tn_background.cu", "tn_fold_guard.cu", "tn_coarsen.cu"]
+SOURCES = ["tn_api.cu", "tn_build.cu", "tn_trace.cu", "tn_ops.cu", "tn_find.cu", "tn_render.cu", "tn_mlp_debug.cu", "tn_walk.cu", "tn_faces.cu", "tn_surface.cu", "tn_normals.cu", "tn_ray_grads.cu", "tn_vertex_grads.cu", "tn_refine.cu", "tn_smoothness.cu", "tn_background.cu", "tn_fold_guard.cu", "tn_coarsen.cu", "tn_flip.cu"]
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 FLAGS = [*ARCH, "-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC", "-shared"]
 

@@ -27,6 +27,45 @@ __device__ __forceinline__ bool orient3d_sign(const float *__restrict__ xyz, uin
     return sign != 0;
 }
 
+// insphere(a, b, c, d, e): Shewchuk's insphere determinant in float64 on the fp32 positions, positive when e lies inside the sphere
+// through a, b, c, d and orient3d(a, b, c, d) > 0 (the sign flips with that orientation).  Every operation rounded individually, in his
+// order (oracle/flip.py restates it), with his forward error bound (16 + 224 eps) eps * permanent: a sign the bound cannot certify is 0.
+__device__ __forceinline__ bool insphere_sign(const float *__restrict__ xyz, uint32_t ia, uint32_t ib, uint32_t ic, uint32_t id, uint32_t ie,
+                                              int &sign) {
+    auto P = [&](uint32_t v, int a) { return (double)__ldg(xyz + 3 * (size_t)v + a); };
+    const double aex = __dsub_rn(P(ia, 0), P(ie, 0)), aey = __dsub_rn(P(ia, 1), P(ie, 1)), aez = __dsub_rn(P(ia, 2), P(ie, 2));
+    const double bex = __dsub_rn(P(ib, 0), P(ie, 0)), bey = __dsub_rn(P(ib, 1), P(ie, 1)), bez = __dsub_rn(P(ib, 2), P(ie, 2));
+    const double cex = __dsub_rn(P(ic, 0), P(ie, 0)), cey = __dsub_rn(P(ic, 1), P(ie, 1)), cez = __dsub_rn(P(ic, 2), P(ie, 2));
+    const double dex = __dsub_rn(P(id, 0), P(ie, 0)), dey = __dsub_rn(P(id, 1), P(ie, 1)), dez = __dsub_rn(P(id, 2), P(ie, 2));
+    const double aexbey = __dmul_rn(aex, bey), bexaey = __dmul_rn(bex, aey), ab = __dsub_rn(aexbey, bexaey);
+    const double bexcey = __dmul_rn(bex, cey), cexbey = __dmul_rn(cex, bey), bc = __dsub_rn(bexcey, cexbey);
+    const double cexdey = __dmul_rn(cex, dey), dexcey = __dmul_rn(dex, cey), cd = __dsub_rn(cexdey, dexcey);
+    const double dexaey = __dmul_rn(dex, aey), aexdey = __dmul_rn(aex, dey), da = __dsub_rn(dexaey, aexdey);
+    const double aexcey = __dmul_rn(aex, cey), cexaey = __dmul_rn(cex, aey), ac = __dsub_rn(aexcey, cexaey);
+    const double bexdey = __dmul_rn(bex, dey), dexbey = __dmul_rn(dex, bey), bd = __dsub_rn(bexdey, dexbey);
+    const double abc = __dadd_rn(__dsub_rn(__dmul_rn(aez, bc), __dmul_rn(bez, ac)), __dmul_rn(cez, ab));
+    const double bcd = __dadd_rn(__dsub_rn(__dmul_rn(bez, cd), __dmul_rn(cez, bd)), __dmul_rn(dez, bc));
+    const double cda = __dadd_rn(__dadd_rn(__dmul_rn(cez, da), __dmul_rn(dez, ac)), __dmul_rn(aez, cd));
+    const double dab = __dadd_rn(__dadd_rn(__dmul_rn(dez, ab), __dmul_rn(aez, bd)), __dmul_rn(bez, da));
+    auto lift = [](double x, double y, double z) { return __dadd_rn(__dadd_rn(__dmul_rn(x, x), __dmul_rn(y, y)), __dmul_rn(z, z)); };
+    const double alift = lift(aex, aey, aez), blift = lift(bex, bey, bez), clift = lift(cex, cey, cez), dlift = lift(dex, dey, dez);
+    const double det = __dadd_rn(__dsub_rn(__dmul_rn(dlift, abc), __dmul_rn(clift, dab)), __dsub_rn(__dmul_rn(blift, cda), __dmul_rn(alift, bcd)));
+    const double az = fabs(aez), bz = fabs(bez), cz = fabs(cez), dz = fabs(dez);
+    const double ab_ = __dadd_rn(fabs(aexbey), fabs(bexaey)), bc_ = __dadd_rn(fabs(bexcey), fabs(cexbey));
+    const double cd_ = __dadd_rn(fabs(cexdey), fabs(dexcey)), da_ = __dadd_rn(fabs(dexaey), fabs(aexdey));
+    const double ac_ = __dadd_rn(fabs(aexcey), fabs(cexaey)), bd_ = __dadd_rn(fabs(bexdey), fabs(dexbey));
+    auto t3 = [](double p, double x, double q, double y, double r, double z) {
+        return __dadd_rn(__dadd_rn(__dmul_rn(p, x), __dmul_rn(q, y)), __dmul_rn(r, z));
+    };
+    const double perm = __dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(t3(cd_, bz, bd_, cz, bc_, dz), alift), __dmul_rn(t3(da_, cz, ac_, dz, cd_, az), blift)),
+                                            __dmul_rn(t3(ab_, dz, bd_, az, da_, bz), clift)),
+                                  __dmul_rn(t3(bc_, az, ac_, bz, ab_, cz), dlift));
+    const double eps = 1.1102230246251565e-16;  // 2^-53
+    const double bound = __dmul_rn(__dmul_rn(__dadd_rn(16.0, __dmul_rn(224.0, eps)), eps), perm);
+    sign = det > bound ? 1 : (-det > bound ? -1 : 0);
+    return sign != 0;
+}
+
 // the vertex of cell c that is not on face f
 __device__ __forceinline__ uint32_t opposite_vertex(const uint4 c, const uint4 f) {
     const uint32_t cv[4] = {c.x, c.y, c.z, c.w};

@@ -133,7 +133,8 @@ class TetrahedraNerfConfig(ModelConfig):
     endpoints, so the field is unchanged and the optimizer gains degrees of freedom where the images need them.  0 = off, nothing
     changes.  With use_biased_sampler a refined ray shares its samples over more records, so renders are not preserved at the moment of
     refinement (by design; the uniform sampler preserves them).  Refinement raises the number of tetrahedra per ray: watch that
-    max_intersected_triangles still covers the rays.  The refined mesh is no longer Delaunay, which nothing downstream requires"""
+    max_intersected_triangles still covers the rays.  The refined mesh is no longer Delaunay, which nothing downstream requires;
+    delaunay_flip_every > 0 flips it back towards Delaunay at the end of every refinement"""
     refine_start: int = 500
     """first training step at which the mesh may be refined"""
     refine_stop: int = 15000
@@ -161,6 +162,16 @@ class TetrahedraNerfConfig(ModelConfig):
     coarsen_passes: int = 3
     """collapse passes per coarsening; a pass removes vertices that share no tetrahedron, so later passes reach the neighbours of
     vertices an earlier pass kept"""
+    delaunay_flip_every: int = 0
+    """> 0: restore the Delaunay property of the mesh as far as flips can (TetrahedraNerf.flip_delaunay, DESIGN §4.19) every
+    delaunay_flip_every training steps and at the end of every refine() and coarsen() that changed the mesh: 2-3 and 3-2 flips of the
+    faces whose opposite vertex lies inside the other tetrahedron's circumsphere, until a pass proposes nothing.  The vertices, the field
+    and the optimizer state do not change; only the tetrahedra do, each new one taking the maximum occupancy of the ones it replaced.
+    Refinement, coarsening and trained vertex positions all leave non-Delaunay faces behind.  0 = off, nothing changes"""
+    delaunay_flip_max_passes: int = 64
+    """flip passes per flip_delaunay at most; a pass applies flips that share no tetrahedron, so later passes reach the faces an earlier
+    pass created or left.  Meshes refined three times took 29 to 47 passes to the fixed point (DESIGN §4.19); when the limit stops the
+    loop first, flip_delaunay's "illegal_left" counts what was not reached, and the next flip continues from there"""
     background_envmap_height: int = 0
     """> 0: learn the light that leaves the mesh as an environment map: the parameter `background_envmap` f32[H, 2H, 3] (H this value;
     "fields" group, in the state dict only when enabled) in the model's frame, z up, equal-area in latitude, initialised to
@@ -679,10 +690,10 @@ class TetrahedraNerf(Model):
     def get_training_callbacks(self, training_callback_attributes: TrainingCallbackAttributes) -> List[TrainingCallback]:
         """with refine_every > 0: after every training iteration, the field-gradient statistics; every refine_every steps in
         [refine_start, refine_stop), `refine` with the trainer's optimizers.  With coarsen_every > 0: every coarsen_every steps in
-        [coarsen_start, coarsen_stop), `coarsen` with them, after the statistics and before a refinement of the same step.  None
-        otherwise"""
+        [coarsen_start, coarsen_stop), `coarsen` with them, after the statistics and before a refinement of the same step.  With
+        delaunay_flip_every > 0: every delaunay_flip_every steps, `flip_delaunay`, after all of those.  None otherwise"""
         c = self.config
-        if c.refine_every <= 0 and c.coarsen_every <= 0:
+        if c.refine_every <= 0 and c.coarsen_every <= 0 and c.delaunay_flip_every <= 0:
             return []
         optimizers = training_callback_attributes.optimizers
 
@@ -694,12 +705,18 @@ class TetrahedraNerf(Model):
             if c.coarsen_start <= step < c.coarsen_stop and step % c.coarsen_every == 0:
                 self.coarsen(optimizers)
 
+        def flip(step: int):
+            if step > 0 and step % c.delaunay_flip_every == 0:
+                self.flip_delaunay(optimizers)
+
         after = [TrainingCallbackLocation.AFTER_TRAIN_ITERATION]
         cbs = [TrainingCallback(after, lambda step: self.accumulate_refine_statistics())] if c.refine_every > 0 else []
         if c.coarsen_every > 0:
             cbs.append(TrainingCallback(after, coarsen))
         if c.refine_every > 0:
             cbs.append(TrainingCallback(after, refine))
+        if c.delaunay_flip_every > 0:
+            cbs.append(TrainingCallback(after, flip))
         return cbs
 
     def accumulate_refine_statistics(self) -> None:
@@ -759,6 +776,8 @@ class TetrahedraNerf(Model):
                 parent_cells.append(out["parent_cell"])
             if parent_edges:
                 self._apply_refinement(parent_edges, parent_cells, xyz, cells, optimizers)
+                if c.delaunay_flip_every > 0:
+                    res["flip"] = self.flip_delaunay(optimizers)
         res["vertices_after"], res["tetrahedra_after"] = len(self.tetrahedra_vertices), len(self.tetrahedra_cells)
         self._grad_acc = self._grad_cnt = None
         if dev.type == "cuda":
@@ -817,7 +836,8 @@ class TetrahedraNerf(Model):
         The Parameter objects stay the same; their .grad is cleared; the tracer is reloaded.  -> counts before / after, per-pass
         proposals and removals, seconds taken ("ready": False when nothing could run), and over all the passes "kept_vertex" / "parent_cell"
         (the old index of each new vertex / tetrahedron; None when nothing was removed), to carry other per-vertex or per-tetrahedron
-        tensors over"""
+        tensors over.  With delaunay_flip_every > 0 the coarsened mesh is then flipped ("flip": flip_delaunay's result); "parent_cell"
+        describes the coarsened tetrahedra before that flip, and the installed ones only when "flip" made no change"""
         import time
 
         from ..b200 import coarsen as cv
@@ -844,6 +864,8 @@ class TetrahedraNerf(Model):
                     xyz, cells, occ = cv.compact_vertices(xyz, k, 0), out["cells"], rf.migrate_cells(occ, p)
                 if kept is not None:
                     self._apply_coarsening(kept, parent, xyz, cells, optimizers)
+                    if c.delaunay_flip_every > 0:
+                        res["flip"] = self.flip_delaunay(optimizers)
                 res["kept_vertex"], res["parent_cell"] = kept, parent
         res["vertices_after"], res["tetrahedra_after"] = len(self.tetrahedra_vertices), len(self.tetrahedra_cells)
         if dev.type == "cuda":
@@ -881,6 +903,65 @@ class TetrahedraNerf(Model):
         if self._tetrahedra_tracer is not None:
             self._tetrahedra_tracer.load_tetrahedra(self.tetrahedra_vertices.detach(), self.tetrahedra_cells)
             self._tracer_vertices = (self.tetrahedra_vertices.data_ptr(), len(xyz), self.tetrahedra_vertices._version)
+            self._keep_guard_start(self.tetrahedra_vertices.detach())
+
+    # ---- Delaunay flips (DESIGN §4.19) ---------------------------------------------------------------------------------------------------
+    def flip_delaunay(self, optimizers=None) -> Dict[str, Any]:
+        """flips the mesh towards Delaunay: passes of `tetranerf.b200.flip.flip_delaunay` until one proposes nothing, at most
+        delaunay_flip_max_passes.  Only the tetrahedra change: the occupancy of each new one is the maximum over the ones its region came
+        from, the tracer is reloaded and the fold guard restarts from the current positions; the positions, the field, the optimizer state
+        (`optimizers` is accepted for the callbacks' sake and left alone) and the refinement statistics are untouched.  When the first
+        pass proposes nothing, nothing is installed.  With optimize_vertices, a vertex step the tracer has not refit yet (an optimizer
+        step since the last forward) first goes through the refit and, with vertex_fold_guard, its guard, so the flips see the positions
+        the next forward would trace and the guard's start is never skipped.  -> counts before / after, per-pass counts (illegal faces,
+        proposals, 2-3 and 3-2 flips), "illegal_left" (faces still certified illegal at the end: stuck ones that no flip of the definition
+        removes, or not yet reached when the pass limit stopped the loop) and the seconds taken"""
+        import time
+
+        from ..b200 import flip as fl
+
+        c = self.config
+        t0 = time.perf_counter()
+        T0 = len(self.tetrahedra_cells)
+        res: Dict[str, Any] = {"tetrahedra_before": T0, "passes": []}
+        dev = self.tetrahedra_field.device
+        if self._tetrahedra_tracer is not None and c.optimize_vertices:
+            self.get_tetrahedra_tracer()  # guard and refit a pending vertex step before flipping on its positions
+        with torch.no_grad():
+            xyz, cells = self.tetrahedra_vertices.detach().contiguous(), self.tetrahedra_cells
+            occ = self.tetrahedra_occupancy.data if c.use_occupancy_field else None
+            changed = False
+            left = None
+            for _ in range(max(0, c.delaunay_flip_max_passes)):
+                out = fl.flip_delaunay(xyz, cells)
+                res["passes"].append({"illegal": out["n_illegal"], "proposed": out["n_proposed"], "flips_23": out["n_23"], "flips_32": out["n_32"]})
+                if out["n_proposed"] == 0:
+                    left = out["n_illegal"]
+                    break
+                changed = True
+                cells = out["cells"]
+                if occ is not None:
+                    occ = fl.migrate_cells_max(occ, out["sources"])
+            if left is None and changed:  # stopped by the pass limit: count what is left without flipping
+                left = fl.flip_delaunay(xyz, cells, max_flips=0)["n_illegal"]
+            if changed:
+                self._apply_flips(cells, occ)
+        res["illegal_left"] = left if left is not None else 0
+        res["tetrahedra_after"] = len(self.tetrahedra_cells)
+        if dev.type == "cuda":
+            torch.cuda.synchronize(dev)
+        res["seconds"] = time.perf_counter() - t0
+        return res
+
+    def _apply_flips(self, cells, occupancy=None) -> None:
+        """installs the flipped cells over the same vertices, with the migrated occupancy (None: without the occupancy field)"""
+        if occupancy is not None:
+            self.tetrahedra_occupancy.data = occupancy
+        self.tetrahedra_cells.data = cells.contiguous()
+        self.config.num_tetrahedra_cells = len(cells)
+        if self._tetrahedra_tracer is not None:
+            self._tetrahedra_tracer.load_tetrahedra(self.tetrahedra_vertices.detach(), self.tetrahedra_cells)
+            self._tracer_vertices = (self.tetrahedra_vertices.data_ptr(), len(self.tetrahedra_vertices), self.tetrahedra_vertices._version)
             self._keep_guard_start(self.tetrahedra_vertices.detach())
 
     # ---- geometry export -----------------------------------------------------------------------------------------------------------------

@@ -85,6 +85,7 @@ _lib.tn_render_set_occupancy2.argtypes = [_vp, _vp, C.c_float, _i]
 _lib.tn_field_smoothness.argtypes = [_vp, C.c_float, _vp, _vp, C.POINTER(_u32), _vp]
 _lib.tn_refine_edges.argtypes = [_i, _vp, _u32, _vp, _u32, _vp, C.c_float, _u32, _vp, _vp, _vp, C.POINTER(_u32), _vp, C.POINTER(C.c_size_t), _vp]
 _lib.tn_coarsen_vertices.argtypes = [_i, _vp, _u32, _vp, _u32, _vp, _u32, _vp, _vp, _vp, C.POINTER(_u32), _vp, C.POINTER(C.c_size_t), _vp]
+_lib.tn_flip_delaunay.argtypes = [_i, _vp, _u32, _vp, _u32, _u32, _vp, _vp, C.POINTER(_u32), _vp, C.POINTER(C.c_size_t), _vp]
 
 LIBRARY_PATH = str(_LIB_PATH)
 
